@@ -49,7 +49,7 @@ from vidu4d_b200.synthetic import SurfelCloud, object_scene, orbit_view, project
 
 NVIEWS = 64
 TAN = 0.5
-L2_MB = 126
+L2_MB = 50          # H100 SXM
 
 
 def parse():
@@ -76,12 +76,15 @@ def parse():
     ap.add_argument("--no-fused", action="store_true", help="e2e through render() instead of render_fused()")
     ap.add_argument("--e2e-streams", type=int, default=1, help="(debug) streams of the eager e2e step when --no-graph")
     ap.add_argument("--streams", type=int, default=8, help="CUDA streams the frames of a step alternate over (value arm)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps of the value arm, write what its last step computed (rendered planes, radii, "
+                         "surfel gradients) as DIR/<name>.npy, float32, at most 64 MB in all")
     return ap.parse_args()
 
 
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region (read-only queries, stopped with the run)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -105,6 +108,8 @@ class ClockSampler:
         if not self.proc:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         self.proc.terminate()
+        self.proc.wait()
+        self.proc = None
         sm, mx, reasons = [], [], set()
         for r in self.rows:
             f = [x.strip() for x in r.split(",")]
@@ -144,6 +149,23 @@ def max_over_ranks(ms: float, world: int, device) -> float:
     t = torch.tensor([ms], dtype=torch.float64, device=device)
     torch.distributed.all_reduce(t, op=torch.distributed.ReduceOp.MAX)
     return float(t.item())
+
+
+DUMP_BYTES = 60_000_000
+
+
+def dump_outputs(path, arrays):
+    """Write each array as path/<name>.npy in float32.  Every array gets an equal share of DUMP_BYTES; a larger one is
+    written as the same seeded sample of its flattened elements (ascending index order) on every run, so that two builds
+    given the same arguments can be compared output for output."""
+    os.makedirs(path, exist_ok=True)
+    cap = DUMP_BYTES // (4 * max(1, len(arrays)))
+    for name, t in arrays.items():
+        a = t.detach().reshape(-1)
+        if a.numel() > cap:
+            idx = torch.randperm(a.numel(), generator=torch.Generator().manual_seed(0))[:cap].sort().values
+            a = a[idx.to(a.device)]
+        np.save(os.path.join(path, name + ".npy"), a.to(torch.float32).cpu().numpy())
 
 
 # ------------------------------------------------------------------------------------------------
@@ -192,7 +214,7 @@ def main():
     g = torch.Generator(device=device).manual_seed(1234)
     dLc = torch.randn((3, RES, RES), device=device, generator=g)
     dLo = torch.randn((8, RES, RES), device=device, generator=g) * 0.1
-    flush = torch.empty((256 << 20,), dtype=torch.uint8, device=device)     # > L2 (126 MB)
+    flush = torch.empty((256 << 20,), dtype=torch.uint8, device=device)     # > L2 (50 MB)
     e = torch.empty((0,), device=device)
 
     with torch.no_grad():
@@ -258,6 +280,8 @@ def main():
     dLo_b = dLo.expand(F, -1, -1, -1).contiguous() if BATCH else None
     value_graph = [None]
     R_last_box = [0]
+    last_fwd = [None, None]     # forward outputs of the value-arm step, per flat-buffer slot (graph outputs stay live)
+    last_slot = [0]
 
     SPLIT = max(1, args.split) if BATCH else 1
     split_rows = torch.zeros((SPLIT, nflt), device=device) if SPLIT > 1 else None
@@ -287,6 +311,7 @@ def main():
             for k in range(SPLIT):
                 main.wait_stream(side[k])
             torch.sum(split_rows, dim=0, out=flat_acc)
+            last_fwd[slot] = o
             return o
         o = C.rasterize_gaussians_batch(bg, t_in["means3D"], e, t_in["opac"], t_in["scales"], t_in["rots"], 1.0, vm_b, pm_b,
                                         TAN, TAN, RES, RES, t_in["shs"], 3, cp_b)
@@ -298,6 +323,8 @@ def main():
         if n != F:      # the 1- and 2-frames-per-call variants: several calls per step accumulate into the flat buffer
             for a_, gi in zip(flat_views, GIDX):
                 a_.add_(gr[gi].reshape(a_.shape))
+        else:
+            last_fwd[slot] = o
         return o
 
     # Two captures of the same step, used alternately, each with its own pinned status words and a "done" event: the host
@@ -330,6 +357,7 @@ def main():
         if BATCH:
             if value_graph[0] is not None:
                 k = step & 1
+                last_slot[0] = k
                 value_graphs[k].replay()
                 if world > 1:
                     # step k's all-reduce (its own flat buffer) goes to the communication stream and overlaps step k+1's
@@ -347,6 +375,7 @@ def main():
                 drain()                     # step k-1 (the other graph): its words landed long ago
                 inflight[0] = k
                 return R_last
+            last_slot[0] = 0
             batch_body()
             if world > 1:
                 torch.distributed.all_reduce(flat_acc)
@@ -361,6 +390,7 @@ def main():
             ctx = torch.cuda.stream(side[k]) if NS > 1 else contextlib.nullcontext()
             with ctx:
                 o, gr = frame_dev(view_of(step, f))
+                last_fwd[0] = o
                 for a_, gi in zip(accs[k], GIDX):
                     if f < NS:
                         a_.copy_(gr[gi].view(a_.shape))
@@ -453,10 +483,22 @@ def main():
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
+        import atexit
+        atexit.register(sampler.stop)       # never leave the sampler running if the run fails
     launches0 = _capi.launch_count() if args.impl == "ours" else 0
     if BATCH:
         arm(value_graph[0])
     total_ms, per_ms, wall_ms = timed(step_dev, K, Wm)
+    if args.dump_outputs:
+        # what a caller of the timed step receives: the last step's rendered planes and radii (all of its frames in batch
+        # mode, its last frame otherwise) and the surfel gradients summed over the step's frames
+        torch.cuda.synchronize()
+        o = last_fwd[last_slot[0]]
+        outs = {"color": o[1], "allmap": o[2], "radii": o[3]}
+        grads = flat_outss[last_slot[0]] if (BATCH and SPLIT == 1) else flat_outs
+        outs.update({"grad_" + k[4:]: v for k, v in grads.items()})
+        if rank == 0:
+            dump_outputs(args.dump_outputs, outs)
     launches = (_capi.launch_count() - launches0) if args.impl == "ours" else None
     if BATCH and value_graph[0] is not None:
         launches = value_graph[0].launches * K          # graph replays do not pass through the library's host-side counter
@@ -762,8 +804,8 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "MEASURED_PEAKS.json (measured)" if peaks else "B200_PROFILING.md fallback 6650 GB/s"
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "MEASURED_PEAKS.json (measured)" if peaks else "H100 SXM data sheet, 3350 GB/s"
     N = RES * RES
     if args.impl == "ours" and rank == 0:
         # The same step as the timed region, eager, with the library's per-kernel CUDA events switched on
@@ -803,29 +845,15 @@ def main():
                 kernels[k]["impl_MB_per_launch"] = round(impl[k] * Fl / 1e6, 2)
         dom = max(kernels, key=lambda k: kernels[k]["ms_per_launch"])
         ach = kernels[dom]["GBps"]
-        ncu = {}
-        try:   # counters of that kernel from the committed `ncu --set full` capture (per launch of ONE frame)
-            ncu = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json"))).get(dom, {})
-        except Exception:
-            pass
-        # the capture is of a batch of `frames_per_launch` frames per launch: rescale to this run's launch
-        nfl = float(ncu.get("frames_per_launch", 1) or 1)
-        traffic = ncu.get("dram_bytes_per_launch")
-        if traffic is not None:
-            traffic = int(traffic * Fl / nfl)
         frame_alg = 1002 * P + 324 * R_inst + 128 * N
         roofline = {"kernel": dom, "bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s",
-                    "frac": round(ach / hbm_peak, 5), "traffic": traffic, "peak_source": peak_src,
+                    "frac": round(ach / hbm_peak, 5), "peak_source": peak_src,
                     "alg_bytes_per_launch": alg.get(dom, 0) * Fl, "impl_bytes_per_launch": impl.get(dom, alg.get(dom, 0)) * Fl,
                     "launch_ms": kernels[dom]["ms_per_launch"], "frames_per_launch": Fl,
-                    "traffic_note": "dram__bytes_read+write of this kernel's launch from the committed ncu --set full capture "
-                                    "(profiles/ncu_traffic.json), rescaled to this run's frames per launch",
-                    "l2_red_sectors": (None if ncu.get("l2_red_sectors") is None else int(ncu["l2_red_sectors"] * Fl / nfl)),
-                    "lanes_active": ncu.get("lanes_active"),
                     "contributing_pairs": pairs_contrib, "visible_surfels": Vv,
                     "note": "the composite kernels are FP32-issue / latency bound by construction (SURVEY 8d): each instance record "
                             "is read once per tile but evaluated against ~10 pixels; algorithmic HBM bytes are small. "
-                            "pairs/s is the explanatory figure, profiles/ holds the ncu pipe utilisation",
+                            "pairs/s is the explanatory figure",
                     "contributing_pairs_per_s": round(pairs_contrib * (K * F * world) / (total_ms * 1e-3), 0),
                     "pair_evals_upper_per_frame": pair_upper,
                     "frame_alg_MB": round(frame_alg / 1e6, 1),
@@ -850,7 +878,7 @@ def main():
                     acc[0].add_(gr[3]); acc[1].add_(gr[5]); acc[2].add_(gr[2]); acc[3].add_(gr[6]); acc[4].add_(gr[7])
             rt, _, _ = timed(ref_step, max(3, K // 2), 3)
             reference_cuda = {"value": round(max(3, K // 2) * F / (rt * 1e-3), 2), "unit": "frames/s",
-                              "what": "unmodified reference extension (oracle/_ref/_C.so, sm_100a), same frames, device-resident"}
+                              "what": "unmodified reference extension (oracle/_ref/_C.so, sm_90a), same frames, device-resident"}
         except Exception as ex:  # pragma: no cover
             reference_cuda = {"unavailable": repr(ex)}
 

@@ -1,5 +1,5 @@
 """Drop-in shim: `from diff_surfel_rasterization import GaussianRasterizationSettings, GaussianRasterizer`
-(gs/gaussian_renderer/__init__.py:14 of yikaiw/Vidu4D) resolves to the B200-native implementation when this
+(gs/gaussian_renderer/__init__.py:14 of yikaiw/Vidu4D) resolves to the H100-native implementation when this
 repository's root is on sys.path ahead of the reference package."""
 from vidu4d_b200.rasterizer import (  # noqa: F401
     GaussianRasterizationSettings,

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Stage-3 stand-in (BASELINE.json configs[2]): the warp -> rasterize -> loss -> Adam inner loop of
-`lab4d/train.py --fg_motion gs-bob` on synthetic data, with the B200 rasterizer dropped in.
+`lab4d/train.py --fg_motion gs-bob` on synthetic data, with this rasterizer dropped in.
 
 What is mirrored from the reference (behaviour, not code):
   * canonical surfels warped per frame by a bag-of-bones dual-quaternion skinning field, kept in PyTorch as

@@ -6,7 +6,7 @@ backward -> Adam -- on a synthetic 32-frame sequence, 300 K surfels, 256x256, M 
   reference   PyTorch warp (the reference's expressions: lab4d/utils/geom_utils.py:48-92, lab4d/nnutils/skinning.py:89-142,
               lab4d/nnutils/deformable_gaussian.py:1033-1046,1395-1434) + the UNMODIFIED reference rasterizer
               (oracle/_ref/_C.so through render()) frame by frame + torch losses
-  ours        the same PyTorch warp + render_loss_batch (batched B200 rasterizer, fused post-processing + losses)
+  ours        the same PyTorch warp + render_loss_batch (batched rasterizer, fused post-processing + losses)
   ours_fused  fused warp kernel (csrc/warp.cu) + render_loss_batch
   ours_full   ours_graph + FlatSurfelModel: flat parameter buffer, one-kernel Adam, densification statistics in the captured step
               (`ours_full_densify`: one densify_and_prune + graph re-capture in the middle of the timed loop)

@@ -1,5 +1,5 @@
 /*
- * surfel_raster.h -- C ABI of the B200-native Gaussian-surfel rasterizer.
+ * surfel_raster.h -- C ABI of the H100-native Gaussian-surfel rasterizer.
  *
  * This is the drop-in boundary for the hot path of yikaiw/Vidu4D's Stage-3
  * ("dynamic Gaussian surfels"): it replaces

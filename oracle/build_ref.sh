@@ -1,16 +1,16 @@
 #!/usr/bin/env bash
 # Build the UNMODIFIED reference rasterizer extension (yikaiw/Vidu4D,
-# gs/submodules/diff-surfel-rasterization) for sm_100a, straight from the
-# sources where they lie under /root/reference, into oracle/_ref/ (git-ignored,
-# travels to the GPU box with gpurun).  No reference source is copied: only the
-# compiled pybind module `_C.so` lands in oracle/_ref/.
+# gs/submodules/diff-surfel-rasterization) for sm_90a (H100), straight from the
+# reference checkout named by REF_ROOT, into oracle/_ref/ (git-ignored build
+# product).  No reference source is copied: only the compiled pybind module
+# `_C.so` lands in oracle/_ref/.
 #
 # This is TEST/BENCH INFRASTRUCTURE (the parity checker and the "reference arm"
 # of bench.py).  Nothing in vidu4d_b200/ may import it.
 #
 # The only deviation from the reference's own setup.py is `-include cstdint`
 # (rasterizer_impl.h:24 uses std::uintptr_t / uint32_t without the header; GCC 13
-# rejects that) and an explicit -gencode for sm_100a.  Device-code flags are
+# rejects that) and an explicit -gencode for sm_90a.  Device-code flags are
 # nvcc defaults (-O3, -fmad=true, IEEE div/sqrt), as setup.py:30 leaves them.
 set -euo pipefail
 REF=${REF_ROOT:-/root/reference}/gs/submodules/diff-surfel-rasterization
@@ -29,7 +29,7 @@ INCS=""
 IFS=':' read -ra PARTS <<<"$TORCH_INC"; for p in "${PARTS[@]}"; do INCS="$INCS -I$p"; done
 COMMON="-std=c++17 -include cstdint -I$REF/third_party/glm/ -I$REF $INCS -I$PY_INC -I/usr/local/cuda/include \
  -DTORCH_EXTENSION_NAME=_C -DTORCH_API_INCLUDE_EXTENSION_H -D_GLIBCXX_USE_CXX11_ABI=1"
-NVFLAGS="-gencode arch=compute_100a,code=sm_100a --expt-relaxed-constexpr -Xcompiler -fPIC -lineinfo \
+NVFLAGS="-gencode arch=compute_90a,code=sm_90a --expt-relaxed-constexpr -Xcompiler -fPIC -lineinfo \
  -D__CUDA_NO_HALF_OPERATORS__ -D__CUDA_NO_HALF_CONVERSIONS__ -D__CUDA_NO_BFLOAT16_CONVERSIONS__ -D__CUDA_NO_HALF2_OPERATORS__"
 pids=()
 for f in cuda_rasterizer/forward.cu cuda_rasterizer/backward.cu cuda_rasterizer/rasterizer_impl.cu rasterize_points.cu; do

@@ -32,7 +32,7 @@
  *
  * Parity pinning: the reference ships NO tests / golden vectors for this path
  * (SURVEY.md section 4).  The oracle is pinned instead against outputs of the
- * unmodified reference extension itself, run on a B200 by
+ * unmodified reference extension itself (its sm_100a build), made by
  * tests/golden/make_golden.py and committed under tests/golden/ (see DESIGN.md).
  *
  * Numerical notes (why CPU and GPU can differ in the last ulp): the reference

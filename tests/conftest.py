@@ -13,7 +13,7 @@ GOLDEN_CASES = ["id_deg3_64", "rigid_bg_96x64", "ragged_80x48_deg1", "precomp_in
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `pytest -m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; run with `pytest -m gpu`)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -2,11 +2,13 @@
 
 The reference (yikaiw/Vidu4D, gs/submodules/diff-surfel-rasterization) has no tests or golden vectors for
 this path (SURVEY.md section 4), and it has no CPU implementation, so its outputs can only be produced on a
-GPU.  This script runs the UNMODIFIED reference extension (oracle/_ref/_C.so, built by oracle/build_ref.sh
-for sm_100a) on seeded scenes on the B200 box and stores inputs + every output / intermediate buffer:
+GPU.  This script runs the UNMODIFIED reference extension (oracle/_ref/_C.so, built by oracle/build_ref.sh) on seeded
+scenes and stores inputs + every output / intermediate buffer:
 
-    gpurun -- python tests/golden/make_golden.py          # writes gpurun_out/golden/*.npz
-    cp gpurun_out/golden/*.npz tests/golden/              # commit
+    python tests/golden/make_golden.py OUTDIR   # writes OUTDIR/*.npz; copy them to tests/golden/ to replace the fixtures
+
+The committed fixtures come from the reference compiled for sm_100a, whose FMA contraction the kernels follow bit for
+bit; the reference compiled for sm_90a differs from them in the last bits of its float buffers.
 
 Fixtures are small (<= ~1.5K surfels, <= 96x64 px).  tests/test_oracle_golden.py (CPU) checks the oracle
 against them; tests/test_gpu_parity.py (GPU) checks the CUDA library against them and against the live
@@ -85,9 +87,8 @@ def run_reference(inp, dev):
     return out
 
 
-def main():
+def main(outdir):
     dev = torch.device("cuda:0")
-    outdir = os.path.join(ROOT, "gpurun_out", "golden")
     os.makedirs(outdir, exist_ok=True)
     for name, kw in CASES.items():
         inp = build_case(**kw)
@@ -98,4 +99,6 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    if len(sys.argv) != 2:
+        sys.exit("usage: python tests/golden/make_golden.py OUTDIR")
+    main(sys.argv[1])

@@ -1,7 +1,7 @@
 """2-GPU NCCL test of SURVEY.md section 8(e)'s parity check with the CUDA path: frames sharded over two ranks, each rank
 renders its frames with ONE batched launch set (render_loss_batch), gradients land in the flat buffer, one NCCL
 all-reduce -- the summed FlatGrads must equal one GPU looping over the same frames, to 1e-5 relative (fp32 summation
-order).  Skipped on boxes with fewer than 2 GPUs (the driver's 1-GPU run); `gpurun --gpus 2` runs it."""
+order).  Skipped on machines with fewer than 2 GPUs."""
 import os
 import sys
 
@@ -59,7 +59,7 @@ def _worker(rank, world, port, out):
 @pytest.mark.timeout(600)
 def test_two_gpu_nccl_allreduce_equals_one_gpu_loop(built, tmp_path):
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run with `gpurun --gpus 2`)")
+        pytest.skip("needs 2 GPUs")
     out = str(tmp_path / "flat.npy")
     port = 29700 + (os.getpid() % 200)
     mp.start_processes(_worker, args=(2, port, out), nprocs=2, join=True, start_method="spawn")

@@ -2,10 +2,10 @@
 libsurfel_raster.so), against
   (1) the committed golden fixtures = outputs of the unmodified reference extension (tests/golden/),
   (2) the CPU oracle on seeded inputs at sizes it finishes in seconds,
-  (3) the live reference extension when oracle/_ref/_C.so travelled with the repo (config C2: 100 K surfels, 512^2),
+  (3) a stored record of the reference extension's outputs at config C2 (100 K surfels, 512^2),
   (4) size-independent properties at BASELINE.json's full size (300 K surfels, 512^2).
 Bar: integer/index work bit-exact; float buffers and gradients within 1e-4 relative (north_star), with the
-tolerance written at each assert.  Nothing here reads /root/reference.
+tolerance written at each assert.  Everything compared against is stored under tests/golden/.
 """
 import os
 
@@ -17,6 +17,10 @@ from .conftest import GOLDEN_CASES, load_golden
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4
+# The kernels follow the FMA contraction of the reference compiled for sm_100a, and reproduce the sm_100a fixtures bit for
+# bit (test_against_reference_golden).  The reference compiled for sm_90a contracts differently: against its records the
+# planes that match the sm_100a build bit for bit differ by a few ulp (measured: <= 8.7e-6 of the plane's max on an H100).
+XBUILD_TOL = 2e-5
 GRADS = ("dL_dmeans2D", "dL_dcolors", "dL_dopacity", "dL_dmeans3D", "dL_dtransMat", "dL_dsh", "dL_dscales", "dL_drotations")
 
 
@@ -72,6 +76,29 @@ def _assert_n_contrib(mine, ref, ranges, W, H):
     nonempty = (rg[:, 1] - rg[:, 0])[t] > 0
     np.testing.assert_array_equal(mine[1][nonempty], ref[1][nonempty])
     assert (mine[1][~nonempty] == 0).all()
+
+
+def _assert_matches_record(r, rec, W, H, near=()):
+    """r: _run_ours() output; rec: a tests/golden/ref_*.npz record (tests/golden/make_reference_records.py).  Index work
+    bit-exact (by digest); every float tensor within TOL of its max magnitude (XBUILD_TOL for the tensors in `near`) at the
+    recorded indices and in that max magnitude."""
+    from tests.golden.make_reference_records import exact_digests, float_tensors
+    assert r["num_rendered"] == int(rec["num_rendered"][0])
+    mine = exact_digests(_np(r["radii"]), _np(r["keys"]), _np(r["point_list"]), _np(r["ranges"]), _np(r["n_contrib"]), W, H)
+    for k, d in mine.items():
+        assert np.array_equal(d, rec["sha_" + k]), f"{k} differs from the reference"
+    nc, rg = _np(r["n_contrib"]), _np(r["ranges"]).astype(np.int64)
+    ys, xs = np.mgrid[0:H, 0:W]
+    empty = (rg[:, 1] == rg[:, 0])[(ys // 16) * ((W + 15) // 16) + xs // 16]
+    assert (nc[1][empty] == 0).all()                  # median contributor of an empty tile: 0 (see _assert_n_contrib)
+    for k, v in float_tensors(_np(r["color"]), _np(r["allmap"]), {g: _np(r["grads"][g]) for g in GRADS}).items():
+        idx, want, mx = rec["idx_" + k], rec["val_" + k], float(rec["max_" + k][0])
+        if idx.size == 0:
+            continue
+        tol = (XBUILD_TOL if k in near else TOL) * max(mx, 1e-30)
+        flat = v.reshape(-1)
+        assert np.abs(flat[idx] - want).max() <= tol, k
+        assert abs(float(np.abs(flat).max()) - mx) <= tol, k
 
 
 def _assert_close_robust(mine, ref, tol, what, outlier_frac=2e-4, outlier_tol=5e-2):
@@ -147,26 +174,13 @@ def test_against_cpu_oracle(P, W, H, seed, rigid, dev):
         _assert_close_robust(_np(r["grads"][k]), og[k], TOL, k)
 
 
-# ----------------------------------------------------------------------------------------------- (3) live reference
-def test_against_live_reference_c2(dev):
-    from oracle import ref_ext
-    if not ref_ext.available():
-        pytest.skip("oracle/_ref/_C.so not present on this box")
-    from tests.golden.make_golden import build_case, run_reference
+# ----------------------------------------------------------------------------------------------- (3) reference record
+def test_against_reference_record_c2(dev):
+    """Config C2 against the reference extension's stored outputs: index work bit-exact, colour within XBUILD_TOL, every
+    allmap plane and gradient within TOL of its max."""
+    from tests.golden.make_golden import build_case
     inp = build_case(100_000, 512, 512, 31, rigid=True)          # BASELINE config[1]
-    ref = run_reference(inp, dev)
-    r = _run_ours(inp, dev)
-    assert r["num_rendered"] == int(ref["num_rendered"][0])
-    for a, b in ((r["radii"], ref["radii"]), (r["keys"], ref["bin_keys"]), (r["point_list"], ref["bin_point_list"]),
-                 (r["ranges"], ref["img_ranges"])):
-        np.testing.assert_array_equal(_np(a), b)
-    _assert_n_contrib(_np(r["n_contrib"]), ref["img_n_contrib"], ref["img_ranges"], 512, 512)
-    assert np.array_equal(_np(r["color"]), ref["color"])
-    assert np.abs(_np(r["allmap"]) - ref["allmap"]).max() <= TOL * np.abs(ref["allmap"]).max()
-    for k in GRADS:
-        b = ref["grad_" + k]
-        a = _np(r["grads"][k]).reshape(b.shape)
-        assert np.abs(a - b).max() <= TOL * (np.abs(b).max() + 1e-30), k
+    _assert_matches_record(_run_ours(inp, dev), load_golden("ref_c2_100k"), 512, 512, near=("color",))
 
 
 # ----------------------------------------------------------------------------------------------- (4) full size

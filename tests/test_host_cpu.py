@@ -125,7 +125,7 @@ def test_product_does_not_import_oracle():
             if f.endswith((".py", ".cu", ".cuh", ".h")):
                 src = open(os.path.join(dirpath, f)).read()
                 assert "surfel_oracle" not in src and "from oracle" not in src and "import oracle" not in src, f
-    assert "oracle" not in open(os.path.join(ROOT, "diff_surfel_rasterization", "__init__.py")).read().replace("B200-native", "")
+    assert "oracle" not in open(os.path.join(ROOT, "diff_surfel_rasterization", "__init__.py")).read().replace("H100-native", "")
 
 
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):

@@ -1,7 +1,7 @@
 """CPU: pin the oracle (oracle/surfel_oracle.c) to outputs of the UNMODIFIED reference extension.
 
-The fixtures in tests/golden/*.npz were produced on a B200 by tests/golden/make_golden.py from
-oracle/_ref/_C.so (the reference has no tests or golden vectors of its own for this path, SURVEY.md section 4).
+The fixtures in tests/golden/*.npz were produced by tests/golden/make_golden.py from the reference extension compiled
+for sm_100a (oracle/_ref/_C.so) (the reference has no tests or golden vectors of its own for this path, SURVEY.md section 4).
 Integer / index work must be bit-exact; float buffers within 1e-4 (north_star tolerance), in practice ~1e-6.
 """
 import numpy as np

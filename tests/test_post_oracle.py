@@ -1,7 +1,7 @@
 """CPU tests pinning oracle/post_oracle.py (float64 NumPy restatement of the reference's render() post-processing and
 Stage-3 image losses):
   (1) against fixtures produced by the REFERENCE's own code (tests/golden/make_post_golden.py executes the source text
-      of gs/utils/point_utils.py and of render() lines 121-145 from /root/reference on the CPU);
+      of gs/utils/point_utils.py and of render() lines 121-145 from the reference checkout on the CPU);
   (2) its hand-written vector-Jacobian products against central finite differences in float64.
 """
 import os

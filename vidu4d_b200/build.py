@@ -1,6 +1,6 @@
-"""Build vidu4d_b200/lib/libsurfel_raster.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build vidu4d_b200/lib/libsurfel_raster.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
-nvcc cross-compiles without a GPU.  The .so is git-ignored but travels to the GPU box with gpurun.
+nvcc cross-compiles without a GPU.  The .so is a build product (git-ignored); build() recompiles whatever is stale.
 Usage: python -m vidu4d_b200.build [--force] [--verbose]
 """
 from __future__ import annotations
@@ -20,7 +20,7 @@ SOURCES = ["api.cu", "preprocess.cu", "sort.cu", "composite_fwd.cu", "composite_
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "composite_common.cuh"), os.path.join(CSRC, "post_common.cuh"),
            os.path.join(HERE, "..", "include", "surfel_raster.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
     # no --use_fast_math: expf / div / sqrt must be the same IEEE / libdevice variants the reference build uses
 ]
@@ -46,8 +46,13 @@ def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(objdir, exist_ok=True)
     nvcc = _nvcc()
     env = dict(os.environ)
-    # the image exports CC/CXX=/opt/gcc/bin/*, nvcc's host compiler should be the system g++
+    # nvcc's host compiler is the system g++ even where CC/CXX point at another toolchain
     ccbin = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else None
+    # objects compiled with other flags (another target architecture) are stale whatever their mtime
+    stamp = os.path.join(objdir, "flags")
+    flags = " ".join(NVCC_FLAGS)
+    if not os.path.exists(stamp) or open(stamp).read() != flags:
+        force = True
 
     def compile_one(src):
         s = os.path.join(CSRC, src)
@@ -68,6 +73,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
         r = subprocess.run(cmd, capture_output=True, text=True, env=env)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
+    with open(stamp, "w") as f:
+        f.write(flags)
     return LIB
 
 

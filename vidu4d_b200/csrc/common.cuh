@@ -1,4 +1,4 @@
-// common.cuh -- shared definitions for the sm_100a surfel rasterizer kernels.
+// common.cuh -- shared definitions for the sm_90a surfel rasterizer kernels.
 //
 // Vocabulary follows the reference (RAST = gs/submodules/diff-surfel-rasterization):
 //   surfel    one 2D Gaussian disc (P of them)
@@ -233,7 +233,7 @@ __device__ __forceinline__ float4 ld_nc_f4(const float4* p) {
 }
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// mbarrier + bulk async copy (TMA 1-D) -- sm_90+/sm_100a
+// mbarrier + bulk async copy (TMA 1-D) -- sm_90+
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }

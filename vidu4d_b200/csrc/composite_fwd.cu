@@ -2,7 +2,7 @@
 //
 // Replaces (behaviour, not code) of the reference's forward renderCUDA, RAST/cuda_rasterizer/forward.cu:265-463.
 //
-// Blackwell design (DESIGN.md "composite"):
+// Design (DESIGN.md "composite"):
 //   * work item = (tile, 8x4 sub-tile) = one warp = one CTA, launched longest-tile-first; each warp streams the
 //     tile's sorted instance records (80 B each, contiguous) through its own double-buffered shared-memory ring
 //     with cp.async.bulk (TMA 1-D) on its own mbarriers -- no CTA-wide synchronisation;

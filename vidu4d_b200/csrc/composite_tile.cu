@@ -12,7 +12,7 @@
 //     any stage lock-step: the warp only re-converges at chunk boundaries.  With ~2 contributions per pixel and
 //     32-instance stage, lock-step at stage granularity evaluates 12.5 pairs per 32-lane iteration on the headline
 //     frame (Poisson noise: the warp waits for its busiest lane every stage); at 256 instances it is 18
-//     (replay of the recorded masks, profiles/README.md r2a).
+//     (replay of the recorded masks).
 //   * No CTA-wide barrier after start-up.  A ring slot is released by an shared-memory counter; the warp whose
 //     release is the eighth issues the next bulk copy into it, so there is no producer warp to wait on.  A warp may
 //     run NSLOT-1 chunks ahead of the slowest warp of its tile.
@@ -377,7 +377,7 @@ cudaError_t opt_in_smem(K kern, size_t bytes) {
 }  // namespace
 
 // Which composite kernels run: SURFEL_COMPOSITE=tile|warp sets both directions, SURFEL_COMPOSITE_FWD / _BWD one of them.
-// Defaults (measured on the headline batch, profiles/README.md r2): forward = one-warp CTAs with private rings (fewer
+// Defaults (measured on the headline batch): forward = one-warp CTAs with private rings (fewer
 // instructions per iteration; the forward is issue bound), backward = tile CTAs with the shared chunk ring (25 % fewer
 // instructions thanks to the per-lane free walk; the backward is bound by L2 reductions and latency).
 bool sr_composite_tile_mode(bool backward) {

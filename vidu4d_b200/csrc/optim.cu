@@ -125,7 +125,8 @@ SR_API int sr_adam_flat(int32_t n_groups, const int64_t* begin /* host, n_groups
     cudaStream_t s = (cudaStream_t)stream_;
     const long long blocks = (total + 1023) / 1024;
     ProfileScope ps("adam_flat", s);
-    adam_flat_kernel<<<(unsigned)(blocks < 148 * 16 ? blocks : 148 * 16), 256, 0, s>>>(G, params, grads, exp_avg, exp_avg_sq, beta1,
+    // grid-stride: at most 16 CTAs per SM of an H100 SXM (132 SMs)
+    adam_flat_kernel<<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, s>>>(G, params, grads, exp_avg, exp_avg_sq, beta1,
                                                                                        beta2, eps, bc1, sqrt_bc2, grad_scale);
     sr_count_launch();
     return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
