@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SR_ABI_VERSION 3
+#define SR_ABI_VERSION 4
 
 #if defined(__GNUC__)
 #define SR_API __attribute__((visibility("default")))
@@ -162,6 +162,46 @@ SR_API int sr_backward_batch(const sr_frame* f, const sr_batch* b,
                 void* geom_buffer, void* binning_buffer, void* image_buffer, int64_t capacity,
                 float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D,
                 float* dL_dtransMat, float* dL_dsh, float* dL_dscales, float* dL_drotations,
+                void* stream);
+
+/*
+ * Batched entry points with per-surfel FEATURE channels composited next to the colour -- the 16+2+3+1-channel vector of
+ * lab4d/nnutils/deformable_gaussian.py:1182-1207 (registration feature, flow, normal, Gaussian mask), which the reference
+ * rasterizer (NUM_CHANNELS 3) cannot render.  Each is the plain batched entry plus:
+ *   features[P*F] per frame at features + frame * features_stride (floats; 0 = shared), 1 <= F <= 32, independent of
+ *       where the colour comes from (shs or colors_precomp);
+ *   background[bg_channels]: 3 (the feature planes get a zero background) or 3+F (feature plane f gets background[3+f]);
+ *   out_color / dL_dout_color: frame m's 3 colour planes at + m * stride (floats; >= 3*H*W), so that colour and features
+ *       can share one (M, 3+F, H, W) tensor (stride (3+F)*H*W, features at out_color + 3*H*W);
+ *   out_features / dL_dout_features: frame m's F planes at + m * stride (floats; >= F*H*W).
+ * Feature plane f = sum_i T_i alpha_i features[i, f] + T_final bg_f over exactly the colour's contributors, weights and
+ * FMA order: a feature column equal to a colour column gives a bit-identical plane.  The colour, out_others, radii and
+ * the three buffers are what sr_forward_batch writes.  F = 0 (features NULL, bg_channels 3, packed colour): the plain
+ * entries.  Backward: grad_scale multiplies dL_dout_color / dL_dout_others as in sr_backward_batch; features_grad_scale
+ * (optional DEVICE scalar, NULL = 1) multiplies dL_dout_features.  dL_dfeatures is fully written (zeroed inside):
+ * (M, P, F), or (P, F) -- the sum over the frames -- for shared features under SR_BATCH_SUM_SHARED; invisible surfels
+ * get 0.  The feature planes' gradient reaches dL_dmeans3D / dL_dscales / dL_drotations / dL_dopacity / dL_dmeans2D
+ * through alpha, as the colour planes' does.  The background gets no gradient.
+ */
+SR_API int sr_forward_batch_features(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+               const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
+               const float* scales, const float* rotations, const float* features, int32_t F, int64_t features_stride,
+               const float* viewmatrix, const float* projmatrix, const float* campos,
+               float* out_color, int64_t out_color_stride, float* out_features, int64_t out_features_stride,
+               float* out_others, int32_t* radii,
+               void* geom_buffer, void* binning_buffer, void* image_buffer, int64_t capacity,
+               uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream);
+
+SR_API int sr_backward_batch_features(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+                const float* means3D, const float* shs, const float* colors_precomp, const float* scales,
+                const float* rotations, const float* features, int32_t F, int64_t features_stride,
+                const float* viewmatrix, const float* projmatrix, const float* campos, const int32_t* radii,
+                const float* dL_dout_color, int64_t dL_dout_color_stride,
+                const float* dL_dout_features, int64_t dL_dout_features_stride,
+                const float* dL_dout_others, const float* grad_scale, const float* features_grad_scale,
+                void* geom_buffer, void* binning_buffer, void* image_buffer, int64_t capacity,
+                float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D,
+                float* dL_dtransMat, float* dL_dsh, float* dL_dscales, float* dL_drotations, float* dL_dfeatures,
                 void* stream);
 
 /* Replaces Rasterizer::markVisible (rasterizer_impl.cu:141-153): present[i] = p_view.z > 0.2 */

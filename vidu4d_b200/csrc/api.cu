@@ -4,6 +4,7 @@
 //   GeometryState/ImageState/BinningState::fromChunk, required<T>   rasterizer_impl.cu:155-194, rasterizer_impl.h:66-72
 // No torch types; no host<->device synchronisation on the forward/backward path (debug mode excepted).
 #include <atomic>
+#include <initializer_list>
 #include <map>
 #include <mutex>
 #include <string>
@@ -141,12 +142,42 @@ int sr_debug_view(int32_t P, int32_t width, int32_t height, int64_t capacity, sr
     return 0;
 }
 
-int sr_forward_batch(const sr_frame* f, const sr_batch* b, const float* background, const float* means3D, const float* shs,
-                     const float* colors_precomp, const float* opacities, const float* scales, const float* rotations,
-                     const float* viewmatrix, const float* projmatrix, const float* campos, float* out_color,
-                     float* out_others, int32_t* radii, void* geom_buffer, void* binning_buffer, void* image_buffer,
-                     int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream_) {
-    (void)projmatrix;   // only feeds dead code in the reference (auxiliary.h:170-172)
+namespace {
+// Feature-channel arguments shared by the two *_features entries: F in [1, SR_FEAT_MAX], background length 3 or 3+F,
+// and the widest vector access (4, 2 or 1 floats) that every feature row / gradient row / frame stride allows.
+int check_features(const sr_frame* f, int32_t F, int32_t bg_channels, const float* features, int64_t features_stride) {
+    if (!f) return fail(SR_EINVAL, "frame descriptor is NULL");
+    if (F < 1 || F > SR_FEAT_MAX) return fail(SR_EINVAL, "features: F must be in [1, %d], got %d", SR_FEAT_MAX, F);
+    if (!features && f->P > 0) return fail(SR_EINVAL, "features pointer is NULL");
+    if (features_stride < 0) return fail(SR_EINVAL, "features: frame stride must be >= 0");
+    if (bg_channels != 3 && bg_channels != 3 + F)
+        return fail(SR_EINVAL, "background must have 3 or 3+F = %d channels, got %d", 3 + F, bg_channels);
+    return 0;
+}
+// F = 0: the *_features entries are the plain ones (no feature pointer, 3-channel background, packed colour)
+int check_no_features(const sr_frame* f, const float* features, int32_t bg_channels, int64_t color_stride) {
+    if (features) return fail(SR_EINVAL, "features: F must be in [1, %d], got 0", SR_FEAT_MAX);
+    if (bg_channels != 3) return fail(SR_EINVAL, "background must have 3 channels when F = 0, got %d", bg_channels);
+    if (f && color_stride != 0 && color_stride != (int64_t)f->width * f->height * 3)
+        return fail(SR_EINVAL, "F = 0: the colour planes must be packed (frame stride 0 or 3*H*W)");
+    return 0;
+}
+int feature_vec(int32_t F, std::initializer_list<uintptr_t> addrs) {
+    for (int v : {4, 2}) {
+        bool ok = F % v == 0;
+        for (uintptr_t p : addrs) ok = ok && (p % (uintptr_t)(4 * v)) == 0;
+        if (ok) return v;
+    }
+    return 1;
+}
+}  // namespace
+
+static int forward_batch(const sr_frame* f, const sr_batch* b, const float* background, const float* means3D, const float* shs,
+                         const float* colors_precomp, const float* opacities, const float* scales, const float* rotations,
+                         const float* viewmatrix, const float* campos, float* out_color, int64_t color_stride,
+                         float* out_others, int32_t* radii, void* geom_buffer, void* binning_buffer, void* image_buffer,
+                         int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream_,
+                         FeatArgs* ft) {
     if (int rc = check_frame(f)) return rc;
     if (!b || b->frames < 1 || b->frames > 65535) return fail(SR_EINVAL, "batch descriptor: frames must be in [1, 65535]");
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -155,10 +186,20 @@ int sr_forward_batch(const sr_frame* f, const sr_batch* b, const float* backgrou
     const size_t N = (size_t)f->width * f->height;
     if (!out_color || !out_others || !num_rendered_dev) return fail(SR_EINVAL, "output pointer is NULL");
     if (!background || !viewmatrix || !campos) return fail(SR_EINVAL, "camera / background pointer is NULL");
+    if (ft) {
+        if (color_stride < (int64_t)(3 * N)) return fail(SR_EINVAL, "out_color frame stride must be >= 3*H*W");
+        if (!ft->out) return fail(SR_EINVAL, "out_features pointer is NULL");
+        if (ft->out_stride < (long long)(ft->F * N) * 4) return fail(SR_EINVAL, "out_features frame stride must be >= F*H*W");
+    }
     CK(cudaMemsetAsync(num_rendered_dev, 0, (size_t)M * 2 * sizeof(uint32_t), stream), "memset(num_rendered)");
     if (P == 0) {
         // rasterize_points.cu:106 -- P == 0 short-circuits to zero-filled outputs
-        CK(cudaMemsetAsync(out_color, 0, (size_t)M * 3 * N * sizeof(float), stream), "memset(out_color)");
+        if (ft) {
+            CK(sr_memset_frames(out_color, (size_t)color_stride * 4, 3 * N * sizeof(float), M, stream), "memset(out_color)");
+            CK(sr_memset_frames(ft->out, (size_t)ft->out_stride, (size_t)ft->F * N * sizeof(float), M, stream), "memset(out_features)");
+        } else {
+            CK(cudaMemsetAsync(out_color, 0, (size_t)M * 3 * N * sizeof(float), stream), "memset(out_color)");
+        }
         CK(cudaMemsetAsync(out_others, 0, (size_t)M * 8 * N * sizeof(float), stream), "memset(out_others)");
         if (num_rendered_host)
             CK(cudaMemcpyAsync(num_rendered_host, num_rendered_dev, (size_t)M * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream), "copy(num_rendered)");
@@ -193,6 +234,7 @@ int sr_forward_batch(const sr_frame* f, const sr_batch* b, const float* backgrou
     fs.means3D = b->means3D * 4; fs.shs = b->shs * 4; fs.colors = b->colors_precomp * 4; fs.opac = b->opacities * 4;
     fs.scales = b->scales * 4; fs.rots = b->rotations * 4; fs.vm = 16 * sizeof(float); fs.campos = 3 * sizeof(float);
     fs.out_color = (long long)(3 * N * sizeof(float)); fs.out_others = (long long)(8 * N * sizeof(float));
+    if (ft) fs.out_color = (long long)color_stride * 4;
     fs.radii = (long long)P * sizeof(int32_t);
 
     // per frame: tile state (ranges .. end of the image buffer); sort control words + digit histograms + look-back status
@@ -206,9 +248,47 @@ int sr_forward_batch(const sr_frame* f, const sr_batch* b, const float* backgrou
     if (sr_composite_tile_mode(false)) { CK(launch_composite_tile_fwd(a), "composite_tile_fwd"); }
     else { CK(launch_composite_fwd(a), "composite_fwd"); }
     DBG("composite_fwd");
+    if (ft) { CK(launch_feature_fwd(a, *ft), "feature_fwd"); DBG("feature_fwd"); }
     if (num_rendered_host)
         CK(cudaMemcpyAsync(num_rendered_host, num_rendered_dev, (size_t)M * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream), "copy(num_rendered)");
     return 0;
+}
+
+int sr_forward_batch(const sr_frame* f, const sr_batch* b, const float* background, const float* means3D, const float* shs,
+                     const float* colors_precomp, const float* opacities, const float* scales, const float* rotations,
+                     const float* viewmatrix, const float* projmatrix, const float* campos, float* out_color,
+                     float* out_others, int32_t* radii, void* geom_buffer, void* binning_buffer, void* image_buffer,
+                     int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream_) {
+    (void)projmatrix;   // only feeds dead code in the reference (auxiliary.h:170-172)
+    return forward_batch(f, b, background, means3D, shs, colors_precomp, opacities, scales, rotations, viewmatrix, campos,
+                         out_color, 0, out_others, radii, geom_buffer, binning_buffer, image_buffer, capacity, num_rendered_dev,
+                         num_rendered_host, stream_, nullptr);
+}
+
+int sr_forward_batch_features(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+                              const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
+                              const float* scales, const float* rotations, const float* features, int32_t F,
+                              int64_t features_stride, const float* viewmatrix, const float* projmatrix, const float* campos,
+                              float* out_color, int64_t out_color_stride, float* out_features, int64_t out_features_stride,
+                              float* out_others, int32_t* radii, void* geom_buffer, void* binning_buffer, void* image_buffer,
+                              int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream_) {
+    (void)projmatrix;
+    if (F == 0) {
+        if (int rc = check_no_features(f, features, bg_channels, out_color_stride)) return rc;
+        return sr_forward_batch(f, b, background, means3D, shs, colors_precomp, opacities, scales, rotations, viewmatrix,
+                                projmatrix, campos, out_color, out_others, radii, geom_buffer, binning_buffer, image_buffer,
+                                capacity, num_rendered_dev, num_rendered_host, stream_);
+    }
+    if (int rc = check_features(f, F, bg_channels, features, features_stride)) return rc;
+    FeatArgs ft{};
+    ft.F = F;
+    ft.vec = feature_vec(F, {(uintptr_t)features, (uintptr_t)(features_stride * 4)});
+    ft.feat = features; ft.feat_stride = features_stride * 4;
+    ft.bg = (bg_channels == 3 + F && background) ? background + 3 : nullptr;
+    ft.out = out_features; ft.out_stride = out_features_stride * 4;
+    return forward_batch(f, b, background, means3D, shs, colors_precomp, opacities, scales, rotations, viewmatrix, campos,
+                         out_color, out_color_stride, out_others, radii, geom_buffer, binning_buffer, image_buffer, capacity,
+                         num_rendered_dev, num_rendered_host, stream_, &ft);
 }
 
 int sr_forward(const sr_frame* f, const float* background, const float* means3D, const float* shs,
@@ -222,14 +302,13 @@ int sr_forward(const sr_frame* f, const float* background, const float* means3D,
                             capacity, num_rendered_dev, num_rendered_host, stream_);
 }
 
-int sr_backward_batch(const sr_frame* f, const sr_batch* b, const float* background, const float* means3D, const float* shs,
-                      const float* colors_precomp, const float* scales, const float* rotations, const float* viewmatrix,
-                      const float* projmatrix, const float* campos, const int32_t* radii, const float* dL_dout_color,
-                      const float* dL_dout_others, const float* grad_scale, void* geom_buffer, void* binning_buffer,
-                      void* image_buffer, int64_t capacity, float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity,
-                      float* dL_dmeans3D, float* dL_dtransMat, float* dL_dsh, float* dL_dscales, float* dL_drotations,
-                      void* stream_) {
-    (void)projmatrix;
+static int backward_batch(const sr_frame* f, const sr_batch* b, const float* background, const float* means3D, const float* shs,
+                          const float* colors_precomp, const float* scales, const float* rotations, const float* viewmatrix,
+                          const float* campos, const int32_t* radii, const float* dL_dout_color, int64_t dcolor_stride,
+                          const float* dL_dout_others, const float* grad_scale, void* geom_buffer, void* binning_buffer,
+                          void* image_buffer, int64_t capacity, float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity,
+                          float* dL_dmeans3D, float* dL_dtransMat, float* dL_dsh, float* dL_dscales, float* dL_drotations,
+                          void* stream_, FeatArgs* ft) {
     if (int rc = check_frame(f)) return rc;
     if (!b || b->frames < 1 || b->frames > 65535) return fail(SR_EINVAL, "batch descriptor: frames must be in [1, 65535]");
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -243,6 +322,12 @@ int sr_backward_batch(const sr_frame* f, const sr_batch* b, const float* backgro
     if (!dL_dtransMat && b->frames == 1 && !(b->flags & SR_BATCH_SUM_SHARED)) return fail(SR_EINVAL, "dL_dtransMat is NULL");
     if (shs && !dL_dsh) return fail(SR_EINVAL, "dL_dsh is NULL");
     if (capacity <= 0) return fail(SR_EINVAL, "capacity must be positive");
+    if (ft) {
+        const long long N = (long long)f->width * f->height;
+        if (dcolor_stride < 3 * N) return fail(SR_EINVAL, "dL_dout_color frame stride must be >= 3*H*W");
+        if (!ft->dout || !ft->dfeat) return fail(SR_EINVAL, "dL_dout_features / dL_dfeatures pointer is NULL");
+        if (ft->dout_stride < ft->F * N * 4) return fail(SR_EINVAL, "dL_dout_features frame stride must be >= F*H*W");
+    }
     if (((uintptr_t)rotations & 15) || ((uintptr_t)scales & 7) || (shs && ((uintptr_t)shs & 15)) ||
         ((uintptr_t)dL_drotations & 15) || ((uintptr_t)dL_dscales & 7) || (dL_dsh && ((uintptr_t)dL_dsh & 15)) ||
         ((b->rotations * 4) & 15) || ((b->scales * 4) & 7) || ((b->shs * 4) & 15))
@@ -268,6 +353,7 @@ int sr_backward_batch(const sr_frame* f, const sr_batch* b, const float* backgro
     fs.scales = b->scales * 4; fs.rots = b->rotations * 4; fs.vm = 16 * sizeof(float); fs.campos = 3 * sizeof(float);
     fs.radii = (long long)P * sizeof(int32_t);
     fs.dcolor = (long long)(3 * N * sizeof(float)); fs.dothers = (long long)(8 * N * sizeof(float));
+    if (ft) fs.dcolor = (long long)dcolor_stride * 4;
     // gradients are written per frame, (M, P, .) -- or, with SR_BATCH_SUM_SHARED, once as the sum over frames, (P, .), for
     // the inputs the frames share (surfel_bwd.cu accumulates them inside the kernel; stride 0 selects that)
     const long long Pl = P;
@@ -279,11 +365,67 @@ int sr_backward_batch(const sr_frame* f, const sr_batch* b, const float* backgro
     fs.g_sh = (sum && b->shs == 0) ? 0 : Pl * a.cam.M * 3 * 4;
     fs.g_scales = (sum && b->scales == 0) ? 0 : Pl * 2 * 4;
     fs.g_rots = (sum && b->rotations == 0) ? 0 : Pl * 4 * 4;
+    if (ft) {
+        // dL/dfeatures: (P,F) summed over the frames when the features are shared and SR_BATCH_SUM_SHARED is set,
+        // else (M,P,F); zeroed here, the feature pass adds into it
+        ft->dfeat_stride = (sum && ft->feat_stride == 0) ? 0 : Pl * ft->F * 4;
+        const size_t rows = ft->dfeat_stride == 0 ? 1 : (size_t)M;
+        CK(cudaMemsetAsync(ft->dfeat, 0, rows * (size_t)Pl * ft->F * sizeof(float), stream), "memset(dL_dfeatures)");
+    }
     if (sr_composite_tile_mode(true)) { CK(launch_composite_tile_bwd(a), "composite_tile_bwd"); }
     else { CK(launch_composite_bwd(a), "composite_bwd"); }
     DBG("composite_bwd");
+    // after composite_bwd (which zeroes the per-surfel accumulator), before surfel_bwd (which reads it)
+    if (ft) { CK(launch_feature_bwd(a, *ft), "feature_bwd"); DBG("feature_bwd"); }
     CK(launch_surfel_bwd(a), "surfel_bwd"); DBG("surfel_bwd");
     return 0;
+}
+
+int sr_backward_batch(const sr_frame* f, const sr_batch* b, const float* background, const float* means3D, const float* shs,
+                      const float* colors_precomp, const float* scales, const float* rotations, const float* viewmatrix,
+                      const float* projmatrix, const float* campos, const int32_t* radii, const float* dL_dout_color,
+                      const float* dL_dout_others, const float* grad_scale, void* geom_buffer, void* binning_buffer,
+                      void* image_buffer, int64_t capacity, float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity,
+                      float* dL_dmeans3D, float* dL_dtransMat, float* dL_dsh, float* dL_dscales, float* dL_drotations,
+                      void* stream_) {
+    (void)projmatrix;
+    return backward_batch(f, b, background, means3D, shs, colors_precomp, scales, rotations, viewmatrix, campos, radii,
+                          dL_dout_color, 0, dL_dout_others, grad_scale, geom_buffer, binning_buffer, image_buffer, capacity,
+                          dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales, dL_drotations,
+                          stream_, nullptr);
+}
+
+int sr_backward_batch_features(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+                               const float* means3D, const float* shs, const float* colors_precomp, const float* scales,
+                               const float* rotations, const float* features, int32_t F, int64_t features_stride,
+                               const float* viewmatrix, const float* projmatrix, const float* campos, const int32_t* radii,
+                               const float* dL_dout_color, int64_t dL_dout_color_stride, const float* dL_dout_features,
+                               int64_t dL_dout_features_stride, const float* dL_dout_others, const float* grad_scale,
+                               const float* features_grad_scale, void* geom_buffer, void* binning_buffer, void* image_buffer,
+                               int64_t capacity, float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity,
+                               float* dL_dmeans3D, float* dL_dtransMat, float* dL_dsh, float* dL_dscales,
+                               float* dL_drotations, float* dL_dfeatures, void* stream_) {
+    (void)projmatrix;
+    if (F == 0) {
+        if (int rc = check_no_features(f, features, bg_channels, dL_dout_color_stride)) return rc;
+        return sr_backward_batch(f, b, background, means3D, shs, colors_precomp, scales, rotations, viewmatrix, projmatrix,
+                                 campos, radii, dL_dout_color, dL_dout_others, grad_scale, geom_buffer, binning_buffer,
+                                 image_buffer, capacity, dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat,
+                                 dL_dsh, dL_dscales, dL_drotations, stream_);
+    }
+    if (int rc = check_features(f, F, bg_channels, features, features_stride)) return rc;
+    FeatArgs ft{};
+    ft.F = F;
+    ft.vec = feature_vec(F, {(uintptr_t)features, (uintptr_t)(features_stride * 4), (uintptr_t)dL_dfeatures});
+    ft.feat = features; ft.feat_stride = features_stride * 4;
+    ft.bg = (bg_channels == 3 + F && background) ? background + 3 : nullptr;
+    ft.dout = dL_dout_features; ft.dout_stride = dL_dout_features_stride * 4;
+    ft.grad_scale = features_grad_scale;
+    ft.dfeat = dL_dfeatures;
+    return backward_batch(f, b, background, means3D, shs, colors_precomp, scales, rotations, viewmatrix, campos, radii,
+                          dL_dout_color, dL_dout_color_stride, dL_dout_others, grad_scale, geom_buffer, binning_buffer,
+                          image_buffer, capacity, dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh,
+                          dL_dscales, dL_drotations, stream_, &ft);
 }
 
 int sr_backward(const sr_frame* f, const float* background, const float* means3D, const float* shs,

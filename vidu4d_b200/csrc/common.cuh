@@ -185,6 +185,21 @@ struct BwdArgs {
     bool debug;
 };
 
+// Per-surfel feature channels composited with the colour's weights (composite_feat.cu).  Strides are in BYTES between
+// consecutive frames (0 = shared by every frame, for `feat` and `dfeat` only).
+#define SR_FEAT_MAX 32           // channels per call
+#define SR_FEAT_CHUNK 8          // channels one CTA accumulates (gridDim.y = ceil(F / SR_FEAT_CHUNK))
+struct FeatArgs {
+    int F;                        // 1..SR_FEAT_MAX
+    int vec;                      // 4, 2 or 1: floats per vector access of a feature row (F % vec == 0, aligned)
+    const float* feat;  long long feat_stride;     // [P*F] per frame
+    const float* bg;                               // DEVICE bg[F] of the feature planes, nullptr = 0
+    float* out;         long long out_stride;      // forward: F planes of H*W per frame
+    const float* dout;  long long dout_stride;     // backward: dL/d(feature planes)
+    const float* grad_scale;                       // optional DEVICE scalar multiplying dout (nullptr = 1)
+    float* dfeat;       long long dfeat_stride;    // backward: dL/dfeatures [P*F], zeroed by the launcher
+};
+
 cudaError_t launch_preprocess_fwd(const FwdArgs& a);      // preprocess.cu
 cudaError_t launch_scan_emit(const FwdArgs& a);           // preprocess.cu
 cudaError_t launch_sort(const FwdArgs& a);                // sort.cu
@@ -196,6 +211,8 @@ cudaError_t launch_surfel_bwd(const BwdArgs& a);          // surfel_bwd.cu
 cudaError_t launch_composite_tile_fwd(const FwdArgs& a);  // composite_tile.cu (one CTA per tile, shared chunk ring)
 cudaError_t launch_composite_tile_bwd(const BwdArgs& a);  // composite_tile.cu
 bool sr_composite_tile_mode(bool backward);               // SURFEL_COMPOSITE[_FWD|_BWD]=tile|warp
+cudaError_t launch_feature_fwd(const FwdArgs& a, const FeatArgs& ft);   // composite_feat.cu (after the composite forward)
+cudaError_t launch_feature_bwd(const BwdArgs& a, const FeatArgs& ft);   // composite_feat.cu (after the composite backward)
 cudaError_t launch_mark_visible(int P, const float* means3D, const float* vm, uint8_t* present, cudaStream_t s);
 // clears `bytes` at p + f * pitch for every frame f of the batch (one 2-D memset)
 cudaError_t sr_memset_frames(void* p, size_t pitch, size_t bytes, int frames, cudaStream_t s);

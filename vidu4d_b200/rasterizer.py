@@ -194,6 +194,25 @@ def _batch_inputs(M: int, **named):
     return out, strides
 
 
+def _check_features(features, P: int, background, batched: bool = False) -> int:
+    """Validate per-surfel feature channels: float (P,F) -- or, batched, (M,P,F) -- with 1 <= F <= 32, on the GPU, and a
+    background of 3 or 3+F values.  Returns F."""
+    if not torch.is_tensor(features):
+        raise RuntimeError("features must be a tensor")
+    if features.ndim not in ((2, 3) if batched else (2,)) or int(features.shape[-2]) != P:
+        want = "(P,F) or (M,P,F)" if batched else "(P,F)"
+        raise RuntimeError(f"features must have dimensions {want} with P = {P}, got {tuple(features.shape)}")
+    F = int(features.shape[-1])
+    if not 1 <= F <= _capi.FEATURES_MAX:
+        raise RuntimeError(f"features must have 1..{_capi.FEATURES_MAX} channels, got {F}")
+    nbg = int(background.numel())
+    if nbg not in (3, 3 + F):
+        raise RuntimeError(f"background must have 3 or 3+F = {3 + F} values with {F} feature channels, got {nbg}")
+    if not features.is_cuda:
+        raise RuntimeError("features must be a CUDA tensor")
+    return F
+
+
 def _as_float(x) -> float:
     # the reference passes CUDA 0-d tensors to pybind `float` params (gaussian_renderer/__init__.py:36-43)
     return float(x.item()) if torch.is_tensor(x) else float(x)
@@ -206,6 +225,45 @@ class _CNamespace:
     def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier,
                             transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height,
                             image_width, sh, degree, campos, prefiltered, debug):
+        return _forward_single(background, means3D, colors, opacity, scales, rotations, scale_modifier, transMat_precomp,
+                               viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
+                               prefiltered, debug, None)
+
+    @staticmethod
+    def rasterize_gaussians_features(background, means3D, colors, opacity, scales, rotations, scale_modifier,
+                                     transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height,
+                                     image_width, sh, degree, campos, prefiltered, debug, features):
+        """rasterize_gaussians plus per-surfel features (P,F), 1 <= F <= 32 (not in the reference): out_color is
+        (3+F,H,W) -- the colour planes, then F feature planes composited with the colour's weights over a background of
+        background[3:] (background of 3+F values) or zeros (background of 3)."""
+        return _forward_single(background, means3D, colors, opacity, scales, rotations, scale_modifier, transMat_precomp,
+                               viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
+                               prefiltered, debug, features)
+
+    @staticmethod
+    def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier,
+                                     transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+                                     dL_dout_color, dL_dout_others, sh, degree, campos, geomBuffer, R,
+                                     binningBuffer, imageBuffer, debug):
+        return _backward_single(background, means3D, radii, colors, scales, rotations, scale_modifier, transMat_precomp,
+                                viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, dL_dout_others, sh, degree,
+                                campos, geomBuffer, R, binningBuffer, imageBuffer, debug, None)
+
+    @staticmethod
+    def rasterize_gaussians_features_backward(background, means3D, radii, colors, scales, rotations, scale_modifier,
+                                              transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+                                              dL_dout_color, dL_dout_others, sh, degree, campos, geomBuffer, R,
+                                              binningBuffer, imageBuffer, debug, features):
+        """Backward of rasterize_gaussians_features: dL_dout_color is (3+F,H,W); returns the eight gradients of
+        rasterize_gaussians_backward and dL_dfeatures (P,F)."""
+        return _backward_single(background, means3D, radii, colors, scales, rotations, scale_modifier, transMat_precomp,
+                                viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, dL_dout_others, sh, degree,
+                                campos, geomBuffer, R, binningBuffer, imageBuffer, debug, features)
+
+    @staticmethod
+    def _forward_single(background, means3D, colors, opacity, scales, rotations, scale_modifier,
+                        transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height,
+                        image_width, sh, degree, campos, prefiltered, debug, features):
         lib = _capi.load()
         if means3D.ndim != 2 or means3D.shape[1] != 3:
             raise RuntimeError("means3D must have dimensions (num_points, 3)")
@@ -224,9 +282,13 @@ class _CNamespace:
         viewmatrix = _f32c(viewmatrix, "viewmatrix"); projmatrix = _f32c(projmatrix, "projmatrix")
         sh = _f32c(sh, "sh"); campos = _f32c(campos, "campos")
         M = int(sh.shape[1]) if sh is not None and sh.numel() != 0 else 0
+        F = 0
+        if features is not None:
+            F = _check_features(features, P, background)
+            features = _f32c(features, "features")
 
         with torch.cuda.device(dev):
-            out_color = torch.empty((3, H, W), dtype=torch.float32, device=dev)
+            out_color = torch.empty((3 + F, H, W), dtype=torch.float32, device=dev)
             out_others = torch.empty((8, H, W), dtype=torch.float32, device=dev)
             radii = torch.empty((P,), dtype=torch.int32, device=dev)
             geom = torch.empty((lib.sr_geom_bytes(P),), dtype=torch.uint8, device=dev)
@@ -241,13 +303,25 @@ class _CNamespace:
                 binning = torch.empty((lib.sr_binning_bytes(cap, W, H),), dtype=torch.uint8, device=dev)
                 nosync = (not _sync_mode) and key in _cap_hint
                 host = _host_slot() if nosync else torch.empty((1, 2), dtype=torch.int32, pin_memory=True)
-                rc = lib.sr_forward(
-                    C.byref(fr), _ptr(background), _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(opacity),
-                    _ptr(scales), _ptr(rotations), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos),
-                    out_color.data_ptr(), out_others.data_ptr(), _ptr(radii), geom.data_ptr(),
-                    binning.data_ptr(), img.data_ptr(), cap, nr_dev.data_ptr(), host.data_ptr(),
-                    stream.cuda_stream)
-                _capi.check(rc, "sr_forward")
+                if F:
+                    N = H * W
+                    bt = _capi.SrBatch(1, 0, 0, 0, 0, 0, 0, 0)
+                    rc = lib.sr_forward_batch_features(
+                        C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh),
+                        _ptr(colors), _ptr(opacity), _ptr(scales), _ptr(rotations), _ptr(features), F, 0,
+                        _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), out_color.data_ptr(), (3 + F) * N,
+                        out_color.data_ptr() + 3 * N * 4, (3 + F) * N, out_others.data_ptr(), _ptr(radii),
+                        geom.data_ptr(), binning.data_ptr(), img.data_ptr(), cap, nr_dev.data_ptr(), host.data_ptr(),
+                        stream.cuda_stream)
+                    _capi.check(rc, "sr_forward_batch_features")
+                else:
+                    rc = lib.sr_forward(
+                        C.byref(fr), _ptr(background), _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(opacity),
+                        _ptr(scales), _ptr(rotations), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos),
+                        out_color.data_ptr(), out_others.data_ptr(), _ptr(radii), geom.data_ptr(),
+                        binning.data_ptr(), img.data_ptr(), cap, nr_dev.data_ptr(), host.data_ptr(),
+                        stream.cuda_stream)
+                    _capi.check(rc, "sr_forward")
                 if nosync:
                     _pending.append((host, key, cap, stream))
                     if len(_pending) > _MAX_PENDING:
@@ -266,14 +340,20 @@ class _CNamespace:
         return num_rendered, out_color, out_others, radii, geom, binning, img
 
     @staticmethod
-    def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier,
-                                     transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
-                                     dL_dout_color, dL_dout_others, sh, degree, campos, geomBuffer, R,
-                                     binningBuffer, imageBuffer, debug):
+    def _backward_single(background, means3D, radii, colors, scales, rotations, scale_modifier,
+                         transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+                         dL_dout_color, dL_dout_others, sh, degree, campos, geomBuffer, R,
+                         binningBuffer, imageBuffer, debug, features):
         lib = _capi.load()
         dev = means3D.device
         P = int(means3D.shape[0])
         H, W = int(dL_dout_color.shape[1]), int(dL_dout_color.shape[2])
+        F = 0
+        if features is not None:
+            F = _check_features(features, P, background)
+            features = _f32c(features, "features")
+            if tuple(dL_dout_color.shape) != (3 + F, H, W):
+                raise RuntimeError(f"dL_dout_color must be (3+F,H,W) = {(3 + F, H, W)}, got {tuple(dL_dout_color.shape)}")
         background = _f32c(background, "background"); means3D = _f32c(means3D, "means3D")
         colors = _f32c(colors, "colors"); scales = _f32c(scales, "scales"); rotations = _f32c(rotations, "rotations")
         viewmatrix = _f32c(viewmatrix, "viewmatrix"); projmatrix = _f32c(projmatrix, "projmatrix")
@@ -286,7 +366,24 @@ class _CNamespace:
             dL_dmeans3D, dL_dmeans2D, dL_dcolors = mk(P, 3), mk(P, 3), mk(P, 3)
             dL_dopacity, dL_dtransMat, dL_dsh = mk(P, 1), mk(P, 9), mk(P, M, 3)
             dL_dscales, dL_drotations = mk(P, 2), mk(P, 4)
-            if P > 0:
+            dL_dfeatures = mk(P, F) if F else None
+            if P > 0 and F:
+                cap = _capacity_from_bytes(int(binningBuffer.numel()), W, H)
+                fr = _capi.SrFrame(P, int(degree), M, W, H, _as_float(tan_fovx), _as_float(tan_fovy),
+                                   float(scale_modifier), 0, int(bool(debug)), 0)
+                N = H * W
+                bt = _capi.SrBatch(1, 0, 0, 0, 0, 0, 0, 0)
+                rc = lib.sr_backward_batch_features(
+                    C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh),
+                    _ptr(colors), _ptr(scales), _ptr(rotations), _ptr(features), F, 0, _ptr(viewmatrix),
+                    _ptr(projmatrix), _ptr(campos), _ptr(radii), _ptr(dL_dout_color), (3 + F) * N,
+                    dL_dout_color.data_ptr() + 3 * N * 4, (3 + F) * N, _ptr(dL_dout_others), None, None,
+                    geomBuffer.data_ptr(), binningBuffer.data_ptr(), imageBuffer.data_ptr(), cap, dL_dmeans2D.data_ptr(),
+                    dL_dcolors.data_ptr(), dL_dopacity.data_ptr(), dL_dmeans3D.data_ptr(), dL_dtransMat.data_ptr(),
+                    dL_dsh.data_ptr() if M > 0 else None, dL_dscales.data_ptr(), dL_drotations.data_ptr(),
+                    dL_dfeatures.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+                _capi.check(rc, "sr_backward_batch_features")
+            elif P > 0:
                 cap = _capacity_from_bytes(int(binningBuffer.numel()), W, H)
                 fr = _capi.SrFrame(P, int(degree), M, W, H, _as_float(tan_fovx), _as_float(tan_fovy),
                                    float(scale_modifier), 0, int(bool(debug)), 0)
@@ -299,17 +396,21 @@ class _CNamespace:
                     dL_dsh.data_ptr() if M > 0 else None, dL_dscales.data_ptr(), dL_drotations.data_ptr(),
                     torch.cuda.current_stream(dev).cuda_stream)
                 _capi.check(rc, "sr_backward")
-        return dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales, dL_drotations
+        grads = (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales, dL_drotations)
+        return grads + (dL_dfeatures,) if F else grads
 
     # ---- batched entry points (SURVEY.md 8(f) N1): M frames in one launch set -------------------------------------
     @staticmethod
     def rasterize_gaussians_batch(background, means3D, colors, opacity, scales, rotations, scale_modifier, viewmatrix,
                                   projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
-                                  prefiltered=False, debug=False):
+                                  prefiltered=False, debug=False, features=None, concat=True):
         """M frames at once.  viewmatrix / projmatrix (M,4,4), campos (M,3).  Every per-surfel input is either shared by
         all frames -- the single-frame shape, e.g. means3D (P,3) -- or per frame with a leading M, e.g. (M,P,3) (Stage 3:
         each frame rasterizes its own warped copy of the surfels).  Returns (num_rendered (list of M ints, or -1 in nosync
-        mode), out_color (M,3,H,W), out_others (M,8,H,W), radii (M,P), geomBuffer, binningBuffer, imgBuffer)."""
+        mode), out_color (M,3,H,W), out_others (M,8,H,W), radii (M,P), geomBuffer, binningBuffer, imgBuffer).
+        features (P,F) shared or (M,P,F) per frame, 1 <= F <= 32: an eighth element, the (M,F,H,W) feature planes, is
+        returned; with concat=True out_color is (M,3+F,H,W) and the feature planes are its view [:, 3:], with concat=False
+        the two are separate tensors."""
         lib = _capi.load()
         M = int(viewmatrix.shape[0])
         if viewmatrix.ndim != 3 or viewmatrix.shape[1:] != (4, 4) or campos.shape != (M, 3):
@@ -318,15 +419,27 @@ class _CNamespace:
         H, W = int(image_height), int(image_width)
         background = _f32c(background, "background"); viewmatrix = _f32c(viewmatrix, "viewmatrix")
         projmatrix = _f32c(projmatrix, "projmatrix"); campos = _f32c(campos, "campos")
+        F = 0
+        if features is not None:
+            F = _check_features(features, int(means3D.shape[-2]), background, batched=True)
         ins, strides = _batch_inputs(M, means3D=(means3D, (3,)), sh=(sh, None), colors=(colors, (3,)), opacity=(opacity, (1,)),
-                                     scales=(scales, (2,)), rotations=(rotations, (4,)))
+                                     scales=(scales, (2,)), rotations=(rotations, (4,)), features=(features, None))
         means3D, sh, colors, opacity, scales, rotations = (ins[k] for k in ("means3D", "sh", "colors", "opacity", "scales", "rotations"))
+        features = ins["features"]
         P = int(means3D.shape[-2])
         Msh = int(sh.shape[-2]) if sh is not None and sh.numel() != 0 else 0
         bt = _capi.SrBatch(M, 0, strides["means3D"], strides["sh"], strides["colors"], strides["opacity"], strides["scales"],
                            strides["rotations"])
+        N = H * W
         with torch.cuda.device(dev):
-            out_color = torch.empty((M, 3, H, W), dtype=torch.float32, device=dev)
+            if F and concat:
+                out_color = torch.empty((M, 3 + F, H, W), dtype=torch.float32, device=dev)
+                out_feat = out_color[:, 3:]
+                cstride = fstride = (3 + F) * N
+            else:
+                out_color = torch.empty((M, 3, H, W), dtype=torch.float32, device=dev)
+                out_feat = torch.empty((M, F, H, W), dtype=torch.float32, device=dev) if F else None
+                cstride, fstride = 3 * N, F * N
             out_others = torch.empty((M, 8, H, W), dtype=torch.float32, device=dev)
             radii = torch.empty((M, P), dtype=torch.int32, device=dev)
             geom = torch.empty((M * lib.sr_geom_bytes(P),), dtype=torch.uint8, device=dev)
@@ -341,12 +454,21 @@ class _CNamespace:
                 binning = torch.empty((M * lib.sr_binning_bytes(cap, W, H),), dtype=torch.uint8, device=dev)
                 nosync = (not _sync_mode) and key in _cap_hint
                 host = _host_slot(M) if nosync else torch.empty((M, 2), dtype=torch.int32, pin_memory=True)
-                rc = lib.sr_forward_batch(
-                    C.byref(fr), C.byref(bt), _ptr(background), _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(opacity),
-                    _ptr(scales), _ptr(rotations), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos),
-                    out_color.data_ptr(), out_others.data_ptr(), _ptr(radii), geom.data_ptr(),
-                    binning.data_ptr(), img.data_ptr(), cap, nr_dev.data_ptr(), host.data_ptr(), stream.cuda_stream)
-                _capi.check(rc, "sr_forward_batch")
+                if F:    # an overflow re-run below re-runs the feature pass too
+                    rc = lib.sr_forward_batch_features(
+                        C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh),
+                        _ptr(colors), _ptr(opacity), _ptr(scales), _ptr(rotations), _ptr(features), F, strides["features"],
+                        _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), out_color.data_ptr(), cstride,
+                        out_feat.data_ptr(), fstride, out_others.data_ptr(), _ptr(radii), geom.data_ptr(),
+                        binning.data_ptr(), img.data_ptr(), cap, nr_dev.data_ptr(), host.data_ptr(), stream.cuda_stream)
+                    _capi.check(rc, "sr_forward_batch_features")
+                else:
+                    rc = lib.sr_forward_batch(
+                        C.byref(fr), C.byref(bt), _ptr(background), _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(opacity),
+                        _ptr(scales), _ptr(rotations), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos),
+                        out_color.data_ptr(), out_others.data_ptr(), _ptr(radii), geom.data_ptr(),
+                        binning.data_ptr(), img.data_ptr(), cap, nr_dev.data_ptr(), host.data_ptr(), stream.cuda_stream)
+                    _capi.check(rc, "sr_forward_batch")
                 if nosync:
                     _pending.append((host, key, cap, stream))
                     num_rendered = -1
@@ -363,13 +485,16 @@ class _CNamespace:
                     cap = _round_cap(int(max(num_rendered) * 1.1) + 4096)
                     continue
                 break
+        if F:
+            return num_rendered, out_color, out_others, radii, geom, binning, img, out_feat
         return num_rendered, out_color, out_others, radii, geom, binning, img
 
     @staticmethod
     def rasterize_gaussians_backward_batch(background, means3D, radii, colors, scales, rotations, scale_modifier, viewmatrix,
                                            projmatrix, tan_fovx, tan_fovy, dL_dout_color, dL_dout_others, sh, degree, campos,
                                            geomBuffer, binningBuffer, imageBuffer, grad_scale=None, debug=False,
-                                           sum_shared=False, opacity_shared=True, want_transmat=True, outs=None):
+                                           sum_shared=False, opacity_shared=True, want_transmat=True, outs=None,
+                                           features=None, dL_dout_features=None, features_grad_scale=None):
         """Backward of rasterize_gaussians_batch.  dL_dout_color (M,3,H,W), dL_dout_others (M,8,H,W); grad_scale: optional
         0-d device tensor multiplying both (the upstream scalar of a fused loss).  Returns the eight gradient tensors
         (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales, dL_drotations), each with a
@@ -378,17 +503,36 @@ class _CNamespace:
         written or reduced; `opacity_shared` says whether the forward's opacities were shared (they are not an input of
         the backward); dL_dmeans2D stays (M,P,3); want_transmat=False skips the (M,P,9) by-product.
         outs: optional {"dL_dmeans3D" | "dL_dsh" | "dL_dopacity" | "dL_dscales" | "dL_drotations" | "dL_dcolors": tensor}
-        of pre-allocated, suitably shaped and aligned outputs (e.g. views of the flat buffer an all-reduce runs over)."""
+        of pre-allocated, suitably shaped and aligned outputs (e.g. views of the flat buffer an all-reduce runs over).
+        features (P,F) or (M,P,F): the gradient of the feature planes is either the tail of dL_dout_color (M,3+F,H,W) or a
+        separate dL_dout_features (M,F,H,W) (then dL_dout_color is (M,3,H,W)); features_grad_scale (optional 0-d device
+        tensor) multiplies it instead of grad_scale.  A ninth gradient, dL_dfeatures, is returned: (M,P,F), or (P,F) for
+        shared features with sum_shared=True."""
         lib = _capi.load()
         M = int(viewmatrix.shape[0])
         dev = means3D.device
         H, W = int(dL_dout_color.shape[-2]), int(dL_dout_color.shape[-1])
+        N = H * W
         background = _f32c(background, "background"); viewmatrix = _f32c(viewmatrix, "viewmatrix")
         projmatrix = _f32c(projmatrix, "projmatrix"); campos = _f32c(campos, "campos")
         dL_dout_color = _f32c(dL_dout_color, "dL_dout_color"); dL_dout_others = _f32c(dL_dout_others, "dL_dout_others")
+        F = 0
+        if features is not None:
+            F = _check_features(features, int(means3D.shape[-2]), background, batched=True)
+            if dL_dout_features is None:
+                if tuple(dL_dout_color.shape) != (M, 3 + F, H, W):
+                    raise RuntimeError(f"dL_dout_color must be (M,3+F,H,W) = {(M, 3 + F, H, W)} without dL_dout_features")
+                cstride = fstride = (3 + F) * N
+                dfeat_ptr = dL_dout_color.data_ptr() + 3 * N * 4
+            else:
+                dL_dout_features = _f32c(dL_dout_features, "dL_dout_features")
+                if tuple(dL_dout_features.shape) != (M, F, H, W) or tuple(dL_dout_color.shape) != (M, 3, H, W):
+                    raise RuntimeError("dL_dout_color must be (M,3,H,W) and dL_dout_features (M,F,H,W)")
+                cstride, fstride, dfeat_ptr = 3 * N, F * N, dL_dout_features.data_ptr()
         ins, strides = _batch_inputs(M, means3D=(means3D, (3,)), sh=(sh, None), colors=(colors, (3,)),
-                                     scales=(scales, (2,)), rotations=(rotations, (4,)))
+                                     scales=(scales, (2,)), rotations=(rotations, (4,)), features=(features, None))
         means3D, sh, colors, scales, rotations = (ins[k] for k in ("means3D", "sh", "colors", "scales", "rotations"))
+        features = ins["features"]
         P = int(means3D.shape[-2])
         Msh = int(sh.shape[-2]) if sh is not None and sh.numel() != 0 else 0
         op_stride = 0 if (opacity_shared or M == 1) else P
@@ -413,6 +557,7 @@ class _CNamespace:
             dL_dtransMat = mk0(M, P, 9) if (want_transmat or (M == 1 and not sum_shared)) else None
             dL_dsh = mk("dL_dsh", strides["sh"] == 0, Msh, 3)
             dL_dscales, dL_drotations = mk("dL_dscales", strides["scales"] == 0, 2), mk("dL_drotations", strides["rotations"] == 0, 4)
+            dL_dfeatures = mk("dL_dfeatures", strides["features"] == 0, F) if F else None
             if P > 0:
                 cap = _capacity_from_bytes(int(binningBuffer.numel()) // M, W, H)
                 fr = _capi.SrFrame(P, int(degree), Msh, W, H, _as_float(tan_fovx), _as_float(tan_fovy),
@@ -420,6 +565,22 @@ class _CNamespace:
                 gs = None
                 if grad_scale is not None:
                     gs = grad_scale.to(device=dev, dtype=torch.float32).reshape(()).contiguous()
+            if P > 0 and F:
+                fgs = None
+                if features_grad_scale is not None:
+                    fgs = features_grad_scale.to(device=dev, dtype=torch.float32).reshape(()).contiguous()
+                rc = lib.sr_backward_batch_features(
+                    C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh),
+                    _ptr(colors), _ptr(scales), _ptr(rotations), _ptr(features), F, strides["features"], _ptr(viewmatrix),
+                    _ptr(projmatrix), _ptr(campos), _ptr(radii), _ptr(dL_dout_color), cstride, dfeat_ptr, fstride,
+                    _ptr(dL_dout_others), gs.data_ptr() if gs is not None else None,
+                    fgs.data_ptr() if fgs is not None else None, geomBuffer.data_ptr(), binningBuffer.data_ptr(),
+                    imageBuffer.data_ptr(), cap, dL_dmeans2D.data_ptr(), dL_dcolors.data_ptr(), dL_dopacity.data_ptr(),
+                    dL_dmeans3D.data_ptr(), dL_dtransMat.data_ptr() if dL_dtransMat is not None else None,
+                    dL_dsh.data_ptr() if Msh > 0 else None, dL_dscales.data_ptr(), dL_drotations.data_ptr(),
+                    dL_dfeatures.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+                _capi.check(rc, "sr_backward_batch_features")
+            elif P > 0:
                 rc = lib.sr_backward_batch(
                     C.byref(fr), C.byref(bt), _ptr(background), _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(scales),
                     _ptr(rotations), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), _ptr(radii),
@@ -429,7 +590,8 @@ class _CNamespace:
                     dL_dtransMat.data_ptr() if dL_dtransMat is not None else None, dL_dsh.data_ptr() if Msh > 0 else None,
                     dL_dscales.data_ptr(), dL_drotations.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
                 _capi.check(rc, "sr_backward_batch")
-        return dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales, dL_drotations
+        grads = (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales, dL_drotations)
+        return grads + (dL_dfeatures,) if F else grads
 
     @staticmethod
     def mark_visible(means3D, viewmatrix, projmatrix):
@@ -448,6 +610,8 @@ class _CNamespace:
 
 
 _C = _CNamespace()
+_forward_single = _CNamespace._forward_single
+_backward_single = _CNamespace._backward_single
 
 
 def cpu_deep_copy_tuple(input_tuple):
@@ -455,36 +619,40 @@ def cpu_deep_copy_tuple(input_tuple):
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        raster_settings):
+                        raster_settings, features=None):
+    """features (P,F), 1 <= F <= 32: the colour output is (3+F,H,W), feature planes after the colour planes."""
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                     cov3Ds_precomp, raster_settings)
+                                     cov3Ds_precomp, raster_settings, features)
 
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings):
+                raster_settings, features=None):
         args = (raster_settings.bg, means3D, colors_precomp, opacities, scales, rotations,
                 raster_settings.scale_modifier, cov3Ds_precomp, raster_settings.viewmatrix,
                 raster_settings.projmatrix, raster_settings.tanfovx, raster_settings.tanfovy,
                 raster_settings.image_height, raster_settings.image_width, sh, raster_settings.sh_degree,
                 raster_settings.campos, raster_settings.prefiltered, raster_settings.debug)
+        fwd = _C.rasterize_gaussians if features is None else \
+            (lambda *a: _C.rasterize_gaussians_features(*a, features))  # noqa: E731
         if raster_settings.debug:
             cpu_args = cpu_deep_copy_tuple(args)
             try:
-                num_rendered, color, depth, radii, geomBuffer, binningBuffer, imgBuffer = _C.rasterize_gaussians(*args)
+                num_rendered, color, depth, radii, geomBuffer, binningBuffer, imgBuffer = fwd(*args)
             except Exception as ex:
                 torch.save(cpu_args, "snapshot_fw.dump")
                 print("\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
                 raise ex
         else:
-            num_rendered, color, depth, radii, geomBuffer, binningBuffer, imgBuffer = _C.rasterize_gaussians(*args)
+            num_rendered, color, depth, radii, geomBuffer, binningBuffer, imgBuffer = fwd(*args)
         ctx.raster_settings = raster_settings
         ctx.num_rendered = num_rendered
+        ctx.has_features = features is not None
         # only inputs + private buffers are saved (never our own outputs): the caller edits `color` in place
         # before backward (deformable_gaussian.py:188-190)
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
-                              binningBuffer, imgBuffer)
+                              binningBuffer, imgBuffer, features)
         ctx.mark_non_differentiable(radii)
         return color, radii, depth
 
@@ -492,9 +660,11 @@ class _RasterizeGaussians(torch.autograd.Function):
     def backward(ctx, grad_out_color, grad_radii, grad_depth):
         num_rendered = ctx.num_rendered
         raster_settings = ctx.raster_settings
-        colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer = ctx.saved_tensors
+        (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer,
+         features) = ctx.saved_tensors
+        F = int(features.shape[-1]) if ctx.has_features else 0
         if grad_out_color is None:
-            grad_out_color = torch.zeros((3, raster_settings.image_height, raster_settings.image_width),
+            grad_out_color = torch.zeros((3 + F, raster_settings.image_height, raster_settings.image_width),
                                          dtype=torch.float32, device=means3D.device)
         if grad_depth is None:
             grad_depth = torch.zeros((8, raster_settings.image_height, raster_settings.image_width),
@@ -503,17 +673,20 @@ class _RasterizeGaussians(torch.autograd.Function):
                 cov3Ds_precomp, raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx,
                 raster_settings.tanfovy, grad_out_color, grad_depth, sh, raster_settings.sh_degree,
                 raster_settings.campos, geomBuffer, num_rendered, binningBuffer, imgBuffer, raster_settings.debug)
+        bwd = _C.rasterize_gaussians_backward if not F else \
+            (lambda *a: _C.rasterize_gaussians_features_backward(*a, features))  # noqa: E731
         if raster_settings.debug:
             cpu_args = cpu_deep_copy_tuple(args)
             try:
-                grads8 = _C.rasterize_gaussians_backward(*args)
+                grads8 = bwd(*args)
             except Exception as ex:
                 torch.save(cpu_args, "snapshot_bw.dump")
                 print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
                 raise ex
         else:
-            grads8 = _C.rasterize_gaussians_backward(*args)
-        grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales, grad_rotations = grads8
+            grads8 = bwd(*args)
+        grad_features = grads8[8] if F else None
+        grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales, grad_rotations = grads8[:8]
         # the reference returns a gradient for every input slot, including the "not provided" empty tensors
         if colors_precomp.numel() == 0:
             grad_colors_precomp = None
@@ -521,8 +694,10 @@ class _RasterizeGaussians(torch.autograd.Function):
             grad_sh = None
         if cov3Ds_precomp.numel() == 0:
             grad_cov3Ds_precomp = None
+        if grad_features is not None:
+            grad_features = grad_features.view(features.shape)
         return (grad_means3D, grad_means2D, grad_sh, grad_colors_precomp, grad_opacities, grad_scales,
-                grad_rotations, grad_cov3Ds_precomp, None)
+                grad_rotations, grad_cov3Ds_precomp, None, grad_features)
 
 
 class BatchRasterizationSettings(NamedTuple):
@@ -555,42 +730,53 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
     means2D is (M,P,3) and only receives the densification proxy gradient, as in the single-frame op."""
 
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, rs):
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, rs, features=None):
+        kw = {} if features is None else {"features": features}
         num_rendered, color, allmap, radii, geomBuffer, binningBuffer, imgBuffer = _C.rasterize_gaussians_batch(
             rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, rs.viewmatrix, rs.projmatrix,
-            rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh, rs.sh_degree, rs.campos, rs.prefiltered, rs.debug)
+            rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh, rs.sh_degree, rs.campos, rs.prefiltered, rs.debug,
+            **kw)[:7]
         ctx.rs = rs
-        ctx.save_for_backward(colors_precomp, means3D, scales, rotations, radii, sh, opacities, geomBuffer, binningBuffer, imgBuffer)
+        ctx.has_features = features is not None
+        ctx.save_for_backward(colors_precomp, means3D, scales, rotations, radii, sh, opacities, geomBuffer, binningBuffer, imgBuffer,
+                              features)
         ctx.mark_non_differentiable(radii)
         return color, radii, allmap
 
     @staticmethod
     def backward(ctx, grad_color, grad_radii, grad_allmap):
         rs = ctx.rs
-        colors_precomp, means3D, scales, rotations, radii, sh, opacities, geomBuffer, binningBuffer, imgBuffer = ctx.saved_tensors
+        (colors_precomp, means3D, scales, rotations, radii, sh, opacities, geomBuffer, binningBuffer, imgBuffer,
+         features) = ctx.saved_tensors
         M = int(rs.viewmatrix.shape[0])
         H, W = rs.image_height, rs.image_width
+        F = int(features.shape[-1]) if ctx.has_features else 0
         if grad_color is None:
-            grad_color = torch.zeros((M, 3, H, W), dtype=torch.float32, device=means3D.device)
+            grad_color = torch.zeros((M, 3 + F, H, W), dtype=torch.float32, device=means3D.device)
         if grad_allmap is None:
             grad_allmap = torch.zeros((M, 8, H, W), dtype=torch.float32, device=means3D.device)
-        g2d, gcol, gop, g3d, gtm, gsh, gsc, grot = _C.rasterize_gaussians_backward_batch(
+        kw = {"features": features} if F else {}
+        grads = _C.rasterize_gaussians_backward_batch(
             rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, rs.viewmatrix, rs.projmatrix,
             rs.tanfovx, rs.tanfovy, grad_color, grad_allmap, sh, rs.sh_degree, rs.campos, geomBuffer, binningBuffer, imgBuffer,
-            None, rs.debug, sum_shared=True, opacity_shared=opacities.ndim == 2, want_transmat=False)
+            None, rs.debug, sum_shared=True, opacity_shared=opacities.ndim == 2, want_transmat=False, **kw)
+        g2d, gcol, gop, g3d, gtm, gsh, gsc, grot = grads[:8]
         return (_reduce_like(g3d, means3D), g2d, _reduce_like(gsh, sh), _reduce_like(gcol, colors_precomp),
-                _reduce_like(gop, opacities), _reduce_like(gsc, scales), _reduce_like(grot, rotations), None)
+                _reduce_like(gop, opacities), _reduce_like(gsc, scales), _reduce_like(grot, rotations), None,
+                _reduce_like(grads[8], features) if F else None)
 
 
-def rasterize_gaussians_batch(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, raster_settings):
-    """Batched twin of rasterize_gaussians: returns (color (M,3,H,W), radii (M,P), allmap (M,8,H,W))."""
+def rasterize_gaussians_batch(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, raster_settings,
+                              features=None):
+    """Batched twin of rasterize_gaussians: returns (color (M,3,H,W), radii (M,P), allmap (M,8,H,W)).
+    features (P,F) shared or (M,P,F) per frame, 1 <= F <= 32: color is (M,3+F,H,W), feature planes after the colour."""
     dev = means3D.device
     empty = lambda: torch.empty((0,), dtype=torch.float32, device=dev)  # noqa: E731
     if (shs is None) == (colors_precomp is None):
         raise Exception('Please provide excatly one of either SHs or precomputed colors!')
     return _RasterizeGaussiansBatch.apply(means3D, means2D, empty() if shs is None else shs,
                                           empty() if colors_precomp is None else colors_precomp, opacities, scales, rotations,
-                                          raster_settings)
+                                          raster_settings, features)
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -621,6 +807,19 @@ class GaussianRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3D_precomp=None):
+        return self._rasterize(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp, None)
+
+    def forward_features(self, means3D, means2D, opacities, features, shs=None, colors_precomp=None, scales=None,
+                         rotations=None, cov3D_precomp=None):
+        """forward() plus per-surfel channels (not in the reference; forward() keeps the reference's signature so that
+        the class stays a drop-in): features (P,F), 1 <= F <= 32, composited with the colour's weights and independent
+        of where the colour comes from.  The returned colour is (3+F,H,W) -- RGB, then the F feature planes (background:
+        raster_settings.bg[3:] when bg has 3+F values, else 0)."""
+        if features is None:
+            raise RuntimeError("forward_features needs a features tensor (P,F)")
+        return self._rasterize(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp, features)
+
+    def _rasterize(self, means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp, features):
         raster_settings = self.raster_settings
         if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
             raise Exception('Please provide excatly one of either SHs or precomputed colors!')
@@ -639,5 +838,7 @@ class GaussianRasterizer(nn.Module):
             rotations = empty()
         if cov3D_precomp is None:
             cov3D_precomp = empty()
+        if features is not None:
+            _check_features(features, int(means3D.shape[0]), raster_settings.bg)
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
-                                   cov3D_precomp, raster_settings)
+                                   cov3D_precomp, raster_settings, features)

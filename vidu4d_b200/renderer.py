@@ -164,8 +164,12 @@ def depth_to_normal(view, depth):
 # ---------------------------------------------------------------------------------------------
 # gs/gaussian_renderer/__init__.py:21-164
 # ---------------------------------------------------------------------------------------------
-def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None):
-    """Render the scene.  Background tensor (bg_color) must be on GPU!"""
+def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None, features=None):
+    """Render the scene.  Background tensor (bg_color) must be on GPU!
+
+    features (P,F), 1 <= F <= 32 (not in the reference): per-surfel channels composited with the colour's weights next to
+    the SH colour; "render" is then (3+F,H,W) -- RGB, then the F feature planes over bg_color[3:] (bg_color of 3+F values)
+    or a zero background (bg_color of 3).  Vidu4D's 22-channel vector (deformable_gaussian.py:1182-1207) goes here."""
     xyz = pc.get_xyz
     screenspace_points = torch.zeros_like(xyz, dtype=xyz.dtype, requires_grad=True, device=xyz.device) + 0
     try:
@@ -211,9 +215,14 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         means3D.retain_grad()
     except Exception:
         pass
-    rendered_image, radii, allmap = rasterizer(
-        means3D=means3D, means2D=means2D, shs=shs, colors_precomp=colors_precomp, opacities=opacity,
-        scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp)
+    if features is None:
+        rendered_image, radii, allmap = rasterizer(
+            means3D=means3D, means2D=means2D, shs=shs, colors_precomp=colors_precomp, opacities=opacity,
+            scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp)
+    else:
+        rendered_image, radii, allmap = rasterizer.forward_features(
+            means3D=means3D, means2D=means2D, opacities=opacity, features=features, shs=shs,
+            colors_precomp=colors_precomp, scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp)
 
     rets = {"render": rendered_image,
             "viewspace_points": means2D,
@@ -288,8 +297,9 @@ class _RenderPost(torch.autograd.Function):
         return g_allmap, None, None, None, None
 
 
-def render_fused(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None):
-    """Same contract and dict keys as render(); the post-processing of `allmap` runs in one fused CUDA kernel each
+def render_fused(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
+                 features=None):
+    """Same contract, `features` and dict keys as render(); the post-processing of `allmap` runs in one fused CUDA kernel each
     way instead of ~35 forward / ~60 backward PyTorch kernels (SURVEY.md section 8(f) row N1).  The three depth
     entries are (3,H,W) broadcast VIEWS of one plane (render() materialises three copies with torch.cat)."""
     xyz = pc.get_xyz
@@ -314,9 +324,9 @@ def render_fused(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_mod
         xyz.retain_grad()
     except Exception:
         pass
-    rendered_image, radii, allmap = rasterizer(
-        means3D=xyz, means2D=screenspace_points, shs=pc.get_features, colors_precomp=override_color,
-        opacities=pc.get_opacity, scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp)
+    kw = dict(means3D=xyz, means2D=screenspace_points, shs=pc.get_features, colors_precomp=override_color,
+              opacities=pc.get_opacity, scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp)
+    rendered_image, radii, allmap = rasterizer(**kw) if features is None else rasterizer.forward_features(features=features, **kw)
     acc, rn, dist, med, ex, sd, sn = _RenderPost.apply(allmap, viewpoint_camera.world_view_transform, tanfovx, tanfovy,
                                                        float(pipe.depth_ratio))
     return {"render": rendered_image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0,
@@ -364,10 +374,11 @@ def stack_cameras(cams) -> BatchCameras:
 
 class _RasterLossBatch(torch.autograd.Function):
     """rasterize M frames -> fused post-processing + losses.  The loss kernel already produced dL/dcolor and dL/dallmap,
-    so backward() is just the rasterizer backward with the upstream scalar as `grad_scale`."""
+    so backward() is just the rasterizer backward with the upstream scalar as `grad_scale`.  Optional feature planes are a
+    further differentiable output; their incoming gradient (already scaled) goes to the same rasterizer backward."""
 
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, bkgd, cfg):
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, bkgd, cfg, features=None):
         from . import _capi
         from .rasterizer import _C
         lib = _capi.load()
@@ -375,9 +386,12 @@ class _RasterLossBatch(torch.autograd.Function):
         M, H, W = len(cams), cams.image_height, cams.image_width
         dev = means3D.device
         e = torch.empty((0,), dtype=torch.float32, device=dev)
-        nr, color, allmap, radii, gb, bb, ib = _C.rasterize_gaussians_batch(
+        kw = {} if features is None else {"features": features, "concat": False}
+        out = _C.rasterize_gaussians_batch(
             bg, means3D, e, opacities, scales, rotations, 1.0, cams.world_view_transform, cams.full_proj_transform, tanx, tany,
-            H, W, sh, sh_degree, cams.camera_center)
+            H, W, sh, sh_degree, cams.camera_center, **kw)
+        nr, color, allmap, radii, gb, bb, ib = out[:7]
+        feat = out[7] if features is not None else None
         terms = torch.empty((M, 4), dtype=torch.float32, device=dev)
         dLc = torch.empty_like(color)
         dLa = torch.empty_like(allmap)
@@ -401,27 +415,39 @@ class _RasterLossBatch(torch.autograd.Function):
         ctx.cfg = (cams, bg, sh_degree, tanx, tany)
         ctx.has_bkgd = bkgd is not None
         ctx.save_for_backward(means3D, scales, rotations, radii, sh, opacities, gb, bb, ib, dLc, dLa,
-                              dLb if dLb is not None else e)
+                              dLb if dLb is not None else e, features)
+        ctx.has_features = features is not None
         ctx.mark_non_differentiable(terms, color, allmap, radii)
-        return total, terms, color, allmap, radii
+        if feat is None:
+            return total, terms, color, allmap, radii
+        return total, terms, color, allmap, radii, feat
 
     @staticmethod
-    def backward(ctx, g_total, g_terms, g_color, g_allmap, g_radii):
+    def backward(ctx, g_total, g_terms, g_color, g_allmap, g_radii, g_feat=None):
         from .rasterizer import _C, _reduce_like
         cams, bg, sh_degree, tanx, tany = ctx.cfg
-        means3D, scales, rotations, radii, sh, opacities, gb, bb, ib, dLc, dLa, dLb = ctx.saved_tensors
+        means3D, scales, rotations, radii, sh, opacities, gb, bb, ib, dLc, dLa, dLb, features = ctx.saved_tensors
         e = torch.empty((0,), dtype=torch.float32, device=means3D.device)
-        g2d, gcol, gop, g3d, gtm, gsh, gsc, grot = _C.rasterize_gaussians_backward_batch(
+        kw = {}
+        if ctx.has_features:
+            if g_feat is None:
+                g_feat = torch.zeros((dLc.shape[0], features.shape[-1]) + tuple(dLc.shape[2:]), dtype=torch.float32,
+                                     device=means3D.device)
+            kw = {"features": features, "dL_dout_features": g_feat}
+        grads = _C.rasterize_gaussians_backward_batch(
             bg, means3D, radii, e, scales, rotations, 1.0, cams.world_view_transform, cams.full_proj_transform, tanx, tany,
             dLc, dLa, sh, sh_degree, cams.camera_center, gb, bb, ib, grad_scale=g_total, sum_shared=True,
-            opacity_shared=opacities.ndim == 2, want_transmat=False)
+            opacity_shared=opacities.ndim == 2, want_transmat=False, **kw)
+        g2d, gcol, gop, g3d, gtm, gsh, gsc, grot = grads[:8]
         g_bk = (dLb.sum(0) * g_total) if ctx.has_bkgd else None
         return (_reduce_like(g3d, means3D), g2d, _reduce_like(gsh, sh), _reduce_like(gop, opacities),
-                _reduce_like(gsc, scales), _reduce_like(grot, rotations), g_bk, None)
+                _reduce_like(gsc, scales), _reduce_like(grot, rotations), g_bk, None,
+                _reduce_like(grads[8], features) if ctx.has_features else None)
 
 
 def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_gt=None, mask_wt=None, learnable_bkgd=None,
-                      w_rgb=1.0, w_mask=0.0, lambda_normal=0.0, lambda_dist=0.0, means3D=None, rotations=None, target_stream=None):
+                      w_rgb=1.0, w_mask=0.0, lambda_normal=0.0, lambda_dist=0.0, means3D=None, rotations=None, target_stream=None,
+                      features=None):
     """The Stage-3 inner loop for M frames in one call: rasterize every frame (batched launch set), post-process and
     evaluate the image losses in one fused kernel, and hand autograd a single scalar.
 
@@ -431,10 +457,13 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
     target_rgb (M,3,H,W); vis2d / mask_gt / mask_wt (M,H,W) or None; learnable_bkgd (3,) or None.
     target_stream: CUDA stream on which target_rgb (and the masks) are still being produced, e.g. an H2D copy running
     beside the rasterizer forward; it is joined right before the loss kernel (None: the tensors are ready).
+    features: optional per-surfel channels, (P,F) shared or (M,P,F) per frame, 1 <= F <= 32, composited with the colour's
+    weights (bg_color may then have 3+F values); they are not part of the fused losses.
 
     Returns {"loss": scalar (sum over frames and terms, differentiable), "terms": (M,4) weighted rgb/mask/normal/dist
     (detached), "render": (M,3,H,W), "allmap": (M,8,H,W), "radii": (M,P), "visibility_filter": (M,P),
-    "viewspace_points": (M,P,3) whose .grad receives the densification proxy}."""
+    "viewspace_points": (M,P,3) whose .grad receives the densification proxy}; with features also "features": (M,F,H,W),
+    differentiable, so that a caller's own feature / flow / mask losses backpropagate through the same rasterizer backward."""
     if not isinstance(cameras, BatchCameras):
         cameras = stack_cameras(cameras)
     M = len(cameras)
@@ -445,7 +474,11 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
     tanx, tany = _cam_tans(cameras)
     cfg = (cameras, bg_color, pc.active_sh_degree, target_rgb, vis2d, mask_gt, mask_wt, float(pipe.depth_ratio),
            w_rgb, w_mask, lambda_normal, lambda_dist, tanx, tany, target_stream)
-    total, terms, color, allmap, radii = _RasterLossBatch.apply(xyz, screenspace_points, pc.get_features, pc.get_opacity,
-                                                                pc.get_scaling, rot, learnable_bkgd, cfg)
-    return {"loss": total, "terms": terms, "render": color, "allmap": allmap, "radii": radii,
-            "visibility_filter": radii > 0, "viewspace_points": screenspace_points}
+    outs = _RasterLossBatch.apply(xyz, screenspace_points, pc.get_features, pc.get_opacity, pc.get_scaling, rot,
+                                  learnable_bkgd, cfg, features)
+    total, terms, color, allmap, radii = outs[:5]
+    out = {"loss": total, "terms": terms, "render": color, "allmap": allmap, "radii": radii,
+           "visibility_filter": radii > 0, "viewspace_points": screenspace_points}
+    if features is not None:
+        out["features"] = outs[5]
+    return out
