@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SR_ABI_VERSION 4
+#define SR_ABI_VERSION 5
 
 #if defined(__GNUC__)
 #define SR_API __attribute__((visibility("default")))
@@ -264,6 +264,25 @@ SR_API int sr_render_loss_batch(int32_t M, int32_t W, int32_t H, float tan_fovx,
                                 const float* learnable_bkgd, float w_rgb, float w_mask, float lambda_normal, float lambda_dist,
                                 float* loss_terms, float* dL_dcolor, float* dL_dallmap, float* dL_dbkgd,
                                 float* surf_depth_scratch, void* stream);
+
+/*
+ * Stage-3 losses on the rasterizer's FEATURE planes (sr_forward_batch_features), forward and gradient, M frames per call.
+ * Replaces lab4d/engine/model.py:663-667 (feature reconstruction) and :742-745 (Gaussian-mask consistency) with their
+ * masking (:952-967) and reduction (:1000-1012):
+ *   feature:        v = ||features[c] - target[c]||_2 over c < Cf, times mask_gt and is_detected[frame]
+ *   reg_gauss_mask: v = (features[gauss_mask_channel] - alpha)^2, alpha = allmap plane 1 (no gradient), unmasked
+ *   term k = weights[k] * mean of v over the pixels of the WHOLE batch where v > 0 (0 if there is none).
+ *   features[M*F*HW]; target[M*Cf*HW] (NULL = no feature term, Cf must then be 0; else 1 <= Cf <= F and mask_gt[M*HW]
+ *   is required); is_detected[M] (NULL = 1); allmap[M*8*HW]; gauss_mask_channel in [Cf, F), or -1 = no term;
+ *   weights[2] = {feature, reg_gauss_mask} DEVICE floats, read at run time (they may change between graph replays).
+ * Writes feature_terms[M*2] = each frame's share of the two weighted terms (their sum over frames is the term),
+ * counts[M*2] = each frame's number of pixels with v > 0, and dL_dfeatures[M*F*HW] = the gradient of the sum of the
+ * two terms (fully written: 0 on channels no term reads).  Two kernels; no allocation, no host synchronisation.
+ */
+SR_API int sr_feature_loss_batch(int32_t M, int32_t W, int32_t H, int32_t F, int32_t Cf, int32_t gauss_mask_channel,
+                                 const float* features, const float* target, const float* mask_gt, const float* is_detected,
+                                 const float* allmap, const float* weights, float* feature_terms, uint32_t* counts,
+                                 float* dL_dfeatures, void* stream);
 
 /*
  * Fused bob-skinning warp (SURVEY.md section 8(f) rows N2/N3): canonical surfels -> every frame's camera space.

@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libsurfel_raster.so")
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 SR_STATUS_OVERFLOW = 1
 SR_STATUS_PREFILTER = 4
 SR_BATCH_SUM_SHARED = 1
@@ -20,7 +20,7 @@ SYMBOLS = (
     "sr_geom_bytes", "sr_image_bytes", "sr_binning_bytes", "sr_forward", "sr_backward",
     "sr_mark_visible", "sr_debug_view", "sr_abi_version", "sr_last_error", "sr_launch_count",
     "sr_set_profiling", "sr_get_profile", "sr_post_forward", "sr_post_backward", "sr_forward_batch", "sr_backward_batch", "sr_render_loss_batch", "sr_bob_warp_table_floats", "sr_bob_warp_forward", "sr_bob_warp_backward", "sr_adam_flat", "sr_surfel_compact", "sr_knn_cells", "sr_knn_mean_dist2",
-    "sr_forward_batch_features", "sr_backward_batch_features",
+    "sr_forward_batch_features", "sr_backward_batch_features", "sr_feature_loss_batch",
 )
 FEATURES_MAX = 32          # channels per call (SR_FEAT_MAX)
 
@@ -105,6 +105,8 @@ def load():
     lib.sr_post_backward.argtypes = [i32, i32, C.c_float, C.c_float, C.c_float] + [vp] * 12
     lib.sr_render_loss_batch.restype = C.c_int
     lib.sr_render_loss_batch.argtypes = [i32, i32, i32, C.c_float, C.c_float, C.c_float] + [vp] * 8 + [C.c_float] * 4 + [vp] * 6
+    lib.sr_feature_loss_batch.restype = C.c_int
+    lib.sr_feature_loss_batch.argtypes = [i32] * 6 + [vp] * 10
     lib.sr_bob_warp_table_floats.restype = C.c_size_t
     lib.sr_bob_warp_table_floats.argtypes = [i32, i32]
     lib.sr_bob_warp_forward.restype = C.c_int

@@ -74,6 +74,8 @@ int check_frame(const sr_frame* f) {
 
 void sr_count_launch(int n) { g_launches.fetch_add((uint64_t)n, std::memory_order_relaxed); }
 
+int sr_fail(int code, const char* msg, int a, int b) { return fail(code, msg, a, b); }
+
 cudaError_t sr_memset_frames(void* p, size_t pitch, size_t bytes, int frames, cudaStream_t s) {
     if (frames == 1) return cudaMemsetAsync(p, 0, bytes, s);
     return cudaMemset2DAsync(p, pitch, 0, bytes, (size_t)frames, s);

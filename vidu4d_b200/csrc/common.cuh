@@ -218,6 +218,8 @@ cudaError_t launch_mark_visible(int P, const float* means3D, const float* vm, ui
 cudaError_t sr_memset_frames(void* p, size_t pitch, size_t bytes, int frames, cudaStream_t s);
 
 void sr_count_launch(int n = 1);
+// sets the message sr_last_error() returns (printf format with up to two int arguments) and returns `code`
+int sr_fail(int code, const char* msg, int a = 0, int b = 0);
 
 // Optional per-kernel timing (sr_set_profiling): CUDA events recorded on the launching stream around each
 // kernel; read back (after a sync) with sr_get_profile().  Off by default: zero overhead on the hot path.

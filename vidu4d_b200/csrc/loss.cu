@@ -200,6 +200,105 @@ loss_grad_kernel(const LossCfg g, const float* __restrict__ color, const float* 
     }
 }
 
+// ---- Stage-3 losses on the feature planes (DESIGN.md section 3.5a):
+//   lab4d/engine/model.py:663-667   feature:        v = ||feat_r - feat_gt||_2 over the Cf target channels
+//   lab4d/engine/model.py:742-745   reg_gauss_mask: v = (gauss_mask_r - acc.detach())^2
+//   lab4d/engine/model.py:952-967   feature masked by the gt mask and the frame's is_detected; reg_gauss_mask unmasked
+//   lab4d/engine/model.py:1000-1012 term = w * mean(v[v > 0]) over the whole batch (v.mean() = 0 when nothing is > 0)
+// The denominator is a batch-wide count, known only after every pixel has been seen, so the pass is two launches:
+// feat_loss_kernel writes the UNSCALED per-pixel gradient (dv/dfeat where v > 0, else 0) and per-frame block-reduced
+// sums and counts; feat_loss_scale_kernel multiplies the touched planes and the sums by w_k / C_k (0 when C_k = 0).
+// Every pixel's gradient is written by its own thread: no atomics on image data, deterministic planes.
+struct FeatLossCfg {
+    int W, H, F, Cf, gm;    // Cf = 0: no feature term; gm = -1: no Gaussian-mask term
+};
+
+__global__ void __launch_bounds__(256)
+feat_loss_kernel(const FeatLossCfg g, const float* __restrict__ feat, const float* __restrict__ target,
+                 const float* __restrict__ mask_gt, const float* __restrict__ is_detected, const float* __restrict__ allmap,
+                 float* __restrict__ terms, uint32_t* __restrict__ counts, float* __restrict__ g_feat) {
+    const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5), f = blockIdx.z;
+    const size_t N = (size_t)g.W * g.H;
+    float part[2] = {0.f, 0.f};
+    uint32_t cnt[2] = {0u, 0u};
+    if (x < g.W && y < g.H) {
+        const size_t p = (size_t)y * g.W + x;
+        const float* fe = feat + (size_t)f * g.F * N + p;
+        float* gf = g_feat + (size_t)f * g.F * N + p;
+        if (g.Cf > 0) {
+            const float* tg = target + (size_t)f * g.Cf * N + p;
+            const float wpx = mask_gt[(size_t)f * N + p] * (is_detected ? __ldg(is_detected + f) : 1.f);
+            float ss = 0.f;
+            for (int c = 0; c < g.Cf; c++) {
+                const float d = fe[c * N] - tg[c * N];
+                ss += d * d;
+            }
+            const float nrm = sqrtf(ss), v = nrm * wpx;
+            const bool on = v > 0.f;                     // also excludes ||d|| = 0, where torch's norm gradient is 0
+            const float k = on ? wpx / nrm : 0.f;
+            for (int c = 0; c < g.Cf; c++) gf[c * N] = (fe[c * N] - tg[c * N]) * k;
+            part[0] = on ? v : 0.f;
+            cnt[0] = on;
+        }
+        for (int c = g.Cf; c < g.F; c++)
+            if (c != g.gm) gf[c * N] = 0.f;
+        if (g.gm >= 0) {
+            const float d = fe[g.gm * N] - allmap[(size_t)f * 8 * N + N + p];
+            const float v = d * d;
+            const bool on = v > 0.f;
+            gf[g.gm * N] = on ? 2.f * d : 0.f;
+            part[1] = on ? v : 0.f;
+            cnt[1] = on;
+        }
+    }
+    // block reduction as in loss_grad_kernel: 2 float + 2 integer atomics per block
+    __shared__ float red[8][2];
+    __shared__ uint32_t redc[8][2];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+        float vs = part[i];
+        uint32_t cs = cnt[i];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            vs += __shfl_xor_sync(0xffffffffu, vs, o);
+            cs += __shfl_xor_sync(0xffffffffu, cs, o);
+        }
+        if (lane == 0) { red[warp][i] = vs; redc[warp][i] = cs; }
+    }
+    __syncthreads();
+    if (threadIdx.x < 2) {
+        float t = 0.f;
+        uint32_t c = 0u;
+#pragma unroll
+        for (int w = 0; w < 8; w++) { t += red[w][threadIdx.x]; c += redc[w][threadIdx.x]; }
+        if (c) {
+            atomicAdd(terms + (size_t)f * 2 + threadIdx.x, t);
+            atomicAdd(counts + (size_t)f * 2 + threadIdx.x, c);
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256)
+feat_loss_scale_kernel(const FeatLossCfg g, const float* __restrict__ weights, const uint32_t* __restrict__ counts,
+                       float* __restrict__ terms, float* __restrict__ g_feat) {
+    const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5), f = blockIdx.z;
+    __shared__ float s[2];
+    if (threadIdx.x < 2) {
+        unsigned long long c = 0;                      // the count over the whole batch: the reference's v[v > 0].mean()
+        for (int m = 0; m < (int)gridDim.z; m++) c += counts[(size_t)m * 2 + threadIdx.x];
+        s[threadIdx.x] = c ? __ldg(weights + threadIdx.x) / (float)c : 0.f;
+        if (blockIdx.x == 0 && blockIdx.y == 0) terms[(size_t)f * 2 + threadIdx.x] *= s[threadIdx.x];
+    }
+    __syncthreads();
+    if (x >= g.W || y >= g.H) return;
+    const size_t N = (size_t)g.W * g.H;
+    float* gf = g_feat + (size_t)f * g.F * N + (size_t)y * g.W + x;
+    const float s0 = s[0];
+    for (int c = 0; c < g.Cf; c++) gf[c * N] *= s0;
+    if (g.gm >= 0) gf[g.gm * N] *= s[1];
+}
+
 }  // namespace
 
 extern "C" {
@@ -226,6 +325,44 @@ SR_API int sr_render_loss_batch(int32_t M, int32_t W, int32_t H, float tanx, flo
         ProfileScope ps("loss_grad", s);
         loss_grad_kernel<<<grid, 256, 0, s>>>(g, color, allmap, world_view_transform, target_rgb, vis2d, mask_gt, mask_wt,
                                              learnable_bkgd, surf_depth_scratch, loss_terms, dL_dcolor, dL_dallmap, dL_dbkgd);
+    }
+    sr_count_launch(2);
+    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+}
+
+SR_API int sr_feature_loss_batch(int32_t M, int32_t W, int32_t H, int32_t F, int32_t Cf, int32_t gauss_mask_channel,
+                                 const float* features, const float* target, const float* mask_gt, const float* is_detected,
+                                 const float* allmap, const float* weights, float* feature_terms, uint32_t* counts,
+                                 float* dL_dfeatures, void* stream_) {
+    if (M < 1 || W <= 0 || H <= 0) return sr_fail(SR_EINVAL, "M, W and H must be positive");
+    if (F < 1) return sr_fail(SR_EINVAL, "F must be >= 1, got %d", F);
+    if (!features || !allmap || !weights || !feature_terms || !counts || !dL_dfeatures)
+        return sr_fail(SR_EINVAL, "features, allmap, weights, feature_terms, counts and dL_dfeatures must not be NULL");
+    if (target) {
+        if (Cf < 1 || Cf > F) return sr_fail(SR_EINVAL, "Cf must be in [1, F = %d] with a target, got %d", F, Cf);
+        if (!mask_gt) return sr_fail(SR_EINVAL, "the feature term needs mask_gt");
+    } else if (Cf != 0) {
+        return sr_fail(SR_EINVAL, "Cf must be 0 without a target, got %d", Cf);
+    }
+    if (gauss_mask_channel < -1 || gauss_mask_channel >= F)
+        return sr_fail(SR_EINVAL, "gauss_mask_channel must be -1 or in [0, F = %d), got %d", F, gauss_mask_channel);
+    if (gauss_mask_channel >= 0 && gauss_mask_channel < Cf)
+        return sr_fail(SR_EINVAL, "gauss_mask_channel %d lies inside the feature target's channels [0, %d)",
+                       gauss_mask_channel, Cf);
+    if (!target && gauss_mask_channel < 0) return sr_fail(SR_EINVAL, "no term: neither a target nor a gauss_mask_channel");
+    cudaStream_t s = (cudaStream_t)stream_;
+    const FeatLossCfg g{W, H, F, Cf, gauss_mask_channel};
+    dim3 grid((W + 31) / 32, (H + 7) / 8, M);
+    if (cudaMemsetAsync(feature_terms, 0, (size_t)M * 2 * sizeof(float), s) != cudaSuccess) return SR_ECUDA;
+    if (cudaMemsetAsync(counts, 0, (size_t)M * 2 * sizeof(uint32_t), s) != cudaSuccess) return SR_ECUDA;
+    {
+        ProfileScope ps("feat_loss", s);
+        feat_loss_kernel<<<grid, 256, 0, s>>>(g, features, target, mask_gt, is_detected, allmap, feature_terms, counts,
+                                              dL_dfeatures);
+    }
+    {
+        ProfileScope ps("feat_loss_scale", s);
+        feat_loss_scale_kernel<<<grid, 256, 0, s>>>(g, weights, counts, feature_terms, dL_dfeatures);
     }
     sr_count_launch(2);
     return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;

@@ -378,7 +378,7 @@ class _RasterLossBatch(torch.autograd.Function):
     further differentiable output; their incoming gradient (already scaled) goes to the same rasterizer backward."""
 
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, bkgd, cfg, features=None):
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, bkgd, cfg, features=None, feature_loss=None):
         from . import _capi
         from .rasterizer import _C
         lib = _capi.load()
@@ -412,25 +412,43 @@ class _RasterLossBatch(torch.autograd.Function):
                                           torch.cuda.current_stream(dev).cuda_stream)
         _capi.check(rc, "sr_render_loss_batch")
         total = terms.sum()
+        dLf = None
+        if feature_loss is not None:        # the losses on the feature planes: csrc/loss.cu, sr_feature_loss_batch
+            ftarget, is_det, gm, weights = feature_loss
+            F = feat.shape[1]
+            fterms = torch.empty((M, 2), dtype=torch.float32, device=dev)
+            counts = torch.empty((M, 2), dtype=torch.int32, device=dev)
+            dLf = torch.empty_like(feat)
+            ftarget, is_det = f32(ftarget), f32(is_det)
+            with torch.cuda.device(dev):
+                rc = lib.sr_feature_loss_batch(M, W, H, F, 0 if ftarget is None else int(ftarget.shape[1]), gm,
+                                               feat.data_ptr(), ptr(ftarget), ptr(mask), ptr(is_det), allmap.data_ptr(),
+                                               weights.data_ptr(), fterms.data_ptr(), counts.data_ptr(), dLf.data_ptr(),
+                                               torch.cuda.current_stream(dev).cuda_stream)
+            _capi.check(rc, "sr_feature_loss_batch")
+            total = total + fterms.sum()
         ctx.cfg = (cams, bg, sh_degree, tanx, tany)
         ctx.has_bkgd = bkgd is not None
         ctx.save_for_backward(means3D, scales, rotations, radii, sh, opacities, gb, bb, ib, dLc, dLa,
-                              dLb if dLb is not None else e, features)
+                              dLb if dLb is not None else e, features, dLf)
         ctx.has_features = features is not None
-        ctx.mark_non_differentiable(terms, color, allmap, radii)
-        if feat is None:
-            return total, terms, color, allmap, radii
-        return total, terms, color, allmap, radii, feat
+        outs = (total, terms, color, allmap, radii) + (() if feat is None else (feat,)) + (() if dLf is None else (fterms, counts))
+        ctx.mark_non_differentiable(terms, color, allmap, radii, *outs[6:])
+        return outs
 
     @staticmethod
-    def backward(ctx, g_total, g_terms, g_color, g_allmap, g_radii, g_feat=None):
+    def backward(ctx, g_total, g_terms, g_color, g_allmap, g_radii, g_feat=None, *_):
         from .rasterizer import _C, _reduce_like
         cams, bg, sh_degree, tanx, tany = ctx.cfg
-        means3D, scales, rotations, radii, sh, opacities, gb, bb, ib, dLc, dLa, dLb, features = ctx.saved_tensors
+        means3D, scales, rotations, radii, sh, opacities, gb, bb, ib, dLc, dLa, dLb, features, dLf = ctx.saved_tensors
         e = torch.empty((0,), dtype=torch.float32, device=means3D.device)
         kw = {}
         if ctx.has_features:
-            if g_feat is None:
+            if dLf is not None:
+                # the fused feature losses' plane gradient scales with the upstream scalar like dLc / dLa; the caller's own
+                # use of out["features"] (g_feat) does not -- so the two are summed here and handed over unscaled
+                g_feat = dLf * g_total if g_feat is None else torch.addcmul(g_feat, dLf, g_total)
+            elif g_feat is None:
                 g_feat = torch.zeros((dLc.shape[0], features.shape[-1]) + tuple(dLc.shape[2:]), dtype=torch.float32,
                                      device=means3D.device)
             kw = {"features": features, "dL_dout_features": g_feat}
@@ -442,12 +460,43 @@ class _RasterLossBatch(torch.autograd.Function):
         g_bk = (dLb.sum(0) * g_total) if ctx.has_bkgd else None
         return (_reduce_like(g3d, means3D), g2d, _reduce_like(gsh, sh), _reduce_like(gop, opacities),
                 _reduce_like(gsc, scales), _reduce_like(grot, rotations), g_bk, None,
-                _reduce_like(grads[8], features) if ctx.has_features else None)
+                _reduce_like(grads[8], features) if ctx.has_features else None, None)
+
+
+def _check_feature_losses(M, H, W, features, feature_target, mask_gt, is_detected, gauss_mask_channel, feature_loss_weights):
+    """Validate the fused feature-loss arguments of render_loss_batch before anything runs on the device (shapes and
+    channels first, then devices); returns (feature_target, is_detected, gauss_mask_channel (-1 = off), weights)."""
+    if features is None:
+        raise RuntimeError("fused feature losses (feature_target / gauss_mask_channel) need features=")
+    F = int(features.shape[-1])
+    Cf = 0
+    if feature_target is not None:
+        Cf = int(feature_target.shape[1]) if feature_target.ndim == 4 else -1
+        if Cf < 1 or Cf > F or tuple(feature_target.shape[::2]) != (M, H) or feature_target.shape[3] != W:
+            raise RuntimeError(f"feature_target must be (M,Cf,H,W) = ({M},Cf,{H},{W}) with 1 <= Cf <= F = {F}, "
+                               f"got {tuple(feature_target.shape)}")
+        if mask_gt is None:
+            raise RuntimeError("the feature term needs mask_gt (the reference masks it with batch['mask'])")
+    gm = -1 if gauss_mask_channel is None else int(gauss_mask_channel)
+    if gauss_mask_channel is not None and not Cf <= gm < F:
+        raise RuntimeError(f"gauss_mask_channel must be in [Cf, F) = [{Cf}, {F}), got {gauss_mask_channel}")
+    if is_detected is not None and tuple(is_detected.shape) != (M,):
+        raise RuntimeError(f"is_detected must be (M,) = ({M},), got {tuple(is_detected.shape)}")
+    if feature_loss_weights is not None and (tuple(feature_loss_weights.shape) != (2,)
+                                             or feature_loss_weights.dtype != torch.float32):
+        raise RuntimeError("feature_loss_weights must be a float32 (2,) tensor [feature_wt, reg_gauss_mask_wt]")
+    for name, t in (("features", features), ("feature_target", feature_target), ("mask_gt", mask_gt),
+                    ("is_detected", is_detected), ("feature_loss_weights", feature_loss_weights)):
+        if t is not None and not t.is_cuda:
+            raise RuntimeError(f"{name} must be a CUDA tensor")
+    if feature_loss_weights is None:        # config.py:82,102 defaults; pass a device tensor to change them without re-capture
+        feature_loss_weights = torch.tensor([1e-2, 1e-2], dtype=torch.float32, device=features.device)
+    return feature_target, is_detected, gm, feature_loss_weights.contiguous()
 
 
 def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_gt=None, mask_wt=None, learnable_bkgd=None,
                       w_rgb=1.0, w_mask=0.0, lambda_normal=0.0, lambda_dist=0.0, means3D=None, rotations=None, target_stream=None,
-                      features=None):
+                      features=None, feature_target=None, is_detected=None, gauss_mask_channel=None, feature_loss_weights=None):
     """The Stage-3 inner loop for M frames in one call: rasterize every frame (batched launch set), post-process and
     evaluate the image losses in one fused kernel, and hand autograd a single scalar.
 
@@ -458,15 +507,30 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
     target_stream: CUDA stream on which target_rgb (and the masks) are still being produced, e.g. an H2D copy running
     beside the rasterizer forward; it is joined right before the loss kernel (None: the tensors are ready).
     features: optional per-surfel channels, (P,F) shared or (M,P,F) per frame, 1 <= F <= 32, composited with the colour's
-    weights (bg_color may then have 3+F values); they are not part of the fused losses.
+    weights (bg_color may then have 3+F values).
+
+    Fused losses on the feature planes (csrc/loss.cu, lab4d/engine/model.py:663-667,742-745,952-967,1000-1012), on when
+    feature_target or gauss_mask_channel is given (both need features=):
+      feature_target (M,Cf,H,W), Cf <= F: feature_wt * mean over the batch's positive values of
+          ||planes[:Cf] - feature_target|| * mask_gt * is_detected[frame]; needs mask_gt.
+      gauss_mask_channel c in [Cf, F): reg_gauss_mask_wt * the same positive mean of (planes[c] - alpha.detach())^2.
+      is_detected (M,) or None (= all detected); feature_loss_weights: (2,) float32 DEVICE tensor
+          [feature_wt, reg_gauss_mask_wt], read by the kernel at run time -- update it in place (e.g. the reference's
+          linear ramp of reg_gauss_mask_wt) between replays of a captured step; None = [1e-2, 1e-2].
 
     Returns {"loss": scalar (sum over frames and terms, differentiable), "terms": (M,4) weighted rgb/mask/normal/dist
     (detached), "render": (M,3,H,W), "allmap": (M,8,H,W), "radii": (M,P), "visibility_filter": (M,P),
     "viewspace_points": (M,P,3) whose .grad receives the densification proxy}; with features also "features": (M,F,H,W),
-    differentiable, so that a caller's own feature / flow / mask losses backpropagate through the same rasterizer backward."""
+    differentiable, so that a caller's own losses on the planes backpropagate through the same rasterizer backward; with
+    the fused feature losses also "feature_terms": (M,2) each frame's share of the weighted feature / reg_gauss_mask
+    terms (detached, included in "loss") and "feature_counts": (M,2) int32, each frame's number of positive values."""
     if not isinstance(cameras, BatchCameras):
         cameras = stack_cameras(cameras)
     M = len(cameras)
+    feature_loss = None
+    if feature_target is not None or gauss_mask_channel is not None:
+        feature_loss = _check_feature_losses(M, cameras.image_height, cameras.image_width, features, feature_target, mask_gt,
+                                             is_detected, gauss_mask_channel, feature_loss_weights)
     xyz = pc.get_xyz if means3D is None else means3D
     rot = pc.get_rotation if rotations is None else rotations
     P = int(xyz.shape[-2])
@@ -475,10 +539,12 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
     cfg = (cameras, bg_color, pc.active_sh_degree, target_rgb, vis2d, mask_gt, mask_wt, float(pipe.depth_ratio),
            w_rgb, w_mask, lambda_normal, lambda_dist, tanx, tany, target_stream)
     outs = _RasterLossBatch.apply(xyz, screenspace_points, pc.get_features, pc.get_opacity, pc.get_scaling, rot,
-                                  learnable_bkgd, cfg, features)
+                                  learnable_bkgd, cfg, features, feature_loss)
     total, terms, color, allmap, radii = outs[:5]
     out = {"loss": total, "terms": terms, "render": color, "allmap": allmap, "radii": radii,
            "visibility_filter": radii > 0, "viewspace_points": screenspace_points}
     if features is not None:
         out["features"] = outs[5]
+    if feature_loss is not None:
+        out["feature_terms"], out["feature_counts"] = outs[6], outs[7]
     return out

@@ -20,6 +20,10 @@ import torch
 from . import _capi
 
 GROUPS = (("xyz", 3), ("f_dc", 3), ("f_rest", 45), ("opacity", 1), ("scaling", 2), ("rotation", 4))
+# the optional seventh group: Stage 3's per-surfel registration feature (lab4d/engine/trainer.py:250, lr feature_lr)
+REGIST_FEAT = ("regist_feat", 16)
+_ATTR = {"xyz": "_xyz", "f_dc": "_features_dc", "f_rest": "_features_rest", "opacity": "_opacity", "scaling": "_scaling",
+         "rotation": "_rotation", "regist_feat": "_regist_feat"}
 
 
 def build_rotation(r):
@@ -33,10 +37,15 @@ def build_rotation(r):
 
 
 class FlatSurfelModel(torch.nn.Module):
-    """Surfel parameters as views of one flat buffer.  Duck-types what render() / render_loss_batch() read from `pc`."""
+    """Surfel parameters as views of one flat buffer.  Duck-types what render() / render_loss_batch() read from `pc`.
+
+    regist_feat (P,16), optional: the registration feature the reference optimises with the surfels
+    (gs/scene/gaussian_model.py:324-325,358-378,405-406,427-428), as a seventh group after the other six (whose layout
+    is then unchanged) -- `_regist_feat`, lr key "regist_feat" (default 0.0025, config.py feature_lr).  Densification
+    carries it along: clones and split children copy their parent's row, pruned surfels drop theirs."""
 
     def __init__(self, xyz, features_dc, features_rest, opacity, scaling, rotation, sh_degree=3, percent_dense=0.01,
-                 lrs=None, betas=(0.9, 0.999), eps=1e-15):
+                 lrs=None, betas=(0.9, 0.999), eps=1e-15, regist_feat=None):
         super().__init__()
         dev = xyz.device
         self.max_sh_degree = 3
@@ -45,7 +54,11 @@ class FlatSurfelModel(torch.nn.Module):
         self.betas, self.eps, self.step_count = betas, eps, 0
         # trainer.py:243-251 defaults (config.py: position_lr_init 1.6e-4 ... ); callers pass their own
         self.lrs = dict(lrs or {"xyz": 1.6e-4, "f_dc": 2.5e-3, "f_rest": 2.5e-3 / 20.0, "opacity": 5e-2, "scaling": 5e-3, "rotation": 1e-3})
-        self._install([xyz, features_dc.reshape(len(xyz), -1), features_rest.reshape(len(xyz), -1), opacity, scaling, rotation], dev)
+        self.groups = GROUPS if regist_feat is None else GROUPS + (REGIST_FEAT,)
+        if regist_feat is not None:
+            self.lrs.setdefault("regist_feat", 2.5e-3)
+        tensors = [xyz, features_dc.reshape(len(xyz), -1), features_rest.reshape(len(xyz), -1), opacity, scaling, rotation]
+        self._install(tensors + ([] if regist_feat is None else [regist_feat]), dev)
         self.exp_avg = torch.zeros_like(self.flat)
         self.exp_avg_sq = torch.zeros_like(self.flat)
         self._reset_stats()
@@ -53,7 +66,7 @@ class FlatSurfelModel(torch.nn.Module):
     # ---- layout -------------------------------------------------------------------------------------------------
     def _offsets(self, P):
         off, o = [], 0
-        for _, k in GROUPS:
+        for _, k in self.groups:
             off.append(o); o += P * k
         return off, o
 
@@ -65,7 +78,7 @@ class FlatSurfelModel(torch.nn.Module):
             pass
         self.P = P
         self.flat = torch.empty((total,), dtype=torch.float32, device=dev)
-        for (name, k), o, t in zip(GROUPS, off, tensors):
+        for (name, k), o, t in zip(self.groups, off, tensors):
             self.flat[o:o + P * k].view(P, k).copy_(t.reshape(P, k))
         self._bind()
 
@@ -74,12 +87,12 @@ class FlatSurfelModel(torch.nn.Module):
         P = self.P
         off, total = self._offsets(P)
         self.grad_flat = torch.zeros((total,), dtype=torch.float32, device=self.flat.device)
-        shapes = {"xyz": (P, 3), "f_dc": (P, 1, 3), "f_rest": (P, 15, 3), "opacity": (P, 1), "scaling": (P, 2), "rotation": (P, 4)}
-        for (name, k), o in zip(GROUPS, off):
+        shapes = {"xyz": (P, 3), "f_dc": (P, 1, 3), "f_rest": (P, 15, 3), "opacity": (P, 1), "scaling": (P, 2), "rotation": (P, 4),
+                  "regist_feat": (P, 16)}
+        for (name, k), o in zip(self.groups, off):
             p = torch.nn.Parameter(self.flat[o:o + P * k].view(shapes[name]))
             p.grad = self.grad_flat[o:o + P * k].view(shapes[name])
-            setattr(self, {"xyz": "_xyz", "f_dc": "_features_dc", "f_rest": "_features_rest", "opacity": "_opacity",
-                           "scaling": "_scaling", "rotation": "_rotation"}[name], p)
+            setattr(self, _ATTR[name], p)
 
     def _reset_stats(self):
         dev = self.flat.device
@@ -95,7 +108,7 @@ class FlatSurfelModel(torch.nn.Module):
     get_features = property(lambda s: torch.cat((s._features_dc, s._features_rest), dim=1))
 
     def flat_params(self):
-        return [self._xyz, self._features_dc, self._features_rest, self._opacity, self._scaling, self._rotation]
+        return [getattr(self, _ATTR[name]) for name, _ in self.groups]
 
     def zero_grad_flat(self):
         self.grad_flat.zero_()
@@ -104,11 +117,11 @@ class FlatSurfelModel(torch.nn.Module):
     def adam_step(self, grad_scale: float = 1.0):
         lib = _capi.load()
         off, total = self._offsets(self.P)
-        begin = (C.c_int64 * (len(GROUPS) + 1))(*off, total)
-        lr = (C.c_float * len(GROUPS))(*[self.lrs[n] for n, _ in GROUPS])
+        begin = (C.c_int64 * (len(self.groups) + 1))(*off, total)
+        lr = (C.c_float * len(self.groups))(*[self.lrs[n] for n, _ in self.groups])
         self.step_count += 1
         with torch.cuda.device(self.flat.device):
-            rc = lib.sr_adam_flat(len(GROUPS), begin, lr, self.betas[0], self.betas[1], self.eps, self.step_count, float(grad_scale),
+            rc = lib.sr_adam_flat(len(self.groups), begin, lr, self.betas[0], self.betas[1], self.eps, self.step_count, float(grad_scale),
                                   self.flat.data_ptr(), self.grad_flat.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(),
                                   torch.cuda.current_stream(self.flat.device).cuda_stream)
         _capi.check(rc, "sr_adam_flat")
@@ -135,8 +148,8 @@ class FlatSurfelModel(torch.nn.Module):
         new_off, new_total = self._offsets(P_new)
         p_new = torch.empty((new_total,), dtype=torch.float32, device=dev)
         m_new, v_new = torch.empty_like(p_new), torch.empty_like(p_new)
-        n = len(GROUPS)
-        width = (C.c_int32 * n)(*[k for _, k in GROUPS])
+        n = len(self.groups)
+        width = (C.c_int32 * n)(*[k for _, k in self.groups])
         ob, nb = (C.c_int64 * n)(*old_off), (C.c_int64 * n)(*new_off)
         src = src.to(torch.int32).contiguous(); kind = kind.to(torch.uint8).contiguous()
         ptr = lambda t: None if t is None else t.contiguous().data_ptr()  # noqa: E731
