@@ -13,9 +13,11 @@
 //     32-instance stage, lock-step at stage granularity evaluates 12.5 pairs per 32-lane iteration on the headline
 //     frame (Poisson noise: the warp waits for its busiest lane every stage); at 256 instances it is 18
 //     (replay of the recorded masks).
-//   * No CTA-wide barrier after start-up.  A ring slot is released by an shared-memory counter; the warp whose
+//   * Forward: no CTA-wide barrier after start-up.  A ring slot is released by an shared-memory counter; the warp whose
 //     release is the eighth issues the next bulk copy into it, so there is no producer warp to wait on.  A warp may
 //     run NSLOT-1 chunks ahead of the slowest warp of its tile.
+//   * Backward: two phases per chunk between CTA barriers (pixel walk -> shared pair buffer -> per-instance sums), so
+//     that gradients reach L2 once per (instance, tile); see composite_tile_bwd_kernel.
 //   * Forward early termination is per lane (T < 1e-4), per warp (all 32 pixels done: the warp only waits for and
 //     releases the remaining chunks) and per CTA (all 8 warps done: no further chunk is requested).
 #include "composite_common.cuh"
@@ -244,8 +246,38 @@ composite_tile_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ range
 }
 
 // ------------------------------------------------------------------------------------------------ backward
-template <int CH, int NSLOT, int MINB>
-__global__ void __launch_bounds__(32 * TWARPS, MINB)
+// Every chunk is processed in two phases separated by CTA barriers, so that each (instance, tile) sends its gradient
+// to L2 as ONE set of vector reductions instead of one set per contributing pixel (12 pairs per (instance, tile) on
+// average on the headline frame; the per-pair reductions were what bounded this kernel):
+//   1. pixel phase (lane = pixel): the reverse walk over the recorded contribution masks, reduced to three scalars per
+//      pair (BwdPixel::pair_scalars) that go to a shared pair buffer.  A pair's slot is its pixel's base -- a CTA-wide
+//      exclusive scan of the per-pixel pair counts of the chunk -- plus its rank in the pixel's back-to-front list.
+//   2. instance phase (thread = instance of the chunk; warp w = stage w): the instance's pixel set is the transpose of
+//      its stage's 32 x 32 (pixel x instance) masks.  For each of its pixels the thread recomputes the pair geometry
+//      (pair_alpha: the same arithmetic on the same inputs, so the same alpha and the same low-pass branch), runs
+//      pair_geom_vjp and sums the 16 + 2 components in registers; one red.v4 x 4 (+ one v2) per instance leaves.
+// A pair whose slot lies beyond the buffer (a dense chunk) takes the direct path in phase 1 -- full VJP and per-pair
+// reductions -- and phase 2 skips it: the capacity changes the order of the float sums, never what is summed.
+constexpr int BWD_CH = 256;        // instances per chunk == threads per CTA (one instance per thread in phase 2)
+constexpr int BWD_NSLOT = 2;
+constexpr int BWD_CAP = 4608;      // pair-buffer slots, 12 B each; headline chunks: 2,200 pairs average, 5,500 p99
+struct BwdSmem {
+    static constexpr int NSTG = BWD_CH / 32;
+    // offsets of the regions that follow the ring
+    static constexpr size_t masks = (size_t)BWD_NSLOT * BWD_CH * REC4 * sizeof(float4);      // masks [warp][stage][lane]
+    static constexpr size_t pd4 = masks + (size_t)TWARPS * NSTG * 32 * sizeof(uint32_t);      // per pixel: dpix0..2, dn0
+    static constexpr size_t pd2 = pd4 + 32 * TWARPS * sizeof(float4);                           // per pixel: dn1, dn2
+    static constexpr size_t buf = pd2 + 32 * TWARPS * sizeof(float2);                           // pair buffer, 3 x BWD_CAP
+    static constexpr size_t sfx = buf + 3 * (size_t)BWD_CAP * sizeof(float);                   // slot table [stage][pixel]
+    static constexpr size_t full = sfx + (size_t)NSTG * 32 * TWARPS * sizeof(uint16_t);        // mbarriers
+    static constexpr size_t wsum = full + BWD_NSLOT * sizeof(uint64_t);                         // pair count per warp
+    static constexpr size_t total = wsum + TWARPS * sizeof(uint32_t);
+};
+static_assert(BWD_CH == 32 * TWARPS, "phase 2 gives every instance of a chunk its own thread");
+static_assert(BwdSmem::full % 8 == 0, "mbarrier alignment");
+static_assert(2 * (BwdSmem::total + 1024) <= 233472, "two CTAs per SM (228 KB, 1 KB reserved per CTA)");
+
+__global__ void __launch_bounds__(32 * TWARPS, 2)
 composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_scale, const uint2* __restrict__ ranges,
                           const uint32_t* __restrict__ tile_order, int tiles_x,
                           const float4* __restrict__ irec, int W, int H, const float* __restrict__ bg,
@@ -253,13 +285,19 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                           const uint32_t* __restrict__ sub_last, const float* __restrict__ dL_dpixels,
                           const float* __restrict__ dL_dothers, const uint32_t* __restrict__ contrib_masks,
                           float* __restrict__ sgrad) {
-    using SM = TileSmem<CH, NSLOT>;
-    constexpr int NSTG = SM::NSTG;
+    using SM = BwdSmem;
+    constexpr int CH = BWD_CH, NSLOT = BWD_NSLOT, NSTG = SM::NSTG, NPIX = 32 * TWARPS;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float4* ring = reinterpret_cast<float4*>(smem_raw);
-    uint32_t* cm_all = reinterpret_cast<uint32_t*>(smem_raw + SM::ring);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + SM::ring + SM::masks);
-    uint32_t* rel = reinterpret_cast<uint32_t*>(full + NSLOT);
+    uint32_t* cm_all = reinterpret_cast<uint32_t*>(smem_raw + SM::masks);
+    float4* pd4 = reinterpret_cast<float4*>(smem_raw + SM::pd4);
+    float2* pd2 = reinterpret_cast<float2*>(smem_raw + SM::pd2);
+    float* buf_a = reinterpret_cast<float*>(smem_raw + SM::buf);     // dL/dalpha (times T, with the background term)
+    float* buf_z = buf_a + BWD_CAP;                                   // dL/dz
+    float* buf_t = buf_z + BWD_CAP;                                   // alpha T
+    uint16_t* sfx = reinterpret_cast<uint16_t*>(smem_raw + SM::sfx);  // first slot of (stage, pixel)'s pairs
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + SM::full);
+    uint32_t* wsum = reinterpret_cast<uint32_t*>(smem_raw + SM::wsum);
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int f = (int)(blockIdx.x % (unsigned)fs.frames);
@@ -279,7 +317,7 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
     const int len = min(rlen, (int)cta_last);
     const int len_w = min(rlen, (int)__shfl_sync(0xffffffffu, my_last, warp));
     const int nchunks = (len + CH - 1) / CH;
-    if (nchunks == 0) return;
+    if (nchunks == 0) return;                      // CTA-uniform
     const int nb_w = (len_w + 31) >> 5;            // stages this sub-tile reads
 
     const int sx0 = (warp & 1) * 8, sy0 = (warp >> 1) * 4;
@@ -288,21 +326,22 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
     auto issue = [&](int k) {   // one thread
         const int c = nchunks - 1 - k, s = k % NSLOT;
         const uint32_t bytes = (uint32_t)min(CH, len - c * CH) * 80u;
-        fence_proxy_async();
+        fence_proxy_async();                       // the slot's previous readers (generic proxy) passed a CTA barrier
         mbar_expect_tx(&full[s], bytes);
         bulk_g2s(ring + (size_t)s * CH * REC4, src + (size_t)c * CH * REC4, bytes, &full[s]);
     };
     if (threadIdx.x == 0) {
 #pragma unroll
-        for (int s = 0; s < NSLOT; s++) { mbar_init(&full[s], 1); rel[s] = 0u; }
+        for (int s = 0; s < NSLOT; s++) mbar_init(&full[s], 1);
         fence_mbar_init();
         for (int k = 0; k < NSLOT && k < nchunks; k++) issue(k);
     }
-    __syncthreads();                               // the only CTA-wide barrier
 
     BwdPixel px;
     px.load(tile_x * SR_TILE + sx0 + (lane & 7), tile_y * SR_TILE + sy0 + (lane >> 3), W, H, bg, final_Ts, n_contrib,
             dL_dpixels, dL_dothers, grad_scale);
+    pd4[threadIdx.x] = make_float4(px.dpix0, px.dpix1, px.dpix2, px.dn0);      // thread == pixel == warp * 32 + lane
+    pd2[threadIdx.x] = make_float2(px.dn1, px.dn2);
 
     uint32_t* cm = cm_all + warp * NSTG * 32 + lane;
     const uint32_t* cm_in = contrib_masks + (((size_t)(range.x >> 5) + tile) * 8 + warp) * 32 + lane;
@@ -319,17 +358,38 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
     for (int k = 0; k < nchunks; k++) {
         const int c = nchunks - 1 - k, s = k % NSLOT;
         uint32_t nz = 0u;
+        int np = 0;
 #pragma unroll
-        for (int st = 0; st < NSTG; st++) { cm[st * 32] = pre[st]; if (pre[st]) nz |= 1u << st; }
+        for (int st = 0; st < NSTG; st++) { cm[st * 32] = pre[st]; if (pre[st]) nz |= 1u << st; np += __popc(pre[st]); }
+        // slot base of this pixel = exclusive scan of the pair counts over the CTA's pixels
+        int incl = np;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += y;
+        }
+        if (lane == 31) wsum[warp] = (uint32_t)incl;
+        __syncthreads();                           // masks and warp totals are in; the previous chunk is finished
+        int base = incl - np;
+        for (int w = 0; w < warp; w++) base += (int)wsum[w];
+        {
+            int run = base;                        // pairs of this pixel in later stages come first (back to front)
+#pragma unroll
+            for (int st = NSTG - 1; st >= 0; st--) {
+                sfx[st * NPIX + threadIdx.x] = (uint16_t)min(run, 0xffff);
+                run += __popc(pre[st]);
+            }
+        }
         if (c > 0) fetch(c - 1);
-        const bool any = __any_sync(0xffffffffu, nz != 0u);
         {
             const uint32_t parity = (uint32_t)((k / NSLOT) & 1);
             while (!mbar_try_wait(&full[s], parity)) { }
         }
-        if (any) {
-            const float4* S = ring + (size_t)s * CH * REC4;
-            int st = 0;
+        const float4* S = ring + (size_t)s * CH * REC4;
+
+        // ---- phase 1: lane = pixel, back to front over its contributors
+        if (__any_sync(0xffffffffu, nz != 0u)) {
+            int st = 0, slot = base;
             uint32_t mym = 0u;
             for (;;) {
                 if (mym == 0u && nz) { st = 31 - __clz(nz); nz &= ~(1u << st); mym = cm[st * 32]; }
@@ -339,24 +399,95 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                 const int jj = 31 - __clz(mym);
                 mym &= ~(1u << jj);
                 const int idx = st * 32 + jj;
-                float v[16];
+                PairAlpha q;
+                float dL_dalpha, dL_dz, aT;
+                px.pair_scalars(S + idx * REC4, c * CH + idx, q, dL_dalpha, dL_dz, aT);
+                if (slot < BWD_CAP) {
+                    buf_a[slot] = dL_dalpha; buf_z[slot] = dL_dz; buf_t[slot] = aT;
+                } else {
+                    float v[16];
 #pragma unroll
-                for (int i = 0; i < 16; i++) v[i] = 0.f;
-                float m2x = 0.f, m2y = 0.f;
-                bool lowpass = false;
-                px.pair(S + idx * REC4, c * CH + idx, v, m2x, m2y, lowpass);
-                red_pixel(sgrad, S + idx * REC4, v, m2x, m2y, lowpass);
+                    for (int i = 0; i < 10; i++) v[i] = 0.f;
+                    float m2x = 0.f, m2y = 0.f;
+                    bool lowpass = false;
+                    px.pair_vjp(S + idx * REC4, q, dL_dalpha, dL_dz, aT, v, m2x, m2y, lowpass);
+                    red_pixel(sgrad, S + idx * REC4, v, m2x, m2y, lowpass);
+                }
+                slot++;
             }
         }
-        __syncwarp();
-        if (lane == 0) {
-            __threadfence_block();
-            if (atomicAdd(&rel[s], 1u) == TWARPS - 1) {
-                rel[s] = 0u;
-                __threadfence_block();
-                if (k + NSLOT < nchunks) issue(k + NSLOT);
+        __syncthreads();                           // pair buffer and slot table complete
+
+        // ---- phase 2: thread = instance warp * 32 + lane of the chunk
+        {
+            uint32_t pw[TWARPS];                   // pw[sw] bit l: pixel l of sub-tile sw has this instance as a contributor
+            uint32_t anyw = 0u;
+#pragma unroll
+            for (int sw = 0; sw < TWARPS; sw++) {
+                pw[sw] = transpose32(cm_all[(sw * NSTG + warp) * 32 + lane], lane);
+                anyw |= pw[sw];
+            }
+            if (anyw) {
+                const float4* R = S + threadIdx.x * REC4;
+                const float4 r0 = R[0], r1 = R[1], r2 = R[2];
+                float acc[16];
+#pragma unroll
+                for (int i = 0; i < 16; i++) acc[i] = 0.f;
+                float a2x = 0.f, a2y = 0.f;
+                bool lowpass_any = false, any_in = false;
+                // one flat walk over the instance's pixels: the warp iterates max over lanes of the pair count
+                uint32_t nzw = 0u;
+#pragma unroll
+                for (int sw = 0; sw < TWARPS; sw++) if (pw[sw]) nzw |= 1u << sw;
+                int sw = 0;
+                uint32_t w = 0u;
+                for (;;) {
+                    if (w == 0u) {
+                        if (nzw == 0u) break;
+                        sw = __ffs(nzw) - 1;
+                        nzw &= nzw - 1u;
+#pragma unroll
+                        for (int q = 0; q < TWARPS; q++) if (q == sw) w = pw[q];
+                    }
+                    const int l = __ffs(w) - 1;
+                    w &= w - 1u;
+                    const int p = sw * 32 + l;
+                    const uint32_t pm = cm_all[(sw * NSTG + warp) * 32 + l];
+                    const int slot = (int)sfx[warp * NPIX + p] + __popc((pm >> lane) >> 1);
+                    if (slot >= BWD_CAP) continue;          // went out directly in phase 1
+                    const int px_ = tile_x * SR_TILE + (sw & 1) * 8 + (l & 7), py_ = tile_y * SR_TILE + (sw >> 1) * 4 + (l >> 3);
+                    const float pixx = (float)px_ + 0.5f, pixy = (float)py_ + 0.5f;
+                    PairAlpha q;
+                    pair_alpha(r0, r1, r2, pixx, pixy, q);
+                    float v[16];
+#pragma unroll
+                    for (int i = 0; i < 10; i++) v[i] = 0.f;
+                    float m2x = 0.f, m2y = 0.f;
+                    bool lowpass = false;
+                    pair_geom_vjp(q, r1, r2.w, pixx, pixy, buf_a[slot], buf_z[slot], v, m2x, m2y, lowpass);
+                    const float aT = buf_t[slot];
+                    const float4 d4 = pd4[p];
+                    const float2 d2 = pd2[p];
+                    v[10] = aT * d4.x; v[11] = aT * d4.y; v[12] = aT * d4.z;
+                    v[13] = aT * d4.w; v[14] = aT * d2.x; v[15] = aT * d2.y;
+#pragma unroll
+                    for (int i = 0; i < 16; i++) acc[i] += v[i];
+                    a2x += m2x; a2y += m2y;
+                    lowpass_any |= lowpass;
+                    any_in = true;
+                }
+                if (any_in) {
+                    float* gp = sgrad + (size_t)__float_as_uint(R[4].z) * SR_GRAD_FLOATS;
+                    red_add<16>(gp, acc);
+                    if (lowpass_any) {
+                        const float w2[16] = {a2x, a2y};
+                        red_add<2>(gp + SR_G_M2D, w2);
+                    }
+                }
             }
         }
+        __syncthreads();                           // ring slot, masks, pair buffer and slot table are free again
+        if (threadIdx.x == 0 && k + NSLOT < nchunks) issue(k + NSLOT);
     }
 }
 
@@ -378,8 +509,8 @@ cudaError_t opt_in_smem(K kern, size_t bytes) {
 
 // Which composite kernels run: SURFEL_COMPOSITE=tile|warp sets both directions, SURFEL_COMPOSITE_FWD / _BWD one of them.
 // Defaults (measured on the headline batch): forward = one-warp CTAs with private rings (fewer
-// instructions per iteration; the forward is issue bound), backward = tile CTAs with the shared chunk ring (25 % fewer
-// instructions thanks to the per-lane free walk; the backward is bound by L2 reductions and latency).
+// instructions per iteration; the forward is issue bound), backward = tile CTAs with the shared chunk ring (the per-lane
+// free walk, and one set of gradient reductions per (instance, tile) instead of one per contributing pixel).
 bool sr_composite_tile_mode(bool backward) {
     static const int mode = [] {
         auto pick = [](const char* name, int dflt) {
@@ -431,26 +562,14 @@ cudaError_t launch_composite_tile_bwd(const BwdArgs& a) {
                                      a.fs.frames, a.stream);
     if (e != cudaSuccess) return e;
     ProfileScope ps("composite_bwd", a.stream);
-    cudaError_t err = cudaSuccess;
-    auto launch = [&](auto kern, size_t smem) {
-        err = opt_in_smem(kern, smem);
-        if (err != cudaSuccess) return;
-        kern<<<a.il.tiles * a.fs.frames, 32 * TWARPS, smem, a.stream>>>(
-            a.fs, a.grad_scale, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles_x,
-            (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, a.cam.bg,
-            (const float*)(a.img + a.il.final_T), (const uint32_t*)(a.img + a.il.n_contrib),
-            (const uint32_t*)(a.img + a.il.tile_last), a.dL_dcolor, a.dL_dothers,
-            (const uint32_t*)(a.bin + a.bl.contrib), (float*)(a.geom + a.gl.sgrad));
-    };
-    switch (comp::tile_cfg_from_env()) {
-        case 2563: launch(composite_tile_bwd_kernel<256, 3, 3>, TileSmem<256, 3>::total); break;
-        case 1282: launch(composite_tile_bwd_kernel<128, 2, 3>, TileSmem<128, 2>::total); break;
-        case 1283: launch(composite_tile_bwd_kernel<128, 3, 3>, TileSmem<128, 3>::total); break;
-        case 1284: launch(composite_tile_bwd_kernel<128, 4, 3>, TileSmem<128, 4>::total); break;
-        case 5122: launch(composite_tile_bwd_kernel<512, 2, 2>, TileSmem<512, 2>::total); break;
-        default: launch(composite_tile_bwd_kernel<256, 2, 3>, TileSmem<256, 2>::total); break;
-    }
-    if (err != cudaSuccess) return err;
+    e = opt_in_smem(composite_tile_bwd_kernel, BwdSmem::total);
+    if (e != cudaSuccess) return e;
+    composite_tile_bwd_kernel<<<a.il.tiles * a.fs.frames, 32 * TWARPS, BwdSmem::total, a.stream>>>(
+        a.fs, a.grad_scale, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles_x,
+        (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, a.cam.bg,
+        (const float*)(a.img + a.il.final_T), (const uint32_t*)(a.img + a.il.n_contrib),
+        (const uint32_t*)(a.img + a.il.tile_last), a.dL_dcolor, a.dL_dothers,
+        (const uint32_t*)(a.bin + a.bl.contrib), (float*)(a.geom + a.gl.sgrad));
     sr_count_launch();
     return cudaGetLastError();
 }
