@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SR_ABI_VERSION 5
+#define SR_ABI_VERSION 6
 
 #if defined(__GNUC__)
 #define SR_API __attribute__((visibility("default")))
@@ -308,6 +308,54 @@ SR_API int sr_bob_warp_backward(int32_t P, int32_t B, int32_t M, const float* xy
                                 const float* se3_d, const float* cam_q, const float* cam_t, const float* g_xyz_cam,
                                 const float* g_rot_cam, const float* g_entropy, float* g_xyz, float* g_rot, float* g_delta,
                                 float* g_tables, void* stream);
+
+/*
+ * Stage 3's feature-matching reprojection loss ("feat_reproj"), in two halves, because the caller's delta-skinning MLP
+ * runs on the matched points between them.  See csrc/match.cu and DESIGN.md section 3.5b.
+ *
+ * sr_global_match_*: replaces lab4d/nnutils/deformable_gaussian.py:1436-1486 (global_match with num_grad = K) without
+ * the (M*H*W, C) score matrix.  feat_px[M*H*W*16] pixel features; regist_feat[P*16], xyz[P*3] canonical surfels;
+ * cand[C] int32 candidate indices into the M-fold expanded surfels (candidate c is surfel cand[c] mod P; indices outside
+ * [0, M*P) are skipped); logsigma[1] DEVICE float (the temperature is exp(logsigma), read at run time).
+ * Per pixel: the K highest scores feat_px . regist_feat[cand[c] mod P] (fp32 FMA chain in channel order; among equal
+ * scores the lower candidate position c wins), softmax of score * exp(logsigma) over them, and
+ * xyz_matched[M*H*W*3] = sum of prob * xyz.  top_idx / top_prob / top_score[M*H*W*K] (candidate position, -1 if none)
+ * are for the backward.  The backward takes g_xyz_matched and writes g_regist_feat[P*16], g_xyz[P*3] and g_logsigma[1]
+ * (all zeroed inside; duplicate surfels among the candidates sum); g_cand[C*19] is scratch.  feat_px gets no gradient.
+ * SR_EINVAL: a NULL required pointer, M, H, W or P < 1, C outside [1, M*P], K outside [1, min(8, C)].
+ *
+ * sr_reproj_loss_*: replaces lab4d/nnutils/deformable_gaussian.py:1488-1513 (forward_project: forward_warp of the matched
+ * points with no rotation, then lab4d/utils/geom_utils.py:17-30 pinhole_projection) and the feat_reproj term of
+ * lab4d/engine/model.py:669-672 (||xy_reproj - hxy[..., :2]||), :915,961-967 (times mask and is_detected) and :994-1012
+ * (mean over the batch's positive values, / train_res, * feat_reproj_wt).  The warp tables are those of
+ * sr_bob_warp_forward (B <= 64); delta[M*H*W*B] or NULL; Kmat[M*9] row-major intrinsics; hxy[M*H*W*hxy_dim]
+ * (hxy_dim 2 or 3; the first two are read); mask[M*H*W]; is_detected[M] or NULL (= 1); weight[1] DEVICE float.
+ * Forward writes xy_reproj[M*H*W*2], terms[M] (each frame's share of the weighted term), counts[M] (pixels with v > 0),
+ * scale[1] = weight / (total count * train_res) (0 if the count is 0) and loss[1] = sum of terms.  Backward takes
+ * g_loss[1] (DEVICE float) and scale, and writes g_xyz_matched[M*H*W*3], g_delta[M*H*W*B] (if non-NULL) and
+ * g_tables[sr_bob_warp_table_floats(B, M)] in sr_bob_warp_backward's order (zeroed inside).  Kmat and hxy get no gradient.
+ * SR_EINVAL: a NULL required pointer, M, H or W < 1, B outside [1, 64], hxy_dim not 2 or 3, train_res <= 0.
+ * No call allocates or synchronises with the host.
+ */
+SR_API int sr_global_match_forward(int32_t M, int32_t H, int32_t W, int32_t P, int32_t C, int32_t K, const float* feat_px,
+                                   const float* regist_feat, const float* xyz, const int32_t* cand, const float* logsigma,
+                                   float* xyz_matched, int32_t* top_idx, float* top_prob, float* top_score, void* stream);
+SR_API int sr_global_match_backward(int32_t M, int32_t H, int32_t W, int32_t P, int32_t C, int32_t K, const float* feat_px,
+                                    const float* xyz, const int32_t* cand, const float* logsigma, const int32_t* top_idx,
+                                    const float* top_prob, const float* top_score, const float* g_xyz_matched, float* g_cand,
+                                    float* g_regist_feat, float* g_xyz, float* g_logsigma, void* stream);
+SR_API int sr_reproj_loss_forward(int32_t M, int32_t H, int32_t W, int32_t B, int32_t hxy_dim, float train_res,
+                                  const float* xyz_matched, const float* o2b_q, const float* o2b_t, const float* inv_gauss,
+                                  const float* delta, const float* se3_r, const float* se3_d, const float* cam_q,
+                                  const float* cam_t, const float* Kmat, const float* hxy, const float* mask,
+                                  const float* is_detected, const float* weight, float* xy_reproj, float* terms,
+                                  uint32_t* counts, float* scale, float* loss, void* stream);
+SR_API int sr_reproj_loss_backward(int32_t M, int32_t H, int32_t W, int32_t B, int32_t hxy_dim, const float* xyz_matched,
+                                   const float* o2b_q, const float* o2b_t, const float* inv_gauss, const float* delta,
+                                   const float* se3_r, const float* se3_d, const float* cam_q, const float* cam_t,
+                                   const float* Kmat, const float* hxy, const float* mask, const float* is_detected,
+                                   const float* scale, const float* g_loss, float* g_xyz_matched, float* g_delta,
+                                   float* g_tables, void* stream);
 
 /*
  * Optimizer-side kernels over the FLAT surfel parameter buffer (SURVEY.md section 8(f) row N4): the Adam step of every

@@ -10,8 +10,15 @@ written in torch on out["features"], alternating in one process, at 256x256 x 2 
 512x512 x 8 frames (headline).  The torch version uses the sync-free form of the reference's positive mean
 (sum(v * (v > 0)) / max(count, 1), equal to it for v >= 0), so that it can be captured too.
 
+--reproj times Stage 3's feature-matching reprojection loss: global_match over 2048 candidates + warp + projection +
+feat_reproj loss, forward + backward, one CUDA graph, L2 flushed between steps, fused (csrc/match.cu) against the same
+statements in torch (global_match's score matrix + topk, oracle/warp_oracle.py in fp32, projection, the sync-free
+positive mean), alternating in one process, at 256x256 x 2 frames with 300 K surfels; and the fused path alone at
+512x512 x 8 frames, where the torch path's score matrix alone is 17 GB.
+
     python tools/bench_features.py --features 4 22 32 [--steps 20 --warmup 5]
     python tools/bench_features.py --losses [--steps 20 --warmup 5]
+    python tools/bench_features.py --reproj [--steps 20 --warmup 5]
 """
 import argparse
 import json
@@ -35,9 +42,12 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--losses", action="store_true")
+    ap.add_argument("--reproj", action="store_true")
     args = ap.parse_args()
     if args.losses:
         return bench_losses(args)
+    if args.reproj:
+        return bench_reproj(args)
     from vidu4d_b200 import _capi, rasterizer as RZ
     from vidu4d_b200.graph import GraphedStep
     from vidu4d_b200.synthetic import object_scene, orbit_view, projection_matrix
@@ -215,6 +225,141 @@ def bench_losses(args):
                           "fps_torch": round(M / (med["torch"] * 1e-3), 1), "launches_per_step_fused": steps["fused"].launches,
                           "kernel_ms_per_launch": kern, "steps": args.steps, "statistic": "median step time",
                           "gpu": gpu}), flush=True)
+    RZ.set_sync_mode(True)
+    RZ._pending.clear()
+
+
+def _reproj_inputs(M, RES, P, B, dev, seed=0):
+    from tests.golden.make_warp_golden import make_inputs
+    wi = {k: v.to(dev) for k, v in make_inputs(seed, P, B, M, False).items() if v is not None}
+    g = torch.Generator(device=dev).manual_seed(seed)
+    d = dict(feat_px=torch.randn((M, RES, RES, 16), device=dev, generator=g),
+             regist=torch.randn((P, 16), device=dev, generator=g).requires_grad_(True),
+             xyz=wi["xyz"].clone().requires_grad_(True), logsigma=torch.tensor([np.log(2.0)], device=dev, dtype=torch.float32))
+    d["logsigma"].requires_grad_(True)
+    for k in ("rest_q", "rest_t", "log_gauss", "art_q", "art_t", "cam_q", "cam_t"):
+        d[k] = wi[k].clone().requires_grad_(True)
+    f = torch.tensor([[1.2 * RES, 0, RES / 2], [0, 1.2 * RES, RES / 2], [0, 0, 1]], device=dev)
+    d["Kmat"] = f[None].expand(M, -1, -1).contiguous()
+    ys, xs = torch.meshgrid(torch.arange(RES, device=dev), torch.arange(RES, device=dev), indexing="ij")
+    d["hxy"] = torch.stack([xs, ys, torch.ones_like(xs)], -1)[None].expand(M, -1, -1, -1).float().contiguous()
+    d["mask"] = (torch.rand((M, RES, RES), device=dev, generator=g) > 0.5).float()
+    d["det"] = torch.ones(M, device=dev)
+    d["delta"] = (torch.randn((M, RES, RES, B), device=dev, generator=g).clamp(min=0) * 0.1).requires_grad_(True)
+    d["w"] = torch.tensor([5e-2], device=dev)
+    d["cand"] = torch.randperm(M * P, generator=torch.Generator().manual_seed(seed))[:2048].to(dev, torch.int32)
+    return d
+
+
+def _q2dq(q, t):
+    from oracle import warp_oracle as wo
+    return q, 0.5 * wo.qmul(torch.cat((torch.zeros_like(t[..., :1]), t), -1), q)
+
+
+def _reproj_fused(d):
+    from vidu4d_b200.registration import global_match, reproj_loss
+    xyz_m = global_match(d["feat_px"], d["regist"], d["xyz"], d["cand"], d["logsigma"], num_grad=8)
+    return reproj_loss(xyz_m, d["hxy"], d["Kmat"], _q2dq(d["rest_q"], d["rest_t"]), _q2dq(d["art_q"], d["art_t"]), d["log_gauss"],
+                       (d["cam_q"], d["cam_t"]), d["mask"], d["det"], weight=d["w"], train_res=256, delta=d["delta"])["loss"], xyz_m
+
+
+def _reproj_torch(d):
+    """Today's caller path: deformable_gaussian.py:1455-1486 statements, oracle/warp_oracle.py in fp32, pinhole
+    projection, model.py's masking and the sync-free positive mean."""
+    from oracle import warp_oracle as wo
+    M, H, W = d["feat_px"].shape[:3]
+    P = d["regist"].shape[0]
+    sidx = d["cand"].long() % P
+    score = d["feat_px"].reshape(-1, 16) @ d["regist"][sidx].T
+    score, idx = torch.topk(score, 8, dim=1, largest=True)
+    prob = torch.softmax(score * d["logsigma"].exp(), 1)
+    xyz_m = (prob[..., None] * d["xyz"][sidx][idx]).sum(1).reshape(M, H, W, 3)
+    rest, art = _q2dq(d["rest_q"], d["rest_t"]), _q2dq(d["art_q"], d["art_t"])
+    rest_m = (rest[0][None].expand(M, -1, -1), rest[1][None].expand(M, -1, -1))
+    se3 = wo.dq_mul(art, wo.dq_inverse(rest_m))
+    rot = torch.zeros((H * W, 4), device=xyz_m.device)
+    rot[:, 0] = 1.0
+    xys = []
+    for m in range(M):
+        xc = wo.bob_warp(xyz_m[m].reshape(-1, 3), rot, rest, torch.exp(-d["log_gauss"]), (se3[0][m:m + 1], se3[1][m:m + 1]),
+                         (d["cam_q"][m:m + 1], d["cam_t"][m:m + 1]), d["delta"][m].reshape(-1, d["delta"].shape[-1]))[0][0]
+        h = xc @ d["Kmat"][m].T
+        xys.append(h[:, :2] / (h[:, 2:] + 1e-6))
+    v = (torch.stack(xys).reshape(M, H, W, 2) - d["hxy"][..., :2]).norm(dim=-1) * d["mask"] * d["det"][:, None, None]
+    on = (v > 0).to(v.dtype)
+    return d["w"][0] * (v * on).sum() / on.sum().clamp(min=1.0) / 256.0, xyz_m
+
+
+def bench_reproj(args):
+    from vidu4d_b200 import _capi, rasterizer as RZ
+    from vidu4d_b200.graph import GraphedStep
+    assert torch.cuda.is_available(), "this measurement needs a GPU"
+    dev = torch.device("cuda:0")
+    _capi.load()
+    gpu = _gpu_name()
+    P, B = args.surfels, 25
+    flush = torch.empty((256 << 20,), dtype=torch.uint8, device=dev)
+    leaves = ("regist", "xyz", "logsigma", "rest_q", "rest_t", "log_gauss", "art_q", "art_t", "cam_q", "cam_t", "delta")
+    for RES, M, arms in ((256, 2, ("fused", "torch")), (512, 8, ("fused",))):
+        d = _reproj_inputs(M, RES, P, B, dev)
+        fns = {"fused": _reproj_fused, "torch": _reproj_torch}
+
+        def make_body(fn):
+            def body():
+                for k in leaves:
+                    d[k].grad = None
+                fn(d)[0].backward()
+            return body
+        bodies = {k: make_body(fns[k]) for k in arms}
+        peak = {}
+        for k, b in bodies.items():                                  # eager peak memory above the inputs
+            torch.cuda.synchronize()
+            base = torch.cuda.memory_allocated()
+            torch.cuda.reset_peak_memory_stats()
+            b()
+            torch.cuda.synchronize()
+            peak[k] = round((torch.cuda.max_memory_allocated() - base) / 2**20, 1)
+        compare = {}
+        if "torch" in arms:                                          # the two paths' outputs on the same inputs
+            with torch.no_grad():
+                lf, xf = _reproj_fused(d)
+                lt, xt = _reproj_torch(d)
+            compare = {"loss_rel_diff": float((lf - lt).abs() / lt.abs()),
+                       "xyz_matched_max_abs_diff_over_max": float((xf - xt).abs().max() / xt.abs().max())}
+        steps = {k: GraphedStep(b, device=dev) for k, b in bodies.items()}
+        for s_ in steps.values():
+            s_()
+            for _ in range(args.warmup):
+                s_(check=False)
+        torch.cuda.synchronize()
+        ms = {k: [] for k in steps}
+        for i in range(args.steps):
+            for k, s_ in steps.items():
+                flush.fill_(i & 255)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record(); s_.graph.replay(); b.record()
+                b.synchronize()
+                ms[k].append(a.elapsed_time(b))
+        RZ._pending.clear()
+        RZ.set_sync_mode(True)
+        bodies["fused"]()
+        torch.cuda.synchronize()
+        _capi.get_profile()
+        _capi.set_profiling(True)
+        for _ in range(5):
+            bodies["fused"]()
+        prof = _capi.get_profile()
+        _capi.set_profiling(False)
+        kern = {k: round(v["ms"] / max(v["count"], 1), 4) for k, v in prof.items()
+                if k in ("match_fwd", "match_bwd", "match_scatter", "reproj_fwd", "reproj_scale", "reproj_bwd")}
+        print(json.dumps({"workload": "feat_reproj step (match + warp + projection + loss, fwd + bwd)", "surfels": P,
+                          "resolution": RES, "frames": M, "candidates": 2048, "num_grad": 8, "bones": B,
+                          "ms_per_step": {k: round(float(np.median(v)), 4) for k, v in ms.items()},
+                          "peak_mem_mb_above_inputs": peak, "kernel_ms_per_launch": kern,
+                          "launches_per_step_fused": steps["fused"].launches, "outputs": compare, "steps": args.steps,
+                          "statistic": "median step time", "gpu": gpu}), flush=True)
+        del steps, bodies, d
+        torch.cuda.empty_cache()
     RZ.set_sync_mode(True)
     RZ._pending.clear()
 

@@ -23,119 +23,9 @@
 //   cam_q (M,4), cam_t (M,3)   field2cam of each frame
 // The backward recomputes the weights (cheaper than storing (P,B) floats) and returns gradients for every input; table
 // gradients are reduced warp -> block (shared memory) -> global (one atomic per value and block).
-#include "common.cuh"
+#include "warp_common.cuh"
 
 namespace {
-
-struct Q4 { float w, x, y, z; };
-__device__ __forceinline__ Q4 qmul(const Q4& a, const Q4& b) {
-    return {a.w * b.w - a.x * b.x - a.y * b.y - a.z * b.z, a.w * b.x + a.x * b.w + a.y * b.z - a.z * b.y,
-            a.w * b.y - a.x * b.z + a.y * b.w + a.z * b.x, a.w * b.z + a.x * b.y - a.y * b.x + a.z * b.w};
-}
-__device__ __forceinline__ Q4 qconj(const Q4& q) { return {q.w, -q.x, -q.y, -q.z}; }
-__device__ __forceinline__ Q4 pure(float x, float y, float z) { return {0.f, x, y, z}; }
-__device__ __forceinline__ Q4 qadd(const Q4& a, const Q4& b) { return {a.w + b.w, a.x + b.x, a.y + b.y, a.z + b.z}; }
-__device__ __forceinline__ Q4 qscale(const Q4& a, float s) { return {a.w * s, a.x * s, a.y * s, a.z * s}; }
-__device__ __forceinline__ float qdot(const Q4& a, const Q4& b) { return a.w * b.w + a.x * b.x + a.y * b.y + a.z * b.z; }
-// v' = q v q*  (general q, as quat_transform.py:259-276)
-__device__ __forceinline__ void qrot(const Q4& q, float vx, float vy, float vz, float& ox, float& oy, float& oz) {
-    const Q4 t = qmul(qmul(q, pure(vx, vy, vz)), qconj(q));
-    ox = t.x; oy = t.y; oz = t.z;
-}
-// vjp of v' = q v q*:  g_v = (q* g q)[1:],  g_q = -2 g (x) q (x) v
-__device__ __forceinline__ void qrot_vjp(const Q4& q, float vx, float vy, float vz, float gx, float gy, float gz, Q4& gq,
-                                         float& gvx, float& gvy, float& gvz) {
-    const Q4 g = pure(gx, gy, gz);
-    const Q4 t = qmul(qmul(qconj(q), g), q);
-    gvx = t.x; gvy = t.y; gvz = t.z;
-    gq = qscale(qmul(qmul(g, q), pure(vx, vy, vz)), -2.0f);
-}
-__device__ __forceinline__ Q4 ldq(const float* p) { return {p[0], p[1], p[2], p[3]}; }
-
-struct WarpDims { int P, B, M; };
-
-// shared-memory tables: o2b_q[B*4] o2b_t[B*3] ig[B*3] se3_r[M*B*4] se3_d[M*B*4] cam_q[M*4] cam_t[M*3]
-struct Tables {
-    const float *oq, *ot, *ig, *sr, *sd, *cq, *ct;
-    __device__ __forceinline__ static int floats(int B, int M) { return B * 10 + M * B * 8 + M * 7; }
-    __device__ __forceinline__ void bind(float* s, int B, int M) {
-        oq = s; ot = oq + B * 4; ig = ot + B * 3; sr = ig + B * 3; sd = sr + M * B * 4; cq = sd + M * B * 4; ct = cq + M * 4;
-    }
-};
-
-__device__ __forceinline__ void load_tables(float* s, const WarpDims d, const float* __restrict__ o2b_q, const float* __restrict__ o2b_t,
-                                            const float* __restrict__ inv_gauss, const float* __restrict__ se3_r,
-                                            const float* __restrict__ se3_d, const float* __restrict__ cam_q,
-                                            const float* __restrict__ cam_t) {
-    const int B = d.B, M = d.M;
-    float* p = s;
-    for (int i = threadIdx.x; i < B * 4; i += blockDim.x) p[i] = __ldg(o2b_q + i);
-    p += B * 4;
-    for (int i = threadIdx.x; i < B * 3; i += blockDim.x) p[i] = __ldg(o2b_t + i);
-    p += B * 3;
-    for (int i = threadIdx.x; i < B * 3; i += blockDim.x) p[i] = __ldg(inv_gauss + i);
-    p += B * 3;
-    for (int i = threadIdx.x; i < M * B * 4; i += blockDim.x) p[i] = __ldg(se3_r + i);
-    p += M * B * 4;
-    for (int i = threadIdx.x; i < M * B * 4; i += blockDim.x) p[i] = __ldg(se3_d + i);
-    p += M * B * 4;
-    for (int i = threadIdx.x; i < M * 4; i += blockDim.x) p[i] = __ldg(cam_q + i);
-    p += M * 4;
-    for (int i = threadIdx.x; i < M * 3; i += blockDim.x) p[i] = __ldg(cam_t + i);
-}
-
-// Skinning weights of one surfel: softmax over bones of -(|x_bone * inv_gauss|^2 + delta); also the arg-max bone and
-// log-sum-exp minus max (= the cross entropy against the arg-max one-hot, loss_utils.py:21-42).
-template <int BMAX>
-__device__ __forceinline__ void skin_weights(const Tables& T, int B, float x, float y, float z, const float* __restrict__ delta_row,
-                                             float (&w)[BMAX], int& anchor, float& entropy) {
-    float mx = -3.4e38f;
-#pragma unroll
-    for (int b = 0; b < BMAX; b++) {
-        w[b] = -3.4e38f;
-        if (b < B) {
-            float bx, by, bz;
-            qrot(ldq(T.oq + 4 * b), x, y, z, bx, by, bz);
-            bx = (bx + T.ot[3 * b]) * T.ig[3 * b]; by = (by + T.ot[3 * b + 1]) * T.ig[3 * b + 1]; bz = (bz + T.ot[3 * b + 2]) * T.ig[3 * b + 2];
-            float l = -(bx * bx + by * by + bz * bz);
-            if (delta_row) l -= __ldg(delta_row + b);
-            w[b] = l;
-            mx = fmaxf(mx, l);
-        }
-    }
-    float Z = 0.f;
-    anchor = 0;
-    bool found = false;
-#pragma unroll
-    for (int b = 0; b < BMAX; b++) {
-        if (b < B) {
-            if (!found && w[b] == mx) { anchor = b; found = true; }      // first arg-max, like torch.argmax
-            w[b] = expf(w[b] - mx);
-            Z += w[b];
-        } else w[b] = 0.f;
-    }
-    const float inv = 1.0f / Z;
-#pragma unroll
-    for (int b = 0; b < BMAX; b++) w[b] *= inv;
-    entropy = logf(Z);
-}
-
-// sign-aligned dual-quaternion blend of frame m (geom_utils.py:66-83): returns the un-normalised QR, QD
-template <int BMAX>
-__device__ __forceinline__ void blend(const Tables& T, int B, int m, const float (&w)[BMAX], int anchor, Q4& QR, Q4& QD) {
-    const float* sr = T.sr + (size_t)m * B * 4;
-    const float* sd = T.sd + (size_t)m * B * 4;
-    const Q4 qa = ldq(sr + 4 * anchor);
-    QR = {0.f, 0.f, 0.f, 0.f}; QD = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int b = 0; b < BMAX; b++) {
-        if (b < B) {
-            const Q4 r = ldq(sr + 4 * b), dq = ldq(sd + 4 * b);
-            const float s = (qdot(qa, r) > 0.f ? 1.f : -1.f) * w[b];
-            QR = qadd(QR, qscale(r, s)); QD = qadd(QD, qscale(dq, s));
-        }
-    }
-}
 
 template <int BMAX>
 __global__ void __launch_bounds__(256)
@@ -174,34 +64,6 @@ bob_warp_fwd_kernel(const WarpDims d, const float* __restrict__ xyz, const float
         const Q4 rc = qmul(qc, rt);
         reinterpret_cast<float4*>(rot_cam)[(size_t)m * d.P + p] = make_float4(rc.w, rc.x, rc.y, rc.z);
     }
-}
-
-// Recursive-halving warp reduction of 32 values: lane L ends with the sum over the warp of v[L].  31 shuffles for 32
-// sums (a plain shuffle tree needs 5 per value) and the 32 results land one per lane, so the shared-memory accumulation
-// that follows is ONE conflict-free atomic instruction instead of 32 single-lane ones.
-__device__ __forceinline__ float butterfly32(float (&v)[32], int lane) {
-#pragma unroll
-    for (int off = 16, n = 16; off >= 1; off >>= 1, n >>= 1) {
-        const bool hi = lane & off;
-#pragma unroll
-        for (int i = 0; i < 16; i++) {
-            if (i < n) {
-                const float keep = hi ? v[i + n] : v[i], send = hi ? v[i] : v[i + n];
-                v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-            }
-        }
-    }
-    return v[0];
-}
-
-// warp sum, then one shared-memory add per warp (only the 8 warps of a block contend on an address)
-__device__ __forceinline__ void acc_table(float* slot, float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0 && v != 0.f) atomicAdd(slot, v);
-}
-__device__ __forceinline__ void acc_q(float* slot, const Q4& q) {
-    acc_table(slot, q.w); acc_table(slot + 1, q.x); acc_table(slot + 2, q.y); acc_table(slot + 3, q.z);
 }
 
 template <int BMAX>
@@ -270,33 +132,7 @@ bob_warp_bwd_kernel(const WarpDims d, const float* __restrict__ xyz, const float
         const Q4 gQD = qscale(gqd, inv);
         const Q4 gQR = qscale(qadd(gq, qscale(q, -(qdot(q, gq) + qdot(qd, gqd)))), inv);
         // ---- blend
-        const float* sr = T.sr + (size_t)m * B * 4;
-        const float* sd = T.sd + (size_t)m * B * 4;
-        const Q4 qa = ldq(sr + 4 * anchor);
-        const int lane = threadIdx.x & 31;
-#pragma unroll
-        for (int c4 = 0; c4 < BMAX / 4; c4++) {
-            if (4 * c4 < B) {                                        // four bones x (4 + 4) components = 32 sums per butterfly
-                float vals[32];
-#pragma unroll
-                for (int j = 0; j < 4; j++) {
-                    const int b = 4 * c4 + j;
-                    float ws = 0.f;
-                    if (b < B) {
-                        const Q4 rb = ldq(sr + 4 * b), db = ldq(sd + 4 * b);
-                        const float s = qdot(qa, rb) > 0.f ? 1.f : -1.f;
-                        gw[b] += s * (qdot(gQR, rb) + qdot(gQD, db));
-                        ws = w[b] * s;
-                    }
-                    vals[8 * j] = gQR.w * ws; vals[8 * j + 1] = gQR.x * ws; vals[8 * j + 2] = gQR.y * ws; vals[8 * j + 3] = gQR.z * ws;
-                    vals[8 * j + 4] = gQD.w * ws; vals[8 * j + 5] = gQD.x * ws; vals[8 * j + 6] = gQD.y * ws; vals[8 * j + 7] = gQD.z * ws;
-                }
-                const float tot = butterfly32(vals, lane);
-                const int b = 4 * c4 + (lane >> 3), comp = lane & 7;
-                if (b < B && tot != 0.f)
-                    atomicAdd((comp < 4 ? g_sr : g_sd) + ((size_t)m * B + b) * 4 + (comp & 3), tot);
-            }
-        }
+        blend_vjp<BMAX>(T, B, m, w, anchor, gQR, gQD, gw, g_sr, g_sd);
     }
     // ---- softmax (+ entropy) backward, then the Gaussian logits
     float dotwg = 0.f;

@@ -89,15 +89,21 @@ class _BobWarp(torch.autograd.Function):
                                           ptr(g_xyz_cam), ptr(g_rot_cam), ptr(g_ent), ptr(g_xyz), ptr(g_rot), ptr(g_delta),
                                           ptr(g_tab), torch.cuda.current_stream(dev).cuda_stream)
         _capi.check(rc, "sr_bob_warp_backward")
-        o = 0
-        outs = []
-        for shape in ((B, 4), (B, 3), (B, 3), (M, B, 4), (M, B, 4), (M, 4), (M, 3)):
-            n = 1
-            for s_ in shape:
-                n *= s_
-            outs.append(g_tab[o:o + n].view(shape)); o += n
-        g_oq, g_ot, g_ig, g_sr, g_sd, g_cq, g_ct = outs
+        g_oq, g_ot, g_ig, g_sr, g_sd, g_cq, g_ct = split_table_grads(g_tab, B, M)
         return g_xyz, g_rot, g_oq, g_ot, g_ig, g_sr, g_sd, g_cq, g_ct, g_delta
+
+
+def split_table_grads(g_tab, B, M):
+    """Views of a flat g_tables buffer (sr_bob_warp_table_floats order): g_o2b_q, g_o2b_t, g_inv_gauss, g_se3_r, g_se3_d,
+    g_cam_q, g_cam_t."""
+    o = 0
+    outs = []
+    for shape in ((B, 4), (B, 3), (B, 3), (M, B, 4), (M, B, 4), (M, 4), (M, 3)):
+        n = 1
+        for s_ in shape:
+            n *= s_
+        outs.append(g_tab[o:o + n].view(shape)); o += n
+    return outs
 
 
 def bob_warp_tables(xyz, rot, o2b_q, o2b_t, inv_gauss, se3, field2cam, delta=None):
@@ -113,6 +119,13 @@ def bob_warp(xyz, rot, rest_articulation, t_articulation, log_gauss, field2cam, 
     object dual quaternions.  log_gauss (B,3).  field2cam ((M,4),(M,3)).  delta (P,B): optional delta skinning term
     (relu(mlp) * 0.1 of skinning.py:104-119; the MLP itself stays in PyTorch).
     Returns xyz_cam (M,P,3), rot_cam (M,P,4), skin_entropy (P,)."""
+    o2b_q, o2b_t, inv_gauss, se3_r, se3_d = warp_tables(rest_articulation, t_articulation, log_gauss)
+    return _BobWarp.apply(xyz, rot, o2b_q, o2b_t, inv_gauss, se3_r, se3_d, field2cam[0], field2cam[1], delta)
+
+
+def warp_tables(rest_articulation, t_articulation, log_gauss):
+    """The per-bone / per-frame tables of the warp kernels from the reference's arguments, with differentiable torch ops:
+    o2b_q (B,4), o2b_t (B,3), inv_gauss (B,3), se3_r (M,B,4), se3_d (M,B,4)."""
     rr, rd = rest_articulation
     # object -> bone of the rest pose: (q, t) of the inverse dual quaternion (transforms.py:20, quat_transform.py:341-349)
     ir, idq = _qconj(rr), _qconj(rd)
@@ -122,4 +135,4 @@ def bob_warp(xyz, rot, rest_articulation, t_articulation, log_gauss, field2cam, 
     tr, td = t_articulation
     se3_r = _qmul(tr, ir[None])
     se3_d = _qmul(tr, idq[None]) + _qmul(td, ir[None])
-    return _BobWarp.apply(xyz, rot, o2b_q, o2b_t, torch.exp(-log_gauss), se3_r, se3_d, field2cam[0], field2cam[1], delta)
+    return o2b_q, o2b_t, torch.exp(-log_gauss), se3_r, se3_d
