@@ -439,38 +439,3 @@ def test_prefiltered_flag_reports_culled_surfels(dev):
         R._C.rasterize_gaussians(t["bg"], t["means3D"], e, t["opacities"], t["scales"], t["rotations"], 1.0, e, t["viewmatrix"],
                                  t["projmatrix"], 0.5, 0.5, 64, 64, t["shs"], 0, t["campos"], True, False)
 
-
-_GROUP_CHILD = r'''
-import sys, numpy as np, torch
-sys.path.insert(0, sys.argv[1])
-from tests.test_gpu_parity import _run_ours
-from tests.golden.make_golden import build_case
-inp = build_case(6000, 112, 80, 77)
-r = _run_ours(inp, torch.device("cuda:0"), with_grads=True)
-np.savez(sys.argv[2], color=r["color"].cpu().numpy(), allmap=r["allmap"].cpu().numpy(),
-         n_contrib=r["n_contrib"].cpu().numpy(), **{"g_" + k: v.cpu().numpy() for k, v in r["grads"].items()})
-'''
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("fwd_g,bwd_g", [(8, 8), (16, 16), (4, 32), (32, 8)])
-def test_alternative_group_sizes_agree_with_default(fwd_g, bwd_g, dev, tmp_path):
-    """The pixel-block size of the composite kernels is a tuning switch read once per process
-    (SURFEL_FWD_GROUPS / SURFEL_BWD_GROUPS): every combination must give the forward planes bit for bit (per-pixel
-    arithmetic and instance order do not depend on it) and the same gradients up to summation order."""
-    import subprocess, sys
-    from tests.golden.make_golden import build_case
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    base = _run_ours(build_case(6000, 112, 80, 77), dev, with_grads=True)
-    out = str(tmp_path / "alt.npz")
-    env = dict(os.environ, SURFEL_FWD_GROUPS=str(fwd_g), SURFEL_BWD_GROUPS=str(bwd_g))
-    r = subprocess.run([sys.executable, "-c", _GROUP_CHILD, root, out], env=env, capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr[-2000:]
-    alt = np.load(out)
-    np.testing.assert_array_equal(alt["color"], _np(base["color"]))
-    np.testing.assert_array_equal(alt["allmap"], _np(base["allmap"]))
-    np.testing.assert_array_equal(alt["n_contrib"][0], _np(base["n_contrib"])[0])
-    for k, v in base["grads"].items():
-        a, b = alt["g_" + k], _np(v)
-        scale = max(float(np.abs(b).max()), 1e-20)
-        assert float(np.abs(a - b).max()) <= 2e-5 * scale, k

@@ -1,7 +1,7 @@
 """A/B of launch strategies on the headline frame set: F frames per step, forward+backward, device resident.
   streams : F single-frame calls alternating over S CUDA streams (round-1 harness)
   batch   : ONE batched call (sr_forward_batch / sr_backward_batch) on one stream
-Each configuration runs in a child process (SURFEL_* switches are read once per process)."""
+Each configuration runs in a child process."""
 import argparse, json, os, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CHILD = r'''
@@ -87,12 +87,8 @@ def main():
     a = ap.parse_args()
     rows = {}
     for cfg in a.configs.split(";"):
-        parts = cfg.split(",")
-        mode, S = parts[0].split(":")
-        env = dict(os.environ)
-        for kv in parts[1:]:
-            k, v = kv.split("="); env["SURFEL_" + k] = v
-        r = subprocess.run([sys.executable, "-c", CHILD, str(a.surfels), str(a.res), str(a.frames), mode, S, str(a.steps)], env=env, capture_output=True, text=True)
+        mode, S = cfg.split(":")
+        r = subprocess.run([sys.executable, "-c", CHILD, str(a.surfels), str(a.res), str(a.frames), mode, S, str(a.steps)], capture_output=True, text=True)
         line = [l for l in r.stdout.splitlines() if l.startswith("RESULT ")]
         if not line:
             print(cfg, "FAILED", r.stderr[-3000:]); continue

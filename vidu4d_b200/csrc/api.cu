@@ -247,7 +247,7 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
     CK(launch_sort(a), "sort"); DBG("sort");
     CK(launch_ranges_gather(a), "ranges_gather"); DBG("ranges_gather");
     CK(launch_tile_order(a), "tile_order"); DBG("tile_order");
-    if (sr_composite_tile_mode(false)) { CK(launch_composite_tile_fwd(a), "composite_tile_fwd"); }
+    if (sr_composite_tile_fwd()) { CK(launch_composite_tile_fwd(a), "composite_tile_fwd"); }
     else { CK(launch_composite_fwd(a), "composite_fwd"); }
     DBG("composite_fwd");
     if (ft) { CK(launch_feature_fwd(a, *ft), "feature_fwd"); DBG("feature_fwd"); }
@@ -374,9 +374,7 @@ static int backward_batch(const sr_frame* f, const sr_batch* b, const float* bac
         const size_t rows = ft->dfeat_stride == 0 ? 1 : (size_t)M;
         CK(cudaMemsetAsync(ft->dfeat, 0, rows * (size_t)Pl * ft->F * sizeof(float), stream), "memset(dL_dfeatures)");
     }
-    if (sr_composite_tile_mode(true)) { CK(launch_composite_tile_bwd(a), "composite_tile_bwd"); }
-    else { CK(launch_composite_bwd(a), "composite_bwd"); }
-    DBG("composite_bwd");
+    CK(launch_composite_tile_bwd(a), "composite_bwd"); DBG("composite_bwd");
     // after composite_bwd (which zeroes the per-surfel accumulator), before surfel_bwd (which reads it)
     if (ft) { CK(launch_feature_bwd(a, *ft), "feature_bwd"); DBG("feature_bwd"); }
     CK(launch_surfel_bwd(a), "surfel_bwd"); DBG("surfel_bwd");

@@ -206,11 +206,10 @@ cudaError_t launch_sort(const FwdArgs& a);                // sort.cu
 cudaError_t launch_ranges_gather(const FwdArgs& a);       // sort.cu
 cudaError_t launch_tile_order(const FwdArgs& a);          // sort.cu
 cudaError_t launch_composite_fwd(const FwdArgs& a);       // composite_fwd.cu
-cudaError_t launch_composite_bwd(const BwdArgs& a);       // composite_bwd.cu
 cudaError_t launch_surfel_bwd(const BwdArgs& a);          // surfel_bwd.cu
 cudaError_t launch_composite_tile_fwd(const FwdArgs& a);  // composite_tile.cu (one CTA per tile, shared chunk ring)
 cudaError_t launch_composite_tile_bwd(const BwdArgs& a);  // composite_tile.cu
-bool sr_composite_tile_mode(bool backward);               // SURFEL_COMPOSITE[_FWD|_BWD]=tile|warp
+bool sr_composite_tile_fwd();                             // SURFEL_COMPOSITE[_FWD]=tile|warp
 cudaError_t launch_feature_fwd(const FwdArgs& a, const FeatArgs& ft);   // composite_feat.cu (after the composite forward)
 cudaError_t launch_feature_bwd(const BwdArgs& a, const FeatArgs& ft);   // composite_feat.cu (after the composite backward)
 cudaError_t launch_mark_visible(int P, const float* means3D, const float* vm, uint8_t* present, cudaStream_t s);

@@ -8,10 +8,10 @@
 //
 // Design (DESIGN.md "feature channels"):
 //   * a separate pass after the composite forward / backward; the pinned composite kernels are untouched.  It reads
-//     only what both composite designs leave behind: the instance records, the per-(stage, pixel) contribution masks,
+//     what either composite forward leaves behind: the instance records, the per-(stage, pixel) contribution masks,
 //     final_T and each 8x4 sub-tile's deepest contributor (sub_last);
 //   * work item = (tile, 8x4 sub-tile) = one warp = one CTA, lane = pixel; the tile's records stream through a private
-//     2-stage ring of 32 records with cp.async.bulk on mbarriers, as in composite_fwd.cu / composite_bwd.cu.  Every lane
+//     2-stage ring of 32 records with cp.async.bulk on mbarriers, as in composite_fwd.cu.  Every lane
 //     walks only its own recorded contributors -- no cull or alpha test is repeated -- and re-evaluates alpha with the
 //     forward's arithmetic (comp::pair_alpha), so each plane is bit-identical to a colour plane of the same values;
 //   * a CTA owns SR_FEAT_CHUNK = 8 channels (gridDim.y = ceil(F/8)): 8 accumulators (forward) or 8 accumulators + 8
@@ -222,7 +222,7 @@ feature_bwd_kernel(const FrameStrides fs, const FeatArgs ft, const uint2* __rest
             PairAlpha q;
             pair_alpha(R[0], r1, r2, pixx, pixy, q);
             const float alpha = q.alpha;
-            const float r1ma = rcp_approx(1.f - alpha);   // as comp::BwdPixel::pair
+            const float r1ma = rcp_approx(1.f - alpha);   // as comp::BwdPixel::pair_scalars
             T = T * r1ma;
             const float aT = alpha * T;
             const uint32_t id = __float_as_uint(R[4].z);

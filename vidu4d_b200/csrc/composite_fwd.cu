@@ -6,11 +6,10 @@
 //   * work item = (tile, 8x4 sub-tile) = one warp = one CTA, launched longest-tile-first; each warp streams the
 //     tile's sorted instance records (80 B each, contiguous) through its own double-buffered shared-memory ring
 //     with cp.async.bulk (TMA 1-D) on its own mbarriers -- no CTA-wide synchronisation;
-//   * the warp is split into G groups of 32/G lanes, each owning a small pixel block of the sub-tile (default G=32:
-//     one pixel per lane).  Per 32-record stage, lane = instance tests the instance's conservative cull rectangle
-//     against the block columns and rows (8 + 4 ballots for G=32); then each group walks its own survivor list, so up
-//     to G different instances are evaluated per warp iteration.  With ~5x5-pixel footprints a whole-warp 8x4 block
-//     wastes most lanes; a finer block never needs more iterations than a coarser one;
+//   * one pixel per lane.  Per 32-record stage, lane = instance turns the instance's conservative cull rectangle into
+//     column and row masks of the sub-tile (group_survivors); then each lane walks its own survivor list, so up to 32
+//     different instances are evaluated per warp iteration.  With ~5x5-pixel footprints a whole-warp 8x4 block
+//     wastes most lanes;
 //   * per stage and pixel the kernel records which instances contributed (one 128-B store per warp): the backward
 //     walks exactly those;
 //   * culling and the rho_cut early-out never change a result: a skipped pair provably has alpha < 1/255;
@@ -21,14 +20,14 @@
 namespace {
 using namespace comp;
 
-template <int G, int ABL = 0>
+constexpr int WPC = 1;      // independent warps per CTA (2 measured slower: register pressure)
+
 __global__ void __launch_bounds__(32 * WPC)
 composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, const uint32_t* __restrict__ tile_order, int n_items, int tiles_x,
                      const float4* __restrict__ irec, int W, int H,
                      const float* __restrict__ bg, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
                      float* __restrict__ out_color, float* __restrict__ out_others, uint32_t* __restrict__ sub_last,
                      uint32_t* __restrict__ contrib_masks) {
-    using GS = GroupShape<G>;
     // WPC independent warps per CTA (the SM holds at most 32 CTAs): work item = (tile, 8x4 sub-tile), tiles in
     // longest-list-first order; the warps of a CTA share nothing
     __shared__ __align__(128) float4 st_all[WPC][NST][WB * REC4];
@@ -51,11 +50,10 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
     const int len = (int)(range.y - range.x);
     const int nb = (len + WB - 1) / WB;
 
-    // warp -> 8x4 sub-tile, group -> block, lane -> pixel
+    // warp -> 8x4 sub-tile, lane -> pixel (slot lane = ly * 8 + lx of the contribution-mask layout)
     const int sx0 = (warp & 1) * 8, sy0 = (warp >> 1) * 4;
-    const int g = lane / GS::GL, l = lane % GS::GL;
-    const int bx0 = sx0 + GS::block_x(g), by0 = sy0 + GS::block_y(g);      // tile-local block origin
-    const int pix_x = tile_x * SR_TILE + bx0 + l % GS::BW, pix_y = tile_y * SR_TILE + by0 + l / GS::BW;
+    const int bx0 = sx0 + lane % 8, by0 = sy0 + lane / 8;      // tile-local pixel
+    const int pix_x = tile_x * SR_TILE + bx0, pix_y = tile_y * SR_TILE + by0;
     const bool inside = pix_x < W && pix_y < H;
     const float pixx = (float)pix_x + 0.5f, pixy = (float)pix_y + 0.5f;
 
@@ -81,8 +79,7 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
     // instances of the current stage that contributed to this lane's pixel, kept for the backward (common.cuh
     // bin_layout: contrib); slot = pixel index inside the 8x4 sub-tile, so a warp's 32 words are one 128-B store
     uint32_t cmask = 0u;
-    uint32_t* cm_out = contrib_masks + (((size_t)(range.x >> 5) + tile) * 8 + warp) * 32
-                       + ((by0 - sy0 + l / GS::BW) * 8 + (bx0 - sx0 + l % GS::BW));
+    uint32_t* cm_out = contrib_masks + (((size_t)(range.x >> 5) + tile) * 8 + warp) * 32 + ((by0 - sy0) * 8 + (bx0 - sx0));
 
     for (int b = 0; b < nb; b++) {
         const int s = b % NST;
@@ -91,12 +88,11 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
         const float4* S = st[s];
         uint32_t cull = 0;
         if (lane < cnt) cull = __float_as_uint(S[lane * REC4 + 4].w);
-        // lane = instance: which groups' blocks does this instance's cull rectangle touch?  (G ballots)
-        uint32_t mym = group_survivors<G>(cull, sx0, sy0, g);
-        {   // a group whose pixels are all finished must not keep the warp iterating over its survivors
+        // lane = instance: which pixels does this instance's cull rectangle touch?
+        uint32_t mym = group_survivors(cull, sx0, sy0, lane);
+        {   // a finished pixel must not keep the warp iterating over its survivors
             const uint32_t db = __ballot_sync(0xffffffffu, done);
-            const uint32_t gm = (GS::GL == 32 ? 0xffffffffu : ((1u << GS::GL) - 1u)) << (g * GS::GL);
-            if ((db & gm) == gm) mym = 0u;
+            if ((db >> lane) & 1u) mym = 0u;
         }
         while (__any_sync(0xffffffffu, mym != 0u)) {
             const bool act = mym != 0u;
@@ -104,8 +100,7 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
             mym &= mym - 1;                              // no-op when mym == 0
             const float rho_cut = cull_rho_cut(__shfl_sync(0xffffffffu, cull, jj));   // before any divergence
             if (!act || done) continue;
-            const int jr = (ABL == 2) ? (jj & 1) : jj;     // ABL (diagnostic): 2 = conflict-free broadcast record loads
-            const float4 r0 = S[jr * REC4], r1 = S[jr * REC4 + 1], r2 = S[jr * REC4 + 2];
+            const float4 r0 = S[jj * REC4], r1 = S[jj * REC4 + 1], r2 = S[jj * REC4 + 2];
             // T rows: Tu=(r0.x,r0.y,r0.z) Tv=(r0.w,r1.x,r1.y) Tw=(r1.z,r1.w,r2.x); xy=(r2.y,r2.z); opac=r2.w
             const float kx = ff(pixx, r1.z, -r0.x), ky = ff(pixx, r1.w, -r0.y), kz = ff(pixx, r2.x, -r0.z);
             const float lx_ = ff(pixy, r1.z, -r0.w), ly_ = ff(pixy, r1.w, -r1.x), lz_ = ff(pixy, r2.x, -r1.y);
@@ -151,7 +146,7 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
             cmask |= 1u << jj;
         }
         __syncwarp();                                   // every lane is done reading stage s
-        if (ABL != 1 || cmask == 0x12345u) cm_out[(size_t)b * SR_CONTRIB_STAGE_WORDS] = cmask;   // ABL 1: no mask store
+        cm_out[(size_t)b * SR_CONTRIB_STAGE_WORDS] = cmask;
         cmask = 0u;
         if (__all_sync(0xffffffffu, done)) {
             // drain the copies still in flight before this warp (and its CTA's smem) goes away
@@ -192,28 +187,11 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
 
 cudaError_t launch_composite_fwd(const FwdArgs& a) {
     ProfileScope ps("composite_fwd", a.stream);
-    const int G = comp::groups_from_env();
-    auto launch = [&](auto kern) {
-        kern<<<((a.il.tiles * 8 + comp::WPC - 1) / comp::WPC) * a.fs.frames, 32 * comp::WPC, 0, a.stream>>>(
-            a.fs, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles * 8, a.il.tiles_x,
-            (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, a.cam.bg,
-            (float*)(a.img + a.il.final_T), (uint32_t*)(a.img + a.il.n_contrib), a.out_color, a.out_others,
-            (uint32_t*)(a.img + a.il.tile_last), (uint32_t*)(a.bin + a.bl.contrib));
-    };
-    switch (G) {
-        case 1: launch(composite_fwd_kernel<1>); break;
-        case 2: launch(composite_fwd_kernel<2>); break;
-        case 4: launch(composite_fwd_kernel<4>); break;
-        case 16: launch(composite_fwd_kernel<16>); break;
-        case 32: {
-            static const int abl = [] { const char* e = getenv("SURFEL_FWD_ABL"); return e ? atoi(e) : 0; }();
-            if (abl == 1) launch(composite_fwd_kernel<32, 1>);
-            else if (abl == 2) launch(composite_fwd_kernel<32, 2>);
-            else launch(composite_fwd_kernel<32>);
-            break;
-        }
-        default: launch(composite_fwd_kernel<8>); break;
-    }
+    composite_fwd_kernel<<<((a.il.tiles * 8 + WPC - 1) / WPC) * a.fs.frames, 32 * WPC, 0, a.stream>>>(
+        a.fs, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles * 8, a.il.tiles_x,
+        (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, a.cam.bg,
+        (float*)(a.img + a.il.final_T), (uint32_t*)(a.img + a.il.n_contrib), a.out_color, a.out_others,
+        (uint32_t*)(a.img + a.il.tile_last), (uint32_t*)(a.bin + a.bl.contrib));
     sr_count_launch();
     return cudaGetLastError();
 }

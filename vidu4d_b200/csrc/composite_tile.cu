@@ -1,9 +1,9 @@
 // composite_tile.cu -- forward and backward composite with one CTA per 16x16 tile and a shared TMA chunk ring.
 //
 // Replaces (behaviour, not code) of the reference's renderCUDA forward / backward,
-// RAST/cuda_rasterizer/forward.cu:265-463 and backward.cu:143-449.  Same per-pair arithmetic, contribution
-// masks, accumulator layout and outputs as composite_fwd.cu / composite_bwd.cu (the one-warp-per-CTA kernels);
-// what changes is how the instance list reaches the lanes:
+// RAST/cuda_rasterizer/forward.cu:265-463 and backward.cu:143-449.  The backward here is the only one; the forward is
+// an alternative to composite_fwd.cu (the one-warp-per-CTA forward, the default) with the same per-pair arithmetic,
+// contribution masks and outputs.  What changes is how the instance list reaches the lanes:
 //
 //   * CTA = one tile = 8 warps (one per 8x4 sub-tile, lane = pixel).  The tile's sorted 80-byte instance records
 //     stream through ONE ring of NSLOT chunks of CH instances, filled by cp.async.bulk (TMA 1-D) and shared by the 8
@@ -20,6 +20,8 @@
 //     that gradients reach L2 once per (instance, tile); see composite_tile_bwd_kernel.
 //   * Forward early termination is per lane (T < 1e-4), per warp (all 32 pixels done: the warp only waits for and
 //     releases the remaining chunks) and per CTA (all 8 warps done: no further chunk is requested).
+#include <cstdlib>
+
 #include "composite_common.cuh"
 
 namespace {
@@ -38,24 +40,24 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     return ok != 0;
 }
 
-template <int CH, int NSLOT>
-struct TileSmem {
-    static constexpr int NSTG = CH / 32;                                         // 32-instance stages per chunk
-    static constexpr size_t ring = (size_t)NSLOT * CH * REC4 * sizeof(float4);
+// ------------------------------------------------------------------------------------------------ forward
+constexpr int FWD_CH = 256;        // instances per chunk
+constexpr int FWD_NSLOT = 2;       // ring slots
+struct FwdSmem {
+    static constexpr int NSTG = FWD_CH / 32;                                     // 32-instance stages per chunk
+    static constexpr size_t ring = (size_t)FWD_NSLOT * FWD_CH * REC4 * sizeof(float4);
     static constexpr size_t masks = (size_t)TWARPS * NSTG * 32 * sizeof(uint32_t);
-    static constexpr size_t total = ring + masks + NSLOT * sizeof(uint64_t) + (NSLOT + 4) * sizeof(uint32_t);
+    static constexpr size_t total = ring + masks + FWD_NSLOT * sizeof(uint64_t) + (FWD_NSLOT + 4) * sizeof(uint32_t);
 };
 
-// ------------------------------------------------------------------------------------------------ forward
-template <int CH, int NSLOT, int MINB>
-__global__ void __launch_bounds__(32 * TWARPS, MINB)
+__global__ void __launch_bounds__(32 * TWARPS, 4)
 composite_tile_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, const uint32_t* __restrict__ tile_order, int tiles_x,
                           const float4* __restrict__ irec, int W, int H, const float* __restrict__ bg,
                           float* __restrict__ final_T, uint32_t* __restrict__ n_contrib, float* __restrict__ out_color,
                           float* __restrict__ out_others, uint32_t* __restrict__ sub_last,
                           uint32_t* __restrict__ contrib_masks) {
-    using SM = TileSmem<CH, NSLOT>;
-    constexpr int NSTG = SM::NSTG;
+    using SM = FwdSmem;
+    constexpr int CH = FWD_CH, NSLOT = FWD_NSLOT, NSTG = SM::NSTG;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float4* ring = reinterpret_cast<float4*>(smem_raw);
     uint32_t* cm_all = reinterpret_cast<uint32_t*>(smem_raw + SM::ring);
@@ -129,7 +131,7 @@ composite_tile_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ range
                 if (st < nst) {
                     const int i = st * 32 + lane;
                     const uint32_t cull = i < cnt ? __float_as_uint(S[i * REC4 + 4].w) : 0u;
-                    const uint32_t m = group_survivors<32>(cull, sx0, sy0, lane);
+                    const uint32_t m = group_survivors(cull, sx0, sy0, lane);
                     cm[st * 32] = m;
                     if (m) nz |= 1u << st;
                 }
@@ -507,52 +509,27 @@ cudaError_t opt_in_smem(K kern, size_t bytes) {
 
 }  // namespace
 
-// Which composite kernels run: SURFEL_COMPOSITE=tile|warp sets both directions, SURFEL_COMPOSITE_FWD / _BWD one of them.
-// Defaults (measured on the headline batch): forward = one-warp CTAs with private rings (fewer
-// instructions per iteration; the forward is issue bound), backward = tile CTAs with the shared chunk ring (the per-lane
-// free walk, and one set of gradient reductions per (instance, tile) instead of one per contributing pixel).
-bool sr_composite_tile_mode(bool backward) {
-    static const int mode = [] {
-        auto pick = [](const char* name, int dflt) {
-            const char* e = getenv(name);
-            if (!e) e = getenv("SURFEL_COMPOSITE");
-            return e ? (e[0] == 't' ? 1 : 0) : dflt;
-        };
-        return pick("SURFEL_COMPOSITE_FWD", 0) | (pick("SURFEL_COMPOSITE_BWD", 1) << 1);
+// Which composite forward runs: SURFEL_COMPOSITE_FWD (or SURFEL_COMPOSITE) = tile|warp.  Default: one-warp CTAs with
+// private rings (composite_fwd.cu).  On the headline 8-frame batch the tile forward is faster, with 1 frame per call
+// slower (DESIGN.md 3.3).
+bool sr_composite_tile_fwd() {
+    static const bool tile = [] {
+        const char* e = getenv("SURFEL_COMPOSITE_FWD");
+        if (!e) e = getenv("SURFEL_COMPOSITE");
+        return e && e[0] == 't';
     }();
-    return backward ? (mode >> 1) & 1 : mode & 1;
-}
-
-int comp::tile_cfg_from_env() {
-    static const int cfg = [] {
-        const char* e = getenv("SURFEL_TILE_CFG");
-        const int v = e ? atoi(e) : 2562;
-        return (v == 2562 || v == 2563 || v == 1283 || v == 1284 || v == 5122 || v == 1282) ? v : 2562;
-    }();
-    return cfg;
+    return tile;
 }
 
 cudaError_t launch_composite_tile_fwd(const FwdArgs& a) {
     ProfileScope ps("composite_fwd", a.stream);
-    cudaError_t err = cudaSuccess;
-    auto launch = [&](auto kern, size_t smem) {
-        err = opt_in_smem(kern, smem);
-        if (err != cudaSuccess) return;
-        kern<<<a.il.tiles * a.fs.frames, 32 * TWARPS, smem, a.stream>>>(
-            a.fs, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles_x,
-            (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, a.cam.bg,
-            (float*)(a.img + a.il.final_T), (uint32_t*)(a.img + a.il.n_contrib), a.out_color, a.out_others,
-            (uint32_t*)(a.img + a.il.tile_last), (uint32_t*)(a.bin + a.bl.contrib));
-    };
-    switch (comp::tile_cfg_from_env()) {
-        case 2563: launch(composite_tile_fwd_kernel<256, 3, 3>, TileSmem<256, 3>::total); break;
-        case 1282: launch(composite_tile_fwd_kernel<128, 2, 4>, TileSmem<128, 2>::total); break;
-        case 1283: launch(composite_tile_fwd_kernel<128, 3, 4>, TileSmem<128, 3>::total); break;
-        case 1284: launch(composite_tile_fwd_kernel<128, 4, 4>, TileSmem<128, 4>::total); break;
-        case 5122: launch(composite_tile_fwd_kernel<512, 2, 2>, TileSmem<512, 2>::total); break;
-        default: launch(composite_tile_fwd_kernel<256, 2, 4>, TileSmem<256, 2>::total); break;
-    }
+    cudaError_t err = opt_in_smem(composite_tile_fwd_kernel, FwdSmem::total);
     if (err != cudaSuccess) return err;
+    composite_tile_fwd_kernel<<<a.il.tiles * a.fs.frames, 32 * TWARPS, FwdSmem::total, a.stream>>>(
+        a.fs, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles_x,
+        (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, a.cam.bg,
+        (float*)(a.img + a.il.final_T), (uint32_t*)(a.img + a.il.n_contrib), a.out_color, a.out_others,
+        (uint32_t*)(a.img + a.il.tile_last), (uint32_t*)(a.bin + a.bl.contrib));
     sr_count_launch();
     return cudaGetLastError();
 }

@@ -96,8 +96,9 @@ sort_plan_kernel(const FrameStrides fs, uint32_t* __restrict__ hist, uint32_t* _
     }
 }
 
-template <int MINB>
-__global__ void __launch_bounds__(SR_SORT_THREADS, MINB)
+// 3 resident blocks per SM (<= 85 registers, no spills) instead of 2: the pass is latency bound (ticket, key loads,
+// look-back), r2g ncu: 24 % warps active, 15 % DRAM.
+__global__ void __launch_bounds__(SR_SORT_THREADS, 3)
 onesweep_pass_kernel(const FrameStrides fs, uint64_t* __restrict__ keys0, uint64_t* __restrict__ keys1,
                      uint32_t* __restrict__ vals0, uint32_t* __restrict__ vals1, const uint32_t* __restrict__ hist,
                      uint32_t* __restrict__ ctl, uint32_t* __restrict__ status, const uint32_t* __restrict__ num_rendered,
@@ -370,19 +371,13 @@ cudaError_t launch_sort(const FwdArgs& a) {
     { ProfileScope ps("sort_plan", a.stream);
       sort_plan_kernel<<<a.fs.frames, 256, 0, a.stream>>>(a.fs, hist, ctl, a.num_rendered_dev, cap, plan); }
     ProfileScope ps("onesweep_passes", a.stream);
-    // 3 resident blocks per SM (<= 85 registers, no spills) instead of 2: the pass is latency bound (ticket, key loads,
-    // look-back), r2g ncu: 24 % warps active, 15 % DRAM.  SURFEL_SORT_MINB=2 selects the old bound for A/B runs.
-    static const int minb = [] { const char* e = getenv("SURFEL_SORT_MINB"); return e && atoi(e) == 2 ? 2 : 3; }();
+    // SURFEL_SORT_INTERLEAVE=0 keeps each frame's blocks together: on the headline batch that pass time was ~1 % lower
+    // with the end-to-end rates unchanged (DESIGN.md 3.2)
     static const int inter = [] { const char* e = getenv("SURFEL_SORT_INTERLEAVE"); return e && atoi(e) == 0 ? 0 : 1; }();
     const unsigned blocks = (unsigned)a.bl.sort_tiles * (unsigned)a.fs.frames;
-    for (int p = 0; p < plan.npass; p++) {
-        if (minb == 2)
-            onesweep_pass_kernel<2><<<blocks, SR_SORT_THREADS, 0, a.stream>>>(
-                a.fs, k0, k1, v0, v1, hist, ctl, status, a.num_rendered_dev, p, plan.shift[p], plan.bits[p], a.bl.sort_tiles, inter);
-        else
-            onesweep_pass_kernel<3><<<blocks, SR_SORT_THREADS, 0, a.stream>>>(
-                a.fs, k0, k1, v0, v1, hist, ctl, status, a.num_rendered_dev, p, plan.shift[p], plan.bits[p], a.bl.sort_tiles, inter);
-    }
+    for (int p = 0; p < plan.npass; p++)
+        onesweep_pass_kernel<<<blocks, SR_SORT_THREADS, 0, a.stream>>>(
+            a.fs, k0, k1, v0, v1, hist, ctl, status, a.num_rendered_dev, p, plan.shift[p], plan.bits[p], a.bl.sort_tiles, inter);
     sr_count_launch(2 + plan.npass);
     return cudaGetLastError();
 }
