@@ -124,9 +124,9 @@ def test_stage3_loss_oracle_gradients_match_finite_differences():
 
 
 # ---- a float64 model of csrc/loss.cu's shared-memory tiling (32x8 tile + one-pixel ring, 80 ring threads, gather signs)
-# against the oracle on ragged image sizes: the index logic of the kernel, checked where the GPU tests use block-aligned
-# images.  The arithmetic is the oracle's; what is restated from the kernel is WHICH stencil lands in WHICH cell and who
-# reads it.
+# against the oracle on ragged image sizes: the index logic of the kernel, checked without a GPU.  The arithmetic is the
+# oracle's; what is restated from the kernel is WHICH stencil lands in WHICH cell and who reads it.  The kernel itself is
+# checked element by element at the same ragged, odd and tiny sizes by tests/test_gpu_loss_bounds.py.
 def _loss_kernel_model(color, allmap, wvt, tanx, tany, depth_ratio, target, vis, mask_gt, mask_wt, w_rgb, w_mask, lam_n, lam_d):
     """Python restatement of csrc/loss.cu:loss_grad_kernel's indexing: 32x8 tiles, sg[6][10][34] ring, 80 ring threads."""
     _, H, W = color.shape

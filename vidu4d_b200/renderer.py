@@ -494,6 +494,26 @@ def _check_feature_losses(M, H, W, features, feature_target, mask_gt, is_detecte
     return feature_target, is_detected, gm, feature_loss_weights.contiguous()
 
 
+def _check_loss_inputs(M, H, W, device, target_rgb, vis2d, mask_gt, mask_wt, learnable_bkgd):
+    """Validate the image-loss arguments of render_loss_batch before anything runs on the device (shapes first, then
+    devices).  The loss kernel reads them as raw (M,3,H,W) / (M,H,W) / (3,) buffers on the rasterizer's device: a (H,W)
+    mask for M > 1 frames or a host tensor would make it read past the end of the buffer."""
+    if target_rgb is None or tuple(target_rgb.shape) != (M, 3, H, W):
+        raise RuntimeError(f"target_rgb must be (M,3,H,W) = ({M},3,{H},{W}), got "
+                           f"{None if target_rgb is None else tuple(target_rgb.shape)}")
+    for name, t in (("vis2d", vis2d), ("mask_gt", mask_gt), ("mask_wt", mask_wt)):
+        if t is not None and tuple(t.shape) != (M, H, W):
+            raise RuntimeError(f"{name} must be (M,H,W) = ({M},{H},{W}) or None, got {tuple(t.shape)}")
+    if mask_wt is not None and mask_gt is None:
+        raise RuntimeError("mask_wt weights the mask term: it needs mask_gt")
+    if learnable_bkgd is not None and learnable_bkgd.numel() != 3:
+        raise RuntimeError(f"learnable_bkgd must have 3 elements, got shape {tuple(learnable_bkgd.shape)}")
+    for name, t in (("target_rgb", target_rgb), ("vis2d", vis2d), ("mask_gt", mask_gt), ("mask_wt", mask_wt),
+                    ("learnable_bkgd", learnable_bkgd)):
+        if t is not None and (not t.is_cuda or t.device != device):
+            raise RuntimeError(f"{name} must be a CUDA tensor on the rasterizer's device {device}, got {t.device}")
+
+
 def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_gt=None, mask_wt=None, learnable_bkgd=None,
                       w_rgb=1.0, w_mask=0.0, lambda_normal=0.0, lambda_dist=0.0, means3D=None, rotations=None, target_stream=None,
                       features=None, feature_target=None, is_detected=None, gauss_mask_channel=None, feature_loss_weights=None):
@@ -527,11 +547,13 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
     if not isinstance(cameras, BatchCameras):
         cameras = stack_cameras(cameras)
     M = len(cameras)
+    xyz = pc.get_xyz if means3D is None else means3D
+    _check_loss_inputs(M, cameras.image_height, cameras.image_width, xyz.device, target_rgb, vis2d, mask_gt, mask_wt,
+                       learnable_bkgd)
     feature_loss = None
     if feature_target is not None or gauss_mask_channel is not None:
         feature_loss = _check_feature_losses(M, cameras.image_height, cameras.image_width, features, feature_target, mask_gt,
                                              is_detected, gauss_mask_channel, feature_loss_weights)
-    xyz = pc.get_xyz if means3D is None else means3D
     rot = pc.get_rotation if rotations is None else rotations
     P = int(xyz.shape[-2])
     screenspace_points = torch.zeros((M, P, 3), dtype=xyz.dtype, requires_grad=True, device=xyz.device)
