@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SR_ABI_VERSION 6
+#define SR_ABI_VERSION 7
 
 #if defined(__GNUC__)
 #define SR_API __attribute__((visibility("default")))
@@ -81,59 +81,45 @@ SR_API size_t sr_image_bytes(int32_t width, int32_t height);
 SR_API size_t sr_binning_bytes(int64_t capacity /* max instances */, int32_t width, int32_t height);
 
 /*
- * Forward.  Replaces Rasterizer::forward (rasterizer_impl.cu:198-342).
+ * Forward and backward.  Replace Rasterizer::forward (rasterizer_impl.cu:198-342) and Rasterizer::backward
+ * (rasterizer_impl.cu:346-448), batched (SURVEY.md section 8(f) row N1): M independent frames -- different cameras, and
+ * optionally different surfel sets, as in Stage 3 where every frame rasterizes its own bob-warped copy of the canonical
+ * surfels (lab4d/nnutils/deformable_gaussian.py:1175-1188 loops frames in Python) -- in ONE launch set: every kernel of
+ * the path gets a frame dimension, so a step costs the same ~15 launches whatever M is and the GPU sees M x the CTAs.
+ * One frame, as the reference renders it, is the M = 1 case: sr_batch {1, 0, 0, ...}.
  *
- *   background[3], means3D[P*3], shs[P*M*3] | colors_precomp[P*3] (exactly one non-NULL),
- *   opacities[P], scales[P*2], rotations[P*4] (w,x,y,z), viewmatrix[16], projmatrix[16], campos[3]
- *   out_color[3*H*W], out_others[8*H*W], radii[P] (int32)           -- written
- *   geom/binning/image buffers: caller-allocated, sizes from sr_*_bytes()
- *   capacity: number of instances the binning buffer was sized for
- *   num_rendered_dev: device uint32[2] -> {num_rendered, status}; also copied
- *       asynchronously to num_rendered_host (pinned host uint32[2]) if non-NULL.
- */
-SR_API int sr_forward(const sr_frame* f,
-               const float* background, const float* means3D, const float* shs,
-               const float* colors_precomp, const float* opacities, const float* scales,
-               const float* rotations, const float* viewmatrix, const float* projmatrix,
-               const float* campos,
-               float* out_color, float* out_others, int32_t* radii,
-               void* geom_buffer, void* binning_buffer, void* image_buffer, int64_t capacity,
-               uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream);
-
-/*
- * Backward.  Replaces Rasterizer::backward (rasterizer_impl.cu:346-448).
- * Inputs as in forward plus dL_dout_color[3*H*W], dL_dout_others[8*H*W] and the
- * three buffers the forward filled.  Outputs (all fully written, no need to zero):
- *   dL_dmeans2D[P*3] (the densification proxy of backward.cu:645-648; z = 0),
- *   dL_dcolors[P*3], dL_dopacity[P], dL_dmeans3D[P*3], dL_dtransMat[P*9],
- *   dL_dsh[P*M*3], dL_dscales[P*2], dL_drotations[P*4]
- */
-SR_API int sr_backward(const sr_frame* f,
-                const float* background, const float* means3D, const float* shs,
-                const float* colors_precomp, const float* scales, const float* rotations,
-                const float* viewmatrix, const float* projmatrix, const float* campos,
-                const int32_t* radii,
-                const float* dL_dout_color, const float* dL_dout_others,
-                void* geom_buffer, void* binning_buffer, void* image_buffer, int64_t capacity,
-                float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D,
-                float* dL_dtransMat, float* dL_dsh, float* dL_dscales, float* dL_drotations,
-                void* stream);
-
-/*
- * Batched entry points (SURVEY.md section 8(f) row N1): M independent frames -- different cameras, and optionally
- * different surfel sets, as in Stage 3 where every frame rasterizes its own bob-warped copy of the canonical surfels
- * (lab4d/nnutils/deformable_gaussian.py:1175-1188 loops frames in Python) -- in ONE launch set: every kernel of the
- * path gets a frame dimension, so a step costs the same ~15 launches whatever M is and the GPU sees M x the CTAs.
+ * Inputs: background[bg_channels], means3D[P*3], shs[P*sh_coeffs*3] | colors_precomp[P*3] (exactly one non-NULL),
+ *   opacities[P], scales[P*2], rotations[P*4] (w,x,y,z), features[P*F]; viewmatrix[M*16], projmatrix[M*16], campos[M*3].
+ *   Per-surfel inputs are addressed as base + frame * stride (in floats; sr_batch, features_stride), stride 0 = shared
+ *   by all frames.
+ * Forward writes frame m's 3 colour planes at out_color + m * out_color_stride, its F feature planes at out_features +
+ *   m * out_features_stride (strides in floats), out_others[M*8*H*W] and radii[M*P] (int32).
+ *   geom/binning/image buffers: caller-allocated, M consecutive per-frame buffers of sr_*_bytes() each; capacity: the
+ *   number of instances each frame's binning buffer was sized for (the same for every frame).
+ *   num_rendered_dev: device uint32[M*2] -> {num_rendered, status} per frame; also copied asynchronously to
+ *   num_rendered_host (pinned host uint32[M*2]) if non-NULL.
+ * Backward takes the forward's inputs, dL_dout_color / dL_dout_features (strided as out_color / out_features),
+ *   dL_dout_others[M*8*H*W] and the three buffers the forward filled.  Outputs (all fully written, no need to zero):
+ *   dL_dmeans2D (the densification proxy of backward.cu:645-648; z = 0), dL_dcolors[P*3], dL_dopacity[P],
+ *   dL_dmeans3D[P*3], dL_dtransMat[P*9], dL_dsh[P*sh_coeffs*3], dL_dscales[P*2], dL_drotations[P*4], dL_dfeatures[P*F],
+ *   each per frame, (M, P, .) -- except, with SR_BATCH_SUM_SHARED, those of shared inputs, which are (P, .) sums over
+ *   the frames; dL_dmeans2D and dL_dtransMat are always per frame.  dL_dtransMat (a by-product) may be NULL unless
+ *   M == 1 without SR_BATCH_SUM_SHARED.  grad_scale (optional DEVICE scalar, NULL = 1) multiplies dL_dout_color and
+ *   dL_dout_others -- the upstream scalar of a fused loss; features_grad_scale (likewise) multiplies dL_dout_features.
  *
- * Layout: viewmatrix[M*16], projmatrix[M*16], campos[M*3]; out_color[M*3*H*W], out_others[M*8*H*W], radii[M*P];
- * geom/binning/image buffers are M consecutive per-frame buffers of sr_*_bytes() each (same capacity for every frame);
- * num_rendered_dev / num_rendered_host are uint32[M*2] = {num_rendered, status} per frame.  Per-surfel inputs are
- * addressed as base + frame * stride (in floats; sr_batch), stride 0 = shared by all frames.  background[3] is shared.
- * Backward: dL_dout_color[M*3*H*W], dL_dout_others[M*8*H*W]; every gradient output is written per frame, (M, P, .)
- * -- except, with SR_BATCH_SUM_SHARED, those of shared inputs, which are (P, .) sums over the frames; dL_dmeans2D is always
- * per frame; dL_dtransMat may be NULL in the batched call (it is only a by-product);
- * grad_scale (optional DEVICE scalar, NULL = 1) multiplies dL_dout_* -- the upstream scalar of a fused loss.
- * sr_forward / sr_backward are the M = 1 case.
+ * F = 0 is the plain rasterizer: features NULL, bg_channels 3, and packed colour (out_color_stride / dL_dout_color_stride
+ * 0 or 3*H*W).  1 <= F <= 32 composites per-surfel FEATURE channels next to the colour -- the 16+2+3+1-channel vector of
+ * lab4d/nnutils/deformable_gaussian.py:1182-1207 (registration feature, flow, normal, Gaussian mask), which the
+ * reference rasterizer (NUM_CHANNELS 3) cannot render:
+ *   features are independent of where the colour comes from (shs or colors_precomp);
+ *   background[bg_channels]: 3 (the feature planes get a zero background) or 3+F (feature plane f gets background[3+f]);
+ *   out_color_stride >= 3*H*W, so that colour and features can share one (M, 3+F, H, W) tensor (stride (3+F)*H*W,
+ *       features at out_color + 3*H*W); out_features_stride >= F*H*W.
+ * Feature plane f = sum_i T_i alpha_i features[i, f] + T_final bg_f over exactly the colour's contributors, weights and
+ * FMA order: a feature column equal to a colour column gives a bit-identical plane.  The colour, out_others, radii and
+ * the three buffers are those F = 0 writes.  dL_dfeatures is zeroed inside; invisible surfels get 0.  The feature planes'
+ * gradient reaches dL_dmeans3D / dL_dscales / dL_drotations / dL_dopacity / dL_dmeans2D through alpha, as the colour
+ * planes' does.  The background gets no gradient.
  */
 #define SR_BATCH_SUM_SHARED 1u   /* backward: an input shared by the frames (stride 0) gets ONE gradient (P, .), the sum over
                                     the frames, accumulated inside the per-surfel kernel and written once -- instead of
@@ -144,46 +130,7 @@ typedef struct sr_batch {
     int64_t means3D, shs, colors_precomp, opacities, scales, rotations;   /* floats between consecutive frames; 0 = shared */
 } sr_batch;
 
-SR_API int sr_forward_batch(const sr_frame* f, const sr_batch* b,
-               const float* background, const float* means3D, const float* shs,
-               const float* colors_precomp, const float* opacities, const float* scales,
-               const float* rotations, const float* viewmatrix, const float* projmatrix,
-               const float* campos,
-               float* out_color, float* out_others, int32_t* radii,
-               void* geom_buffer, void* binning_buffer, void* image_buffer, int64_t capacity,
-               uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream);
-
-SR_API int sr_backward_batch(const sr_frame* f, const sr_batch* b,
-                const float* background, const float* means3D, const float* shs,
-                const float* colors_precomp, const float* scales, const float* rotations,
-                const float* viewmatrix, const float* projmatrix, const float* campos,
-                const int32_t* radii,
-                const float* dL_dout_color, const float* dL_dout_others, const float* grad_scale,
-                void* geom_buffer, void* binning_buffer, void* image_buffer, int64_t capacity,
-                float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D,
-                float* dL_dtransMat, float* dL_dsh, float* dL_dscales, float* dL_drotations,
-                void* stream);
-
-/*
- * Batched entry points with per-surfel FEATURE channels composited next to the colour -- the 16+2+3+1-channel vector of
- * lab4d/nnutils/deformable_gaussian.py:1182-1207 (registration feature, flow, normal, Gaussian mask), which the reference
- * rasterizer (NUM_CHANNELS 3) cannot render.  Each is the plain batched entry plus:
- *   features[P*F] per frame at features + frame * features_stride (floats; 0 = shared), 1 <= F <= 32, independent of
- *       where the colour comes from (shs or colors_precomp);
- *   background[bg_channels]: 3 (the feature planes get a zero background) or 3+F (feature plane f gets background[3+f]);
- *   out_color / dL_dout_color: frame m's 3 colour planes at + m * stride (floats; >= 3*H*W), so that colour and features
- *       can share one (M, 3+F, H, W) tensor (stride (3+F)*H*W, features at out_color + 3*H*W);
- *   out_features / dL_dout_features: frame m's F planes at + m * stride (floats; >= F*H*W).
- * Feature plane f = sum_i T_i alpha_i features[i, f] + T_final bg_f over exactly the colour's contributors, weights and
- * FMA order: a feature column equal to a colour column gives a bit-identical plane.  The colour, out_others, radii and
- * the three buffers are what sr_forward_batch writes.  F = 0 (features NULL, bg_channels 3, packed colour): the plain
- * entries.  Backward: grad_scale multiplies dL_dout_color / dL_dout_others as in sr_backward_batch; features_grad_scale
- * (optional DEVICE scalar, NULL = 1) multiplies dL_dout_features.  dL_dfeatures is fully written (zeroed inside):
- * (M, P, F), or (P, F) -- the sum over the frames -- for shared features under SR_BATCH_SUM_SHARED; invisible surfels
- * get 0.  The feature planes' gradient reaches dL_dmeans3D / dL_dscales / dL_drotations / dL_dopacity / dL_dmeans2D
- * through alpha, as the colour planes' does.  The background gets no gradient.
- */
-SR_API int sr_forward_batch_features(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+SR_API int sr_forward(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
                const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
                const float* scales, const float* rotations, const float* features, int32_t F, int64_t features_stride,
                const float* viewmatrix, const float* projmatrix, const float* campos,
@@ -192,7 +139,7 @@ SR_API int sr_forward_batch_features(const sr_frame* f, const sr_batch* b, const
                void* geom_buffer, void* binning_buffer, void* image_buffer, int64_t capacity,
                uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream);
 
-SR_API int sr_backward_batch_features(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+SR_API int sr_backward(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
                 const float* means3D, const float* shs, const float* colors_precomp, const float* scales,
                 const float* rotations, const float* features, int32_t F, int64_t features_stride,
                 const float* viewmatrix, const float* projmatrix, const float* campos, const int32_t* radii,
@@ -266,7 +213,7 @@ SR_API int sr_render_loss_batch(int32_t M, int32_t W, int32_t H, float tan_fovx,
                                 float* surf_depth_scratch, void* stream);
 
 /*
- * Stage-3 losses on the rasterizer's FEATURE planes (sr_forward_batch_features), forward and gradient, M frames per call.
+ * Stage-3 losses on the rasterizer's FEATURE planes (sr_forward with F > 0), forward and gradient, M frames per call.
  * Replaces lab4d/engine/model.py:663-667 (feature reconstruction) and :742-745 (Gaussian-mask consistency) with their
  * masking (:952-967) and reduction (:1000-1012):
  *   feature:        v = ||features[c] - target[c]||_2 over c < Cf, times mask_gt and is_detected[frame]
@@ -293,7 +240,7 @@ SR_API int sr_feature_loss_batch(int32_t M, int32_t W, int32_t H, int32_t F, int
  *   xyz[P*3], rot[P*4] (w,x,y,z): canonical surfels;  o2b_q[B*4], o2b_t[B*3]: object->bone transform of the rest pose;
  *   inv_gauss[B*3] = exp(-log_gauss);  delta[P*B] or NULL;  se3_r, se3_d[M*B*4]: per frame and bone dual quaternion
  *   t_articulation o rest_articulation^-1;  cam_q[M*4], cam_t[M*3]: field2cam.   B <= 64.
- * forward writes xyz_cam[M*P*3], rot_cam[M*P*4] (feed them to sr_forward_batch with per-frame strides) and
+ * forward writes xyz_cam[M*P*3], rot_cam[M*P*4] (feed them to sr_forward with per-frame strides) and
  * skin_entropy[P] (may be NULL).  backward takes their gradients (g_entropy may be NULL) and writes g_xyz[P*3], g_rot[P*4],
  * g_delta[P*B] (if non-NULL) and g_tables[sr_bob_warp_table_floats(B, M)] = gradients of {o2b_q, o2b_t, inv_gauss, se3_r,
  * se3_d, cam_q, cam_t} in that order (zeroed inside).

@@ -14,7 +14,7 @@ def _frame(P=10, W=64, H=64):
 
 
 def _fwd_args(F, bg_channels, features=True):
-    """sr_forward_batch_features arguments with dummy (never dereferenced) pointers."""
+    """sr_forward arguments with dummy (never dereferenced) pointers."""
     from vidu4d_b200 import _capi
     fr, bt = _frame(), _capi.SrBatch(1, 0, 0, 0, 0, 0, 0, 0)
     d = 4096
@@ -31,10 +31,10 @@ def _bwd_args(F, bg_channels, features=True):
 
 
 @pytest.mark.parametrize("entry", ["forward", "backward"])
-def test_c_abi_rejects_bad_feature_arguments(built, entry):
+def test_sr_forward_backward_reject_bad_feature_arguments(built, entry):
     from vidu4d_b200 import _capi
     lib = _capi.load()
-    fn, mk = (lib.sr_forward_batch_features, _fwd_args) if entry == "forward" else (lib.sr_backward_batch_features, _bwd_args)
+    fn, mk = (lib.sr_forward, _fwd_args) if entry == "forward" else (lib.sr_backward, _bwd_args)
     assert fn(*mk(33, 36)) == -1 and b"F must be in [1, 32]" in lib.sr_last_error()
     assert fn(*mk(-1, 3)) == -1 and b"F must be in [1, 32]" in lib.sr_last_error()
     assert fn(*mk(0, 3)) == -1 and b"got 0" in lib.sr_last_error()           # F = 0 with a features pointer

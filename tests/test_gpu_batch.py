@@ -1,4 +1,4 @@
-"""GPU tests of the batched entry points (sr_forward_batch / sr_backward_batch, SURVEY.md 8(f) row N1): M frames in one
+"""GPU tests of batched calls (sr_forward / sr_backward with M frames, SURVEY.md 8(f) row N1): M frames in one
 launch set must equal M single-frame calls -- forward planes, sorted lists and contributor counts bit for bit, gradients
 up to the order of the atomic reductions -- for shared and for per-frame surfel sets, and through autograd."""
 import numpy as np

@@ -1,4 +1,4 @@
-"""GPU tests of per-surfel feature channels (sr_forward_batch_features / sr_backward_batch_features): F channels composited
+"""GPU tests of per-surfel feature channels (sr_forward / sr_backward with F >= 1): F channels composited
 with the colour's weights next to the colour.  The colour path must not change at all; a feature plane must be bit for bit
 what the colour path renders for the same values; the backward is pinned by linearity against colour-only renders."""
 import numpy as np

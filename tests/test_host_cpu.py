@@ -55,18 +55,30 @@ def test_debug_layout_is_aligned(built):
             assert x % 256 == 0, (name, x)
 
 
-def test_argument_validation_without_gpu(built):
+def _null_forward_args(fr, bt):
+    """sr_forward arguments with F = 0, a 3-channel background and every pointer but the descriptors NULL."""
+    return ([C.byref(fr), None if bt is None else C.byref(bt), None, 3] + [None] * 7 + [0, 0] + [None] * 3
+            + [None, 0, None, 0] + [None] * 5 + [0] + [None] * 3)
+
+
+def _null_backward_args(fr, bt):
+    """sr_backward arguments with F = 0, a 3-channel background and every pointer but the descriptors NULL."""
+    return ([C.byref(fr), C.byref(bt), None, 3] + [None] * 6 + [0, 0] + [None] * 4 + [None, 0, None, 0] + [None] * 6
+            + [0] + [None] * 10)
+
+
+def test_sr_forward_rejects_bad_frame_without_gpu(built):
     """Bad arguments are rejected before any CUDA call (so this runs on a CPU-only box)."""
     from vidu4d_b200 import _capi
     lib = _capi.load()
-    nul = [None] * 16 + [0] + [None] * 3      # 16 pointers, capacity, 3 pointers
+    one = _capi.SrBatch(1, 0, 0, 0, 0, 0, 0, 0)
     fr = _capi.SrFrame(10, 3, 16, -5, 64, 0.5, 0.5, 1.0, 0, 0, 0)
-    rc = lib.sr_forward(C.byref(fr), *nul)
+    rc = lib.sr_forward(*_null_forward_args(fr, one))
     assert rc == -1 and b"image size" in lib.sr_last_error()
     fr = _capi.SrFrame(10, 5, 16, 64, 64, 0.5, 0.5, 1.0, 0, 0, 0)
-    assert lib.sr_forward(C.byref(fr), *nul) == -1 and b"sh_degree" in lib.sr_last_error()
+    assert lib.sr_forward(*_null_forward_args(fr, one)) == -1 and b"sh_degree" in lib.sr_last_error()
     fr = _capi.SrFrame(10, 3, 4, 64, 64, 0.5, 0.5, 1.0, 0, 0, 0)
-    assert lib.sr_forward(C.byref(fr), *nul) == -1 and b"coefficients" in lib.sr_last_error()
+    assert lib.sr_forward(*_null_forward_args(fr, one)) == -1 and b"coefficients" in lib.sr_last_error()
     assert lib.sr_mark_visible(-1, None, None, None, None, None) == -1
 
 
@@ -228,20 +240,18 @@ def test_check_overflow_bookkeeping_without_a_gpu(built, monkeypatch):
         R._pending[:] = saved[0]; R._cap_hint.clear(); R._cap_hint.update(saved[1]); R._host_next = saved[2]
 
 
-def test_batch_descriptor_and_validation_without_gpu(built):
-    """The batched entry points validate their descriptor before any CUDA call; sr_batch's ctypes layout matches the C one."""
+def test_sr_batch_descriptor_and_validation_without_gpu(built):
+    """sr_forward / sr_backward validate their batch descriptor before any CUDA call; sr_batch's ctypes layout matches the C one."""
     from vidu4d_b200 import _capi
     lib = _capi.load()
     assert C.sizeof(_capi.SrBatch) == 8 + 6 * 8                      # int32 frames, uint32 flags, six int64 strides
     fr = _capi.SrFrame(10, 3, 16, 64, 64, 0.5, 0.5, 1.0, 0, 0, 0)
-    nul = [None] * 16 + [0] + [None] * 3
     for frames in (0, -3, 70000):
         bt = _capi.SrBatch(frames, 0, 0, 0, 0, 0, 0, 0)
-        assert lib.sr_forward_batch(C.byref(fr), C.byref(bt), *nul) == -1 and b"frames" in lib.sr_last_error()
-    assert lib.sr_forward_batch(C.byref(fr), None, *nul) == -1
+        assert lib.sr_forward(*_null_forward_args(fr, bt)) == -1 and b"frames" in lib.sr_last_error()
+    assert lib.sr_forward(*_null_forward_args(fr, None)) == -1
     bt = _capi.SrBatch(2, 0, 0, 0, 0, 0, 0, 0)
-    nulb = [None] * 13 + [None, None, None, 0] + [None] * 9
-    assert lib.sr_backward_batch(C.byref(fr), C.byref(bt), *nulb) == -1 and b"NULL" in lib.sr_last_error()
+    assert lib.sr_backward(*_null_backward_args(fr, bt)) == -1 and b"NULL" in lib.sr_last_error()
     # pure host helpers
     assert lib.sr_bob_warp_table_floats(25, 2) == 25 * 10 + 2 * 25 * 8 + 2 * 7
     assert lib.sr_bob_warp_forward(10, 65, 1, *([None] * 14)) == -1                 # more than 64 bones

@@ -1,6 +1,6 @@
 """A/B of launch strategies on the headline frame set: F frames per step, forward+backward, device resident.
   streams : F single-frame calls alternating over S CUDA streams (round-1 harness)
-  batch   : ONE batched call (sr_forward_batch / sr_backward_batch) on one stream
+  batch   : ONE batched call (sr_forward / sr_backward over F frames) on one stream
 Each configuration runs in a child process."""
 import argparse, json, os, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libsurfel_raster.so")
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 SR_STATUS_OVERFLOW = 1
 SR_STATUS_PREFILTER = 4
 SR_BATCH_SUM_SHARED = 1
@@ -19,9 +19,8 @@ SR_BATCH_SUM_SHARED = 1
 SYMBOLS = (
     "sr_geom_bytes", "sr_image_bytes", "sr_binning_bytes", "sr_forward", "sr_backward",
     "sr_mark_visible", "sr_debug_view", "sr_abi_version", "sr_last_error", "sr_launch_count",
-    "sr_set_profiling", "sr_get_profile", "sr_post_forward", "sr_post_backward", "sr_forward_batch", "sr_backward_batch", "sr_render_loss_batch", "sr_bob_warp_table_floats", "sr_bob_warp_forward", "sr_bob_warp_backward", "sr_adam_flat", "sr_surfel_compact", "sr_knn_cells", "sr_knn_mean_dist2",
-    "sr_forward_batch_features", "sr_backward_batch_features", "sr_feature_loss_batch",
-    "sr_global_match_forward", "sr_global_match_backward", "sr_reproj_loss_forward", "sr_reproj_loss_backward",
+    "sr_set_profiling", "sr_get_profile", "sr_post_forward", "sr_post_backward", "sr_render_loss_batch", "sr_bob_warp_table_floats", "sr_bob_warp_forward", "sr_bob_warp_backward", "sr_adam_flat", "sr_surfel_compact", "sr_knn_cells", "sr_knn_mean_dist2",
+    "sr_feature_loss_batch", "sr_global_match_forward", "sr_global_match_backward", "sr_reproj_loss_forward", "sr_reproj_loss_backward",
 )
 FEATURES_MAX = 32          # channels per call (SR_FEAT_MAX)
 
@@ -82,20 +81,12 @@ def load():
     lib.sr_binning_bytes.restype = C.c_size_t
     lib.sr_binning_bytes.argtypes = [i64, i32, i32]
     lib.sr_forward.restype = C.c_int
-    lib.sr_forward.argtypes = [C.POINTER(SrFrame)] + [f32p] * 10 + [vp, vp, vp] + [vp, vp, vp, i64, vp, vp, vp]
+    lib.sr_forward.argtypes = ([C.POINTER(SrFrame), C.POINTER(SrBatch), f32p, i32] + [f32p] * 7 + [i32, i64]
+                               + [f32p] * 3 + [vp, i64, vp, i64] + [vp] * 5 + [i64, vp, vp, vp])
     lib.sr_backward.restype = C.c_int
-    lib.sr_backward.argtypes = [C.POINTER(SrFrame)] + [f32p] * 9 + [vp] + [f32p] * 2 + [vp, vp, vp, i64] + [f32p] * 8 + [vp]
-    lib.sr_forward_batch.restype = C.c_int
-    lib.sr_forward_batch.argtypes = [C.POINTER(SrFrame), C.POINTER(SrBatch)] + [f32p] * 10 + [vp, vp, vp] + [vp, vp, vp, i64, vp, vp, vp]
-    lib.sr_backward_batch.restype = C.c_int
-    lib.sr_backward_batch.argtypes = [C.POINTER(SrFrame), C.POINTER(SrBatch)] + [f32p] * 9 + [vp] + [f32p] * 3 + [vp, vp, vp, i64] + [f32p] * 8 + [vp]
-    lib.sr_forward_batch_features.restype = C.c_int
-    lib.sr_forward_batch_features.argtypes = ([C.POINTER(SrFrame), C.POINTER(SrBatch), f32p, i32] + [f32p] * 7 + [i32, i64]
-                                              + [f32p] * 3 + [vp, i64, vp, i64] + [vp] * 5 + [i64, vp, vp, vp])
-    lib.sr_backward_batch_features.restype = C.c_int
-    lib.sr_backward_batch_features.argtypes = ([C.POINTER(SrFrame), C.POINTER(SrBatch), f32p, i32] + [f32p] * 6 + [i32, i64]
-                                               + [f32p] * 3 + [vp] + [f32p, i64, f32p, i64] + [f32p] * 3 + [vp] * 3 + [i64]
-                                               + [f32p] * 9 + [vp])
+    lib.sr_backward.argtypes = ([C.POINTER(SrFrame), C.POINTER(SrBatch), f32p, i32] + [f32p] * 6 + [i32, i64]
+                                + [f32p] * 3 + [vp] + [f32p, i64, f32p, i64] + [f32p] * 3 + [vp] * 3 + [i64]
+                                + [f32p] * 9 + [vp])
     lib.sr_mark_visible.restype = C.c_int
     lib.sr_mark_visible.argtypes = [i32, f32p, f32p, f32p, vp, vp]
     lib.sr_debug_view.restype = C.c_int

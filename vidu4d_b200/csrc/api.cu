@@ -145,7 +145,7 @@ int sr_debug_view(int32_t P, int32_t width, int32_t height, int64_t capacity, sr
 }
 
 namespace {
-// Feature-channel arguments shared by the two *_features entries: F in [1, SR_FEAT_MAX], background length 3 or 3+F,
+// Feature-channel arguments of sr_forward / sr_backward with F > 0: F in [1, SR_FEAT_MAX], background length 3 or 3+F,
 // and the widest vector access (4, 2 or 1 floats) that every feature row / gradient row / frame stride allows.
 int check_features(const sr_frame* f, int32_t F, int32_t bg_channels, const float* features, int64_t features_stride) {
     if (!f) return fail(SR_EINVAL, "frame descriptor is NULL");
@@ -156,7 +156,7 @@ int check_features(const sr_frame* f, int32_t F, int32_t bg_channels, const floa
         return fail(SR_EINVAL, "background must have 3 or 3+F = %d channels, got %d", 3 + F, bg_channels);
     return 0;
 }
-// F = 0: the *_features entries are the plain ones (no feature pointer, 3-channel background, packed colour)
+// F = 0: the plain rasterizer (no feature pointer, 3-channel background, packed colour)
 int check_no_features(const sr_frame* f, const float* features, int32_t bg_channels, int64_t color_stride) {
     if (features) return fail(SR_EINVAL, "features: F must be in [1, %d], got 0", SR_FEAT_MAX);
     if (bg_channels != 3) return fail(SR_EINVAL, "background must have 3 channels when F = 0, got %d", bg_channels);
@@ -256,30 +256,19 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
     return 0;
 }
 
-int sr_forward_batch(const sr_frame* f, const sr_batch* b, const float* background, const float* means3D, const float* shs,
-                     const float* colors_precomp, const float* opacities, const float* scales, const float* rotations,
-                     const float* viewmatrix, const float* projmatrix, const float* campos, float* out_color,
-                     float* out_others, int32_t* radii, void* geom_buffer, void* binning_buffer, void* image_buffer,
-                     int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream_) {
+int sr_forward(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels, const float* means3D,
+               const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
+               const float* rotations, const float* features, int32_t F, int64_t features_stride, const float* viewmatrix,
+               const float* projmatrix, const float* campos, float* out_color, int64_t out_color_stride,
+               float* out_features, int64_t out_features_stride, float* out_others, int32_t* radii, void* geom_buffer,
+               void* binning_buffer, void* image_buffer, int64_t capacity, uint32_t* num_rendered_dev,
+               uint32_t* num_rendered_host, void* stream_) {
     (void)projmatrix;   // only feeds dead code in the reference (auxiliary.h:170-172)
-    return forward_batch(f, b, background, means3D, shs, colors_precomp, opacities, scales, rotations, viewmatrix, campos,
-                         out_color, 0, out_others, radii, geom_buffer, binning_buffer, image_buffer, capacity, num_rendered_dev,
-                         num_rendered_host, stream_, nullptr);
-}
-
-int sr_forward_batch_features(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
-                              const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
-                              const float* scales, const float* rotations, const float* features, int32_t F,
-                              int64_t features_stride, const float* viewmatrix, const float* projmatrix, const float* campos,
-                              float* out_color, int64_t out_color_stride, float* out_features, int64_t out_features_stride,
-                              float* out_others, int32_t* radii, void* geom_buffer, void* binning_buffer, void* image_buffer,
-                              int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream_) {
-    (void)projmatrix;
     if (F == 0) {
         if (int rc = check_no_features(f, features, bg_channels, out_color_stride)) return rc;
-        return sr_forward_batch(f, b, background, means3D, shs, colors_precomp, opacities, scales, rotations, viewmatrix,
-                                projmatrix, campos, out_color, out_others, radii, geom_buffer, binning_buffer, image_buffer,
-                                capacity, num_rendered_dev, num_rendered_host, stream_);
+        return forward_batch(f, b, background, means3D, shs, colors_precomp, opacities, scales, rotations, viewmatrix, campos,
+                             out_color, 0, out_others, radii, geom_buffer, binning_buffer, image_buffer, capacity,
+                             num_rendered_dev, num_rendered_host, stream_, nullptr);
     }
     if (int rc = check_features(f, F, bg_channels, features, features_stride)) return rc;
     FeatArgs ft{};
@@ -291,17 +280,6 @@ int sr_forward_batch_features(const sr_frame* f, const sr_batch* b, const float*
     return forward_batch(f, b, background, means3D, shs, colors_precomp, opacities, scales, rotations, viewmatrix, campos,
                          out_color, out_color_stride, out_others, radii, geom_buffer, binning_buffer, image_buffer, capacity,
                          num_rendered_dev, num_rendered_host, stream_, &ft);
-}
-
-int sr_forward(const sr_frame* f, const float* background, const float* means3D, const float* shs,
-               const float* colors_precomp, const float* opacities, const float* scales, const float* rotations,
-               const float* viewmatrix, const float* projmatrix, const float* campos, float* out_color,
-               float* out_others, int32_t* radii, void* geom_buffer, void* binning_buffer, void* image_buffer,
-               int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream_) {
-    const sr_batch one = {1, 0u, 0, 0, 0, 0, 0, 0};
-    return sr_forward_batch(f, &one, background, means3D, shs, colors_precomp, opacities, scales, rotations, viewmatrix,
-                            projmatrix, campos, out_color, out_others, radii, geom_buffer, binning_buffer, image_buffer,
-                            capacity, num_rendered_dev, num_rendered_host, stream_);
 }
 
 static int backward_batch(const sr_frame* f, const sr_batch* b, const float* background, const float* means3D, const float* shs,
@@ -381,37 +359,22 @@ static int backward_batch(const sr_frame* f, const sr_batch* b, const float* bac
     return 0;
 }
 
-int sr_backward_batch(const sr_frame* f, const sr_batch* b, const float* background, const float* means3D, const float* shs,
-                      const float* colors_precomp, const float* scales, const float* rotations, const float* viewmatrix,
-                      const float* projmatrix, const float* campos, const int32_t* radii, const float* dL_dout_color,
-                      const float* dL_dout_others, const float* grad_scale, void* geom_buffer, void* binning_buffer,
-                      void* image_buffer, int64_t capacity, float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity,
-                      float* dL_dmeans3D, float* dL_dtransMat, float* dL_dsh, float* dL_dscales, float* dL_drotations,
-                      void* stream_) {
-    (void)projmatrix;
-    return backward_batch(f, b, background, means3D, shs, colors_precomp, scales, rotations, viewmatrix, campos, radii,
-                          dL_dout_color, 0, dL_dout_others, grad_scale, geom_buffer, binning_buffer, image_buffer, capacity,
-                          dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales, dL_drotations,
-                          stream_, nullptr);
-}
-
-int sr_backward_batch_features(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
-                               const float* means3D, const float* shs, const float* colors_precomp, const float* scales,
-                               const float* rotations, const float* features, int32_t F, int64_t features_stride,
-                               const float* viewmatrix, const float* projmatrix, const float* campos, const int32_t* radii,
-                               const float* dL_dout_color, int64_t dL_dout_color_stride, const float* dL_dout_features,
-                               int64_t dL_dout_features_stride, const float* dL_dout_others, const float* grad_scale,
-                               const float* features_grad_scale, void* geom_buffer, void* binning_buffer, void* image_buffer,
-                               int64_t capacity, float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity,
-                               float* dL_dmeans3D, float* dL_dtransMat, float* dL_dsh, float* dL_dscales,
-                               float* dL_drotations, float* dL_dfeatures, void* stream_) {
+int sr_backward(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels, const float* means3D,
+                const float* shs, const float* colors_precomp, const float* scales, const float* rotations,
+                const float* features, int32_t F, int64_t features_stride, const float* viewmatrix, const float* projmatrix,
+                const float* campos, const int32_t* radii, const float* dL_dout_color, int64_t dL_dout_color_stride,
+                const float* dL_dout_features, int64_t dL_dout_features_stride, const float* dL_dout_others,
+                const float* grad_scale, const float* features_grad_scale, void* geom_buffer, void* binning_buffer,
+                void* image_buffer, int64_t capacity, float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity,
+                float* dL_dmeans3D, float* dL_dtransMat, float* dL_dsh, float* dL_dscales, float* dL_drotations,
+                float* dL_dfeatures, void* stream_) {
     (void)projmatrix;
     if (F == 0) {
         if (int rc = check_no_features(f, features, bg_channels, dL_dout_color_stride)) return rc;
-        return sr_backward_batch(f, b, background, means3D, shs, colors_precomp, scales, rotations, viewmatrix, projmatrix,
-                                 campos, radii, dL_dout_color, dL_dout_others, grad_scale, geom_buffer, binning_buffer,
-                                 image_buffer, capacity, dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat,
-                                 dL_dsh, dL_dscales, dL_drotations, stream_);
+        return backward_batch(f, b, background, means3D, shs, colors_precomp, scales, rotations, viewmatrix, campos, radii,
+                              dL_dout_color, 0, dL_dout_others, grad_scale, geom_buffer, binning_buffer, image_buffer,
+                              capacity, dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales,
+                              dL_drotations, stream_, nullptr);
     }
     if (int rc = check_features(f, F, bg_channels, features, features_stride)) return rc;
     FeatArgs ft{};
@@ -426,19 +389,6 @@ int sr_backward_batch_features(const sr_frame* f, const sr_batch* b, const float
                           dL_dout_color, dL_dout_color_stride, dL_dout_others, grad_scale, geom_buffer, binning_buffer,
                           image_buffer, capacity, dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh,
                           dL_dscales, dL_drotations, stream_, &ft);
-}
-
-int sr_backward(const sr_frame* f, const float* background, const float* means3D, const float* shs,
-                const float* colors_precomp, const float* scales, const float* rotations, const float* viewmatrix,
-                const float* projmatrix, const float* campos, const int32_t* radii, const float* dL_dout_color,
-                const float* dL_dout_others, void* geom_buffer, void* binning_buffer, void* image_buffer,
-                int64_t capacity, float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D,
-                float* dL_dtransMat, float* dL_dsh, float* dL_dscales, float* dL_drotations, void* stream_) {
-    const sr_batch one = {1, 0u, 0, 0, 0, 0, 0, 0};
-    return sr_backward_batch(f, &one, background, means3D, shs, colors_precomp, scales, rotations, viewmatrix, projmatrix,
-                             campos, radii, dL_dout_color, dL_dout_others, nullptr, geom_buffer, binning_buffer, image_buffer,
-                             capacity, dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales,
-                             dL_drotations, stream_);
 }
 
 int sr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,

@@ -11,7 +11,7 @@
 //
 // The losses are scalars whose gradient with respect to the rasterizer's outputs is analytic, so ONE kernel computes the
 // four loss terms (block reduction + 4 atomics per block) and writes dL/dcolor and dL/dallmap directly; the rasterizer
-// backward consumes them (times the upstream scalar, sr_backward_batch's grad_scale).  The surf_normal stencil is
+// backward consumes them (times the upstream scalar, sr_backward's grad_scale).  The surf_normal stencil is
 // handled as a gather: a block evaluates the stencils of its 32x8 tile plus a one-pixel ring once each into shared memory
 // and every pixel picks up its four neighbours' results, so there are no atomics on image data and the result is
 // deterministic.  Batched: blockIdx.z = frame.

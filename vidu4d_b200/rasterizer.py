@@ -218,16 +218,149 @@ def _as_float(x) -> float:
     return float(x.item()) if torch.is_tensor(x) else float(x)
 
 
+_STRIDED = ("means3D", "sh", "colors", "opacity", "scales", "rotations")     # sr_batch's per-surfel strides, in its order
+
+
+def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, scales, rotations, features, viewmatrix,
+             projmatrix, campos, H, W, degree, tan_fovx, tan_fovy, scale_modifier, prefiltered, debug, concat=True):
+    """The one sr_forward call behind every _C forward: M frames, F = 0 without features.  The caller has validated the
+    inputs and made them contiguous float32 CUDA tensors; `strides` gives the floats between consecutive frames of each
+    per-surfel input (absent = shared).  The outputs get a leading frame dimension iff frame_dim.  In sync mode an
+    overflowed call is re-run with a larger instance buffer; in nosync mode the status words join _pending.
+    Returns (num_rendered (list of M ints, or -1 in nosync mode), out_color, out_others, radii, geom, binning, img,
+    out_feat): with concat, out_color holds 3+F planes per frame and out_feat is the view of the last F; None when F = 0."""
+    lib = _capi.load()
+    dev = means3D.device
+    P, N = int(means3D.shape[-2]), H * W
+    Msh = int(sh.shape[-2]) if sh is not None and sh.numel() != 0 else 0
+    F = int(features.shape[-1]) if features is not None else 0
+    lead = (M,) if frame_dim else ()
+    fr = _capi.SrFrame(P, int(degree), Msh, W, H, _as_float(tan_fovx), _as_float(tan_fovy), float(scale_modifier),
+                       int(bool(prefiltered)), int(bool(debug)), 0)
+    bt = _capi.SrBatch(M, 0, *(strides.get(k, 0) for k in _STRIDED))
+    with torch.cuda.device(dev):
+        if F and concat:
+            out_color = torch.empty(lead + (3 + F, H, W), dtype=torch.float32, device=dev)
+            out_feat = out_color[..., 3:, :, :]
+            cstride = fstride = (3 + F) * N
+        else:
+            out_color = torch.empty(lead + (3, H, W), dtype=torch.float32, device=dev)
+            out_feat = torch.empty(lead + (F, H, W), dtype=torch.float32, device=dev) if F else None
+            cstride, fstride = 3 * N, F * N
+        out_others = torch.empty(lead + (8, H, W), dtype=torch.float32, device=dev)
+        radii = torch.empty(lead + (P,), dtype=torch.int32, device=dev)
+        geom = torch.empty((M * lib.sr_geom_bytes(P),), dtype=torch.uint8, device=dev)
+        img = torch.empty((M * lib.sr_image_bytes(W, H),), dtype=torch.uint8, device=dev)
+        nr_dev = torch.empty((M, 2), dtype=torch.int32, device=dev)
+        stream = torch.cuda.current_stream(dev)
+        key = (dev.index, W, H)
+        cap = _pick_capacity(key, P)
+        while True:
+            binning = torch.empty((M * lib.sr_binning_bytes(cap, W, H),), dtype=torch.uint8, device=dev)
+            nosync = (not _sync_mode) and key in _cap_hint
+            host = _host_slot(M) if nosync else torch.empty((M, 2), dtype=torch.int32, pin_memory=True)
+            # an overflow re-run below re-runs the feature pass too
+            rc = lib.sr_forward(
+                C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh), _ptr(colors),
+                _ptr(opacity), _ptr(scales), _ptr(rotations), _ptr(features), F, strides.get("features", 0),
+                _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), out_color.data_ptr(), cstride, _ptr(out_feat), fstride,
+                out_others.data_ptr(), _ptr(radii), geom.data_ptr(), binning.data_ptr(), img.data_ptr(), cap,
+                nr_dev.data_ptr(), host.data_ptr(), stream.cuda_stream)
+            _capi.check(rc, "sr_forward")
+            if nosync:
+                _pending.append((host, key, cap, stream))
+                if len(_pending) > _MAX_PENDING:
+                    check_overflow()      # an unchecked backlog must not grow without bound (nor hide dropped frames)
+                num_rendered = -1
+                break
+            stream.synchronize()
+            words = host.tolist()
+            num_rendered = [r for r, _ in words]
+            status = 0
+            for _, s in words:
+                status |= s
+            _cap_hint[key] = max(_cap_hint.get(key, 0), max(num_rendered)) if not _sync_mode else max(num_rendered)
+            if status & _capi.SR_STATUS_PREFILTER:
+                raise RuntimeError("Point is filtered although prefiltered is set. This shouldn't happen!")
+            if status & _capi.SR_STATUS_OVERFLOW:
+                cap = _round_cap(int(max(num_rendered) * 1.1) + 4096)
+                continue
+            break
+    return num_rendered, out_color, out_others, radii, geom, binning, img, out_feat
+
+
+def _backward(M, frame_dim, strides, background, means3D, sh, colors, scales, rotations, features, viewmatrix, projmatrix,
+              campos, radii, dL_dout_color, dL_dout_features, dL_dout_others, geomBuffer, binningBuffer, imageBuffer, degree,
+              tan_fovx, tan_fovy, scale_modifier, debug, grad_scale=None, features_grad_scale=None, sum_shared=False,
+              want_transmat=True, outs=None):
+    """The one sr_backward call behind every _C backward; none when P = 0, whose gradients are zero-filled.  Inputs as
+    for _forward; strides["opacity"] is the forward's opacity stride.  The feature planes' gradient is dL_dout_features,
+    or the tail of dL_dout_color when that is None.  Each gradient is (M,P,.), or (P,.) without frame_dim and, under
+    sum_shared, for an input the frames share.  Returns (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D,
+    dL_dtransMat, dL_dsh, dL_dscales, dL_drotations), and dL_dfeatures ninth when there are features."""
+    lib = _capi.load()
+    dev = means3D.device
+    P, H, W = int(means3D.shape[-2]), int(dL_dout_color.shape[-2]), int(dL_dout_color.shape[-1])
+    N = H * W
+    Msh = int(sh.shape[-2]) if sh is not None and sh.numel() != 0 else 0
+    F = int(features.shape[-1]) if features is not None else 0
+    cstride, fstride, dfeat_ptr = 3 * N, F * N, _ptr(dL_dout_features) if F else None
+    if F and dL_dout_features is None:
+        cstride = fstride = (3 + F) * N
+        dfeat_ptr = dL_dout_color.data_ptr() + 3 * N * 4
+    lead = (M,) if frame_dim else ()
+    with torch.cuda.device(dev):
+        alloc = torch.empty if P > 0 else torch.zeros
+
+        def mk(name, *tail):   # (P,.) when the input is shared and the kernel sums over frames
+            shape = ((P,) if (sum_shared and M > 1 and strides.get(name, 0) == 0) else lead + (P,)) + tail
+            o = outs.get("dL_d" + name) if outs else None
+            if o is not None:
+                if (o.numel() != int(torch.Size(shape).numel()) or not o.is_contiguous() or o.dtype != torch.float32
+                        or o.data_ptr() % 16 != 0):
+                    raise RuntimeError(f"outs['dL_d{name}'] must be a contiguous, 16-byte aligned float32 tensor of {shape}")
+                return o.view(shape)
+            return alloc(shape, dtype=torch.float32, device=dev)
+        dL_dmeans2D = alloc(lead + (P, 3), dtype=torch.float32, device=dev)
+        dL_dmeans3D, dL_dcolors, dL_dopacity = mk("means3D", 3), mk("colors", 3), mk("opacity", 1)
+        dL_dtransMat = alloc(lead + (P, 9), dtype=torch.float32, device=dev) \
+            if (want_transmat or (M == 1 and not sum_shared)) else None
+        dL_dsh, dL_dscales, dL_drotations = mk("sh", Msh, 3), mk("scales", 2), mk("rotations", 4)
+        dL_dfeatures = mk("features", F) if F else None
+        if P > 0:
+            cap = _capacity_from_bytes(int(binningBuffer.numel()) // M, W, H)
+            fr = _capi.SrFrame(P, int(degree), Msh, W, H, _as_float(tan_fovx), _as_float(tan_fovy),
+                               float(scale_modifier), 0, int(bool(debug)), 0)
+            bt = _capi.SrBatch(M, _capi.SR_BATCH_SUM_SHARED if sum_shared else 0, *(strides.get(k, 0) for k in _STRIDED))
+            gs = fgs = None
+            if grad_scale is not None:
+                gs = grad_scale.to(device=dev, dtype=torch.float32).reshape(()).contiguous()
+            if F and features_grad_scale is not None:
+                fgs = features_grad_scale.to(device=dev, dtype=torch.float32).reshape(()).contiguous()
+            rc = lib.sr_backward(
+                C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh), _ptr(colors),
+                _ptr(scales), _ptr(rotations), _ptr(features), F, strides.get("features", 0), _ptr(viewmatrix),
+                _ptr(projmatrix), _ptr(campos), _ptr(radii), _ptr(dL_dout_color), cstride, dfeat_ptr, fstride,
+                _ptr(dL_dout_others), _ptr(gs), _ptr(fgs), geomBuffer.data_ptr(), binningBuffer.data_ptr(),
+                imageBuffer.data_ptr(), cap, dL_dmeans2D.data_ptr(), dL_dcolors.data_ptr(), dL_dopacity.data_ptr(),
+                dL_dmeans3D.data_ptr(), _ptr(dL_dtransMat), _ptr(dL_dsh), dL_dscales.data_ptr(), dL_drotations.data_ptr(),
+                _ptr(dL_dfeatures), torch.cuda.current_stream(dev).cuda_stream)
+            _capi.check(rc, "sr_backward")
+    grads = (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales, dL_drotations)
+    return grads + (dL_dfeatures,) if F else grads
+
+
 class _CNamespace:
-    """Stand-in for the reference's pybind module `_C` with the same three entry points."""
+    """Stand-in for the reference's pybind module `_C` with the same three entry points, plus the feature and batched
+    variants.  Each checks its arguments' shapes and hands _forward / _backward normalised inputs."""
 
     @staticmethod
     def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier,
                             transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height,
                             image_width, sh, degree, campos, prefiltered, debug):
-        return _forward_single(background, means3D, colors, opacity, scales, rotations, scale_modifier, transMat_precomp,
-                               viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
-                               prefiltered, debug, None)
+        return _CNamespace.rasterize_gaussians_features(
+            background, means3D, colors, opacity, scales, rotations, scale_modifier, transMat_precomp, viewmatrix,
+            projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, debug, None)
 
     @staticmethod
     def rasterize_gaussians_features(background, means3D, colors, opacity, scales, rotations, scale_modifier,
@@ -235,36 +368,7 @@ class _CNamespace:
                                      image_width, sh, degree, campos, prefiltered, debug, features):
         """rasterize_gaussians plus per-surfel features (P,F), 1 <= F <= 32 (not in the reference): out_color is
         (3+F,H,W) -- the colour planes, then F feature planes composited with the colour's weights over a background of
-        background[3:] (background of 3+F values) or zeros (background of 3)."""
-        return _forward_single(background, means3D, colors, opacity, scales, rotations, scale_modifier, transMat_precomp,
-                               viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
-                               prefiltered, debug, features)
-
-    @staticmethod
-    def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier,
-                                     transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
-                                     dL_dout_color, dL_dout_others, sh, degree, campos, geomBuffer, R,
-                                     binningBuffer, imageBuffer, debug):
-        return _backward_single(background, means3D, radii, colors, scales, rotations, scale_modifier, transMat_precomp,
-                                viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, dL_dout_others, sh, degree,
-                                campos, geomBuffer, R, binningBuffer, imageBuffer, debug, None)
-
-    @staticmethod
-    def rasterize_gaussians_features_backward(background, means3D, radii, colors, scales, rotations, scale_modifier,
-                                              transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
-                                              dL_dout_color, dL_dout_others, sh, degree, campos, geomBuffer, R,
-                                              binningBuffer, imageBuffer, debug, features):
-        """Backward of rasterize_gaussians_features: dL_dout_color is (3+F,H,W); returns the eight gradients of
-        rasterize_gaussians_backward and dL_dfeatures (P,F)."""
-        return _backward_single(background, means3D, radii, colors, scales, rotations, scale_modifier, transMat_precomp,
-                                viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, dL_dout_others, sh, degree,
-                                campos, geomBuffer, R, binningBuffer, imageBuffer, debug, features)
-
-    @staticmethod
-    def _forward_single(background, means3D, colors, opacity, scales, rotations, scale_modifier,
-                        transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height,
-                        image_width, sh, degree, campos, prefiltered, debug, features):
-        lib = _capi.load()
+        background[3:] (background of 3+F values) or zeros (background of 3).  features=None is rasterize_gaussians."""
         if means3D.ndim != 2 or means3D.shape[1] != 3:
             raise RuntimeError("means3D must have dimensions (num_points, 3)")
         if scales.ndim != 2 or scales.shape[1] != 2:
@@ -274,84 +378,41 @@ class _CNamespace:
         if transMat_precomp is not None and transMat_precomp.numel() != 0:
             raise RuntimeError("precomputed transMat / cov3D is not supported (the reference path for it is "
                                "broken: forward.cu:214-218 leaves the normal uninitialised)")
-        dev = means3D.device
-        P, H, W = int(means3D.shape[0]), int(image_height), int(image_width)
         background = _f32c(background, "background"); means3D = _f32c(means3D, "means3D")
         colors = _f32c(colors, "colors"); opacity = _f32c(opacity, "opacity")
         scales = _f32c(scales, "scales"); rotations = _f32c(rotations, "rotations")
         viewmatrix = _f32c(viewmatrix, "viewmatrix"); projmatrix = _f32c(projmatrix, "projmatrix")
         sh = _f32c(sh, "sh"); campos = _f32c(campos, "campos")
-        M = int(sh.shape[1]) if sh is not None and sh.numel() != 0 else 0
-        F = 0
         if features is not None:
-            F = _check_features(features, P, background)
+            _check_features(features, int(means3D.shape[0]), background)
             features = _f32c(features, "features")
-
-        with torch.cuda.device(dev):
-            out_color = torch.empty((3 + F, H, W), dtype=torch.float32, device=dev)
-            out_others = torch.empty((8, H, W), dtype=torch.float32, device=dev)
-            radii = torch.empty((P,), dtype=torch.int32, device=dev)
-            geom = torch.empty((lib.sr_geom_bytes(P),), dtype=torch.uint8, device=dev)
-            img = torch.empty((lib.sr_image_bytes(W, H),), dtype=torch.uint8, device=dev)
-            nr_dev = torch.empty((2,), dtype=torch.int32, device=dev)
-            stream = torch.cuda.current_stream(dev)
-            key = (dev.index, W, H)
-            cap = _pick_capacity(key, P)
-            while True:
-                fr = _capi.SrFrame(P, int(degree), M, W, H, _as_float(tan_fovx), _as_float(tan_fovy),
-                                   float(scale_modifier), int(bool(prefiltered)), int(bool(debug)), 0)
-                binning = torch.empty((lib.sr_binning_bytes(cap, W, H),), dtype=torch.uint8, device=dev)
-                nosync = (not _sync_mode) and key in _cap_hint
-                host = _host_slot() if nosync else torch.empty((1, 2), dtype=torch.int32, pin_memory=True)
-                if F:
-                    N = H * W
-                    bt = _capi.SrBatch(1, 0, 0, 0, 0, 0, 0, 0)
-                    rc = lib.sr_forward_batch_features(
-                        C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh),
-                        _ptr(colors), _ptr(opacity), _ptr(scales), _ptr(rotations), _ptr(features), F, 0,
-                        _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), out_color.data_ptr(), (3 + F) * N,
-                        out_color.data_ptr() + 3 * N * 4, (3 + F) * N, out_others.data_ptr(), _ptr(radii),
-                        geom.data_ptr(), binning.data_ptr(), img.data_ptr(), cap, nr_dev.data_ptr(), host.data_ptr(),
-                        stream.cuda_stream)
-                    _capi.check(rc, "sr_forward_batch_features")
-                else:
-                    rc = lib.sr_forward(
-                        C.byref(fr), _ptr(background), _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(opacity),
-                        _ptr(scales), _ptr(rotations), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos),
-                        out_color.data_ptr(), out_others.data_ptr(), _ptr(radii), geom.data_ptr(),
-                        binning.data_ptr(), img.data_ptr(), cap, nr_dev.data_ptr(), host.data_ptr(),
-                        stream.cuda_stream)
-                    _capi.check(rc, "sr_forward")
-                if nosync:
-                    _pending.append((host, key, cap, stream))
-                    if len(_pending) > _MAX_PENDING:
-                        check_overflow()      # an unchecked backlog must not grow without bound (nor hide dropped frames)
-                    num_rendered = -1
-                    break
-                stream.synchronize()
-                num_rendered, status = int(host[0, 0]), int(host[0, 1])
-                _cap_hint[key] = max(_cap_hint.get(key, 0), num_rendered) if not _sync_mode else num_rendered
-                if status & _capi.SR_STATUS_PREFILTER:
-                    raise RuntimeError("Point is filtered although prefiltered is set. This shouldn't happen!")
-                if status & _capi.SR_STATUS_OVERFLOW:
-                    cap = _round_cap(int(num_rendered * 1.1) + 4096)
-                    continue
-                break
-        return num_rendered, out_color, out_others, radii, geom, binning, img
+        # one frame: M = 1 explicitly (viewmatrix is (4,4), campos (3,)), outputs without a frame dimension
+        out = _forward(1, False, {}, background, means3D, sh, colors, opacity, scales, rotations, features, viewmatrix,
+                       projmatrix, campos, int(image_height), int(image_width), degree, tan_fovx, tan_fovy, scale_modifier,
+                       prefiltered, debug)
+        return (-1 if out[0] == -1 else out[0][0],) + out[1:7]
 
     @staticmethod
-    def _backward_single(background, means3D, radii, colors, scales, rotations, scale_modifier,
-                         transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
-                         dL_dout_color, dL_dout_others, sh, degree, campos, geomBuffer, R,
-                         binningBuffer, imageBuffer, debug, features):
-        lib = _capi.load()
-        dev = means3D.device
-        P = int(means3D.shape[0])
-        H, W = int(dL_dout_color.shape[1]), int(dL_dout_color.shape[2])
-        F = 0
+    def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier,
+                                     transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+                                     dL_dout_color, dL_dout_others, sh, degree, campos, geomBuffer, R,
+                                     binningBuffer, imageBuffer, debug):
+        return _CNamespace.rasterize_gaussians_features_backward(
+            background, means3D, radii, colors, scales, rotations, scale_modifier, transMat_precomp, viewmatrix,
+            projmatrix, tan_fovx, tan_fovy, dL_dout_color, dL_dout_others, sh, degree, campos, geomBuffer, R,
+            binningBuffer, imageBuffer, debug, None)
+
+    @staticmethod
+    def rasterize_gaussians_features_backward(background, means3D, radii, colors, scales, rotations, scale_modifier,
+                                              transMat_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+                                              dL_dout_color, dL_dout_others, sh, degree, campos, geomBuffer, R,
+                                              binningBuffer, imageBuffer, debug, features):
+        """Backward of rasterize_gaussians_features: dL_dout_color is (3+F,H,W); returns the eight gradients of
+        rasterize_gaussians_backward and dL_dfeatures (P,F).  features=None is rasterize_gaussians_backward."""
         if features is not None:
-            F = _check_features(features, P, background)
+            F = _check_features(features, int(means3D.shape[0]), background)
             features = _f32c(features, "features")
+            H, W = int(dL_dout_color.shape[1]), int(dL_dout_color.shape[2])
             if tuple(dL_dout_color.shape) != (3 + F, H, W):
                 raise RuntimeError(f"dL_dout_color must be (3+F,H,W) = {(3 + F, H, W)}, got {tuple(dL_dout_color.shape)}")
         background = _f32c(background, "background"); means3D = _f32c(means3D, "means3D")
@@ -359,45 +420,9 @@ class _CNamespace:
         viewmatrix = _f32c(viewmatrix, "viewmatrix"); projmatrix = _f32c(projmatrix, "projmatrix")
         sh = _f32c(sh, "sh"); campos = _f32c(campos, "campos")
         dL_dout_color = _f32c(dL_dout_color, "dL_dout_color"); dL_dout_others = _f32c(dL_dout_others, "dL_dout_others")
-        M = int(sh.shape[1]) if sh is not None and sh.numel() != 0 else 0
-        with torch.cuda.device(dev):
-            mk = (lambda *s: torch.empty(s, dtype=torch.float32, device=dev)) if P > 0 else \
-                 (lambda *s: torch.zeros(s, dtype=torch.float32, device=dev))
-            dL_dmeans3D, dL_dmeans2D, dL_dcolors = mk(P, 3), mk(P, 3), mk(P, 3)
-            dL_dopacity, dL_dtransMat, dL_dsh = mk(P, 1), mk(P, 9), mk(P, M, 3)
-            dL_dscales, dL_drotations = mk(P, 2), mk(P, 4)
-            dL_dfeatures = mk(P, F) if F else None
-            if P > 0 and F:
-                cap = _capacity_from_bytes(int(binningBuffer.numel()), W, H)
-                fr = _capi.SrFrame(P, int(degree), M, W, H, _as_float(tan_fovx), _as_float(tan_fovy),
-                                   float(scale_modifier), 0, int(bool(debug)), 0)
-                N = H * W
-                bt = _capi.SrBatch(1, 0, 0, 0, 0, 0, 0, 0)
-                rc = lib.sr_backward_batch_features(
-                    C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh),
-                    _ptr(colors), _ptr(scales), _ptr(rotations), _ptr(features), F, 0, _ptr(viewmatrix),
-                    _ptr(projmatrix), _ptr(campos), _ptr(radii), _ptr(dL_dout_color), (3 + F) * N,
-                    dL_dout_color.data_ptr() + 3 * N * 4, (3 + F) * N, _ptr(dL_dout_others), None, None,
-                    geomBuffer.data_ptr(), binningBuffer.data_ptr(), imageBuffer.data_ptr(), cap, dL_dmeans2D.data_ptr(),
-                    dL_dcolors.data_ptr(), dL_dopacity.data_ptr(), dL_dmeans3D.data_ptr(), dL_dtransMat.data_ptr(),
-                    dL_dsh.data_ptr() if M > 0 else None, dL_dscales.data_ptr(), dL_drotations.data_ptr(),
-                    dL_dfeatures.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-                _capi.check(rc, "sr_backward_batch_features")
-            elif P > 0:
-                cap = _capacity_from_bytes(int(binningBuffer.numel()), W, H)
-                fr = _capi.SrFrame(P, int(degree), M, W, H, _as_float(tan_fovx), _as_float(tan_fovy),
-                                   float(scale_modifier), 0, int(bool(debug)), 0)
-                rc = lib.sr_backward(
-                    C.byref(fr), _ptr(background), _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(scales),
-                    _ptr(rotations), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), _ptr(radii),
-                    _ptr(dL_dout_color), _ptr(dL_dout_others), geomBuffer.data_ptr(), binningBuffer.data_ptr(),
-                    imageBuffer.data_ptr(), cap, dL_dmeans2D.data_ptr(), dL_dcolors.data_ptr(),
-                    dL_dopacity.data_ptr(), dL_dmeans3D.data_ptr(), dL_dtransMat.data_ptr(),
-                    dL_dsh.data_ptr() if M > 0 else None, dL_dscales.data_ptr(), dL_drotations.data_ptr(),
-                    torch.cuda.current_stream(dev).cuda_stream)
-                _capi.check(rc, "sr_backward")
-        grads = (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales, dL_drotations)
-        return grads + (dL_dfeatures,) if F else grads
+        return _backward(1, False, {}, background, means3D, sh, colors, scales, rotations, features, viewmatrix, projmatrix,
+                         campos, radii, dL_dout_color, None, dL_dout_others, geomBuffer, binningBuffer, imageBuffer, degree,
+                         tan_fovx, tan_fovy, scale_modifier, debug)
 
     # ---- batched entry points (SURVEY.md 8(f) N1): M frames in one launch set -------------------------------------
     @staticmethod
@@ -411,83 +436,19 @@ class _CNamespace:
         features (P,F) shared or (M,P,F) per frame, 1 <= F <= 32: an eighth element, the (M,F,H,W) feature planes, is
         returned; with concat=True out_color is (M,3+F,H,W) and the feature planes are its view [:, 3:], with concat=False
         the two are separate tensors."""
-        lib = _capi.load()
         M = int(viewmatrix.shape[0])
         if viewmatrix.ndim != 3 or viewmatrix.shape[1:] != (4, 4) or campos.shape != (M, 3):
             raise RuntimeError("batched cameras: viewmatrix must be (M,4,4) and campos (M,3)")
-        dev = means3D.device
-        H, W = int(image_height), int(image_width)
         background = _f32c(background, "background"); viewmatrix = _f32c(viewmatrix, "viewmatrix")
         projmatrix = _f32c(projmatrix, "projmatrix"); campos = _f32c(campos, "campos")
-        F = 0
         if features is not None:
-            F = _check_features(features, int(means3D.shape[-2]), background, batched=True)
+            _check_features(features, int(means3D.shape[-2]), background, batched=True)
         ins, strides = _batch_inputs(M, means3D=(means3D, (3,)), sh=(sh, None), colors=(colors, (3,)), opacity=(opacity, (1,)),
                                      scales=(scales, (2,)), rotations=(rotations, (4,)), features=(features, None))
-        means3D, sh, colors, opacity, scales, rotations = (ins[k] for k in ("means3D", "sh", "colors", "opacity", "scales", "rotations"))
-        features = ins["features"]
-        P = int(means3D.shape[-2])
-        Msh = int(sh.shape[-2]) if sh is not None and sh.numel() != 0 else 0
-        bt = _capi.SrBatch(M, 0, strides["means3D"], strides["sh"], strides["colors"], strides["opacity"], strides["scales"],
-                           strides["rotations"])
-        N = H * W
-        with torch.cuda.device(dev):
-            if F and concat:
-                out_color = torch.empty((M, 3 + F, H, W), dtype=torch.float32, device=dev)
-                out_feat = out_color[:, 3:]
-                cstride = fstride = (3 + F) * N
-            else:
-                out_color = torch.empty((M, 3, H, W), dtype=torch.float32, device=dev)
-                out_feat = torch.empty((M, F, H, W), dtype=torch.float32, device=dev) if F else None
-                cstride, fstride = 3 * N, F * N
-            out_others = torch.empty((M, 8, H, W), dtype=torch.float32, device=dev)
-            radii = torch.empty((M, P), dtype=torch.int32, device=dev)
-            geom = torch.empty((M * lib.sr_geom_bytes(P),), dtype=torch.uint8, device=dev)
-            img = torch.empty((M * lib.sr_image_bytes(W, H),), dtype=torch.uint8, device=dev)
-            nr_dev = torch.empty((M, 2), dtype=torch.int32, device=dev)
-            stream = torch.cuda.current_stream(dev)
-            key = (dev.index, W, H)
-            cap = _pick_capacity(key, P)
-            while True:
-                fr = _capi.SrFrame(P, int(degree), Msh, W, H, _as_float(tan_fovx), _as_float(tan_fovy),
-                                   float(scale_modifier), int(bool(prefiltered)), int(bool(debug)), 0)
-                binning = torch.empty((M * lib.sr_binning_bytes(cap, W, H),), dtype=torch.uint8, device=dev)
-                nosync = (not _sync_mode) and key in _cap_hint
-                host = _host_slot(M) if nosync else torch.empty((M, 2), dtype=torch.int32, pin_memory=True)
-                if F:    # an overflow re-run below re-runs the feature pass too
-                    rc = lib.sr_forward_batch_features(
-                        C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh),
-                        _ptr(colors), _ptr(opacity), _ptr(scales), _ptr(rotations), _ptr(features), F, strides["features"],
-                        _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), out_color.data_ptr(), cstride,
-                        out_feat.data_ptr(), fstride, out_others.data_ptr(), _ptr(radii), geom.data_ptr(),
-                        binning.data_ptr(), img.data_ptr(), cap, nr_dev.data_ptr(), host.data_ptr(), stream.cuda_stream)
-                    _capi.check(rc, "sr_forward_batch_features")
-                else:
-                    rc = lib.sr_forward_batch(
-                        C.byref(fr), C.byref(bt), _ptr(background), _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(opacity),
-                        _ptr(scales), _ptr(rotations), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos),
-                        out_color.data_ptr(), out_others.data_ptr(), _ptr(radii), geom.data_ptr(),
-                        binning.data_ptr(), img.data_ptr(), cap, nr_dev.data_ptr(), host.data_ptr(), stream.cuda_stream)
-                    _capi.check(rc, "sr_forward_batch")
-                if nosync:
-                    _pending.append((host, key, cap, stream))
-                    num_rendered = -1
-                    break
-                stream.synchronize()
-                num_rendered = [int(v) for v in host[:, 0]]
-                status = 0
-                for v in host[:, 1]:
-                    status |= int(v)
-                _cap_hint[key] = max(_cap_hint.get(key, 0), max(num_rendered)) if not _sync_mode else max(num_rendered)
-                if status & _capi.SR_STATUS_PREFILTER:
-                    raise RuntimeError("Point is filtered although prefiltered is set. This shouldn't happen!")
-                if status & _capi.SR_STATUS_OVERFLOW:
-                    cap = _round_cap(int(max(num_rendered) * 1.1) + 4096)
-                    continue
-                break
-        if F:
-            return num_rendered, out_color, out_others, radii, geom, binning, img, out_feat
-        return num_rendered, out_color, out_others, radii, geom, binning, img
+        out = _forward(M, True, strides, background, ins["means3D"], ins["sh"], ins["colors"], ins["opacity"], ins["scales"],
+                       ins["rotations"], ins["features"], viewmatrix, projmatrix, campos, int(image_height),
+                       int(image_width), degree, tan_fovx, tan_fovy, scale_modifier, prefiltered, debug, concat)
+        return out if features is not None else out[:7]
 
     @staticmethod
     def rasterize_gaussians_backward_batch(background, means3D, radii, colors, scales, rotations, scale_modifier, viewmatrix,
@@ -508,90 +469,27 @@ class _CNamespace:
         separate dL_dout_features (M,F,H,W) (then dL_dout_color is (M,3,H,W)); features_grad_scale (optional 0-d device
         tensor) multiplies it instead of grad_scale.  A ninth gradient, dL_dfeatures, is returned: (M,P,F), or (P,F) for
         shared features with sum_shared=True."""
-        lib = _capi.load()
         M = int(viewmatrix.shape[0])
-        dev = means3D.device
         H, W = int(dL_dout_color.shape[-2]), int(dL_dout_color.shape[-1])
-        N = H * W
         background = _f32c(background, "background"); viewmatrix = _f32c(viewmatrix, "viewmatrix")
         projmatrix = _f32c(projmatrix, "projmatrix"); campos = _f32c(campos, "campos")
         dL_dout_color = _f32c(dL_dout_color, "dL_dout_color"); dL_dout_others = _f32c(dL_dout_others, "dL_dout_others")
-        F = 0
         if features is not None:
             F = _check_features(features, int(means3D.shape[-2]), background, batched=True)
             if dL_dout_features is None:
                 if tuple(dL_dout_color.shape) != (M, 3 + F, H, W):
                     raise RuntimeError(f"dL_dout_color must be (M,3+F,H,W) = {(M, 3 + F, H, W)} without dL_dout_features")
-                cstride = fstride = (3 + F) * N
-                dfeat_ptr = dL_dout_color.data_ptr() + 3 * N * 4
             else:
                 dL_dout_features = _f32c(dL_dout_features, "dL_dout_features")
                 if tuple(dL_dout_features.shape) != (M, F, H, W) or tuple(dL_dout_color.shape) != (M, 3, H, W):
                     raise RuntimeError("dL_dout_color must be (M,3,H,W) and dL_dout_features (M,F,H,W)")
-                cstride, fstride, dfeat_ptr = 3 * N, F * N, dL_dout_features.data_ptr()
         ins, strides = _batch_inputs(M, means3D=(means3D, (3,)), sh=(sh, None), colors=(colors, (3,)),
                                      scales=(scales, (2,)), rotations=(rotations, (4,)), features=(features, None))
-        means3D, sh, colors, scales, rotations = (ins[k] for k in ("means3D", "sh", "colors", "scales", "rotations"))
-        features = ins["features"]
-        P = int(means3D.shape[-2])
-        Msh = int(sh.shape[-2]) if sh is not None and sh.numel() != 0 else 0
-        op_stride = 0 if (opacity_shared or M == 1) else P
-        bt = _capi.SrBatch(M, _capi.SR_BATCH_SUM_SHARED if sum_shared else 0, strides["means3D"], strides["sh"], strides["colors"],
-                           op_stride, strides["scales"], strides["rotations"])
-        with torch.cuda.device(dev):
-            mk0 = (lambda *s: torch.empty(s, dtype=torch.float32, device=dev)) if P > 0 else \
-                  (lambda *s: torch.zeros(s, dtype=torch.float32, device=dev))
-
-            def mk(name, shared, *tail):   # (M,P,.) per frame, or (P,.) when the input is shared and the kernel sums over frames
-                shape = (P,) + tail if (sum_shared and shared and M > 1) else (M, P) + tail
-                o = outs.get(name) if outs else None
-                if o is not None:
-                    if (o.numel() != int(torch.Size(shape).numel()) or not o.is_contiguous() or o.dtype != torch.float32
-                            or o.data_ptr() % 16 != 0):
-                        raise RuntimeError(f"outs[{name!r}] must be a contiguous, 16-byte aligned float32 tensor of {shape}")
-                    return o.view(shape)
-                return mk0(*shape)
-            dL_dmeans2D = mk0(M, P, 3)
-            dL_dmeans3D, dL_dcolors = mk("dL_dmeans3D", strides["means3D"] == 0, 3), mk("dL_dcolors", strides["colors"] == 0, 3)
-            dL_dopacity = mk("dL_dopacity", op_stride == 0, 1)
-            dL_dtransMat = mk0(M, P, 9) if (want_transmat or (M == 1 and not sum_shared)) else None
-            dL_dsh = mk("dL_dsh", strides["sh"] == 0, Msh, 3)
-            dL_dscales, dL_drotations = mk("dL_dscales", strides["scales"] == 0, 2), mk("dL_drotations", strides["rotations"] == 0, 4)
-            dL_dfeatures = mk("dL_dfeatures", strides["features"] == 0, F) if F else None
-            if P > 0:
-                cap = _capacity_from_bytes(int(binningBuffer.numel()) // M, W, H)
-                fr = _capi.SrFrame(P, int(degree), Msh, W, H, _as_float(tan_fovx), _as_float(tan_fovy),
-                                   float(scale_modifier), 0, int(bool(debug)), 0)
-                gs = None
-                if grad_scale is not None:
-                    gs = grad_scale.to(device=dev, dtype=torch.float32).reshape(()).contiguous()
-            if P > 0 and F:
-                fgs = None
-                if features_grad_scale is not None:
-                    fgs = features_grad_scale.to(device=dev, dtype=torch.float32).reshape(()).contiguous()
-                rc = lib.sr_backward_batch_features(
-                    C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh),
-                    _ptr(colors), _ptr(scales), _ptr(rotations), _ptr(features), F, strides["features"], _ptr(viewmatrix),
-                    _ptr(projmatrix), _ptr(campos), _ptr(radii), _ptr(dL_dout_color), cstride, dfeat_ptr, fstride,
-                    _ptr(dL_dout_others), gs.data_ptr() if gs is not None else None,
-                    fgs.data_ptr() if fgs is not None else None, geomBuffer.data_ptr(), binningBuffer.data_ptr(),
-                    imageBuffer.data_ptr(), cap, dL_dmeans2D.data_ptr(), dL_dcolors.data_ptr(), dL_dopacity.data_ptr(),
-                    dL_dmeans3D.data_ptr(), dL_dtransMat.data_ptr() if dL_dtransMat is not None else None,
-                    dL_dsh.data_ptr() if Msh > 0 else None, dL_dscales.data_ptr(), dL_drotations.data_ptr(),
-                    dL_dfeatures.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-                _capi.check(rc, "sr_backward_batch_features")
-            elif P > 0:
-                rc = lib.sr_backward_batch(
-                    C.byref(fr), C.byref(bt), _ptr(background), _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(scales),
-                    _ptr(rotations), _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), _ptr(radii),
-                    _ptr(dL_dout_color), _ptr(dL_dout_others), gs.data_ptr() if gs is not None else None,
-                    geomBuffer.data_ptr(), binningBuffer.data_ptr(), imageBuffer.data_ptr(), cap,
-                    dL_dmeans2D.data_ptr(), dL_dcolors.data_ptr(), dL_dopacity.data_ptr(), dL_dmeans3D.data_ptr(),
-                    dL_dtransMat.data_ptr() if dL_dtransMat is not None else None, dL_dsh.data_ptr() if Msh > 0 else None,
-                    dL_dscales.data_ptr(), dL_drotations.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-                _capi.check(rc, "sr_backward_batch")
-        grads = (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales, dL_drotations)
-        return grads + (dL_dfeatures,) if F else grads
+        strides["opacity"] = 0 if (opacity_shared or M == 1) else int(ins["means3D"].shape[-2])
+        return _backward(M, True, strides, background, ins["means3D"], ins["sh"], ins["colors"], ins["scales"],
+                         ins["rotations"], ins["features"], viewmatrix, projmatrix, campos, radii, dL_dout_color,
+                         dL_dout_features, dL_dout_others, geomBuffer, binningBuffer, imageBuffer, degree, tan_fovx,
+                         tan_fovy, scale_modifier, debug, grad_scale, features_grad_scale, sum_shared, want_transmat, outs)
 
     @staticmethod
     def mark_visible(means3D, viewmatrix, projmatrix):
@@ -610,8 +508,6 @@ class _CNamespace:
 
 
 _C = _CNamespace()
-_forward_single = _CNamespace._forward_single
-_backward_single = _CNamespace._backward_single
 
 
 def cpu_deep_copy_tuple(input_tuple):
