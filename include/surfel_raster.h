@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SR_ABI_VERSION 7
+#define SR_ABI_VERSION 8
 
 #if defined(__GNUC__)
 #define SR_API __attribute__((visibility("default")))
@@ -303,6 +303,38 @@ SR_API int sr_reproj_loss_backward(int32_t M, int32_t H, int32_t W, int32_t B, i
                                    const float* Kmat, const float* hxy, const float* mask, const float* is_detected,
                                    const float* scale, const float* g_loss, float* g_xyz_matched, float* g_delta,
                                    float* g_tables, void* stream);
+
+/*
+ * Stage 3's deformation-cycle regulariser with the backward warp's skin-entropy and delta-skin terms (csrc/cycle.cu,
+ * DESIGN.md section 3.5c).  Replaces lab4d/nnutils/deformable_gaussian.py:1272-1275,1517-1574 (cycle_loss: :738-764
+ * cam_to_field, then lab4d/nnutils/warping.py:378-444 SkinningWarp.forward with backward=True, then apply_qt_to_gaussian
+ * and |x_cycled - x|), and lab4d/engine/model.py:850-853 (reg_deform_cyc, reg_delta_skin, reg_skin_entropy) with their
+ * :994-1012 reduction (v[v > 0].mean() times the term's weight).
+ *   xyz[P*3]: canonical surfels;  xyz_cam[M*P*3]: the same surfels in every frame's camera space (sr_bob_warp_forward's
+ *   output);  o2b_q[M*B*4], o2b_t[M*B*3]: object->bone transform of each frame's t_articulation;  inv_gauss[B*3] =
+ *   exp(-log_gauss);  delta[M*P*B] or NULL: the frame-conditioned delta skinning term;  se3_r, se3_d[M*B*4]: per frame
+ *   and bone dual quaternion rest_articulation o t_articulation^-1;  cam_q[M*4], cam_t[M*3]: field2cam;
+ *   weights[3] DEVICE floats {reg_deform_cyc, reg_delta_skin, reg_skin_entropy} read at run time.
+ * Per frame m and surfel p: v = {|x_cycled - xyz[p]|, mean_b delta^2 (0 without delta), logsumexp - max of the logits}.
+ * Forward writes terms[M*3] (each frame's share of each weighted term), counts[M*3] (values > 0), scale[3] =
+ * weights / (total count) (0 where the count is 0) and loss[1] = sum of terms.  Backward takes scale and g_loss[1]
+ * (DEVICE float); a value > 0 gets g_loss * scale_k, a value = 0 none.  It writes g_xyz_cam[M*P*3], g_xyz[P*3],
+ * g_delta[M*P*B] (if non-NULL) and g_tables[sr_cycle_loss_table_floats(B, M)] = gradients of {o2b_q, o2b_t, inv_gauss,
+ * se3_r, se3_d, cam_q, cam_t} in that order (zeroed inside).
+ * SR_EINVAL: a NULL required pointer, P < 0, M < 1, B outside [1, 64], tables of (B, M) beyond 200 KB of shared memory
+ * (twice sr_cycle_loss_table_floats floats; at B = 64 that is M <= 26), g_delta without delta.
+ * No call allocates or synchronises with the host.
+ */
+SR_API size_t sr_cycle_loss_table_floats(int32_t B, int32_t M);
+SR_API int sr_cycle_loss_forward(int32_t P, int32_t B, int32_t M, const float* xyz, const float* xyz_cam, const float* o2b_q,
+                                 const float* o2b_t, const float* inv_gauss, const float* delta, const float* se3_r,
+                                 const float* se3_d, const float* cam_q, const float* cam_t, const float* weights, float* terms,
+                                 uint32_t* counts, float* scale, float* loss, void* stream);
+SR_API int sr_cycle_loss_backward(int32_t P, int32_t B, int32_t M, const float* xyz, const float* xyz_cam, const float* o2b_q,
+                                  const float* o2b_t, const float* inv_gauss, const float* delta, const float* se3_r,
+                                  const float* se3_d, const float* cam_q, const float* cam_t, const float* scale,
+                                  const float* g_loss, float* g_xyz_cam, float* g_xyz, float* g_delta, float* g_tables,
+                                  void* stream);
 
 /*
  * Optimizer-side kernels over the FLAT surfel parameter buffer (SURVEY.md section 8(f) row N4): the Adam step of every

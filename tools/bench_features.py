@@ -16,9 +16,15 @@ statements in torch (global_match's score matrix + topk, oracle/warp_oracle.py i
 positive mean), alternating in one process, at 256x256 x 2 frames with 300 K surfels; and the fused path alone at
 512x512 x 8 frames, where the torch path's score matrix alone is 17 GB.
 
+--cycle times Stage 3's deformation-cycle regulariser: the fused forward warp (bob_warp) -> cycle loss -> backward at
+300 K surfels, B = 25 with delta, M = 2 and M = 8, one CUDA graph, L2 flushed between steps, with the cycle loss fused
+(csrc/cycle.cu) against the same statements in torch (tests/cycle_model.py cycle_values in fp32 and the sync-free
+positive means), alternating in one process.
+
     python tools/bench_features.py --features 4 22 32 [--steps 20 --warmup 5]
     python tools/bench_features.py --losses [--steps 20 --warmup 5]
     python tools/bench_features.py --reproj [--steps 20 --warmup 5]
+    python tools/bench_features.py --cycle [--steps 20 --warmup 5]
 """
 import argparse
 import json
@@ -43,7 +49,10 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--losses", action="store_true")
     ap.add_argument("--reproj", action="store_true")
+    ap.add_argument("--cycle", action="store_true")
     args = ap.parse_args()
+    if args.cycle:
+        return bench_cycle(args)
     if args.losses:
         return bench_losses(args)
     if args.reproj:
@@ -358,6 +367,122 @@ def bench_reproj(args):
                           "peak_mem_mb_above_inputs": peak, "kernel_ms_per_launch": kern,
                           "launches_per_step_fused": steps["fused"].launches, "outputs": compare, "steps": args.steps,
                           "statistic": "median step time", "gpu": gpu}), flush=True)
+        del steps, bodies, d
+        torch.cuda.empty_cache()
+    RZ.set_sync_mode(True)
+    RZ._pending.clear()
+
+
+CYCLE_LEAVES = ("xyz", "rot", "rest_q", "rest_t", "log_gauss", "art_q", "art_t", "cam_q", "cam_t", "delta", "cdelta")
+
+
+def _cycle_inputs(M, P, B, dev, seed=0):
+    from tests.golden.make_warp_golden import make_inputs
+    d = {k: v.to(dev).requires_grad_(True) for k, v in make_inputs(seed, P, B, M, True).items()}
+    g = torch.Generator(device=dev).manual_seed(seed)
+    d["cdelta"] = (torch.randn((M, P, B), device=dev, generator=g).clamp(min=0) * 0.1).requires_grad_(True)
+    d["w"] = torch.tensor([0.01, 5e-3, 5e-4], device=dev)
+    return d
+
+
+def _cycle_warp(d):
+    from vidu4d_b200.warp import bob_warp
+    rest, art = _q2dq(d["rest_q"], d["rest_t"]), _q2dq(d["art_q"], d["art_t"])
+    xc, _, _ = bob_warp(d["xyz"], d["rot"], rest, art, d["log_gauss"], (d["cam_q"], d["cam_t"]), d["delta"])
+    return xc, rest, art
+
+
+def _cycle_fused(d):
+    from vidu4d_b200.warp import cycle_loss
+    xc, rest, art = _cycle_warp(d)
+    out = cycle_loss(d["xyz"], xc, rest, art, d["log_gauss"], (d["cam_q"], d["cam_t"]), d["cdelta"], weights=d["w"])
+    return out["loss"], out["terms"].sum(0)
+
+
+def _cycle_torch(d):
+    """Today's caller path after the fused warp: deformable_gaussian.py:1517-1574 as tests/cycle_model.py's statements
+    in fp32, and model.py's reduction as the sync-free positive mean."""
+    from tests import cycle_model as cm
+    xc, rest, art = _cycle_warp(d)
+    vals = cm.cycle_values(d["xyz"], xc, rest, art, torch.exp(-d["log_gauss"]), (d["cam_q"], d["cam_t"]), d["cdelta"])
+    terms = []
+    for k, v in enumerate(vals):
+        on = (v > 0).to(v.dtype)
+        terms.append(d["w"][k] * (v * on).sum() / on.sum().clamp(min=1.0))
+    terms = torch.stack(terms)
+    return terms.sum(), terms
+
+
+def bench_cycle(args):
+    from vidu4d_b200 import _capi, rasterizer as RZ
+    from vidu4d_b200.graph import GraphedStep
+    assert torch.cuda.is_available(), "this measurement needs a GPU"
+    dev = torch.device("cuda:0")
+    _capi.load()
+    gpu = _gpu_name()
+    P, B = args.surfels, 25
+    flush = torch.empty((256 << 20,), dtype=torch.uint8, device=dev)
+    for M in (2, 8):
+        d = _cycle_inputs(M, P, B, dev)
+        fns = {"fused": _cycle_fused, "torch": _cycle_torch}
+
+        def make_body(fn):
+            def body():
+                for k in CYCLE_LEAVES:
+                    d[k].grad = None
+                fn(d)[0].backward()
+            return body
+        bodies = {k: make_body(f) for k, f in fns.items()}
+        peak = {}
+        for k, b in bodies.items():                                  # eager peak memory above the inputs
+            torch.cuda.synchronize()
+            base = torch.cuda.memory_allocated()
+            torch.cuda.reset_peak_memory_stats()
+            b()
+            torch.cuda.synchronize()
+            peak[k] = round((torch.cuda.max_memory_allocated() - base) / 2**20, 1)
+        grads = {}
+        for k, b in bodies.items():                                  # the two paths on the same inputs
+            b()
+            grads[k] = {n: d[n].grad.clone() for n in ("xyz", "art_q", "log_gauss", "cdelta")}
+        with torch.no_grad():
+            lf, tf = _cycle_fused(d)
+            lt, tt = _cycle_torch(d)
+        compare = {"loss_rel_diff": float((lf - lt).abs() / lt.abs()),
+                   "terms_rel_diff": [float(v) for v in ((tf - tt).abs() / tt.abs().clamp(min=1e-30))],
+                   "grad_max_abs_diff_over_max": {n: float((grads["fused"][n] - grads["torch"][n]).abs().max()
+                                                           / grads["torch"][n].abs().max()) for n in grads["fused"]}}
+        steps = {k: GraphedStep(b, device=dev) for k, b in bodies.items()}
+        for s_ in steps.values():
+            s_()
+            for _ in range(args.warmup):
+                s_(check=False)
+        torch.cuda.synchronize()
+        ms = {k: [] for k in steps}
+        for i in range(args.steps):
+            for k, s_ in steps.items():
+                flush.fill_(i & 255)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record(); s_.graph.replay(); b.record()
+                b.synchronize()
+                ms[k].append(a.elapsed_time(b))
+        RZ._pending.clear()
+        RZ.set_sync_mode(True)
+        bodies["fused"]()
+        torch.cuda.synchronize()
+        _capi.get_profile()
+        _capi.set_profiling(True)
+        for _ in range(5):
+            bodies["fused"]()
+        prof = _capi.get_profile()
+        _capi.set_profiling(False)
+        kern = {k: round(v["ms"] / max(v["count"], 1), 4) for k, v in prof.items()
+                if k in ("bob_warp_fwd", "bob_warp_bwd", "cycle_fwd", "cycle_scale", "cycle_bwd")}
+        print(json.dumps({"workload": "bob_warp -> cycle loss -> backward (fwd + bwd)", "surfels": P, "frames": M, "bones": B,
+                          "delta": True, "ms_per_step": {k: round(float(np.median(v)), 4) for k, v in ms.items()},
+                          "peak_mem_mb_above_inputs": peak, "kernel_ms_per_launch": kern,
+                          "launches_per_step": {k: s_.launches for k, s_ in steps.items()}, "outputs": compare,
+                          "steps": args.steps, "statistic": "median step time", "gpu": gpu}), flush=True)
         del steps, bodies, d
         torch.cuda.empty_cache()
     RZ.set_sync_mode(True)

@@ -16,7 +16,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libsurfel_raster.so")
 SOURCES = ["api.cu", "preprocess.cu", "sort.cu", "composite_fwd.cu", "composite_tile.cu", "composite_feat.cu", "surfel_bwd.cu",
-           "postprocess.cu", "loss.cu", "warp.cu", "match.cu", "optim.cu", "knn.cu"]
+           "postprocess.cu", "loss.cu", "warp.cu", "match.cu", "cycle.cu", "optim.cu", "knn.cu"]
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "composite_common.cuh"), os.path.join(CSRC, "post_common.cuh"),
            os.path.join(CSRC, "warp_common.cuh"),
            os.path.join(HERE, "..", "include", "surfel_raster.h")]

@@ -356,7 +356,7 @@ reproj_bwd_kernel(const ReprojDims d, const float* __restrict__ xyz_m, const flo
 #pragma unroll
     for (int b = 0; b < BMAX; b++) gw[b] = 0.f;
     blend_vjp<BMAX>(T, B, m, w, anchor, gQR, gQD, gw, g_sr, g_sd);
-    skin_vjp<BMAX>(T, B, x, y, z, w, gw, anchor, nullptr, n, live, lv, g_delta, g_oq, g_ot, g_ig, gxx, gxy, gxz);
+    skin_vjp<BMAX>(T, B, x, y, z, w, gw, anchor, 0.f, n, live, lv, g_delta, nullptr, 0.f, g_oq, g_ot, g_ig, gxx, gxy, gxz);
     if (live) { g_xyz_m[3 * n] = gxx; g_xyz_m[3 * n + 1] = gxy; g_xyz_m[3 * n + 2] = gxz; }
     __syncthreads();
     for (int j = threadIdx.x; j < nt; j += blockDim.x)

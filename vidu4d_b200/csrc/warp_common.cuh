@@ -179,20 +179,20 @@ __device__ __forceinline__ void blend_vjp(const Tables& T, int B, int m, const f
     }
 }
 
-// vjp of the skinning weights of point ps given dL/dw (gw) and dL/dentropy (g_entropy[ps], NULL = 0): softmax, then the
-// Gaussian logits.  Writes dL/ddelta to g_delta[ps*B..] (if non-NULL), adds dL/dx to (gxx, gxy, gxz) and reduces
-// dL/do2b_q, dL/do2b_t, dL/dinv_gauss over the warp into g_oq, g_ot, g_ig.  A dead lane (live = false, lv = 0) takes
-// part with zeros: every lane of the warp must call it.  bob_warp_bwd_kernel keeps its own inline copy of this loop:
-// calling this function there changes that kernel's instruction schedule, which is kept as it was.
+// vjp of the skinning weights of point ps given dL/dw (gw) and dL/dentropy (ge; 0 on a dead lane): softmax, then the
+// Gaussian logits.  Writes dL/ddelta to g_delta[ps*B..] (if non-NULL), plus g_d2 * delta_row[b] where delta also feeds a
+// term in delta^2 (delta_row non-NULL), adds dL/dx to (gxx, gxy, gxz) and reduces dL/do2b_q, dL/do2b_t, dL/dinv_gauss over
+// the warp into g_oq, g_ot, g_ig.  A dead lane (live = false, lv = 0) takes part with zeros: every lane of the warp must
+// call it.  bob_warp_bwd_kernel keeps its own inline copy of this loop: calling this function there changes that kernel's
+// instruction schedule, which is kept as it was.
 template <int BMAX>
 __device__ __forceinline__ void skin_vjp(const Tables& T, int B, float x, float y, float z, const float (&w)[BMAX],
-                                         const float (&gw)[BMAX], int anchor, const float* __restrict__ g_entropy, size_t ps,
-                                         bool live, float lv, float* __restrict__ g_delta, float* g_oq, float* g_ot, float* g_ig,
-                                         float& gxx, float& gxy, float& gxz) {
+                                         const float (&gw)[BMAX], int anchor, float ge, size_t ps, bool live, float lv,
+                                         float* __restrict__ g_delta, const float* __restrict__ delta_row, float g_d2, float* g_oq,
+                                         float* g_ot, float* g_ig, float& gxx, float& gxy, float& gxz) {
     float dotwg = 0.f;
 #pragma unroll
     for (int b = 0; b < BMAX; b++) dotwg += w[b] * gw[b];
-    const float ge = (g_entropy && live) ? g_entropy[ps] : 0.f;
     const int lane = threadIdx.x & 31;
 #pragma unroll
     for (int c3 = 0; c3 < (BMAX + 2) / 3; c3++) {
@@ -206,7 +206,7 @@ __device__ __forceinline__ void skin_vjp(const Tables& T, int B, float x, float 
                 for (int i = 0; i < 10; i++) vals[10 * j + i] = 0.f;
                 if (b < B && b < BMAX) {
                     const float gl = (w[b] * (gw[b] - dotwg) + ge * (w[b] - (b == anchor ? 1.f : 0.f))) * lv;
-                    if (g_delta && live) g_delta[ps * B + b] = -gl;
+                    if (g_delta && live) g_delta[ps * B + b] = delta_row ? g_d2 * __ldg(delta_row + b) - gl : -gl;
                     const Q4 qb = ldq(T.oq + 4 * b);
                     float bx, by, bz;
                     qrot(qb, x, y, z, bx, by, bz);
