@@ -139,146 +139,171 @@ __device__ __forceinline__ void cull_bbox(const float* T, float cx, float cy, fl
     by = (uint32_t)fy0 | ((uint32_t)fy1 << 16);
 }
 
+// The block's SH coefficients (rows x 3M floats, contiguous) are staged in shared memory with coalesced 128-bit loads;
+// each thread then reads its own padded row (stride 3M+1: conflict-free) instead of 48 scalar loads at a 192-byte lane
+// stride.
+__device__ __forceinline__ void stage_sh(float* shbuf, const float* __restrict__ gsrc, int rows, int M3) {
+    const int stride = M3 + 1, total = rows * M3;
+    if ((M3 & 3) == 0) {
+        const float4* g4 = reinterpret_cast<const float4*>(gsrc);
+        for (int i = threadIdx.x; i < total / 4; i += 256) {
+            const float4 v = __ldg(g4 + i);
+            const int e = i * 4, r = e / M3, col = e - r * M3;
+            float* d = shbuf + r * stride + col;
+            d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
+        }
+    } else {
+        for (int i = threadIdx.x; i < total; i += 256) { const int r = i / M3; shbuf[r * stride + (i - r * M3)] = __ldg(gsrc + i); }
+    }
+}
+
+// computeTransMat's rotation matrix R (row-major) of the quaternion q = (w,x,y,z); glm names .x=w .y=x .z=y .w=z
+__device__ __forceinline__ void rot_matrix(float4 q, float R[9]) {
+    const float n2 = ff(q.z, q.z, ff(q.y, q.y, ff(q.w, q.w, fm(q.x, q.x))));
+    const float s = rsqrtf(n2);
+    const float w = fm(q.x, s), x = fm(q.y, s), y = fm(q.z, s), z = fm(q.w, s);
+    const float wz = fm(w, z), wy = fm(w, y), wx = fm(w, x), yy = fm(y, y), zz = fm(z, z);
+    float t;
+    t = fa(yy, zz);        R[0] = fa(1.f, -fa(t, t));
+    t = ff(x, y, wz);      R[1] = fa(t, t);
+    t = ff(x, z, -wy);     R[2] = fa(t, t);
+    t = ff(x, y, -wz);     R[3] = fa(t, t);
+    t = ff(x, x, zz);      R[4] = fa(1.f, -fa(t, t));
+    t = ff(y, z, wx);      R[5] = fa(t, t);
+    t = ff(x, z, wy);      R[6] = fa(t, t);
+    t = ff(y, z, -wx);     R[7] = fa(t, t);
+    t = ff(x, x, yy);      R[8] = fa(1.f, -fa(t, t));
+}
+
+// One thread owns one surfel for every frame of the batch (grid = ceil(P/256) blocks).  An input whose frame stride is 0
+// is shared by all frames and is read once per launch: at the headline the SH table alone is larger than L2, so a
+// per-frame block grid re-read it from HBM for every frame.  Per-frame inputs are read inside the frame loop.  Each
+// frame runs the same operations in the same order as a single-frame launch, so its outputs are bit-identical to one.
 __global__ void __launch_bounds__(256)
-preprocess_fwd_kernel(const CamParams c_, const FrameStrides fs, const float* __restrict__ means3D, const float* __restrict__ shs,
+preprocess_fwd_kernel(const CamParams c0, const FrameStrides fs, const float* __restrict__ means3D, const float* __restrict__ shs,
                       const float* __restrict__ colors_precomp, const float* __restrict__ opacities,
                       const float2* __restrict__ scales, const float4* __restrict__ rotations,
                       int* __restrict__ radii, float4* __restrict__ srec, float* __restrict__ depths,
                       uint32_t* __restrict__ tiles_touched, uint8_t* __restrict__ clamped_out,
                       uint32_t* __restrict__ block_sums, uint32_t* __restrict__ status, int prefiltered) {
-    const int f = blockIdx.y;                       // frame of the batch
-    const CamParams c = cam_of_frame(c_, fs, f);
-    means3D = fr(means3D, fs.means3D, f); shs = fr(shs, fs.shs, f); colors_precomp = fr(colors_precomp, fs.colors, f);
-    opacities = fr(opacities, fs.opac, f); scales = fr(scales, fs.scales, f); rotations = fr(rotations, fs.rots, f);
-    radii = fr(radii, fs.radii, f); srec = fr(srec, fs.geom, f); depths = fr(depths, fs.geom, f);
-    tiles_touched = fr(tiles_touched, fs.geom, f); clamped_out = fr(clamped_out, fs.geom, f);
-    block_sums = fr(block_sums, fs.geom, f); status = fr(status, fs.nr, f);
-    // The block's SH coefficients (256 x 3M floats, contiguous) are staged in shared memory with coalesced 128-bit
-    // loads; each thread then reads its own padded row (stride 3M+1: conflict-free) instead of 48 scalar loads at a
-    // 192-byte lane stride.
     extern __shared__ float shbuf[];
+    __shared__ uint32_t wsum[2][8];                 // per-warp tile counts, double-buffered over frames
     const int idx = blockIdx.x * 256 + threadIdx.x;
-    const int M3 = 3 * c.M, stride = M3 + 1;
-    if (colors_precomp == nullptr) {
-        const int base = blockIdx.x * 256;
-        const int total = min(256, c.P - base) * M3;
-        const float* gsrc = shs + (size_t)base * M3;
-        if ((M3 & 3) == 0) {
-            const float4* g4 = reinterpret_cast<const float4*>(gsrc);
-            for (int i = threadIdx.x; i < total / 4; i += 256) {
-                const float4 v = __ldg(g4 + i);
-                const int e = i * 4, r = e / M3, col = e - r * M3;
-                float* d = shbuf + r * stride + col;
-                d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
-            }
-        } else {
-            for (int i = threadIdx.x; i < total; i += 256) { const int r = i / M3; shbuf[r * stride + (i - r * M3)] = __ldg(gsrc + i); }
-        }
+    const bool live = idx < c0.P;
+    const int M3 = 3 * c0.M, stride = M3 + 1;
+    const int rows = min(256, c0.P - (int)blockIdx.x * 256);
+    const bool use_sh = colors_precomp == nullptr;
+    if (use_sh && fs.shs == 0) {
+        stage_sh(shbuf, shs + (size_t)blockIdx.x * 256 * M3, rows, M3);
         __syncthreads();
     }
-    uint32_t touched = 0;
-    int radius_i = 0;
-    if (idx < c.P) {
-        const View V = load_view(c.vm);
-        const float px = __ldg(means3D + 3 * (size_t)idx), py = __ldg(means3D + 3 * (size_t)idx + 1),
-                    pz = __ldg(means3D + 3 * (size_t)idx + 2);
-        const float depth = view_z(V, px, py, pz);
-        if (depth > 0.2f) {
-            // ---- computeTransMat ----
-            const float4 q = __ldg(rotations + idx);   // (w,x,y,z); glm names .x=w .y=x .z=y .w=z
-            const float2 sc = __ldg(scales + idx);
-            const float n2 = ff(q.z, q.z, ff(q.y, q.y, ff(q.w, q.w, fm(q.x, q.x))));
-            const float s = rsqrtf(n2);
-            const float w = fm(q.x, s), x = fm(q.y, s), y = fm(q.z, s), z = fm(q.w, s);
-            const float wz = fm(w, z), wy = fm(w, y), wx = fm(w, x), yy = fm(y, y), zz = fm(z, z);
-            float t;
-            t = fa(yy, zz);        const float R0 = fa(1.f, -fa(t, t));
-            t = ff(x, y, wz);      const float R1 = fa(t, t);
-            t = ff(x, z, -wy);     const float R2 = fa(t, t);
-            t = ff(x, y, -wz);     const float R3 = fa(t, t);
-            t = ff(x, x, zz);      const float R4 = fa(1.f, -fa(t, t));
-            t = ff(y, z, wx);      const float R5 = fa(t, t);
-            t = ff(x, z, wy);      const float R6 = fa(t, t);
-            t = ff(y, z, -wx);     const float R7 = fa(t, t);
-            t = ff(x, x, yy);      const float R8 = fa(1.f, -fa(t, t));
-            const float3 pv0 = w_mul(V, make_float3(px, py, pz));
-            const float3 pv = make_float3(fa(pv0.x, V.m[12]), fa(pv0.y, V.m[13]), fa(pv0.z, V.m[14]));
-            const float3 M0 = w_mul(V, make_float3(fm(R0, sc.x), fm(R1, sc.x), fm(R2, sc.x)));
-            const float3 M1 = w_mul(V, make_float3(fm(R3, sc.y), fm(R4, sc.y), fm(R5, sc.y)));
-            float3 tn = w_mul(V, make_float3(R6, R7, R8));
-            const float cosv = ff(-pv.z, tn.z, ff(pv.y, -tn.y, -fm(pv.x, tn.x)));
-            if (cosv != 0.0f) {
-                const float mult = cosv > 0.f ? 1.f : -1.f;
-                tn.x = fm(tn.x, mult); tn.y = fm(tn.y, mult); tn.z = fm(tn.z, mult);
-                float T[9];
-                T[0] = ff(M0.z, c.cx, fm(c.focal_x, M0.x));
-                T[1] = ff(M1.z, c.cx, fm(c.focal_x, M1.x));
-                T[2] = ff(pv.z, c.cx, fm(c.focal_x, pv.x));
-                T[3] = ff(M0.z, c.cy, fm(c.focal_y, M0.y));
-                T[4] = ff(M1.z, c.cy, fm(c.focal_y, M1.y));
-                T[5] = ff(pv.z, c.cy, fm(c.focal_y, pv.y));
-                T[6] = M0.z; T[7] = M1.z; T[8] = pv.z;
-                // ---- computeAABB ----
-                const float d = ff(-T[8], T[8], ff(T[6], T[6], fm(T[7], T[7])));
-                if (d != 0.0f) {
-                    const float r = __fdiv_rn(1.0f, d);
-                    const float cxp = ff(fm(T[2], T[8]), -r, ff(fm(T[1], T[7]), r, fm(fm(T[0], T[6]), r)));
-                    const float cyp = ff(fm(T[5], T[8]), -r, ff(fm(T[4], T[7]), r, fm(fm(T[3], T[6]), r)));
-                    const float nqx = ff(fm(T[2], T[2]), r, -ff(fm(T[1], T[1]), r, fm(fm(T[0], T[0]), r)));
-                    const float nqy = ff(fm(T[5], T[5]), r, -ff(fm(T[4], T[4]), r, fm(fm(T[3], T[3]), r)));
-                    const float ex = __fsqrt_rn(fmaxf(0.0f, ff(cxp, cxp, nqx)));
-                    const float ey = __fsqrt_rn(fmaxf(0.0f, ff(cyp, cyp, nqy)));
-                    // forward.cu:239 -- FilterSize is a double literal: max / *3 / ceil happen in double
-                    double e = (double)fmaxf(ex, ey);
-                    e = fmax(e, 0.7071067811865476);
-                    const float radius = (float)ceil(3.0 * e);
-                    const int ri = (int)radius;
-                    uint2 rmin, rmax;
-                    get_rect(cxp, cyp, ri, c.tiles_x, c.tiles_y, rmin, rmax);
-                    const uint32_t area = (rmax.x - rmin.x) * (rmax.y - rmin.y);
-                    if (area != 0) {
-                        uint32_t cl = 0;
-                        float3 rgb;
-                        if (colors_precomp == nullptr) {
-                            rgb = sh_to_rgb(c.D, c.M, make_float3(px, py, pz), c.campos, shbuf + threadIdx.x * stride, cl);
-                        } else {
-                            rgb = make_float3(__ldg(colors_precomp + 3 * (size_t)idx), __ldg(colors_precomp + 3 * (size_t)idx + 1),
-                                              __ldg(colors_precomp + 3 * (size_t)idx + 2));
+    float px = 0.f, py = 0.f, pz = 0.f, R[9], opac = 0.f;
+    float2 sc = make_float2(0.f, 0.f);
+    if (live) {
+        if (fs.means3D == 0) { px = __ldg(means3D + 3 * (size_t)idx); py = __ldg(means3D + 3 * (size_t)idx + 1); pz = __ldg(means3D + 3 * (size_t)idx + 2); }
+        if (fs.rots == 0) rot_matrix(__ldg(rotations + idx), R);
+        if (fs.scales == 0) sc = __ldg(scales + idx);
+        if (fs.opac == 0) opac = __ldg(opacities + idx);
+    }
+    for (int f = 0; f < fs.frames; f++) {
+        const CamParams c = cam_of_frame(c0, fs, f);
+        if (use_sh && fs.shs != 0) {
+            // the previous frame's __syncthreads below already ordered every read of shbuf before this overwrite
+            stage_sh(shbuf, fr(shs, fs.shs, f) + (size_t)blockIdx.x * 256 * M3, rows, M3);
+            __syncthreads();
+        }
+        uint32_t touched = 0;
+        if (live) {
+            int radius_i = 0;
+            if (fs.means3D != 0) {
+                const float* m = fr(means3D, fs.means3D, f) + 3 * (size_t)idx;
+                px = __ldg(m); py = __ldg(m + 1); pz = __ldg(m + 2);
+            }
+            const View V = load_view(c.vm);
+            const float depth = view_z(V, px, py, pz);
+            if (depth > 0.2f) {
+                // ---- computeTransMat ----
+                if (fs.rots != 0) rot_matrix(__ldg(fr(rotations, fs.rots, f) + idx), R);
+                if (fs.scales != 0) sc = __ldg(fr(scales, fs.scales, f) + idx);
+                const float3 pv0 = w_mul(V, make_float3(px, py, pz));
+                const float3 pv = make_float3(fa(pv0.x, V.m[12]), fa(pv0.y, V.m[13]), fa(pv0.z, V.m[14]));
+                const float3 M0 = w_mul(V, make_float3(fm(R[0], sc.x), fm(R[1], sc.x), fm(R[2], sc.x)));
+                const float3 M1 = w_mul(V, make_float3(fm(R[3], sc.y), fm(R[4], sc.y), fm(R[5], sc.y)));
+                float3 tn = w_mul(V, make_float3(R[6], R[7], R[8]));
+                const float cosv = ff(-pv.z, tn.z, ff(pv.y, -tn.y, -fm(pv.x, tn.x)));
+                if (cosv != 0.0f) {
+                    const float mult = cosv > 0.f ? 1.f : -1.f;
+                    tn.x = fm(tn.x, mult); tn.y = fm(tn.y, mult); tn.z = fm(tn.z, mult);
+                    float T[9];
+                    T[0] = ff(M0.z, c.cx, fm(c.focal_x, M0.x));
+                    T[1] = ff(M1.z, c.cx, fm(c.focal_x, M1.x));
+                    T[2] = ff(pv.z, c.cx, fm(c.focal_x, pv.x));
+                    T[3] = ff(M0.z, c.cy, fm(c.focal_y, M0.y));
+                    T[4] = ff(M1.z, c.cy, fm(c.focal_y, M1.y));
+                    T[5] = ff(pv.z, c.cy, fm(c.focal_y, pv.y));
+                    T[6] = M0.z; T[7] = M1.z; T[8] = pv.z;
+                    // ---- computeAABB ----
+                    const float d = ff(-T[8], T[8], ff(T[6], T[6], fm(T[7], T[7])));
+                    if (d != 0.0f) {
+                        const float r = __fdiv_rn(1.0f, d);
+                        const float cxp = ff(fm(T[2], T[8]), -r, ff(fm(T[1], T[7]), r, fm(fm(T[0], T[6]), r)));
+                        const float cyp = ff(fm(T[5], T[8]), -r, ff(fm(T[4], T[7]), r, fm(fm(T[3], T[6]), r)));
+                        const float nqx = ff(fm(T[2], T[2]), r, -ff(fm(T[1], T[1]), r, fm(fm(T[0], T[0]), r)));
+                        const float nqy = ff(fm(T[5], T[5]), r, -ff(fm(T[4], T[4]), r, fm(fm(T[3], T[3]), r)));
+                        const float ex = __fsqrt_rn(fmaxf(0.0f, ff(cxp, cxp, nqx)));
+                        const float ey = __fsqrt_rn(fmaxf(0.0f, ff(cyp, cyp, nqy)));
+                        // forward.cu:239 -- FilterSize is a double literal: max / *3 / ceil happen in double
+                        double e = (double)fmaxf(ex, ey);
+                        e = fmax(e, 0.7071067811865476);
+                        const float radius = (float)ceil(3.0 * e);
+                        const int ri = (int)radius;
+                        uint2 rmin, rmax;
+                        get_rect(cxp, cyp, ri, c.tiles_x, c.tiles_y, rmin, rmax);
+                        const uint32_t area = (rmax.x - rmin.x) * (rmax.y - rmin.y);
+                        if (area != 0) {
+                            uint32_t cl = 0;
+                            float3 rgb;
+                            if (use_sh) {
+                                rgb = sh_to_rgb(c.D, c.M, make_float3(px, py, pz), c.campos, shbuf + threadIdx.x * stride, cl);
+                            } else {
+                                const float* cp = fr(colors_precomp, fs.colors, f) + 3 * (size_t)idx;
+                                rgb = make_float3(__ldg(cp), __ldg(cp + 1), __ldg(cp + 2));
+                            }
+                            if (fs.opac != 0) opac = __ldg(fr(opacities, fs.opac, f) + idx);
+                            uint32_t bx, by;
+                            cull_bbox(T, cxp, cyp, opac, c.W, c.H, bx, by);
+                            float4* o = fr(srec, fs.geom, f) + (size_t)idx * 5;
+                            o[0] = make_float4(T[0], T[1], T[2], T[3]);
+                            o[1] = make_float4(T[4], T[5], T[6], T[7]);
+                            o[2] = make_float4(T[8], cxp, cyp, opac);
+                            o[3] = make_float4(tn.x, tn.y, tn.z, rgb.x);
+                            o[4] = make_float4(rgb.y, rgb.z, __uint_as_float(bx), __uint_as_float(by));
+                            fr(depths, fs.geom, f)[idx] = depth;
+                            fr(clamped_out, fs.geom, f)[idx] = (uint8_t)cl;
+                            radius_i = ri;
+                            touched = area;
                         }
-                        const float opac = __ldg(opacities + idx);
-                        uint32_t bx, by;
-                        cull_bbox(T, cxp, cyp, opac, c.W, c.H, bx, by);
-                        float4* o = srec + (size_t)idx * 5;
-                        o[0] = make_float4(T[0], T[1], T[2], T[3]);
-                        o[1] = make_float4(T[4], T[5], T[6], T[7]);
-                        o[2] = make_float4(T[8], cxp, cyp, opac);
-                        o[3] = make_float4(tn.x, tn.y, tn.z, rgb.x);
-                        o[4] = make_float4(rgb.y, rgb.z, __uint_as_float(bx), __uint_as_float(by));
-                        depths[idx] = depth;
-                        clamped_out[idx] = (uint8_t)cl;
-                        radius_i = ri;
-                        touched = area;
                     }
                 }
+            } else if (prefiltered) {
+                atomicOr(fr(status, fs.nr, f), 4u);   // the reference __trap()s here (auxiliary.h:177-181)
             }
-        } else if (prefiltered) {
-            atomicOr(status, 4u);   // the reference __trap()s here (auxiliary.h:177-181)
+            fr(radii, fs.radii, f)[idx] = radius_i;
+            fr(tiles_touched, fs.geom, f)[idx] = touched;
         }
-        radii[idx] = radius_i;
-        tiles_touched[idx] = touched;
-    }
-    // block sum of tiles_touched -> block_sums[blockIdx.x]
-    __shared__ uint32_t wsum[8];
-    uint32_t v = touched;
+        // block sum of this frame's tiles_touched -> block_sums[blockIdx.x] of the frame.  Thread 0 reads wsum[f & 1]
+        // before it reaches the next frame's barrier, and nobody writes that half again until the frame after.
+        uint32_t v = touched;
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = v;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        uint32_t tot = 0;
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if ((threadIdx.x & 31) == 0) wsum[f & 1][threadIdx.x >> 5] = v;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            uint32_t tot = 0;
 #pragma unroll
-        for (int i = 0; i < 8; i++) tot += wsum[i];
-        block_sums[blockIdx.x] = tot;
+            for (int i = 0; i < 8; i++) tot += wsum[f & 1][i];
+            fr(block_sums, fs.geom, f)[blockIdx.x] = tot;
+        }
     }
 }
 
@@ -403,7 +428,7 @@ cudaError_t launch_preprocess_fwd(const FwdArgs& a) {
         if (e != cudaSuccess) return e;
     }
     ProfileScope ps("preprocess_fwd", a.stream);
-    preprocess_fwd_kernel<<<dim3(nb, a.fs.frames), 256, smem, a.stream>>>(
+    preprocess_fwd_kernel<<<nb, 256, smem, a.stream>>>(
         a.cam, a.fs, a.means3D, a.shs, a.colors_precomp, a.opacities, (const float2*)a.scales, (const float4*)a.rotations,
         a.radii, (float4*)(a.geom + a.gl.surfel_rec), (float*)(a.geom + a.gl.depths),
         (uint32_t*)(a.geom + a.gl.tiles_touched), (uint8_t*)(a.geom + a.gl.clamped),
