@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SR_ABI_VERSION 8
+#define SR_ABI_VERSION 9
 
 #if defined(__GNUC__)
 #define SR_API __attribute__((visibility("default")))
@@ -357,6 +357,27 @@ SR_API int sr_surfel_compact(int32_t n_groups, const int32_t* width, const int64
 SR_API int64_t sr_knn_cells(int32_t P, const float* bbox_min, const float* bbox_max, float* h_out, int32_t* dims_out);
 SR_API int sr_knn_mean_dist2(int32_t P, const float* points, const float* bbox_min, const float* bbox_max, float* out,
                              int32_t* scratch, void* stream);
+
+/*
+ * Radius outlier filter (csrc/outlier.cu, DESIGN.md section 3.9): Stage 3's periodic
+ * `pcd.remove_radius_outlier(nb_points=20, radius=0.004)` (lab4d/engine/trainer.py:573-588) on the device.
+ *   count_i = #{ j in [0,P) : d2(i,j) < r2 }, j = i included, with
+ *   d2 = ((xi-xj)^2 + (yi-yj)^2) + (zi-zj)^2: coordinates widened to float64, every difference, product and sum rounded
+ *   on its own (no FMA contraction), and r2 = radius * radius in float64.
+ *   keep[i] = count_i > nb_points (1 / 0); counts[i] (nullable) = min(count_i, nb_points + 1).
+ * A point with a NaN or Inf coordinate is nobody's neighbour, not even its own: it is never kept and changes no other
+ * count.  nb_points = 0 keeps every finite point.  This is Open3D's RemoveRadiusOutliers as we understand it (a KD-tree
+ * radius search with a strict < on the squared distance, the query point counted, kept iff the count exceeds nb_points);
+ * it was not checked against Open3D itself.  The two can differ only on pairs at distance exactly `radius`.
+ * points[P*3] (DEVICE float32), keep[P], counts[P]; scratch: DEVICE, at least sr_radius_outlier_scratch_bytes(P) bytes,
+ * which depends on P alone.  Counts are integers, so the result is bit-identical run to run and independent of the
+ * order of the points.  No allocation, no host synchronisation: the call can be captured in a CUDA graph.
+ * SR_EINVAL, before any device work: P < 0, nb_points < 0, radius not finite or <= 0, scratch_bytes below the size
+ * query, a NULL points / keep / scratch.  P = 0 does nothing.
+ */
+SR_API int64_t sr_radius_outlier_scratch_bytes(int32_t P);
+SR_API int sr_radius_outlier_mask(int32_t P, const float* points, double radius, int32_t nb_points, uint8_t* keep,
+                                  int32_t* counts, void* scratch, int64_t scratch_bytes, void* stream);
 
 SR_API int sr_abi_version(void);
 SR_API const char* sr_last_error(void);

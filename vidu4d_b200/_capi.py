@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libsurfel_raster.so")
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 SR_STATUS_OVERFLOW = 1
 SR_STATUS_PREFILTER = 4
 SR_BATCH_SUM_SHARED = 1
@@ -22,6 +22,7 @@ SYMBOLS = (
     "sr_set_profiling", "sr_get_profile", "sr_post_forward", "sr_post_backward", "sr_render_loss_batch", "sr_bob_warp_table_floats", "sr_bob_warp_forward", "sr_bob_warp_backward", "sr_adam_flat", "sr_surfel_compact", "sr_knn_cells", "sr_knn_mean_dist2",
     "sr_feature_loss_batch", "sr_global_match_forward", "sr_global_match_backward", "sr_reproj_loss_forward", "sr_reproj_loss_backward",
     "sr_cycle_loss_table_floats", "sr_cycle_loss_forward", "sr_cycle_loss_backward",
+    "sr_radius_outlier_scratch_bytes", "sr_radius_outlier_mask",
 )
 FEATURES_MAX = 32          # channels per call (SR_FEAT_MAX)
 
@@ -128,6 +129,10 @@ def load():
     lib.sr_knn_cells.argtypes = [i32, vp, vp, vp, vp]
     lib.sr_knn_mean_dist2.restype = C.c_int
     lib.sr_knn_mean_dist2.argtypes = [i32, vp, vp, vp, vp, vp, vp]
+    lib.sr_radius_outlier_scratch_bytes.restype = C.c_int64
+    lib.sr_radius_outlier_scratch_bytes.argtypes = [i32]
+    lib.sr_radius_outlier_mask.restype = C.c_int
+    lib.sr_radius_outlier_mask.argtypes = [i32, vp, C.c_double, i32, vp, vp, vp, i64, vp]
     lib.sr_set_profiling.restype = None
     lib.sr_set_profiling.argtypes = [C.c_int]
     lib.sr_get_profile.restype = C.c_char_p

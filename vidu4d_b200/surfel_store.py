@@ -171,6 +171,18 @@ class FlatSurfelModel(torch.nn.Module):
         self.xyz_gradient_accum, self.denom, self.max_radii2D = stats
 
     @torch.no_grad()
+    def remove_radius_outliers(self, nb_points: int = 20, radius: float = 0.004) -> int:
+        """lab4d/engine/trainer.py:573-588 (Open3D's remove_radius_outlier, then prune_points) on the device: prunes every
+        surfel with at most nb_points surfels, itself included, strictly closer than `radius` (knn.radius_outlier_mask).
+        Returns the number pruned.  When none is, the buffers are left as they are (same addresses for a captured step)."""
+        from .knn import radius_outlier_mask
+        mask = radius_outlier_mask(self._xyz, nb_points, radius)
+        n = int(mask.sum())
+        if n:
+            self.prune_points(mask)
+        return n
+
+    @torch.no_grad()
     def densify_and_prune(self, max_grad, min_opacity, extent, max_screen_size, generator=None):
         """gaussian_model.py:431-446 in ONE pass over the buffers.  The reference builds the result in four steps (clone ->
         cat; split -> cat, prune the split parents; prune by opacity / size), re-creating every parameter and both Adam

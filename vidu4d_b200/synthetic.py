@@ -98,6 +98,21 @@ def object_scene(P: int, seed: int = 0, radius: float = 0.35, center=(0.0, 0.0, 
     return Scene(f32(xyz), f32(scales), f32(q), f32(op), f32(shs), sh_degree)
 
 
+def shell_with_strays(P: int, seed: int = 0, radius: float = 0.15, thickness: float = 0.002, stray_frac: float = 0.01,
+                      center=(0.0, 0.0, 1.0)) -> np.ndarray:
+    """(P,3) float32 surfel centres like a densified Stage-3 object: a thin noisy sphere dense enough that a point has ~50
+    others within 0.004 (the reference's outlier radius), plus stray_frac of the points scattered uniformly over a box
+    three radii wide, far from the surface (lab4d/engine/trainer.py:573-588 exists to prune those)."""
+    rng = np.random.default_rng(seed)
+    n_stray = int(round(P * stray_frac))
+    d = rng.normal(size=(P - n_stray, 3))
+    d /= np.linalg.norm(d, axis=1, keepdims=True)
+    shell = d * (radius + thickness * rng.normal(size=(P - n_stray, 1)))
+    strays = rng.uniform(-3 * radius, 3 * radius, size=(n_stray, 3))
+    xyz = np.concatenate([shell, strays])[rng.permutation(P)] + np.asarray(center, dtype=np.float64)[None]
+    return np.ascontiguousarray(xyz, dtype=np.float32)
+
+
 def random_rotation(rng) -> np.ndarray:
     q = rng.normal(size=4)
     q /= np.linalg.norm(q)
