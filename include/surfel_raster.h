@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SR_ABI_VERSION 9
+#define SR_ABI_VERSION 10
 
 #if defined(__GNUC__)
 #define SR_API __attribute__((visibility("default")))
@@ -335,6 +335,40 @@ SR_API int sr_cycle_loss_backward(int32_t P, int32_t B, int32_t M, const float* 
                                   const float* se3_d, const float* cam_q, const float* cam_t, const float* scale,
                                   const float* g_loss, float* g_xyz_cam, float* g_xyz, float* g_delta, float* g_tables,
                                   void* stream);
+
+/*
+ * Stage 3's per-surfel feature rows (csrc/feature_rows.cu, DESIGN.md section 3.5d): the (M,P,Cf+6) rows the rasterizer
+ * composites next to the colour.  Replaces lab4d/nnutils/deformable_gaussian.py:1106-1182 (query_field's normal, flow,
+ * flow scale and row concatenation), :817-883 (compute_flow with flip_pair), :1742-1769 with lab4d/nnutils/warping.py:463-495
+ * and lab4d/utils/transforms.py:28-40 (the Gaussian-bone density), with their autograd.
+ *   regist[P*Cf] (may be NULL when Cf = 0; 8-byte alignment suffices);  xyz[P*3]: canonical surfels;  scaling[P*2]: the
+ *   two tangent scales;  xyz_cam[M*P*3], rot_cam[M*P*4]: sr_bob_warp_forward's outputs;  Kmat[M*9]: intrinsics (all
+ *   three rows used);  cam_q[M*4]: field2cam's quaternion;  centres[B*3]: translations of the rest bones;  beta[1] =
+ *   exp(logibeta).  All DEVICE float32.
+ * Row (m, p) = [regist[p] | flow[m,p] / s | normal[m,p] | density[p]], with
+ *   flow[m,p] = pi(K[m'], xyz_cam[m',p]) - pi(K[m], xyz_cam[m,p]), pi(K,x) = (Kx)[0:2] / (Kx)[2], m' = m xor 1 (M = 1:
+ *   m' = m, flow 0);  s = max |flow| over all M*P*2 values + 1e-6 (= max(max(flow), |min(flow)|) + 1e-6);
+ *   normal = cam_q[m] (rot_cam[m,p] e_a rot_cam[m,p]*) cam_q[m]*, e_a = e_x or e_y, the arg-min of the two scales (e_x on
+ *   ties), quaternions not normalised;  density = beta * max_b exp(-0.5 |xyz - centres[b]|^2 / 0.01^2).
+ * Forward writes rows[M*P*(Cf+6)], density[P], flow_scale[1] = s and aux[3] (uint32: the bits of max |flow|, the number
+ * of flow values equal to +max|flow| and to -max|flow|; keep it for the backward).  Rows are bit-identical run to run.
+ * Backward takes g_rows[M*P*(Cf+6)], g_density[P] or NULL and g_flow_scale[1] (DEVICE) or NULL.  dL/ds (the caller's
+ * g_flow_scale plus the rows' -sum(g * flow) / s^2) reaches the tied extreme flow values as torch's autograd sends it:
+ * halved when both +max|flow| and -max|flow| occur, then spread evenly over the equal elements, times -1 for the
+ * minimum's.  It writes g_regist[P*Cf], g_xyz[P*3], g_xyz_cam[M*P*3], g_rot_cam[M*P*4] directly and g_tables[M*4 + B*3 + 2]
+ * = gradients of {cam_q, centres, beta} in that order, then one float of scratch (zeroed inside).
+ * SR_EINVAL, before any device work: a NULL required pointer (the per-surfel arrays may be NULL when P = 0), P < 0, M not
+ * 1 and not even or above 1024, B outside [1, 64], Cf < 0 or Cf + 6 > 32.  No call allocates or synchronises with the host.
+ */
+SR_API int sr_feature_rows_forward(int32_t P, int32_t M, int32_t B, int32_t Cf, const float* regist, const float* xyz,
+                                   const float* scaling, const float* xyz_cam, const float* rot_cam, const float* Kmat,
+                                   const float* cam_q, const float* centres, const float* beta, float* rows, float* density,
+                                   float* flow_scale, uint32_t* aux, void* stream);
+SR_API int sr_feature_rows_backward(int32_t P, int32_t M, int32_t B, int32_t Cf, const float* xyz, const float* scaling,
+                                    const float* xyz_cam, const float* rot_cam, const float* Kmat, const float* cam_q,
+                                    const float* centres, const float* beta, const float* flow_scale, const uint32_t* aux,
+                                    const float* g_rows, const float* g_density, const float* g_flow_scale, float* g_regist,
+                                    float* g_xyz, float* g_xyz_cam, float* g_rot_cam, float* g_tables, void* stream);
 
 /*
  * Optimizer-side kernels over the FLAT surfel parameter buffer (SURVEY.md section 8(f) row N4): the Adam step of every

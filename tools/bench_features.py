@@ -21,10 +21,16 @@ positive mean), alternating in one process, at 256x256 x 2 frames with 300 K sur
 (csrc/cycle.cu) against the same statements in torch (tests/cycle_model.py cycle_values in fp32 and the sync-free
 positive means), alternating in one process.
 
+--rows times Stage 3's per-surfel feature rows alone: [regist | flow / s | normal | Gaussian-bone density] for every
+frame, forward + backward with seeded upstream gradients, at 300 K surfels, B = 25, Cf = 16, M = 2 and M = 8, one CUDA
+graph, L2 flushed between steps, fused (csrc/feature_rows.cu) against the reference's statements in fp32 torch
+(tests/feature_rows_model.py), alternating in one process.
+
     python tools/bench_features.py --features 4 22 32 [--steps 20 --warmup 5]
     python tools/bench_features.py --losses [--steps 20 --warmup 5]
     python tools/bench_features.py --reproj [--steps 20 --warmup 5]
     python tools/bench_features.py --cycle [--steps 20 --warmup 5]
+    python tools/bench_features.py --rows [--steps 20 --warmup 5]
 """
 import argparse
 import json
@@ -50,7 +56,10 @@ def main():
     ap.add_argument("--losses", action="store_true")
     ap.add_argument("--reproj", action="store_true")
     ap.add_argument("--cycle", action="store_true")
+    ap.add_argument("--rows", action="store_true")
     args = ap.parse_args()
+    if args.rows:
+        return bench_rows(args)
     if args.cycle:
         return bench_cycle(args)
     if args.losses:
@@ -482,6 +491,122 @@ def bench_cycle(args):
                           "delta": True, "ms_per_step": {k: round(float(np.median(v)), 4) for k, v in ms.items()},
                           "peak_mem_mb_above_inputs": peak, "kernel_ms_per_launch": kern,
                           "launches_per_step": {k: s_.launches for k, s_ in steps.items()}, "outputs": compare,
+                          "steps": args.steps, "statistic": "median step time", "gpu": gpu}), flush=True)
+        del steps, bodies, d
+        torch.cuda.empty_cache()
+    RZ.set_sync_mode(True)
+    RZ._pending.clear()
+
+
+ROWS_LEAVES = ("regist", "xyz", "xyz_cam", "rot_cam", "cam_q", "rest_q", "rest_t", "logibeta")
+
+
+def _rows_inputs(M, P, B, dev, seed=0):
+    """make_feature_rows_golden.make_case's inputs at full size; xyz_cam / rot_cam are the fused forward warp's."""
+    from tests.golden.make_feature_rows_golden import make_case
+    from vidu4d_b200.warp import bob_warp
+    inp = make_case(seed, P, B, M)
+    d = {k: v.to(dev) for k, v in inp.items()}
+    with torch.no_grad():
+        d["xyz_cam"], d["rot_cam"], _ = bob_warp(d["xyz"], d["rot"], _q2dq(d["rest_q"], d["rest_t"]), _q2dq(d["art_q"], d["art_t"]),
+                                                 d["log_gauss"], (d["cam_q"], d["cam_t"]), d["delta"])
+    d["Kmat"] = torch.linalg.inv(d["Kinv"])
+    for k in ROWS_LEAVES:
+        d[k].requires_grad_(True)
+    g = torch.Generator(device=dev).manual_seed(seed)
+    d["g_rows"] = torch.randn((M, P, inp["regist"].shape[1] + 6), device=dev, generator=g)
+    d["g_s"] = torch.randn((), device=dev, generator=g)
+    d["g_dens"] = torch.randn((P, 1), device=dev, generator=g)
+    return d
+
+
+def _rows_fused(d):
+    from vidu4d_b200.warp import feature_rows
+    o = feature_rows(d["regist"], d["xyz"], d["scaling"], d["xyz_cam"], d["rot_cam"], d["Kmat"], (d["cam_q"], d["cam_t"]),
+                     _q2dq(d["rest_q"], d["rest_t"]), d["logibeta"])
+    return o["rows"], o["flow_scale"], o["gauss_density"]
+
+
+def _rows_torch(d):
+    """deformable_gaussian.py:1106-1182 as tests/feature_rows_model.py's statements, in fp32."""
+    from tests import feature_rows_model as fm
+    rows, s, dens, _ = fm.feature_rows(d["regist"], d["xyz"], d["scaling"], d["xyz_cam"], d["rot_cam"], d["Kmat"],
+                                       (d["cam_q"], d["cam_t"]), _q2dq(d["rest_q"], d["rest_t"]), d["logibeta"])
+    return rows, s, dens
+
+
+def bench_rows(args):
+    from vidu4d_b200 import _capi, rasterizer as RZ
+    from vidu4d_b200.graph import GraphedStep
+    assert torch.cuda.is_available(), "this measurement needs a GPU"
+    dev = torch.device("cuda:0")
+    _capi.load()
+    gpu = _gpu_name()
+    P, B = args.surfels, 25
+    flush = torch.empty((256 << 20,), dtype=torch.uint8, device=dev)
+    for M in (2, 8):
+        d = _rows_inputs(M, P, B, dev)
+        fns = {"fused": _rows_fused, "torch": _rows_torch}
+
+        def make_body(fn):
+            def body():
+                for k in ROWS_LEAVES:
+                    d[k].grad = None
+                torch.autograd.backward(fn(d), (d["g_rows"], d["g_s"], d["g_dens"]))
+            return body
+        bodies = {k: make_body(f) for k, f in fns.items()}
+        peak = {}
+        for k, b in bodies.items():                                  # eager peak memory above the inputs
+            torch.cuda.synchronize()
+            base = torch.cuda.memory_allocated()
+            torch.cuda.reset_peak_memory_stats()
+            b()
+            torch.cuda.synchronize()
+            peak[k] = round((torch.cuda.max_memory_allocated() - base) / 2**20, 1)
+        grads = {}
+        for k, b in bodies.items():                                  # the two paths on the same inputs
+            b()
+            grads[k] = {n: d[n].grad.clone() for n in ROWS_LEAVES}
+        with torch.no_grad():
+            of, ot = _rows_fused(d), _rows_torch(d)
+        rel = lambda a, b: float((a - b).abs().max() / b.abs().max().clamp(min=1e-30))  # noqa: E731
+        compare = {"outputs_max_abs_diff_over_max": {n: rel(a, b) for n, a, b in zip(("rows", "flow_scale", "gauss_density"), of, ot)},
+                   "grad_max_abs_diff_over_max": {n: rel(grads["fused"][n], grads["torch"][n]) for n in ROWS_LEAVES}}
+        launches = {}
+        for k, b in bodies.items():                                  # GPU activities (kernels, memsets, copies) of one step
+            with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as tp:
+                b()
+                torch.cuda.synchronize()
+            launches[k] = sum(e.count for e in tp.key_averages() if e.device_type == torch.autograd.DeviceType.CUDA)
+        steps = {k: GraphedStep(b, device=dev) for k, b in bodies.items()}
+        for s_ in steps.values():
+            s_()
+            for _ in range(args.warmup):
+                s_(check=False)
+        torch.cuda.synchronize()
+        ms = {k: [] for k in steps}
+        for i in range(args.steps):
+            for k, s_ in steps.items():
+                flush.fill_(i & 255)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record(); s_.graph.replay(); b.record()
+                b.synchronize()
+                ms[k].append(a.elapsed_time(b))
+        RZ._pending.clear()
+        RZ.set_sync_mode(True)
+        bodies["fused"]()
+        torch.cuda.synchronize()
+        _capi.get_profile()
+        _capi.set_profiling(True)
+        for _ in range(5):
+            bodies["fused"]()
+        prof = _capi.get_profile()
+        _capi.set_profiling(False)
+        kern = {k: round(v["ms"] / max(v["count"], 1), 4) for k, v in prof.items() if k.startswith("frows_")}
+        print(json.dumps({"workload": "feature rows (fwd + bwd)", "surfels": P, "frames": M, "bones": B,
+                          "regist_channels": int(d["regist"].shape[1]), "ms_per_step": {k: round(float(np.median(v)), 4) for k, v in ms.items()},
+                          "peak_mem_mb_above_inputs": peak, "kernel_ms_per_launch": kern,
+                          "gpu_activities_per_step": launches, "library_launches_per_step": steps["fused"].launches, "outputs": compare,
                           "steps": args.steps, "statistic": "median step time", "gpu": gpu}), flush=True)
         del steps, bodies, d
         torch.cuda.empty_cache()

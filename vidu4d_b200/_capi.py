@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libsurfel_raster.so")
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 SR_STATUS_OVERFLOW = 1
 SR_STATUS_PREFILTER = 4
 SR_BATCH_SUM_SHARED = 1
@@ -22,7 +22,7 @@ SYMBOLS = (
     "sr_set_profiling", "sr_get_profile", "sr_post_forward", "sr_post_backward", "sr_render_loss_batch", "sr_bob_warp_table_floats", "sr_bob_warp_forward", "sr_bob_warp_backward", "sr_adam_flat", "sr_surfel_compact", "sr_knn_cells", "sr_knn_mean_dist2",
     "sr_feature_loss_batch", "sr_global_match_forward", "sr_global_match_backward", "sr_reproj_loss_forward", "sr_reproj_loss_backward",
     "sr_cycle_loss_table_floats", "sr_cycle_loss_forward", "sr_cycle_loss_backward",
-    "sr_radius_outlier_scratch_bytes", "sr_radius_outlier_mask",
+    "sr_radius_outlier_scratch_bytes", "sr_radius_outlier_mask", "sr_feature_rows_forward", "sr_feature_rows_backward",
 )
 FEATURES_MAX = 32          # channels per call (SR_FEAT_MAX)
 
@@ -121,6 +121,10 @@ def load():
     lib.sr_cycle_loss_forward.argtypes = [i32] * 3 + [vp] * 16
     lib.sr_cycle_loss_backward.restype = C.c_int
     lib.sr_cycle_loss_backward.argtypes = [i32] * 3 + [vp] * 17
+    lib.sr_feature_rows_forward.restype = C.c_int
+    lib.sr_feature_rows_forward.argtypes = [i32] * 4 + [vp] * 14
+    lib.sr_feature_rows_backward.restype = C.c_int
+    lib.sr_feature_rows_backward.argtypes = [i32] * 4 + [vp] * 19
     lib.sr_adam_flat.restype = C.c_int
     lib.sr_adam_flat.argtypes = [i32, vp, vp, C.c_float, C.c_float, C.c_float, i64, C.c_float, vp, vp, vp, vp, vp]
     lib.sr_surfel_compact.restype = C.c_int

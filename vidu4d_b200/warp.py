@@ -277,3 +277,136 @@ def cycle_loss(xyz, xyz_cam, rest_articulation, t_articulation, log_gauss, field
     loss, terms, counts = _CycleLoss.apply(xyz, xyz_cam, o2b_q, o2b_t, inv_gauss, se3_r, se3_d, field2cam[0], field2cam[1],
                                            delta, weights, (P, B, M))
     return {"loss": loss, "terms": terms, "counts": counts}
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Per-surfel feature rows (csrc/feature_rows.cu): [regist | flow / s | normal | Gaussian-bone density] per frame, the
+# (M,P,Cf+6) channels render_loss_batch(features=) composites next to the colour.
+
+FEATURE_ROWS_MAX = 32
+
+
+def _check_feature_rows(regist_feat, xyz, scaling, xyz_cam, rot_cam, Kmat, field2cam, rest_articulation, logibeta):
+    if xyz.dim() != 2 or xyz.shape[1] != 3:
+        raise RuntimeError(f"xyz must be (P,3), got {tuple(xyz.shape)}")
+    P = int(xyz.shape[0])
+    if regist_feat.dim() != 2 or regist_feat.shape[0] != P or regist_feat.shape[1] + 6 > FEATURE_ROWS_MAX:
+        raise RuntimeError(f"regist_feat must be (P,Cf) with P = {P} and Cf + 6 <= {FEATURE_ROWS_MAX}, got {tuple(regist_feat.shape)}")
+    Cf = int(regist_feat.shape[1])
+    if tuple(scaling.shape) != (P, 2):
+        raise RuntimeError(f"scaling must be (P,2) (the two tangent scales) with P = {P}, got {tuple(scaling.shape)}")
+    if xyz_cam.dim() != 3 or tuple(xyz_cam.shape[1:]) != (P, 3) or xyz_cam.shape[0] < 1:
+        raise RuntimeError(f"xyz_cam must be (M,P,3) with P = {P}, got {tuple(xyz_cam.shape)}")
+    M = int(xyz_cam.shape[0])
+    if M > 1 and M % 2:
+        raise RuntimeError(f"M must be 1 or even: the flow pairs frames 2k and 2k+1 (flip_pair), got M = {M}")
+    if M > 1024:
+        raise RuntimeError(f"M must be at most 1024, got {M}")
+    if tuple(rot_cam.shape) != (M, P, 4):
+        raise RuntimeError(f"rot_cam must be (M,P,4) = ({M},{P},4), got {tuple(rot_cam.shape)}")
+    if tuple(Kmat.shape) != (M, 3, 3):
+        raise RuntimeError(f"Kmat must be (M,3,3) with M = {M}, got {tuple(Kmat.shape)}")
+    if len(field2cam) != 2 or tuple(field2cam[0].shape) != (M, 4):
+        raise RuntimeError(f"field2cam must be ((M,4),(M,3)) with M = {M}, got {[tuple(t.shape) for t in field2cam]}")
+    B = int(rest_articulation[0].shape[0]) if rest_articulation[0].dim() == 2 else -1
+    if (len(rest_articulation) != 2 or not 1 <= B <= B_MAX or tuple(rest_articulation[0].shape) != (B, 4)
+            or tuple(rest_articulation[1].shape) != (B, 4)):
+        raise RuntimeError(f"rest_articulation must be ((B,4),(B,4)) with 1 <= B <= {B_MAX}, "
+                           f"got {[tuple(t.shape) for t in rest_articulation]}")
+    if logibeta.numel() != 1:
+        raise RuntimeError(f"logibeta must hold one value, got shape {tuple(logibeta.shape)}")
+    named = [("regist_feat", regist_feat), ("xyz", xyz), ("scaling", scaling), ("xyz_cam", xyz_cam), ("rot_cam", rot_cam),
+             ("Kmat", Kmat), ("field2cam", field2cam[0]), ("rest_articulation", rest_articulation[0]),
+             ("rest_articulation", rest_articulation[1]), ("logibeta", logibeta)]
+    for name, t in named:
+        if t.dtype != torch.float32:
+            raise RuntimeError(f"{name} must be float32, got {t.dtype}")
+    for name, t in named:
+        if not t.is_cuda:
+            raise RuntimeError(f"{name} must be a CUDA tensor (there is no CPU fallback)")
+        if t.device != xyz.device:
+            raise RuntimeError(f"{name} is on {t.device}, xyz on {xyz.device}")
+    return P, M, B, Cf
+
+
+class _FeatureRows(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, regist, xyz, xyz_cam, rot_cam, cam_q, centres, beta, scaling, Kmat, dims):
+        P, M, B, Cf = dims
+        lib = _capi.load()
+        f = lambda t: t.detach().contiguous()  # noqa: E731
+        regist, xyz, xyz_cam, rot_cam, cam_q, centres, beta, scaling, Kmat = map(f, (regist, xyz, xyz_cam, rot_cam, cam_q, centres,
+                                                                                    beta, scaling, Kmat))
+        dev = xyz.device
+        rows = torch.empty((M, P, Cf + 6), dtype=torch.float32, device=dev)
+        density = torch.empty((P, 1), dtype=torch.float32, device=dev)
+        s = torch.empty((), dtype=torch.float32, device=dev)
+        aux = torch.empty((3,), dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            rc = lib.sr_feature_rows_forward(P, M, B, Cf, regist.data_ptr() if Cf else None, xyz.data_ptr(), scaling.data_ptr(),
+                                             xyz_cam.data_ptr(), rot_cam.data_ptr(), Kmat.data_ptr(), cam_q.data_ptr(),
+                                             centres.data_ptr(), beta.data_ptr(), rows.data_ptr(), density.data_ptr(), s.data_ptr(),
+                                             aux.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        _capi.check(rc, "sr_feature_rows_forward")
+        ctx.dims = dims
+        ctx.save_for_backward(xyz, scaling, xyz_cam, rot_cam, Kmat, cam_q, centres, beta, s, aux)
+        return rows, s, density
+
+    @staticmethod
+    def backward(ctx, g_rows, g_s, g_density):
+        P, M, B, Cf = ctx.dims
+        xyz, scaling, xyz_cam, rot_cam, Kmat, cam_q, centres, beta, s, aux = ctx.saved_tensors
+        dev = xyz.device
+        g_rows = torch.zeros((M, P, Cf + 6), dtype=torch.float32, device=dev) if g_rows is None else g_rows.to(torch.float32).contiguous()
+        g_s = None if g_s is None else g_s.to(torch.float32).contiguous()
+        g_density = None if g_density is None else g_density.to(torch.float32).contiguous()
+        g_regist = torch.empty((P, Cf), dtype=torch.float32, device=dev)
+        g_xyz = torch.empty((P, 3), dtype=torch.float32, device=dev)
+        g_xyz_cam = torch.empty((M, P, 3), dtype=torch.float32, device=dev)
+        g_rot_cam = torch.empty((M, P, 4), dtype=torch.float32, device=dev)
+        g_tab = torch.empty((M * 4 + B * 3 + 2,), dtype=torch.float32, device=dev)
+        ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        lib = _capi.load()
+        with torch.cuda.device(dev):
+            rc = lib.sr_feature_rows_backward(P, M, B, Cf, ptr(xyz), ptr(scaling), ptr(xyz_cam), ptr(rot_cam), ptr(Kmat), ptr(cam_q),
+                                              ptr(centres), ptr(beta), ptr(s), ptr(aux), ptr(g_rows), ptr(g_density), ptr(g_s),
+                                              ptr(g_regist) if Cf else None, ptr(g_xyz), ptr(g_xyz_cam), ptr(g_rot_cam), ptr(g_tab),
+                                              torch.cuda.current_stream(dev).cuda_stream)
+        _capi.check(rc, "sr_feature_rows_backward")
+        g_cq = g_tab[:M * 4].view(M, 4)
+        g_cen = g_tab[M * 4:M * 4 + B * 3].view(B, 3)
+        g_beta = g_tab[M * 4 + B * 3:M * 4 + B * 3 + 1]
+        return g_regist, g_xyz, g_xyz_cam, g_rot_cam, g_cq, g_cen, g_beta, None, None, None
+
+
+def feature_rows(regist_feat, xyz, scaling, xyz_cam, rot_cam, Kmat, field2cam, rest_articulation, logibeta):
+    """Stage 3's per-surfel feature rows (deformable_gaussian.py:1106-1182): for frame m and surfel p the row
+    [regist_feat[p] (Cf) | flow[m,p] / s (2) | normal[m,p] (3) | gauss_density[p] (1)], the channels the reference renders
+    next to the colour (render_view(override_color=concated_feat)); the Gaussian-mask channel is Cf + 5.
+
+    regist_feat (P,Cf): `_regist_feat` (a FlatSurfelModel view is fine).  xyz (P,3): the canonical `_xyz`.  scaling (P,2):
+    `get_scaling`.  xyz_cam (M,P,3), rot_cam (M,P,4): bob_warp's first two outputs.  Kmat (M,3,3): Kmatinv(Kinv).
+    field2cam ((M,4),(M,3)).  rest_articulation ((B,4),(B,4)): the rest bones as dual quaternions
+    (samples_dict["rest_articulation"][..][0]).  logibeta (1,): the SkinningWarp's.  M is 1 or even: frames 2k and 2k+1
+    are each other's flow partner (compute_flow's flip_pair); a single frame is its own partner and its flow is 0.
+
+      flow[m,p] = pi(K[m'], xyz_cam[m',p]) - pi(K[m], xyz_cam[m,p]), pi(K,x) = (Kx)[0:2] / (Kx)[2], m' = m xor 1;
+      s = max(max(flow), |min(flow)|) + 1e-6, NOT detached (as in the reference);
+      normal = field2cam[0][m] applied to rot_cam[m,p] applied to e_a, where e_a is e_x or e_y, whichever of the two
+          tangent scales is smaller (e_x on ties) -- the reference's axis, which is never the surfel normal e_z; rot_cam
+          already holds the camera rotation, which is applied a second time as in the reference; no quaternion is
+          normalised;
+      gauss_density = exp(logibeta) * max_b exp(-0.5 |xyz - c_b|^2 / 0.01^2), c_b the rest bones' translations.
+
+    Returns {"rows": (M,P,Cf+6), "flow_scale": 0-d tensor s, "gauss_density": (P,1)}, all differentiable: gradients reach
+    regist_feat, xyz, xyz_cam, rot_cam (through bob_warp: the canonical surfels and the articulations), field2cam[0],
+    rest_articulation and logibeta.  scaling, Kmat and field2cam[1] are data.  The caller multiplies the flow planes it
+    renders back by flow_scale (:1193), which adds its own gradient to s.  No host synchronisation; nothing is allocated
+    beyond the outputs and the gradients."""
+    P, M, B, Cf = _check_feature_rows(regist_feat, xyz, scaling, xyz_cam, rot_cam, Kmat, field2cam, rest_articulation, logibeta)
+    rr, rd = rest_articulation
+    centres = 2.0 * _qmul(rd, _qconj(rr))[..., 1:]              # dual_quaternion_to_quaternion_translation
+    beta = torch.exp(logibeta.reshape(1))
+    rows, s, density = _FeatureRows.apply(regist_feat, xyz, xyz_cam, rot_cam, field2cam[0], centres, beta, scaling, Kmat,
+                                          (P, M, B, Cf))
+    return {"rows": rows, "flow_scale": s, "gauss_density": density}
