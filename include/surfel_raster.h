@@ -183,6 +183,7 @@ SR_API int sr_debug_view(int32_t P, int32_t width, int32_t height, int64_t capac
  * world_view_transform is the camera's (4,4) W2C^T exactly as GaussianRasterizationSettings.viewmatrix.
  * forward writes acc[HW], rend_normal[3HW], rend_dist[HW], depth_median[HW], depth_expected[HW], surf_depth[HW],
  * surf_normal[3HW]; backward takes their gradients and writes g_allmap[8HW] (fully, no need to zero).
+ * SR_EINVAL: a NULL pointer (other than stream).
  */
 SR_API int sr_post_forward(int32_t W, int32_t H, float tan_fovx, float tan_fovy, float depth_ratio, const float* allmap,
                            const float* world_view_transform, float* acc, float* rend_normal, float* rend_dist,

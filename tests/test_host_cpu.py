@@ -22,6 +22,26 @@ def test_library_exports_declared_abi(built):
         assert hasattr(lib, sym), f"{sym} declared in the header but not exported"
     assert declared == set(_capi.SYMBOLS)
     assert lib.sr_abi_version() == _capi.ABI_VERSION
+    # each prototype's return and parameter kinds against the ctypes declaration
+    c_kinds = {"int": "int32", "int32_t": "int32", "int64_t": "int64", "uint64_t": "uint64", "size_t": "uint64",
+               "float": "float", "double": "double", "void": None}
+    py_kinds = {C.c_int32: "int32", C.c_int64: "int64", C.c_uint64: "uint64", C.c_float: "float", C.c_double: "double"}
+
+    def c_kind(decl):
+        return "pointer" if "*" in decl else c_kinds[decl.replace("const", "").split()[0]]
+
+    def py_kind(t):
+        if t is None:
+            return None
+        return "pointer" if t in (C.c_void_p, C.c_char_p) or issubclass(t, C._Pointer) else py_kinds[t]
+    body = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
+    protos = re.findall(r"SR_API\s+([\w\s\*]+?)\b(sr_\w+)\s*\(([^)]*)\)", body)
+    assert {name for _, name, _ in protos} == declared
+    for ret, name, params in protos:
+        params = [p for p in params.split(",") if p.strip() not in ("", "void")]
+        restype, argtypes = _capi.PROTOTYPES[name]
+        assert py_kind(restype) == c_kind(ret), name
+        assert [py_kind(t) for t in argtypes] == [c_kind(p) for p in params], name
 
 
 def test_buffer_sizing_monotonic_and_invertible(built):

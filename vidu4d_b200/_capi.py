@@ -15,16 +15,7 @@ ABI_VERSION = 10
 SR_STATUS_OVERFLOW = 1
 SR_STATUS_PREFILTER = 4
 SR_BATCH_SUM_SHARED = 1
-
-SYMBOLS = (
-    "sr_geom_bytes", "sr_image_bytes", "sr_binning_bytes", "sr_forward", "sr_backward",
-    "sr_mark_visible", "sr_debug_view", "sr_abi_version", "sr_last_error", "sr_launch_count",
-    "sr_set_profiling", "sr_get_profile", "sr_post_forward", "sr_post_backward", "sr_render_loss_batch", "sr_bob_warp_table_floats", "sr_bob_warp_forward", "sr_bob_warp_backward", "sr_adam_flat", "sr_surfel_compact", "sr_knn_cells", "sr_knn_mean_dist2",
-    "sr_feature_loss_batch", "sr_global_match_forward", "sr_global_match_backward", "sr_reproj_loss_forward", "sr_reproj_loss_backward",
-    "sr_cycle_loss_table_floats", "sr_cycle_loss_forward", "sr_cycle_loss_backward",
-    "sr_radius_outlier_scratch_bytes", "sr_radius_outlier_mask", "sr_feature_rows_forward", "sr_feature_rows_backward",
-)
-FEATURES_MAX = 32          # channels per call (SR_FEAT_MAX)
+FEATURES_MAX = 32          # channels per call (SR_FEAT_MAX); also the widest feature row sr_feature_rows_* writes
 
 
 class SrFrame(C.Structure):
@@ -56,6 +47,51 @@ class SurfelRasterError(RuntimeError):
     pass
 
 
+# restype and argtypes of every entry point, in include/surfel_raster.h's order (tests/test_host_cpu.py checks them against
+# the header).  Device pointers are c_void_p; the trailing c_void_p of most entry points is the stream.
+_p, _i32, _i64, _f32, _f64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_double
+_FRAME, _BATCH = C.POINTER(SrFrame), C.POINTER(SrBatch)
+PROTOTYPES = {
+    "sr_geom_bytes": (C.c_size_t, [_i32]),
+    "sr_image_bytes": (C.c_size_t, [_i32, _i32]),
+    "sr_binning_bytes": (C.c_size_t, [_i64, _i32, _i32]),
+    "sr_forward": (C.c_int, [_FRAME, _BATCH, _p, _i32] + [_p] * 7 + [_i32, _i64] + [_p] * 3 + [_p, _i64, _p, _i64] + [_p] * 5
+                   + [_i64, _p, _p, _p]),
+    "sr_backward": (C.c_int, [_FRAME, _BATCH, _p, _i32] + [_p] * 6 + [_i32, _i64] + [_p] * 4 + [_p, _i64, _p, _i64] + [_p] * 6
+                    + [_i64] + [_p] * 10),
+    "sr_mark_visible": (C.c_int, [_i32] + [_p] * 5),
+    "sr_debug_view": (C.c_int, [_i32, _i32, _i32, _i64, C.POINTER(SrDebugLayout)]),
+    "sr_post_forward": (C.c_int, [_i32, _i32, _f32, _f32, _f32] + [_p] * 10),
+    "sr_post_backward": (C.c_int, [_i32, _i32, _f32, _f32, _f32] + [_p] * 12),
+    "sr_render_loss_batch": (C.c_int, [_i32, _i32, _i32, _f32, _f32, _f32] + [_p] * 8 + [_f32] * 4 + [_p] * 6),
+    "sr_feature_loss_batch": (C.c_int, [_i32] * 6 + [_p] * 10),
+    "sr_bob_warp_table_floats": (C.c_size_t, [_i32, _i32]),
+    "sr_bob_warp_forward": (C.c_int, [_i32] * 3 + [_p] * 14),
+    "sr_bob_warp_backward": (C.c_int, [_i32] * 3 + [_p] * 18),
+    "sr_global_match_forward": (C.c_int, [_i32] * 6 + [_p] * 10),
+    "sr_global_match_backward": (C.c_int, [_i32] * 6 + [_p] * 13),
+    "sr_reproj_loss_forward": (C.c_int, [_i32] * 5 + [_f32] + [_p] * 20),
+    "sr_reproj_loss_backward": (C.c_int, [_i32] * 5 + [_p] * 19),
+    "sr_cycle_loss_table_floats": (C.c_size_t, [_i32, _i32]),
+    "sr_cycle_loss_forward": (C.c_int, [_i32] * 3 + [_p] * 16),
+    "sr_cycle_loss_backward": (C.c_int, [_i32] * 3 + [_p] * 17),
+    "sr_feature_rows_forward": (C.c_int, [_i32] * 4 + [_p] * 14),
+    "sr_feature_rows_backward": (C.c_int, [_i32] * 4 + [_p] * 19),
+    "sr_adam_flat": (C.c_int, [_i32, _p, _p, _f32, _f32, _f32, _i64, _f32] + [_p] * 5),
+    "sr_surfel_compact": (C.c_int, [_i32, _p, _p, _p, _i32, _i32, _i32] + [_p] * 12),
+    "sr_knn_cells": (C.c_int64, [_i32, _p, _p, _p, _p]),
+    "sr_knn_mean_dist2": (C.c_int, [_i32] + [_p] * 6),
+    "sr_radius_outlier_scratch_bytes": (C.c_int64, [_i32]),
+    "sr_radius_outlier_mask": (C.c_int, [_i32, _p, _f64, _i32, _p, _p, _p, _i64, _p]),
+    "sr_abi_version": (C.c_int, []),
+    "sr_last_error": (C.c_char_p, []),
+    "sr_launch_count": (C.c_uint64, []),
+    "sr_set_profiling": (None, [C.c_int]),
+    "sr_get_profile": (C.c_char_p, []),
+}
+SYMBOLS = tuple(PROTOTYPES)
+
+
 _lib = None
 
 
@@ -72,74 +108,9 @@ def load():
     for s in SYMBOLS:
         if not hasattr(lib, s):
             raise SurfelRasterError(f"{LIB_PATH} does not export {s}")
-    vp, i32, i64, f32p = C.c_void_p, C.c_int32, C.c_int64, C.c_void_p
-    lib.sr_abi_version.restype = C.c_int
-    lib.sr_last_error.restype = C.c_char_p
-    lib.sr_launch_count.restype = C.c_uint64
-    lib.sr_geom_bytes.restype = C.c_size_t
-    lib.sr_geom_bytes.argtypes = [i32]
-    lib.sr_image_bytes.restype = C.c_size_t
-    lib.sr_image_bytes.argtypes = [i32, i32]
-    lib.sr_binning_bytes.restype = C.c_size_t
-    lib.sr_binning_bytes.argtypes = [i64, i32, i32]
-    lib.sr_forward.restype = C.c_int
-    lib.sr_forward.argtypes = ([C.POINTER(SrFrame), C.POINTER(SrBatch), f32p, i32] + [f32p] * 7 + [i32, i64]
-                               + [f32p] * 3 + [vp, i64, vp, i64] + [vp] * 5 + [i64, vp, vp, vp])
-    lib.sr_backward.restype = C.c_int
-    lib.sr_backward.argtypes = ([C.POINTER(SrFrame), C.POINTER(SrBatch), f32p, i32] + [f32p] * 6 + [i32, i64]
-                                + [f32p] * 3 + [vp] + [f32p, i64, f32p, i64] + [f32p] * 3 + [vp] * 3 + [i64]
-                                + [f32p] * 9 + [vp])
-    lib.sr_mark_visible.restype = C.c_int
-    lib.sr_mark_visible.argtypes = [i32, f32p, f32p, f32p, vp, vp]
-    lib.sr_debug_view.restype = C.c_int
-    lib.sr_debug_view.argtypes = [i32, i32, i32, i64, C.POINTER(SrDebugLayout)]
-    lib.sr_post_forward.restype = C.c_int
-    lib.sr_post_forward.argtypes = [i32, i32, C.c_float, C.c_float, C.c_float] + [vp] * 10
-    lib.sr_post_backward.restype = C.c_int
-    lib.sr_post_backward.argtypes = [i32, i32, C.c_float, C.c_float, C.c_float] + [vp] * 12
-    lib.sr_render_loss_batch.restype = C.c_int
-    lib.sr_render_loss_batch.argtypes = [i32, i32, i32, C.c_float, C.c_float, C.c_float] + [vp] * 8 + [C.c_float] * 4 + [vp] * 6
-    lib.sr_feature_loss_batch.restype = C.c_int
-    lib.sr_feature_loss_batch.argtypes = [i32] * 6 + [vp] * 10
-    lib.sr_bob_warp_table_floats.restype = C.c_size_t
-    lib.sr_bob_warp_table_floats.argtypes = [i32, i32]
-    lib.sr_bob_warp_forward.restype = C.c_int
-    lib.sr_bob_warp_forward.argtypes = [i32, i32, i32] + [vp] * 14
-    lib.sr_bob_warp_backward.restype = C.c_int
-    lib.sr_bob_warp_backward.argtypes = [i32, i32, i32] + [vp] * 18
-    lib.sr_global_match_forward.restype = C.c_int
-    lib.sr_global_match_forward.argtypes = [i32] * 6 + [vp] * 10
-    lib.sr_global_match_backward.restype = C.c_int
-    lib.sr_global_match_backward.argtypes = [i32] * 6 + [vp] * 13
-    lib.sr_reproj_loss_forward.restype = C.c_int
-    lib.sr_reproj_loss_forward.argtypes = [i32] * 5 + [C.c_float] + [vp] * 20
-    lib.sr_reproj_loss_backward.restype = C.c_int
-    lib.sr_reproj_loss_backward.argtypes = [i32] * 5 + [vp] * 19
-    lib.sr_cycle_loss_table_floats.restype = C.c_size_t
-    lib.sr_cycle_loss_table_floats.argtypes = [i32, i32]
-    lib.sr_cycle_loss_forward.restype = C.c_int
-    lib.sr_cycle_loss_forward.argtypes = [i32] * 3 + [vp] * 16
-    lib.sr_cycle_loss_backward.restype = C.c_int
-    lib.sr_cycle_loss_backward.argtypes = [i32] * 3 + [vp] * 17
-    lib.sr_feature_rows_forward.restype = C.c_int
-    lib.sr_feature_rows_forward.argtypes = [i32] * 4 + [vp] * 14
-    lib.sr_feature_rows_backward.restype = C.c_int
-    lib.sr_feature_rows_backward.argtypes = [i32] * 4 + [vp] * 19
-    lib.sr_adam_flat.restype = C.c_int
-    lib.sr_adam_flat.argtypes = [i32, vp, vp, C.c_float, C.c_float, C.c_float, i64, C.c_float, vp, vp, vp, vp, vp]
-    lib.sr_surfel_compact.restype = C.c_int
-    lib.sr_surfel_compact.argtypes = [i32, vp, vp, vp, i32, i32, i32] + [vp] * 12
-    lib.sr_knn_cells.restype = C.c_int64
-    lib.sr_knn_cells.argtypes = [i32, vp, vp, vp, vp]
-    lib.sr_knn_mean_dist2.restype = C.c_int
-    lib.sr_knn_mean_dist2.argtypes = [i32, vp, vp, vp, vp, vp, vp]
-    lib.sr_radius_outlier_scratch_bytes.restype = C.c_int64
-    lib.sr_radius_outlier_scratch_bytes.argtypes = [i32]
-    lib.sr_radius_outlier_mask.restype = C.c_int
-    lib.sr_radius_outlier_mask.argtypes = [i32, vp, C.c_double, i32, vp, vp, vp, i64, vp]
-    lib.sr_set_profiling.restype = None
-    lib.sr_set_profiling.argtypes = [C.c_int]
-    lib.sr_get_profile.restype = C.c_char_p
+    for name, (restype, argtypes) in PROTOTYPES.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     if lib.sr_abi_version() != ABI_VERSION:
         raise SurfelRasterError(f"ABI mismatch: library {lib.sr_abi_version()} != binding {ABI_VERSION}")
     _lib = lib
@@ -150,6 +121,31 @@ def check(rc: int, what: str):
     if rc != 0:
         msg = load().sr_last_error().decode("utf-8", "replace")
         raise SurfelRasterError(f"{what} failed (code {rc}): {msg}")
+
+
+def call(name: str, device, *args):
+    """Run entry point `name` on `device`'s current stream, which is passed as the last argument.  A tensor argument
+    passes as its data_ptr(); ints, floats, None (NULL) and ctypes objects pass unchanged.  Raises SurfelRasterError
+    with the library's message if the call fails."""
+    import torch
+    fn = getattr(load(), name)
+    args = [a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args]
+    with torch.cuda.device(device):
+        check(fn(*args, torch.cuda.current_stream(device).cuda_stream), name)
+
+
+def check_tensors(named, ref_name: str, ref, floats=None):
+    """Raise RuntimeError unless every tensor of `floats` ((name, tensor) pairs; default `named`) is float32 and every
+    tensor of `named` is a CUDA tensor on `ref`'s device."""
+    import torch
+    for name, t in named if floats is None else floats:
+        if t.dtype != torch.float32:
+            raise RuntimeError(f"{name} must be float32, got {t.dtype}")
+    for name, t in named:
+        if not t.is_cuda:
+            raise RuntimeError(f"{name} must be a CUDA tensor (there is no CPU fallback)")
+        if t.device != ref.device:
+            raise RuntimeError(f"{name} is on {t.device}, {ref_name} on {ref.device}")
 
 
 def launch_count() -> int:

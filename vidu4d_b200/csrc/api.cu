@@ -19,21 +19,6 @@ namespace {
 thread_local char g_err[512] = "";
 std::atomic<uint64_t> g_launches{0};
 
-int fail(int code, const char* fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_err, sizeof(g_err), fmt, ap);
-    va_end(ap);
-    return code;
-}
-int cuda_fail(cudaError_t e, const char* where) {
-    return fail(SR_ECUDA, "CUDA error in %s: %s", where, cudaGetErrorString(e));
-}
-#define CK(call, where)                                      \
-    do {                                                     \
-        cudaError_t e_ = (call);                             \
-        if (e_ != cudaSuccess) return cuda_fail(e_, where);  \
-    } while (0)
 #define DBG(where)                                           \
     do {                                                     \
         if (debug) CK(cudaStreamSynchronize(stream), where); \
@@ -59,22 +44,48 @@ CamParams make_cam(const sr_frame* f, const float* vm, const float* campos, cons
 }
 
 int check_frame(const sr_frame* f) {
-    if (!f) return fail(SR_EINVAL, "frame descriptor is NULL");
-    if (f->P < 0) return fail(SR_EINVAL, "P must be >= 0");
-    if (f->width <= 0 || f->height <= 0) return fail(SR_EINVAL, "image size must be positive");
-    if (f->width > 65535 || f->height > 65535) return fail(SR_EINVAL, "image side must be < 65536");
-    if (f->sh_degree < 0 || f->sh_degree > 3) return fail(SR_EINVAL, "sh_degree must be 0..3");
-    if (f->sh_coeffs < 0) return fail(SR_EINVAL, "sh_coeffs must be >= 0");
+    if (!f) return sr_fail(SR_EINVAL, "frame descriptor is NULL");
+    if (f->P < 0) return sr_fail(SR_EINVAL, "P must be >= 0");
+    if (f->width <= 0 || f->height <= 0) return sr_fail(SR_EINVAL, "image size must be positive");
+    if (f->width > 65535 || f->height > 65535) return sr_fail(SR_EINVAL, "image side must be < 65536");
+    if (f->sh_degree < 0 || f->sh_degree > 3) return sr_fail(SR_EINVAL, "sh_degree must be 0..3");
+    if (f->sh_coeffs < 0) return sr_fail(SR_EINVAL, "sh_coeffs must be >= 0");
     if (f->sh_coeffs > 0 && (f->sh_degree + 1) * (f->sh_degree + 1) > f->sh_coeffs)
-        return fail(SR_EINVAL, "sh_degree %d needs %d coefficients, shs has %d", f->sh_degree,
-                    (f->sh_degree + 1) * (f->sh_degree + 1), f->sh_coeffs);
+        return sr_fail(SR_EINVAL, "sh_degree %d needs %d coefficients, shs has %d", f->sh_degree,
+                       (f->sh_degree + 1) * (f->sh_degree + 1), f->sh_coeffs);
     return 0;
 }
 }  // namespace
 
 void sr_count_launch(int n) { g_launches.fetch_add((uint64_t)n, std::memory_order_relaxed); }
 
-int sr_fail(int code, const char* msg, int a, int b) { return fail(code, msg, a, b); }
+int sr_fail(int code, const char* fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(g_err, sizeof(g_err), fmt, ap);
+    va_end(ap);
+    return code;
+}
+
+int sr_launched(int n, const char* where) {
+    sr_count_launch(n);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_fail(e, where);
+}
+
+cudaError_t sr_opt_in_smem(const void* kern, size_t bytes) {
+    if (bytes <= 48 * 1024) return cudaSuccess;
+    int dev = 0;
+    if (cudaError_t e = cudaGetDevice(&dev)) return e;
+    static std::mutex mu;
+    static std::map<std::pair<const void*, int>, size_t> done;   // largest size set per (kernel, device)
+    std::lock_guard<std::mutex> lk(mu);
+    size_t& have = done[{kern, dev}];
+    if (bytes <= have) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e == cudaSuccess) have = bytes;
+    return e;
+}
 
 cudaError_t sr_memset_frames(void* p, size_t pitch, size_t bytes, int frames, cudaStream_t s) {
     if (frames == 1) return cudaMemsetAsync(p, 0, bytes, s);
@@ -132,7 +143,7 @@ size_t sr_binning_bytes(int64_t capacity, int32_t width, int32_t height) {
 }
 
 int sr_debug_view(int32_t P, int32_t width, int32_t height, int64_t capacity, sr_debug_layout* out) {
-    if (!out) return fail(SR_EINVAL, "out is NULL");
+    if (!out) return sr_fail(SR_EINVAL, "out is NULL");
     const GeomLayout g = geom_layout(P);
     const ImageLayout i = image_layout(width, height);
     const BinLayout b = bin_layout(capacity, i.tiles);
@@ -148,20 +159,20 @@ namespace {
 // Feature-channel arguments of sr_forward / sr_backward with F > 0: F in [1, SR_FEAT_MAX], background length 3 or 3+F,
 // and the widest vector access (4, 2 or 1 floats) that every feature row / gradient row / frame stride allows.
 int check_features(const sr_frame* f, int32_t F, int32_t bg_channels, const float* features, int64_t features_stride) {
-    if (!f) return fail(SR_EINVAL, "frame descriptor is NULL");
-    if (F < 1 || F > SR_FEAT_MAX) return fail(SR_EINVAL, "features: F must be in [1, %d], got %d", SR_FEAT_MAX, F);
-    if (!features && f->P > 0) return fail(SR_EINVAL, "features pointer is NULL");
-    if (features_stride < 0) return fail(SR_EINVAL, "features: frame stride must be >= 0");
+    if (!f) return sr_fail(SR_EINVAL, "frame descriptor is NULL");
+    if (F < 1 || F > SR_FEAT_MAX) return sr_fail(SR_EINVAL, "features: F must be in [1, %d], got %d", SR_FEAT_MAX, F);
+    if (!features && f->P > 0) return sr_fail(SR_EINVAL, "features pointer is NULL");
+    if (features_stride < 0) return sr_fail(SR_EINVAL, "features: frame stride must be >= 0");
     if (bg_channels != 3 && bg_channels != 3 + F)
-        return fail(SR_EINVAL, "background must have 3 or 3+F = %d channels, got %d", 3 + F, bg_channels);
+        return sr_fail(SR_EINVAL, "background must have 3 or 3+F = %d channels, got %d", 3 + F, bg_channels);
     return 0;
 }
 // F = 0: the plain rasterizer (no feature pointer, 3-channel background, packed colour)
 int check_no_features(const sr_frame* f, const float* features, int32_t bg_channels, int64_t color_stride) {
-    if (features) return fail(SR_EINVAL, "features: F must be in [1, %d], got 0", SR_FEAT_MAX);
-    if (bg_channels != 3) return fail(SR_EINVAL, "background must have 3 channels when F = 0, got %d", bg_channels);
+    if (features) return sr_fail(SR_EINVAL, "features: F must be in [1, %d], got 0", SR_FEAT_MAX);
+    if (bg_channels != 3) return sr_fail(SR_EINVAL, "background must have 3 channels when F = 0, got %d", bg_channels);
     if (f && color_stride != 0 && color_stride != (int64_t)f->width * f->height * 3)
-        return fail(SR_EINVAL, "F = 0: the colour planes must be packed (frame stride 0 or 3*H*W)");
+        return sr_fail(SR_EINVAL, "F = 0: the colour planes must be packed (frame stride 0 or 3*H*W)");
     return 0;
 }
 int feature_vec(int32_t F, std::initializer_list<uintptr_t> addrs) {
@@ -181,17 +192,17 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
                          int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream_,
                          FeatArgs* ft) {
     if (int rc = check_frame(f)) return rc;
-    if (!b || b->frames < 1 || b->frames > 65535) return fail(SR_EINVAL, "batch descriptor: frames must be in [1, 65535]");
+    if (!b || b->frames < 1 || b->frames > 65535) return sr_fail(SR_EINVAL, "batch descriptor: frames must be in [1, 65535]");
     cudaStream_t stream = (cudaStream_t)stream_;
     const bool debug = f->debug != 0;
     const int P = f->P, M = b->frames;
     const size_t N = (size_t)f->width * f->height;
-    if (!out_color || !out_others || !num_rendered_dev) return fail(SR_EINVAL, "output pointer is NULL");
-    if (!background || !viewmatrix || !campos) return fail(SR_EINVAL, "camera / background pointer is NULL");
+    if (!out_color || !out_others || !num_rendered_dev) return sr_fail(SR_EINVAL, "output pointer is NULL");
+    if (!background || !viewmatrix || !campos) return sr_fail(SR_EINVAL, "camera / background pointer is NULL");
     if (ft) {
-        if (color_stride < (int64_t)(3 * N)) return fail(SR_EINVAL, "out_color frame stride must be >= 3*H*W");
-        if (!ft->out) return fail(SR_EINVAL, "out_features pointer is NULL");
-        if (ft->out_stride < (long long)(ft->F * N) * 4) return fail(SR_EINVAL, "out_features frame stride must be >= F*H*W");
+        if (color_stride < (int64_t)(3 * N)) return sr_fail(SR_EINVAL, "out_color frame stride must be >= 3*H*W");
+        if (!ft->out) return sr_fail(SR_EINVAL, "out_features pointer is NULL");
+        if (ft->out_stride < (long long)(ft->F * N) * 4) return sr_fail(SR_EINVAL, "out_features frame stride must be >= F*H*W");
     }
     CK(cudaMemsetAsync(num_rendered_dev, 0, (size_t)M * 2 * sizeof(uint32_t), stream), "memset(num_rendered)");
     if (P == 0) {
@@ -207,16 +218,16 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
             CK(cudaMemcpyAsync(num_rendered_host, num_rendered_dev, (size_t)M * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream), "copy(num_rendered)");
         return 0;
     }
-    if (!means3D || !opacities || !scales || !rotations || !radii) return fail(SR_EINVAL, "surfel attribute pointer is NULL");
+    if (!means3D || !opacities || !scales || !rotations || !radii) return sr_fail(SR_EINVAL, "surfel attribute pointer is NULL");
     if ((shs == nullptr) == (colors_precomp == nullptr))
-        return fail(SR_EINVAL, "provide exactly one of shs / colors_precomp");
-    if (shs && f->sh_coeffs == 0) return fail(SR_EINVAL, "shs given but sh_coeffs == 0");
-    if (!geom_buffer || !binning_buffer || !image_buffer) return fail(SR_EINVAL, "scratch buffer is NULL");
-    if (capacity <= 0 || capacity >= (1ll << 30)) return fail(SR_EINVAL, "capacity must be in (0, 2^30)");
+        return sr_fail(SR_EINVAL, "provide exactly one of shs / colors_precomp");
+    if (shs && f->sh_coeffs == 0) return sr_fail(SR_EINVAL, "shs given but sh_coeffs == 0");
+    if (!geom_buffer || !binning_buffer || !image_buffer) return sr_fail(SR_EINVAL, "scratch buffer is NULL");
+    if (capacity <= 0 || capacity >= (1ll << 30)) return sr_fail(SR_EINVAL, "capacity must be in (0, 2^30)");
     // 128-bit / 64-bit vector loads: rotations as float4, scales as float2, SH rows as float4 when 3M % 4 == 0
     if (((uintptr_t)rotations & 15) || ((uintptr_t)scales & 7) || (shs && ((uintptr_t)shs & 15)) ||
         ((b->rotations * 4) & 15) || ((b->scales * 4) & 7) || ((b->shs * 4) & 15))
-        return fail(SR_EINVAL, "rotations / shs must be 16-byte aligned and scales 8-byte aligned (per frame)");
+        return sr_fail(SR_EINVAL, "rotations / shs must be 16-byte aligned and scales 8-byte aligned (per frame)");
 
     FwdArgs a{};
     a.cam = make_cam(f, viewmatrix, campos, background);
@@ -290,28 +301,28 @@ static int backward_batch(const sr_frame* f, const sr_batch* b, const float* bac
                           float* dL_dmeans3D, float* dL_dtransMat, float* dL_dsh, float* dL_dscales, float* dL_drotations,
                           void* stream_, FeatArgs* ft) {
     if (int rc = check_frame(f)) return rc;
-    if (!b || b->frames < 1 || b->frames > 65535) return fail(SR_EINVAL, "batch descriptor: frames must be in [1, 65535]");
+    if (!b || b->frames < 1 || b->frames > 65535) return sr_fail(SR_EINVAL, "batch descriptor: frames must be in [1, 65535]");
     cudaStream_t stream = (cudaStream_t)stream_;
     const bool debug = f->debug != 0;
     if (f->P == 0) return 0;   // rasterize_points.cu:204
     if (!background || !means3D || !scales || !rotations || !viewmatrix || !campos || !radii || !dL_dout_color ||
         !dL_dout_others || !geom_buffer || !binning_buffer || !image_buffer)
-        return fail(SR_EINVAL, "input pointer is NULL");
+        return sr_fail(SR_EINVAL, "input pointer is NULL");
     if (!dL_dmeans2D || !dL_dcolors || !dL_dopacity || !dL_dmeans3D || !dL_dscales || !dL_drotations)
-        return fail(SR_EINVAL, "gradient output pointer is NULL");
-    if (!dL_dtransMat && b->frames == 1 && !(b->flags & SR_BATCH_SUM_SHARED)) return fail(SR_EINVAL, "dL_dtransMat is NULL");
-    if (shs && !dL_dsh) return fail(SR_EINVAL, "dL_dsh is NULL");
-    if (capacity <= 0) return fail(SR_EINVAL, "capacity must be positive");
+        return sr_fail(SR_EINVAL, "gradient output pointer is NULL");
+    if (!dL_dtransMat && b->frames == 1 && !(b->flags & SR_BATCH_SUM_SHARED)) return sr_fail(SR_EINVAL, "dL_dtransMat is NULL");
+    if (shs && !dL_dsh) return sr_fail(SR_EINVAL, "dL_dsh is NULL");
+    if (capacity <= 0) return sr_fail(SR_EINVAL, "capacity must be positive");
     if (ft) {
         const long long N = (long long)f->width * f->height;
-        if (dcolor_stride < 3 * N) return fail(SR_EINVAL, "dL_dout_color frame stride must be >= 3*H*W");
-        if (!ft->dout || !ft->dfeat) return fail(SR_EINVAL, "dL_dout_features / dL_dfeatures pointer is NULL");
-        if (ft->dout_stride < ft->F * N * 4) return fail(SR_EINVAL, "dL_dout_features frame stride must be >= F*H*W");
+        if (dcolor_stride < 3 * N) return sr_fail(SR_EINVAL, "dL_dout_color frame stride must be >= 3*H*W");
+        if (!ft->dout || !ft->dfeat) return sr_fail(SR_EINVAL, "dL_dout_features / dL_dfeatures pointer is NULL");
+        if (ft->dout_stride < ft->F * N * 4) return sr_fail(SR_EINVAL, "dL_dout_features frame stride must be >= F*H*W");
     }
     if (((uintptr_t)rotations & 15) || ((uintptr_t)scales & 7) || (shs && ((uintptr_t)shs & 15)) ||
         ((uintptr_t)dL_drotations & 15) || ((uintptr_t)dL_dscales & 7) || (dL_dsh && ((uintptr_t)dL_dsh & 15)) ||
         ((b->rotations * 4) & 15) || ((b->scales * 4) & 7) || ((b->shs * 4) & 15))
-        return fail(SR_EINVAL, "rotations / shs (and their gradients) must be 16-byte aligned, scales 8-byte aligned");
+        return sr_fail(SR_EINVAL, "rotations / shs (and their gradients) must be 16-byte aligned, scales 8-byte aligned");
 
     const int P = f->P, M = b->frames;
     const size_t N = (size_t)f->width * f->height;
@@ -394,9 +405,9 @@ int sr_backward(const sr_frame* f, const sr_batch* b, const float* background, i
 int sr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                     uint8_t* present, void* stream_) {
     (void)projmatrix;
-    if (P < 0) return fail(SR_EINVAL, "P must be >= 0");
+    if (P < 0) return sr_fail(SR_EINVAL, "P must be >= 0");
     if (P == 0) return 0;
-    if (!means3D || !viewmatrix || !present) return fail(SR_EINVAL, "pointer is NULL");
+    if (!means3D || !viewmatrix || !present) return sr_fail(SR_EINVAL, "pointer is NULL");
     CK(launch_mark_visible(P, means3D, viewmatrix, present, (cudaStream_t)stream_), "mark_visible");
     return 0;
 }

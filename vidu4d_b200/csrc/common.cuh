@@ -217,8 +217,30 @@ cudaError_t launch_mark_visible(int P, const float* means3D, const float* vm, ui
 cudaError_t sr_memset_frames(void* p, size_t pitch, size_t bytes, int frames, cudaStream_t s);
 
 void sr_count_launch(int n = 1);
-// sets the message sr_last_error() returns (printf format with up to two int arguments) and returns `code`
-int sr_fail(int code, const char* msg, int a = 0, int b = 0);
+
+// ---- error reporting: every failing entry point sets the message sr_last_error() returns ---------------------------
+// sets the calling thread's message (printf format) and returns `code`
+int sr_fail(int code, const char* fmt, ...) __attribute__((format(printf, 2, 3)));
+static inline int cuda_fail(cudaError_t e, const char* where) {
+    return sr_fail(SR_ECUDA, "CUDA error in %s: %s", where, cudaGetErrorString(e));
+}
+// returns SR_ECUDA (naming `where`) from the enclosing function if a CUDA runtime call fails
+#define CK(call, where)                                      \
+    do {                                                     \
+        cudaError_t e_ = (call);                             \
+        if (e_ != cudaSuccess) return cuda_fail(e_, where);  \
+    } while (0)
+// epilogue of an entry point that launched `n` kernels: counts them, then turns a pending launch error into SR_ECUDA
+int sr_launched(int n, const char* where);
+
+// Opts `kern` in to `bytes` of dynamic shared memory.  Nothing to do up to the default 48 KB; above it the attribute
+// belongs to the current device's context, so the largest size set so far is remembered per (kernel, device) and a
+// request within it costs no driver call.  Safe to call from several threads.
+cudaError_t sr_opt_in_smem(const void* kern, size_t bytes);
+template <class K>
+cudaError_t sr_opt_in_smem(K* kern, size_t bytes) { return sr_opt_in_smem((const void*)kern, bytes); }
+// dynamic shared memory the bone / frame tables of the warp, reprojection and cycle kernels may take (B <= 64)
+#define SR_TABLE_SMEM_MAX (200 * 1024)
 
 // Optional per-kernel timing (sr_set_profiling): CUDA events recorded on the launching stream around each
 // kernel; read back (after a sync) with sr_get_profile().  Off by default: zero overhead on the hot path.

@@ -493,20 +493,6 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
     }
 }
 
-template <typename K>
-cudaError_t opt_in_smem(K kern, size_t bytes) {
-    // per device: cudaFuncSetAttribute applies to the current device's context only
-    static bool set[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64 || !set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-        if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < 64) set[dev] = true;
-    }
-    return cudaSuccess;
-}
-
 }  // namespace
 
 // Which composite forward runs: SURFEL_COMPOSITE_FWD (or SURFEL_COMPOSITE) = tile|warp.  Default: one-warp CTAs with
@@ -523,7 +509,7 @@ bool sr_composite_tile_fwd() {
 
 cudaError_t launch_composite_tile_fwd(const FwdArgs& a) {
     ProfileScope ps("composite_fwd", a.stream);
-    cudaError_t err = opt_in_smem(composite_tile_fwd_kernel, FwdSmem::total);
+    cudaError_t err = sr_opt_in_smem(composite_tile_fwd_kernel, FwdSmem::total);
     if (err != cudaSuccess) return err;
     composite_tile_fwd_kernel<<<a.il.tiles * a.fs.frames, 32 * TWARPS, FwdSmem::total, a.stream>>>(
         a.fs, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles_x,
@@ -539,7 +525,7 @@ cudaError_t launch_composite_tile_bwd(const BwdArgs& a) {
                                      a.fs.frames, a.stream);
     if (e != cudaSuccess) return e;
     ProfileScope ps("composite_bwd", a.stream);
-    e = opt_in_smem(composite_tile_bwd_kernel, BwdSmem::total);
+    e = sr_opt_in_smem(composite_tile_bwd_kernel, BwdSmem::total);
     if (e != cudaSuccess) return e;
     composite_tile_bwd_kernel<<<a.il.tiles * a.fs.frames, 32 * TWARPS, BwdSmem::total, a.stream>>>(
         a.fs, a.grad_scale, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles_x,

@@ -38,7 +38,6 @@ namespace {
 
 constexpr int CYC_FWD_THREADS = 256;
 constexpr int CYC_BWD_THREADS = 128;     // w[B] and gw[B] live in registers, as in bob_warp_bwd / reproj_bwd
-constexpr size_t CYC_SMEM_MAX = 200 * 1024;
 
 struct CycleDims { int P, B, M; };
 
@@ -239,7 +238,7 @@ int check_cycle(int32_t P, int32_t B, int32_t M) {
     if (P < 0) return sr_fail(SR_EINVAL, "P must be >= 0, got %d", P);
     if (M < 1) return sr_fail(SR_EINVAL, "M must be >= 1, got %d", M);
     if (B < 1 || B > 64) return sr_fail(SR_EINVAL, "B must be in [1, 64], got %d", B);
-    if (2 * CycleTables::floats(B, M) * sizeof(float) > CYC_SMEM_MAX)
+    if (2 * CycleTables::floats(B, M) * sizeof(float) > SR_TABLE_SMEM_MAX)
         return sr_fail(SR_EINVAL, "the bone / frame tables of B = %d, M = %d frames do not fit in shared memory", B, M);
     return 0;
 }
@@ -259,17 +258,15 @@ SR_API int sr_cycle_loss_forward(int32_t P, int32_t B, int32_t M, const float* x
         !counts || !scale || !loss)
         return sr_fail(SR_EINVAL, "sr_cycle_loss_forward: a required pointer is NULL");
     cudaStream_t s = (cudaStream_t)stream_;
-    if (cudaMemsetAsync(terms, 0, (size_t)M * 3 * sizeof(float), s) != cudaSuccess ||
-        cudaMemsetAsync(counts, 0, (size_t)M * 3 * sizeof(uint32_t), s) != cudaSuccess)
-        return SR_ECUDA;
+    CK(cudaMemsetAsync(terms, 0, (size_t)M * 3 * sizeof(float), s), "sr_cycle_loss_forward: memset(terms)");
+    CK(cudaMemsetAsync(counts, 0, (size_t)M * 3 * sizeof(uint32_t), s), "sr_cycle_loss_forward: memset(counts)");
     int launches = 1;
     if (P > 0) {
         const CycleDims d{P, B, M};
         const CycleIn in{o2b_q, o2b_t, inv_gauss, se3_r, se3_d, cam_q, cam_t};
         const size_t smem = CycleTables::floats(B, M) * sizeof(float) + (size_t)M * 3 * 8;
         auto launch = [&](auto kern) -> int {
-            if (smem > 48 * 1024 && cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-                return SR_ECUDA;
+            CK(sr_opt_in_smem(kern, smem), "sr_cycle_loss_forward: shared-memory opt-in");
             ProfileScope ps("cycle_fwd", s);
             kern<<<(P + CYC_FWD_THREADS - 1) / CYC_FWD_THREADS, CYC_FWD_THREADS, smem, s>>>(d, xyz, xyz_cam, in, delta, terms, counts);
             return 0;
@@ -281,8 +278,7 @@ SR_API int sr_cycle_loss_forward(int32_t P, int32_t B, int32_t M, const float* x
         ProfileScope ps("cycle_scale", s);
         cycle_scale_kernel<<<1, 32, 0, s>>>(M, weights, counts, terms, scale, loss);
     }
-    sr_count_launch(launches);
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(launches, "sr_cycle_loss_forward");
 }
 
 SR_API int sr_cycle_loss_backward(int32_t P, int32_t B, int32_t M, const float* xyz, const float* xyz_cam, const float* o2b_q,
@@ -297,22 +293,20 @@ SR_API int sr_cycle_loss_backward(int32_t P, int32_t B, int32_t M, const float* 
     if (g_delta && !delta) return sr_fail(SR_EINVAL, "sr_cycle_loss_backward: g_delta without delta");
     cudaStream_t s = (cudaStream_t)stream_;
     const size_t nt = CycleTables::floats(B, M);
-    if (cudaMemsetAsync(g_tables, 0, nt * sizeof(float), s) != cudaSuccess) return SR_ECUDA;
+    CK(cudaMemsetAsync(g_tables, 0, nt * sizeof(float), s), "sr_cycle_loss_backward: memset(g_tables)");
     if (P == 0) return 0;
     const CycleDims d{P, B, M};
     const CycleIn in{o2b_q, o2b_t, inv_gauss, se3_r, se3_d, cam_q, cam_t};
     const size_t smem = 2 * nt * sizeof(float);
     auto launch = [&](auto kern) -> int {
-        if (smem > 48 * 1024 && cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-            return SR_ECUDA;
+        CK(sr_opt_in_smem(kern, smem), "sr_cycle_loss_backward: shared-memory opt-in");
         ProfileScope ps("cycle_bwd", s);
         kern<<<(P + CYC_BWD_THREADS - 1) / CYC_BWD_THREADS, CYC_BWD_THREADS, smem, s>>>(d, xyz, xyz_cam, in, delta, scale, g_loss,
                                                                                    g_xyz_cam, g_xyz, g_delta, g_tables);
         return 0;
     };
     if (int rc = B <= 32 ? launch(cycle_bwd_kernel<32>) : launch(cycle_bwd_kernel<64>)) return rc;
-    sr_count_launch();
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(1, "sr_cycle_loss_backward");
 }
 
 }  // extern "C"

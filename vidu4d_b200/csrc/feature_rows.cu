@@ -348,7 +348,7 @@ SR_API int sr_feature_rows_forward(int32_t P, int32_t M, int32_t B, int32_t Cf, 
         !centres || !beta || !flow_scale || !aux)
         return sr_fail(SR_EINVAL, "sr_feature_rows_forward: a required pointer is NULL");
     cudaStream_t s = (cudaStream_t)stream_;
-    if (cudaMemsetAsync(aux, 0, 3 * sizeof(uint32_t), s) != cudaSuccess) return SR_ECUDA;
+    CK(cudaMemsetAsync(aux, 0, 3 * sizeof(uint32_t), s), "sr_feature_rows_forward: memset(aux)");
     const FrDims d{P, M, B, Cf, row_vec(Cf, regist, rows)};
     const int blocks = (P + FR_THREADS - 1) / FR_THREADS;
     int launches = 1;
@@ -363,8 +363,7 @@ SR_API int sr_feature_rows_forward(int32_t P, int32_t M, int32_t B, int32_t Cf, 
                                                                                           Kmat, cam_q, centres, beta, rows, density,
                                                                                           flow_scale, aux);
     }
-    sr_count_launch(launches);
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(launches, "sr_feature_rows_forward");
 }
 
 SR_API int sr_feature_rows_backward(int32_t P, int32_t M, int32_t B, int32_t Cf, const float* xyz, const float* scaling,
@@ -379,7 +378,7 @@ SR_API int sr_feature_rows_backward(int32_t P, int32_t M, int32_t B, int32_t Cf,
         return sr_fail(SR_EINVAL, "sr_feature_rows_backward: a required pointer is NULL");
     cudaStream_t s = (cudaStream_t)stream_;
     const int ntab = M * 4 + B * 3 + 1;
-    if (cudaMemsetAsync(g_tables, 0, (ntab + 1) * sizeof(float), s) != cudaSuccess) return SR_ECUDA;
+    CK(cudaMemsetAsync(g_tables, 0, (ntab + 1) * sizeof(float), s), "sr_feature_rows_backward: memset(g_tables)");
     if (P == 0) return 0;
     const FrDims d{P, M, B, Cf, row_vec(Cf, g_rows, g_regist)};
     const int blocks = (P + FR_THREADS - 1) / FR_THREADS;
@@ -394,8 +393,7 @@ SR_API int sr_feature_rows_backward(int32_t P, int32_t M, int32_t B, int32_t Cf,
                                                           aux, g_rows, g_density, g_flow_scale, g_regist, g_xyz, g_xyz_cam,
                                                           g_rot_cam, g_tables);
     }
-    sr_count_launch(2);
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(2, "sr_feature_rows_backward");
 }
 
 }  // extern "C"

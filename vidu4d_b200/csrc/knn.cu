@@ -133,22 +133,21 @@ SR_API int64_t sr_knn_cells(int32_t P, const float* bbox_min, const float* bbox_
 
 SR_API int sr_knn_mean_dist2(int32_t P, const float* points, const float* bbox_min, const float* bbox_max, float* out,
                              int32_t* scratch, void* stream_) {
-    if (P < 0) return SR_EINVAL;
+    if (P < 0) return sr_fail(SR_EINVAL, "sr_knn_mean_dist2: P must be >= 0, got %d", P);
     if (P == 0) return 0;
-    if (!points || !bbox_min || !bbox_max || !out || !scratch) return SR_EINVAL;
+    if (!points || !bbox_min || !bbox_max || !out || !scratch) return sr_fail(SR_EINVAL, "sr_knn_mean_dist2: a required pointer is NULL");
     float h; int dims[3];
     const int64_t cells = sr_knn_cells(P, bbox_min, bbox_max, &h, dims);
     Grid g{bbox_min[0], bbox_min[1], bbox_min[2], 1.0f / h, h, dims[0], dims[1], dims[2]};
     cudaStream_t s = (cudaStream_t)stream_;
     int* cell = scratch; int* order = cell + P; int* count = order + P; int* start = count + cells; int* cursor = start + cells;
-    if (cudaMemsetAsync(count, 0, (size_t)cells * 3 * sizeof(int), s) != cudaSuccess) return SR_ECUDA;
+    CK(cudaMemsetAsync(count, 0, (size_t)cells * 3 * sizeof(int), s), "sr_knn_mean_dist2: memset(scratch)");
     const int nb = (P + 255) / 256;
     knn_count_kernel<<<nb, 256, 0, s>>>(g, P, points, cell, count);
     knn_scan_kernel<<<1, 1024, 0, s>>>(count, start, (long long)cells);
     knn_scatter_kernel<<<nb, 256, 0, s>>>(P, cell, start, cursor, order);
     knn_query_kernel<<<nb, 256, 0, s>>>(g, P, points, start, count, order, out);
-    sr_count_launch(4);
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(4, "sr_knn_mean_dist2");
 }
 
 }  // extern "C"

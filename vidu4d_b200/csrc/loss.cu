@@ -309,14 +309,14 @@ SR_API int sr_render_loss_batch(int32_t M, int32_t W, int32_t H, float tanx, flo
                                 const float* learnable_bkgd, float w_rgb, float w_mask, float lambda_normal, float lambda_dist,
                                 float* loss_terms, float* dL_dcolor, float* dL_dallmap, float* dL_dbkgd, float* surf_depth_scratch,
                                 void* stream_) {
-    if (M < 1 || W <= 0 || H <= 0 || !color || !allmap || !world_view_transform || !target_rgb || !loss_terms || !dL_dcolor ||
-        !dL_dallmap || !surf_depth_scratch)
-        return SR_EINVAL;
+    if (M < 1 || W <= 0 || H <= 0) return sr_fail(SR_EINVAL, "sr_render_loss_batch: M, W and H must be positive");
+    if (!color || !allmap || !world_view_transform || !target_rgb || !loss_terms || !dL_dcolor || !dL_dallmap || !surf_depth_scratch)
+        return sr_fail(SR_EINVAL, "sr_render_loss_batch: a required pointer is NULL");
     cudaStream_t s = (cudaStream_t)stream_;
     LossCfg g{W, H, tanx, tany, depth_ratio, w_rgb, w_mask, lambda_normal, lambda_dist};
     dim3 grid((W + 31) / 32, (H + 7) / 8, M);
-    if (cudaMemsetAsync(loss_terms, 0, (size_t)M * 4 * sizeof(float), s) != cudaSuccess) return SR_ECUDA;
-    if (dL_dbkgd && cudaMemsetAsync(dL_dbkgd, 0, (size_t)M * 3 * sizeof(float), s) != cudaSuccess) return SR_ECUDA;
+    CK(cudaMemsetAsync(loss_terms, 0, (size_t)M * 4 * sizeof(float), s), "sr_render_loss_batch: memset(loss_terms)");
+    if (dL_dbkgd) CK(cudaMemsetAsync(dL_dbkgd, 0, (size_t)M * 3 * sizeof(float), s), "sr_render_loss_batch: memset(dL_dbkgd)");
     {
         ProfileScope ps("loss_depth", s);
         loss_depth_kernel<<<grid, 256, 0, s>>>(g, allmap, surf_depth_scratch);
@@ -326,8 +326,7 @@ SR_API int sr_render_loss_batch(int32_t M, int32_t W, int32_t H, float tanx, flo
         loss_grad_kernel<<<grid, 256, 0, s>>>(g, color, allmap, world_view_transform, target_rgb, vis2d, mask_gt, mask_wt,
                                              learnable_bkgd, surf_depth_scratch, loss_terms, dL_dcolor, dL_dallmap, dL_dbkgd);
     }
-    sr_count_launch(2);
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(2, "sr_render_loss_batch");
 }
 
 SR_API int sr_feature_loss_batch(int32_t M, int32_t W, int32_t H, int32_t F, int32_t Cf, int32_t gauss_mask_channel,
@@ -353,8 +352,8 @@ SR_API int sr_feature_loss_batch(int32_t M, int32_t W, int32_t H, int32_t F, int
     cudaStream_t s = (cudaStream_t)stream_;
     const FeatLossCfg g{W, H, F, Cf, gauss_mask_channel};
     dim3 grid((W + 31) / 32, (H + 7) / 8, M);
-    if (cudaMemsetAsync(feature_terms, 0, (size_t)M * 2 * sizeof(float), s) != cudaSuccess) return SR_ECUDA;
-    if (cudaMemsetAsync(counts, 0, (size_t)M * 2 * sizeof(uint32_t), s) != cudaSuccess) return SR_ECUDA;
+    CK(cudaMemsetAsync(feature_terms, 0, (size_t)M * 2 * sizeof(float), s), "sr_feature_loss_batch: memset(feature_terms)");
+    CK(cudaMemsetAsync(counts, 0, (size_t)M * 2 * sizeof(uint32_t), s), "sr_feature_loss_batch: memset(counts)");
     {
         ProfileScope ps("feat_loss", s);
         feat_loss_kernel<<<grid, 256, 0, s>>>(g, features, target, mask_gt, is_detected, allmap, feature_terms, counts,
@@ -364,8 +363,7 @@ SR_API int sr_feature_loss_batch(int32_t M, int32_t W, int32_t H, int32_t F, int
         ProfileScope ps("feat_loss_scale", s);
         feat_loss_scale_kernel<<<grid, 256, 0, s>>>(g, weights, counts, feature_terms, dL_dfeatures);
     }
-    sr_count_launch(2);
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(2, "sr_feature_loss_batch");
 }
 
 }  // extern "C"

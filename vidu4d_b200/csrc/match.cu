@@ -375,7 +375,7 @@ int check_reproj(int32_t M, int32_t H, int32_t W, int32_t B, int32_t hxy_dim, fl
     if (B < 1 || B > 64) return sr_fail(SR_EINVAL, "B must be in [1, 64], got %d", B);
     if (hxy_dim != 2 && hxy_dim != 3) return sr_fail(SR_EINVAL, "hxy_dim must be 2 or 3, got %d", hxy_dim);
     if (!(train_res > 0.f)) return sr_fail(SR_EINVAL, "train_res must be > 0");
-    if (sr_bob_warp_table_floats(B, M) * 2 * sizeof(float) > 200 * 1024)
+    if (sr_bob_warp_table_floats(B, M) * 2 * sizeof(float) > SR_TABLE_SMEM_MAX)
         return sr_fail(SR_EINVAL, "the bone / frame tables of B = %d, M = %d frames do not fit in shared memory", B, M);
     return 0;
 }
@@ -397,8 +397,7 @@ SR_API int sr_global_match_forward(int32_t M, int32_t H, int32_t W, int32_t P, i
         match_fwd_kernel<<<(unsigned)((d.N + MATCH_THREADS - 1) / MATCH_THREADS), MATCH_THREADS, 0, s>>>(
             d, feat_px, regist_feat, xyz, cand, logsigma, xyz_matched, top_idx, top_prob, top_score);
     }
-    sr_count_launch();
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(1, "sr_global_match_forward");
 }
 
 SR_API int sr_global_match_backward(int32_t M, int32_t H, int32_t W, int32_t P, int32_t C, int32_t K, const float* feat_px,
@@ -411,15 +410,12 @@ SR_API int sr_global_match_backward(int32_t M, int32_t H, int32_t W, int32_t P, 
         return sr_fail(SR_EINVAL, "sr_global_match_backward: a required pointer is NULL");
     const MatchDims d{(long long)M * H * W, P, C, K, (long long)M * P};
     cudaStream_t s = (cudaStream_t)stream_;
-    if (cudaMemsetAsync(g_cand, 0, (size_t)C * ROW * sizeof(float), s) != cudaSuccess ||
-        cudaMemsetAsync(g_regist_feat, 0, (size_t)P * FEAT * sizeof(float), s) != cudaSuccess ||
-        cudaMemsetAsync(g_xyz, 0, (size_t)P * 3 * sizeof(float), s) != cudaSuccess ||
-        cudaMemsetAsync(g_logsigma, 0, sizeof(float), s) != cudaSuccess)
-        return SR_ECUDA;
+    CK(cudaMemsetAsync(g_cand, 0, (size_t)C * ROW * sizeof(float), s), "sr_global_match_backward: memset(g_cand)");
+    CK(cudaMemsetAsync(g_regist_feat, 0, (size_t)P * FEAT * sizeof(float), s), "sr_global_match_backward: memset(g_regist_feat)");
+    CK(cudaMemsetAsync(g_xyz, 0, (size_t)P * 3 * sizeof(float), s), "sr_global_match_backward: memset(g_xyz)");
+    CK(cudaMemsetAsync(g_logsigma, 0, sizeof(float), s), "sr_global_match_backward: memset(g_logsigma)");
     const size_t smem = (size_t)C * ROW * sizeof(float);
-    if (smem > 48 * 1024 &&
-        cudaFuncSetAttribute(match_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-        return SR_ECUDA;
+    CK(sr_opt_in_smem(match_bwd_kernel, smem), "sr_global_match_backward: shared-memory opt-in");
     int dev = 0, sms = 132, per_sm = 1;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -436,8 +432,7 @@ SR_API int sr_global_match_backward(int32_t M, int32_t H, int32_t W, int32_t P, 
         ProfileScope ps("match_scatter", s);
         match_scatter_kernel<<<(C * ROW + 255) / 256, 256, 0, s>>>(d, cand, g_cand, g_regist_feat, g_xyz);
     }
-    sr_count_launch(2);
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(2, "sr_global_match_backward");
 }
 
 SR_API int sr_reproj_loss_forward(int32_t M, int32_t H, int32_t W, int32_t B, int32_t hxy_dim, float train_res,
@@ -452,14 +447,12 @@ SR_API int sr_reproj_loss_forward(int32_t M, int32_t H, int32_t W, int32_t B, in
         return sr_fail(SR_EINVAL, "sr_reproj_loss_forward: a required pointer is NULL");
     const ReprojDims d{M, H * W, B, hxy_dim};
     cudaStream_t s = (cudaStream_t)stream_;
-    if (cudaMemsetAsync(terms, 0, (size_t)M * sizeof(float), s) != cudaSuccess ||
-        cudaMemsetAsync(counts, 0, (size_t)M * sizeof(uint32_t), s) != cudaSuccess)
-        return SR_ECUDA;
+    CK(cudaMemsetAsync(terms, 0, (size_t)M * sizeof(float), s), "sr_reproj_loss_forward: memset(terms)");
+    CK(cudaMemsetAsync(counts, 0, (size_t)M * sizeof(uint32_t), s), "sr_reproj_loss_forward: memset(counts)");
     const size_t smem = sr_bob_warp_table_floats(B, M) * sizeof(float);
     const dim3 grid((d.HW + REPROJ_THREADS - 1) / REPROJ_THREADS, M);
     auto launch = [&](auto kern) -> int {
-        if (smem > 48 * 1024 && cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-            return SR_ECUDA;
+        CK(sr_opt_in_smem(kern, smem), "sr_reproj_loss_forward: shared-memory opt-in");
         ProfileScope ps("reproj_fwd", s);
         kern<<<grid, REPROJ_THREADS, smem, s>>>(d, xyz_matched, o2b_q, o2b_t, inv_gauss, delta, se3_r, se3_d, cam_q, cam_t, Kmat,
                                                 hxy, mask, is_detected, xy_reproj, terms, counts);
@@ -470,8 +463,7 @@ SR_API int sr_reproj_loss_forward(int32_t M, int32_t H, int32_t W, int32_t B, in
         ProfileScope ps("reproj_scale", s);
         reproj_scale_kernel<<<1, 32, 0, s>>>(M, train_res, weight, counts, terms, scale, loss);
     }
-    sr_count_launch(2);
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(2, "sr_reproj_loss_forward");
 }
 
 SR_API int sr_reproj_loss_backward(int32_t M, int32_t H, int32_t W, int32_t B, int32_t hxy_dim, const float* xyz_matched,
@@ -488,20 +480,18 @@ SR_API int sr_reproj_loss_backward(int32_t M, int32_t H, int32_t W, int32_t B, i
     const ReprojDims d{M, H * W, B, hxy_dim};
     cudaStream_t s = (cudaStream_t)stream_;
     const size_t nt = sr_bob_warp_table_floats(B, M);
-    if (cudaMemsetAsync(g_tables, 0, nt * sizeof(float), s) != cudaSuccess) return SR_ECUDA;
+    CK(cudaMemsetAsync(g_tables, 0, nt * sizeof(float), s), "sr_reproj_loss_backward: memset(g_tables)");
     const size_t smem = 2 * nt * sizeof(float);
     const dim3 grid((d.HW + REPROJ_THREADS - 1) / REPROJ_THREADS, M);
     auto launch = [&](auto kern) -> int {
-        if (smem > 48 * 1024 && cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-            return SR_ECUDA;
+        CK(sr_opt_in_smem(kern, smem), "sr_reproj_loss_backward: shared-memory opt-in");
         ProfileScope ps("reproj_bwd", s);
         kern<<<grid, REPROJ_THREADS, smem, s>>>(d, xyz_matched, o2b_q, o2b_t, inv_gauss, delta, se3_r, se3_d, cam_q, cam_t, Kmat,
                                                 hxy, mask, is_detected, scale, g_loss, g_xyz_matched, g_delta, g_tables);
         return 0;
     };
     if (int rc = B <= 32 ? launch(reproj_bwd_kernel<32>) : launch(reproj_bwd_kernel<64>)) return rc;
-    sr_count_launch();
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(1, "sr_reproj_loss_backward");
 }
 
 }  // extern "C"

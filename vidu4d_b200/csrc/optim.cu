@@ -112,8 +112,11 @@ extern "C" {
 SR_API int sr_adam_flat(int32_t n_groups, const int64_t* begin /* host, n_groups + 1 */, const float* lr /* host, n_groups */,
                         float beta1, float beta2, float eps, int64_t step, float grad_scale, float* params, const float* grads,
                         float* exp_avg, float* exp_avg_sq, void* stream_) {
-    if (n_groups < 1 || n_groups > MAXG || !begin || !lr || !params || !grads || !exp_avg || !exp_avg_sq || step < 1) return SR_EINVAL;
-    if (((uintptr_t)params | (uintptr_t)grads | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) & 15) return SR_EINVAL;
+    if (n_groups < 1 || n_groups > MAXG) return sr_fail(SR_EINVAL, "sr_adam_flat: n_groups must be in [1, %d], got %d", MAXG, n_groups);
+    if (!begin || !lr || !params || !grads || !exp_avg || !exp_avg_sq) return sr_fail(SR_EINVAL, "sr_adam_flat: a required pointer is NULL");
+    if (step < 1) return sr_fail(SR_EINVAL, "sr_adam_flat: step must be >= 1, got %lld", (long long)step);
+    if (((uintptr_t)params | (uintptr_t)grads | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) & 15)
+        return sr_fail(SR_EINVAL, "sr_adam_flat: params, grads, exp_avg and exp_avg_sq must be 16-byte aligned");
     AdamGroups G{};
     G.n = n_groups;
     for (int i = 0; i <= n_groups; i++) G.begin[i] = begin[i];
@@ -128,8 +131,7 @@ SR_API int sr_adam_flat(int32_t n_groups, const int64_t* begin /* host, n_groups
     // grid-stride: at most 16 CTAs per SM of an H100 SXM (132 SMs)
     adam_flat_kernel<<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, s>>>(G, params, grads, exp_avg, exp_avg_sq, beta1,
                                                                                        beta2, eps, bc1, sqrt_bc2, grad_scale);
-    sr_count_launch();
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(1, "sr_adam_flat");
 }
 
 /* Gather the surfel rows of every parameter group (and both Adam moments) into new flat buffers: new row s = old row
@@ -139,9 +141,13 @@ SR_API int sr_surfel_compact(int32_t n_groups, const int32_t* width, const int64
                              int32_t xyz_group, int32_t scaling_group, int32_t P_new, const int32_t* src, const uint8_t* kind,
                              const int32_t* child_slot, const float* child_xyz, const float* child_scaling, const float* p_old,
                              const float* m_old, const float* v_old, float* p_new, float* m_new, float* v_new, void* stream_) {
-    if (n_groups < 1 || n_groups > MAXG || !width || !old_begin || !new_begin || P_new < 0) return SR_EINVAL;
+    if (n_groups < 1 || n_groups > MAXG)
+        return sr_fail(SR_EINVAL, "sr_surfel_compact: n_groups must be in [1, %d], got %d", MAXG, n_groups);
+    if (!width || !old_begin || !new_begin) return sr_fail(SR_EINVAL, "sr_surfel_compact: width / old_begin / new_begin is NULL");
+    if (P_new < 0) return sr_fail(SR_EINVAL, "sr_surfel_compact: P_new must be >= 0, got %d", P_new);
     if (P_new == 0) return 0;
-    if (!src || !kind || !p_old || !m_old || !v_old || !p_new || !m_new || !v_new) return SR_EINVAL;
+    if (!src || !kind || !p_old || !m_old || !v_old || !p_new || !m_new || !v_new)
+        return sr_fail(SR_EINVAL, "sr_surfel_compact: a required pointer is NULL");
     CompactGroups G{};
     G.n = n_groups; G.xyz_group = xyz_group; G.scaling_group = scaling_group;
     for (int i = 0; i < n_groups; i++) { G.width[i] = width[i]; G.old_begin[i] = old_begin[i]; G.new_begin[i] = new_begin[i]; }
@@ -149,8 +155,7 @@ SR_API int sr_surfel_compact(int32_t n_groups, const int32_t* width, const int64
     ProfileScope ps("surfel_compact", s);
     compact_kernel<<<(P_new + 7) / 8, 256, 0, s>>>(G, P_new, src, kind, child_slot, child_xyz, child_scaling, p_old, m_old, v_old,
                                                    p_new, m_new, v_new);
-    sr_count_launch();
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(1, "sr_surfel_compact");
 }
 
 }  // extern "C"

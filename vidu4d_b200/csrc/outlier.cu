@@ -147,8 +147,8 @@ SR_API int sr_radius_outlier_mask(int32_t P, const float* points, double radius,
     cub::DoubleBuffer<uint64_t> keys((uint64_t*)(base + L.keys[0]), (uint64_t*)(base + L.keys[1]));
     cub::DoubleBuffer<int> idx((int*)(base + L.idx[0]), (int*)(base + L.idx[1]));
     size_t cub_bytes = 0;
-    if (cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, keys, idx, (int)P, 0, 3 * RO_BITS) != cudaSuccess)
-        return sr_fail(SR_ECUDA, "sr_radius_outlier_mask: cub radix sort size query failed");
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, keys, idx, (int)P, 0, 3 * RO_BITS),
+       "sr_radius_outlier_mask: cub radix sort size query");
     if (cub_bytes > L.total - L.cub)
         return sr_fail(SR_ECUDA, "sr_radius_outlier_mask: cub needs more temporary storage than reserved for P = %d", P);
     cudaStream_t s = (cudaStream_t)stream_;
@@ -160,8 +160,7 @@ SR_API int sr_radius_outlier_mask(int32_t P, const float* points, double radius,
     {
         ProfileScope ps("outlier_sort", s);
         size_t tb = L.total - L.cub;
-        if (cub::DeviceRadixSort::SortPairs(base + L.cub, tb, keys, idx, (int)P, 0, 3 * RO_BITS, s) != cudaSuccess)
-            return sr_fail(SR_ECUDA, "sr_radius_outlier_mask: cub radix sort failed");
+        CK(cub::DeviceRadixSort::SortPairs(base + L.cub, tb, keys, idx, (int)P, 0, 3 * RO_BITS, s), "sr_radius_outlier_mask: cub radix sort");
     }
     float4* sorted = (float4*)(base + L.sorted);
     {
@@ -173,8 +172,7 @@ SR_API int sr_radius_outlier_mask(int32_t P, const float* points, double radius,
         ro_query_kernel<<<nb, RO_THREADS, 0, s>>>(P, sorted, keys.Current(), idx.Current(), inv_h, r2, (long long)nb_points + 1,
                                                   keep, counts);
     }
-    sr_count_launch(3);
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(3, "sr_radius_outlier_mask");
 }
 
 }  // extern "C"

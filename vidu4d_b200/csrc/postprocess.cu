@@ -135,6 +135,9 @@ extern "C" {
 SR_API int sr_post_forward(int32_t W, int32_t H, float tanx, float tany, float depth_ratio, const float* allmap,
                            const float* world_view_transform, float* acc, float* rend_normal, float* rend_dist,
                            float* depth_median, float* depth_expected, float* surf_depth, float* surf_normal, void* stream_) {
+    if (!allmap || !world_view_transform || !acc || !rend_normal || !rend_dist || !depth_median || !depth_expected || !surf_depth ||
+        !surf_normal)
+        return sr_fail(SR_EINVAL, "sr_post_forward: a required pointer is NULL");
     cudaStream_t s = (cudaStream_t)stream_;
     dim3 grid((W + 31) / 32, (H + 7) / 8);
     {
@@ -144,8 +147,7 @@ SR_API int sr_post_forward(int32_t W, int32_t H, float tanx, float tany, float d
     }
     ProfileScope ps("post_normal", s);
     post_normal_kernel<<<grid, 256, 0, s>>>(W, H, tanx, tany, allmap, world_view_transform, surf_depth, surf_normal);
-    sr_count_launch(2);
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(2, "sr_post_forward");
 }
 
 SR_API int sr_post_backward(int32_t W, int32_t H, float tanx, float tany, float depth_ratio, const float* allmap,
@@ -153,14 +155,16 @@ SR_API int sr_post_backward(int32_t W, int32_t H, float tanx, float tany, float 
                             const float* g_rend_normal, const float* g_rend_dist, const float* g_depth_median,
                             const float* g_depth_expected, const float* g_surf_depth, const float* g_surf_normal,
                             float* g_allmap, void* stream_) {
+    if (!allmap || !world_view_transform || !surf_depth || !g_acc || !g_rend_normal || !g_rend_dist || !g_depth_median ||
+        !g_depth_expected || !g_surf_depth || !g_surf_normal || !g_allmap)
+        return sr_fail(SR_EINVAL, "sr_post_backward: a required pointer is NULL");
     cudaStream_t s = (cudaStream_t)stream_;
     dim3 grid((W + 31) / 32, (H + 7) / 8);
     ProfileScope ps("post_bwd", s);
     post_bwd_kernel<<<grid, 256, 0, s>>>(W, H, tanx, tany, depth_ratio, allmap, world_view_transform, surf_depth, g_acc,
                                         g_rend_normal, g_rend_dist, g_depth_median, g_depth_expected, g_surf_depth,
                                         g_surf_normal, g_allmap);
-    sr_count_launch();
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    return sr_launched(1, "sr_post_backward");
 }
 
 }  // extern "C"

@@ -423,10 +423,7 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D, co
 cudaError_t launch_preprocess_fwd(const FwdArgs& a) {
     const int nb = a.gl.nblocks;
     const size_t smem = a.colors_precomp ? 0 : (size_t)256 * (3 * a.cam.M + 1) * sizeof(float);
-    if (smem > 48 * 1024) {   // > 48 KB dynamic shared memory is an opt-in per device context: cheap, not a stream operation
-        cudaError_t e = cudaFuncSetAttribute(preprocess_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-    }
+    if (cudaError_t e = sr_opt_in_smem(preprocess_fwd_kernel, smem)) return e;
     ProfileScope ps("preprocess_fwd", a.stream);
     preprocess_fwd_kernel<<<nb, 256, smem, a.stream>>>(
         a.cam, a.fs, a.means3D, a.shs, a.colors_precomp, a.opacities, (const float2*)a.scales, (const float4*)a.rotations,

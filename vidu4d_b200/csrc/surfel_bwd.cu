@@ -333,10 +333,7 @@ surfel_bwd_body(const CamParams& c, const int idx, const int M, const float* shv
 cudaError_t launch_surfel_bwd(const BwdArgs& a) {
     const int nb = (a.cam.P + SB - 1) / SB;
     const size_t smem = (size_t)2 * SB * (3 * a.cam.M + 1) * sizeof(float);
-    if (smem > 48 * 1024) {   // per device context; cheap, not a stream operation
-        cudaError_t e = cudaFuncSetAttribute(surfel_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-    }
+    if (cudaError_t e = sr_opt_in_smem(surfel_bwd_kernel, smem)) return e;
     ProfileScope ps("surfel_bwd", a.stream);
     surfel_bwd_kernel<<<nb, SB, smem, a.stream>>>(
         a.cam, a.fs, a.means3D, a.shs, (const float2*)a.scales, (const float4*)a.rotations, a.radii,

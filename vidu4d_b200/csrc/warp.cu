@@ -186,6 +186,13 @@ bob_warp_bwd_kernel(const WarpDims d, const float* __restrict__ xyz, const float
         if (gacc[i] != 0.f) atomicAdd(g_tables + i, gacc[i]);
 }
 
+int check_warp(int32_t P, int32_t B, int32_t M) {
+    if (P < 0) return sr_fail(SR_EINVAL, "P must be >= 0, got %d", P);
+    if (B < 1 || B > 64) return sr_fail(SR_EINVAL, "B must be in [1, 64], got %d", B);
+    if (M < 1) return sr_fail(SR_EINVAL, "M must be >= 1, got %d", M);
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -196,25 +203,25 @@ SR_API int sr_bob_warp_forward(int32_t P, int32_t B, int32_t M, const float* xyz
                                const float* o2b_t, const float* inv_gauss, const float* delta, const float* se3_r,
                                const float* se3_d, const float* cam_q, const float* cam_t, float* xyz_cam, float* rot_cam,
                                float* skin_entropy, void* stream_) {
-    if (P < 0 || B < 1 || B > 64 || M < 1) return SR_EINVAL;
+    if (int rc = check_warp(P, B, M)) return rc;
     if (P == 0) return 0;
-    if (!xyz || !rot || !o2b_q || !o2b_t || !inv_gauss || !se3_r || !se3_d || !cam_q || !cam_t || !xyz_cam || !rot_cam) return SR_EINVAL;
-    if (((uintptr_t)rot_cam & 15)) return SR_EINVAL;
+    if (!xyz || !rot || !o2b_q || !o2b_t || !inv_gauss || !se3_r || !se3_d || !cam_q || !cam_t || !xyz_cam || !rot_cam)
+        return sr_fail(SR_EINVAL, "sr_bob_warp_forward: a required pointer is NULL");
+    if (((uintptr_t)rot_cam & 15)) return sr_fail(SR_EINVAL, "sr_bob_warp_forward: rot_cam must be 16-byte aligned");
     const WarpDims d{P, B, M};
     const size_t smem = sr_bob_warp_table_floats(B, M) * sizeof(float);
-    if (smem > 200 * 1024) return SR_EINVAL;          // split the frames over several calls
+    if (smem > SR_TABLE_SMEM_MAX)                    // split the frames over several calls
+        return sr_fail(SR_EINVAL, "sr_bob_warp_forward: the tables of B = %d, M = %d frames do not fit in shared memory", B, M);
     cudaStream_t s = (cudaStream_t)stream_;
     ProfileScope ps("bob_warp_fwd", s);
     auto launch = [&](auto kern) -> int {
-        if (smem > 48 * 1024 && cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return SR_ECUDA;
+        CK(sr_opt_in_smem(kern, smem), "sr_bob_warp_forward: shared-memory opt-in");
         kern<<<(P + 255) / 256, 256, smem, s>>>(d, xyz, rot, o2b_q, o2b_t, inv_gauss, delta, se3_r, se3_d, cam_q, cam_t, xyz_cam,
                                                  rot_cam, skin_entropy);
         return 0;
     };
-    const int rc = B <= 32 ? launch(bob_warp_fwd_kernel<32>) : launch(bob_warp_fwd_kernel<64>);
-    if (rc) return rc;
-    sr_count_launch();
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    if (int rc = B <= 32 ? launch(bob_warp_fwd_kernel<32>) : launch(bob_warp_fwd_kernel<64>)) return rc;
+    return sr_launched(1, "sr_bob_warp_forward");
 }
 
 /* g_tables: float[sr_bob_warp_table_floats(B, M)], laid out o2b_q[B*4] o2b_t[B*3] inv_gauss[B*3] se3_r[M*B*4] se3_d[M*B*4]
@@ -224,31 +231,32 @@ SR_API int sr_bob_warp_backward(int32_t P, int32_t B, int32_t M, const float* xy
                                 const float* se3_d, const float* cam_q, const float* cam_t, const float* g_xyz_cam,
                                 const float* g_rot_cam, const float* g_entropy, float* g_xyz, float* g_rot, float* g_delta,
                                 float* g_tables, void* stream_) {
-    if (P < 0 || B < 1 || B > 64 || M < 1) return SR_EINVAL;
-    if (!g_tables) return SR_EINVAL;
+    if (int rc = check_warp(P, B, M)) return rc;
+    if (!g_tables) return sr_fail(SR_EINVAL, "sr_bob_warp_backward: g_tables is NULL");
     cudaStream_t s = (cudaStream_t)stream_;
     const size_t nt = sr_bob_warp_table_floats(B, M);
-    if (cudaMemsetAsync(g_tables, 0, nt * sizeof(float), s) != cudaSuccess) return SR_ECUDA;
+    CK(cudaMemsetAsync(g_tables, 0, nt * sizeof(float), s), "sr_bob_warp_backward: memset(g_tables)");
     if (P == 0) return 0;
     if (!xyz || !rot || !o2b_q || !o2b_t || !inv_gauss || !se3_r || !se3_d || !cam_q || !cam_t || !g_xyz_cam || !g_rot_cam ||
         !g_xyz || !g_rot)
-        return SR_EINVAL;
-    if (((uintptr_t)g_rot_cam & 15) || ((uintptr_t)g_rot & 15)) return SR_EINVAL;
+        return sr_fail(SR_EINVAL, "sr_bob_warp_backward: a required pointer is NULL");
+    if (((uintptr_t)g_rot_cam & 15) || ((uintptr_t)g_rot & 15))
+        return sr_fail(SR_EINVAL, "sr_bob_warp_backward: g_rot_cam and g_rot must be 16-byte aligned");
     const WarpDims d{P, B, M};
     const size_t smem = 2 * nt * sizeof(float);
-    if (smem > 200 * 1024) return SR_EINVAL;
+    if (smem > SR_TABLE_SMEM_MAX)
+        return sr_fail(SR_EINVAL, "sr_bob_warp_backward: the tables and their gradients of B = %d, M = %d frames do not fit in "
+                       "shared memory", B, M);
     ProfileScope ps("bob_warp_bwd", s);
     auto launch = [&](auto kern) -> int {
-        if (smem > 48 * 1024 && cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return SR_ECUDA;
+        CK(sr_opt_in_smem(kern, smem), "sr_bob_warp_backward: shared-memory opt-in");
         // 128-thread blocks: the kernel holds ~200 registers per thread (B weights + B weight gradients)
         kern<<<(P + 127) / 128, 128, smem, s>>>(d, xyz, rot, o2b_q, o2b_t, inv_gauss, delta, se3_r, se3_d, cam_q, cam_t, g_xyz_cam,
                                                  g_rot_cam, g_entropy, g_xyz, g_rot, g_delta, g_tables);
         return 0;
     };
-    const int rc = B <= 32 ? launch(bob_warp_bwd_kernel<32>) : launch(bob_warp_bwd_kernel<64>);
-    if (rc) return rc;
-    sr_count_launch();
-    return cudaGetLastError() == cudaSuccess ? 0 : SR_ECUDA;
+    if (int rc = B <= 32 ? launch(bob_warp_bwd_kernel<32>) : launch(bob_warp_bwd_kernel<64>)) return rc;
+    return sr_launched(1, "sr_bob_warp_backward");
 }
 
 }  // extern "C"

@@ -26,10 +26,7 @@ def distCUDA2(points: torch.Tensor) -> torch.Tensor:
     bmin = (C.c_float * 3)(*[float(v) for v in lo]); bmax = (C.c_float * 3)(*[float(v) for v in hi])
     cells = int(lib.sr_knn_cells(P, bmin, bmax, None, None))
     scratch = torch.empty((2 * P + 3 * cells,), dtype=torch.int32, device=pts.device)
-    with torch.cuda.device(pts.device):
-        rc = lib.sr_knn_mean_dist2(P, pts.data_ptr(), bmin, bmax, out.data_ptr(), scratch.data_ptr(),
-                                   torch.cuda.current_stream(pts.device).cuda_stream)
-    _capi.check(rc, "sr_knn_mean_dist2")
+    _capi.call("sr_knn_mean_dist2", pts.device, P, pts, bmin, bmax, out, scratch)
     return out
 
 
@@ -51,10 +48,6 @@ def radius_outlier_mask(points: torch.Tensor, nb_points: int = 20, radius: float
     counts = torch.empty((P,), dtype=torch.int32, device=pts.device) if return_counts else None
     nbytes = int(lib.sr_radius_outlier_scratch_bytes(P))
     scratch = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=pts.device)
-    with torch.cuda.device(pts.device):
-        rc = lib.sr_radius_outlier_mask(P, pts.data_ptr(), float(radius), int(nb_points), keep.data_ptr(),
-                                        None if counts is None else counts.data_ptr(), scratch.data_ptr(), nbytes,
-                                        torch.cuda.current_stream(pts.device).cuda_stream)
-    _capi.check(rc, "sr_radius_outlier_mask")
+    _capi.call("sr_radius_outlier_mask", pts.device, P, pts, float(radius), int(nb_points), keep, counts, scratch, nbytes)
     prune = keep == 0
     return (prune, counts) if return_counts else prune

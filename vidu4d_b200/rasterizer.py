@@ -260,13 +260,10 @@ def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, sc
             nosync = (not _sync_mode) and key in _cap_hint
             host = _host_slot(M) if nosync else torch.empty((M, 2), dtype=torch.int32, pin_memory=True)
             # an overflow re-run below re-runs the feature pass too
-            rc = lib.sr_forward(
-                C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh), _ptr(colors),
-                _ptr(opacity), _ptr(scales), _ptr(rotations), _ptr(features), F, strides.get("features", 0),
-                _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), out_color.data_ptr(), cstride, _ptr(out_feat), fstride,
-                out_others.data_ptr(), _ptr(radii), geom.data_ptr(), binning.data_ptr(), img.data_ptr(), cap,
-                nr_dev.data_ptr(), host.data_ptr(), stream.cuda_stream)
-            _capi.check(rc, "sr_forward")
+            _capi.call("sr_forward", dev, C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh),
+                       _ptr(colors), _ptr(opacity), _ptr(scales), _ptr(rotations), _ptr(features), F, strides.get("features", 0),
+                       _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), out_color, cstride, _ptr(out_feat), fstride, out_others,
+                       _ptr(radii), geom, binning, img, cap, nr_dev, host)
             if nosync:
                 _pending.append((host, key, cap, stream))
                 if len(_pending) > _MAX_PENDING:
@@ -298,7 +295,6 @@ def _backward(M, frame_dim, strides, background, means3D, sh, colors, scales, ro
     or the tail of dL_dout_color when that is None.  Each gradient is (M,P,.), or (P,.) without frame_dim and, under
     sum_shared, for an input the frames share.  Returns (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D,
     dL_dtransMat, dL_dsh, dL_dscales, dL_drotations), and dL_dfeatures ninth when there are features."""
-    lib = _capi.load()
     dev = means3D.device
     P, H, W = int(means3D.shape[-2]), int(dL_dout_color.shape[-2]), int(dL_dout_color.shape[-1])
     N = H * W
@@ -337,15 +333,12 @@ def _backward(M, frame_dim, strides, background, means3D, sh, colors, scales, ro
                 gs = grad_scale.to(device=dev, dtype=torch.float32).reshape(()).contiguous()
             if F and features_grad_scale is not None:
                 fgs = features_grad_scale.to(device=dev, dtype=torch.float32).reshape(()).contiguous()
-            rc = lib.sr_backward(
-                C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh), _ptr(colors),
-                _ptr(scales), _ptr(rotations), _ptr(features), F, strides.get("features", 0), _ptr(viewmatrix),
-                _ptr(projmatrix), _ptr(campos), _ptr(radii), _ptr(dL_dout_color), cstride, dfeat_ptr, fstride,
-                _ptr(dL_dout_others), _ptr(gs), _ptr(fgs), geomBuffer.data_ptr(), binningBuffer.data_ptr(),
-                imageBuffer.data_ptr(), cap, dL_dmeans2D.data_ptr(), dL_dcolors.data_ptr(), dL_dopacity.data_ptr(),
-                dL_dmeans3D.data_ptr(), _ptr(dL_dtransMat), _ptr(dL_dsh), dL_dscales.data_ptr(), dL_drotations.data_ptr(),
-                _ptr(dL_dfeatures), torch.cuda.current_stream(dev).cuda_stream)
-            _capi.check(rc, "sr_backward")
+            _capi.call("sr_backward", dev, C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D),
+                       _ptr(sh), _ptr(colors), _ptr(scales), _ptr(rotations), _ptr(features), F, strides.get("features", 0),
+                       _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), _ptr(radii), _ptr(dL_dout_color), cstride, dfeat_ptr,
+                       fstride, _ptr(dL_dout_others), _ptr(gs), _ptr(fgs), geomBuffer, binningBuffer, imageBuffer, cap,
+                       dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, _ptr(dL_dtransMat), _ptr(dL_dsh), dL_dscales,
+                       dL_drotations, _ptr(dL_dfeatures))
     grads = (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales, dL_drotations)
     return grads + (dL_dfeatures,) if F else grads
 
@@ -493,17 +486,13 @@ class _CNamespace:
 
     @staticmethod
     def mark_visible(means3D, viewmatrix, projmatrix):
-        lib = _capi.load()
         dev = means3D.device
         P = int(means3D.shape[0])
         present = torch.zeros((P,), dtype=torch.bool, device=dev)
         if P:
             means3D = _f32c(means3D, "means3D"); viewmatrix = _f32c(viewmatrix, "viewmatrix")
             projmatrix = _f32c(projmatrix, "projmatrix")
-            with torch.cuda.device(dev):
-                rc = lib.sr_mark_visible(P, _ptr(means3D), _ptr(viewmatrix), _ptr(projmatrix), present.data_ptr(),
-                                         torch.cuda.current_stream(dev).cuda_stream)
-            _capi.check(rc, "sr_mark_visible")
+            _capi.call("sr_mark_visible", dev, P, _ptr(means3D), _ptr(viewmatrix), _ptr(projmatrix), present)
         return present
 
 

@@ -22,11 +22,10 @@ from __future__ import annotations
 import torch
 
 from . import _capi
-from .warp import split_table_grads, warp_tables
+from .warp import B_MAX, check_articulations, split_table_grads, warp_tables
 
 FEAT = 16          # width of the registration feature (_regist_feat)
 NUM_GRAD_MAX = 8
-B_MAX = 64
 
 
 def draw_candidates(M: int, P: int, num_candidates: int = 2048, generator=None, device=None):
@@ -36,14 +35,6 @@ def draw_candidates(M: int, P: int, num_candidates: int = 2048, generator=None, 
     C = min(int(num_candidates), M * P)
     gdev = generator.device if generator is not None else "cpu"
     return torch.randperm(M * P, generator=generator, device=gdev)[:C].to(device=device, dtype=torch.int32)
-
-
-def _ptr(t):
-    return None if t is None else t.data_ptr()
-
-
-def _stream(dev):
-    return torch.cuda.current_stream(dev).cuda_stream
 
 
 def _check_match(feat_px, regist_feat, xyz, cand, logsigma, num_grad):
@@ -63,14 +54,8 @@ def _check_match(feat_px, regist_feat, xyz, cand, logsigma, num_grad):
     C = int(cand.shape[0])
     if not isinstance(num_grad, int) or isinstance(num_grad, bool) or not 1 <= num_grad <= min(NUM_GRAD_MAX, C):
         raise RuntimeError(f"num_grad must be an int in [1, min({NUM_GRAD_MAX}, C = {C})], got {num_grad!r}")
-    for name, t in (("feat_px", feat_px), ("regist_feat", regist_feat), ("xyz", xyz), ("logsigma", logsigma)):
-        if t.dtype != torch.float32:
-            raise RuntimeError(f"{name} must be float32, got {t.dtype}")
-    for name, t in (("feat_px", feat_px), ("regist_feat", regist_feat), ("xyz", xyz), ("cand", cand), ("logsigma", logsigma)):
-        if not t.is_cuda:
-            raise RuntimeError(f"{name} must be a CUDA tensor (there is no CPU fallback)")
-        if t.device != feat_px.device:
-            raise RuntimeError(f"{name} is on {t.device}, feat_px on {feat_px.device}")
+    floats = (("feat_px", feat_px), ("regist_feat", regist_feat), ("xyz", xyz), ("logsigma", logsigma))
+    _capi.check_tensors(floats[:3] + (("cand", cand),) + floats[3:], "feat_px", feat_px, floats=floats)
     return M, int(feat_px.shape[1]), int(feat_px.shape[2]), P, C
 
 
@@ -78,17 +63,14 @@ class _GlobalMatch(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feat_px, regist_feat, xyz, cand, logsigma, dims):
         M, H, W, P, C, K = dims
-        lib = _capi.load()
         feat_px, regist_feat, xyz, cand, logsigma = (t.detach().contiguous() for t in (feat_px, regist_feat, xyz, cand, logsigma))
         dev = feat_px.device
         xyz_m = torch.empty((M, H, W, 3), dtype=torch.float32, device=dev)
         idx = torch.empty((M, H, W, K), dtype=torch.int32, device=dev)
         prob = torch.empty((M, H, W, K), dtype=torch.float32, device=dev)
         score = torch.empty((M, H, W, K), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            rc = lib.sr_global_match_forward(M, H, W, P, C, K, _ptr(feat_px), _ptr(regist_feat), _ptr(xyz), _ptr(cand),
-                                             _ptr(logsigma), _ptr(xyz_m), _ptr(idx), _ptr(prob), _ptr(score), _stream(dev))
-        _capi.check(rc, "sr_global_match_forward")
+        _capi.call("sr_global_match_forward", dev, M, H, W, P, C, K, feat_px, regist_feat, xyz, cand, logsigma, xyz_m, idx, prob,
+                   score)
         ctx.dims = dims
         ctx.save_for_backward(feat_px, xyz, cand, logsigma, idx, prob, score)
         ctx.mark_non_differentiable(idx, prob)
@@ -106,12 +88,8 @@ class _GlobalMatch(torch.autograd.Function):
         g_rf = torch.empty((P, FEAT), dtype=torch.float32, device=dev)
         g_xyz = torch.empty((P, 3), dtype=torch.float32, device=dev)
         g_log = torch.empty((1,), dtype=torch.float32, device=dev)
-        lib = _capi.load()
-        with torch.cuda.device(dev):
-            rc = lib.sr_global_match_backward(M, H, W, P, C, K, _ptr(feat_px), _ptr(xyz), _ptr(cand), _ptr(logsigma), _ptr(idx),
-                                              _ptr(prob), _ptr(score), _ptr(g), _ptr(g_cand), _ptr(g_rf), _ptr(g_xyz),
-                                              _ptr(g_log), _stream(dev))
-        _capi.check(rc, "sr_global_match_backward")
+        _capi.call("sr_global_match_backward", dev, M, H, W, P, C, K, feat_px, xyz, cand, logsigma, idx, prob, score, g, g_cand,
+                   g_rf, g_xyz, g_log)
         return None, g_rf, g_xyz, None, g_log.view(logsigma.shape), None
 
 
@@ -144,11 +122,7 @@ def _check_reproj(xyz_m, hxy, Kmat, rest_articulation, t_articulation, log_gauss
     B = int(log_gauss.shape[0])
     if not 1 <= B <= B_MAX or tuple(log_gauss.shape) != (B, 3):
         raise RuntimeError(f"log_gauss must be (B,3) with 1 <= B <= {B_MAX}, got {tuple(log_gauss.shape)}")
-    for name, pair, shapes in (("rest_articulation", rest_articulation, ((B, 4), (B, 4))),
-                               ("t_articulation", t_articulation, ((M, B, 4), (M, B, 4))),
-                               ("field2cam", field2cam, ((M, 4), (M, 3)))):
-        if len(pair) != 2 or tuple(pair[0].shape) != shapes[0] or tuple(pair[1].shape) != shapes[1]:
-            raise RuntimeError(f"{name} must be tensors of shapes {shapes}, got {[tuple(t.shape) for t in pair]}")
+    check_articulations(B, M, rest_articulation, t_articulation, field2cam)
     if delta is not None and tuple(delta.shape) != (M, H, W, B):
         raise RuntimeError(f"delta must be (M,H,W,B) = ({M},{H},{W},{B}), got {tuple(delta.shape)}")
     if torch.is_tensor(weight) and (weight.numel() != 1 or weight.dtype != torch.float32):
@@ -160,11 +134,7 @@ def _check_reproj(xyz_m, hxy, Kmat, rest_articulation, t_articulation, log_gauss
              ("t_articulation", t_articulation[0]), ("t_articulation", t_articulation[1]), ("field2cam", field2cam[0]),
              ("field2cam", field2cam[1])]
     named += [(n, t) for n, t in (("is_detected", is_detected), ("delta", delta), ("weight", weight)) if torch.is_tensor(t)]
-    for name, t in named:
-        if not t.is_cuda:
-            raise RuntimeError(f"{name} must be a CUDA tensor (there is no CPU fallback)")
-        if t.device != xyz_m.device:
-            raise RuntimeError(f"{name} is on {t.device}, xyz_matched on {xyz_m.device}")
+    _capi.check_tensors(named, "xyz_matched", xyz_m, floats=())     # the forward converts to float32
     return M, H, W, B
 
 
@@ -172,7 +142,6 @@ class _ReprojLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz_m, o2b_q, o2b_t, inv_gauss, se3_r, se3_d, cam_q, cam_t, delta, Kmat, hxy, mask, det, weight, cfg):
         M, H, W, B, train_res = cfg
-        lib = _capi.load()
         f = lambda t: None if t is None else t.detach().to(torch.float32).contiguous()  # noqa: E731
         ins = tuple(map(f, (xyz_m, o2b_q, o2b_t, inv_gauss, se3_r, se3_d, cam_q, cam_t, delta, Kmat, hxy, mask, det, weight)))
         xyz_m, o2b_q, o2b_t, inv_gauss, se3_r, se3_d, cam_q, cam_t, delta, Kmat, hxy, mask, det, weight = ins
@@ -182,12 +151,8 @@ class _ReprojLoss(torch.autograd.Function):
         counts = torch.empty((M,), dtype=torch.int32, device=dev)
         scale = torch.empty((1,), dtype=torch.float32, device=dev)
         loss = torch.empty((), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            rc = lib.sr_reproj_loss_forward(M, H, W, B, int(hxy.shape[-1]), float(train_res), _ptr(xyz_m), _ptr(o2b_q),
-                                            _ptr(o2b_t), _ptr(inv_gauss), _ptr(delta), _ptr(se3_r), _ptr(se3_d), _ptr(cam_q),
-                                            _ptr(cam_t), _ptr(Kmat), _ptr(hxy), _ptr(mask), _ptr(det), _ptr(weight), _ptr(xy),
-                                            _ptr(terms), _ptr(counts), _ptr(scale), _ptr(loss), _stream(dev))
-        _capi.check(rc, "sr_reproj_loss_forward")
+        _capi.call("sr_reproj_loss_forward", dev, M, H, W, B, int(hxy.shape[-1]), float(train_res), xyz_m, o2b_q, o2b_t, inv_gauss,
+                   delta, se3_r, se3_d, cam_q, cam_t, Kmat, hxy, mask, det, weight, xy, terms, counts, scale, loss)
         ctx.cfg = cfg
         ctx.ins = ins
         ctx.scale = scale
@@ -205,14 +170,9 @@ class _ReprojLoss(torch.autograd.Function):
         g_loss = g_loss.to(torch.float32).contiguous()
         g_xyz_m = torch.empty((M, H, W, 3), dtype=torch.float32, device=dev)
         g_delta = torch.empty((M, H, W, B), dtype=torch.float32, device=dev) if delta is not None else None
-        lib = _capi.load()
-        g_tab = torch.empty((int(lib.sr_bob_warp_table_floats(B, M)),), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            rc = lib.sr_reproj_loss_backward(M, H, W, B, int(hxy.shape[-1]), _ptr(xyz_m), _ptr(o2b_q), _ptr(o2b_t),
-                                             _ptr(inv_gauss), _ptr(delta), _ptr(se3_r), _ptr(se3_d), _ptr(cam_q), _ptr(cam_t),
-                                             _ptr(Kmat), _ptr(hxy), _ptr(mask), _ptr(det), _ptr(ctx.scale), _ptr(g_loss),
-                                             _ptr(g_xyz_m), _ptr(g_delta), _ptr(g_tab), _stream(dev))
-        _capi.check(rc, "sr_reproj_loss_backward")
+        g_tab = torch.empty((int(_capi.load().sr_bob_warp_table_floats(B, M)),), dtype=torch.float32, device=dev)
+        _capi.call("sr_reproj_loss_backward", dev, M, H, W, B, int(hxy.shape[-1]), xyz_m, o2b_q, o2b_t, inv_gauss, delta, se3_r,
+                   se3_d, cam_q, cam_t, Kmat, hxy, mask, det, ctx.scale, g_loss, g_xyz_m, g_delta, g_tab)
         g_oq, g_ot, g_ig, g_sr, g_sd, g_cq, g_ct = split_table_grads(g_tab, B, M)
         return (g_xyz_m, g_oq, g_ot, g_ig, g_sr, g_sd, g_cq, g_ct, g_delta) + none
 

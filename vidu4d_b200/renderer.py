@@ -262,18 +262,13 @@ class _RenderPost(torch.autograd.Function):
     @staticmethod
     def forward(ctx, allmap, wvt, tanx, tany, depth_ratio):
         from . import _capi
-        lib = _capi.load()
         allmap = allmap.contiguous()
         wvt = wvt.contiguous()
         _, H, W = allmap.shape
         dev = allmap.device
         mk = lambda c: torch.empty((c, H, W), dtype=torch.float32, device=dev)  # noqa: E731
         acc, rn, dist, med, ex, sd, sn = mk(1), mk(3), mk(1), mk(1), mk(1), mk(1), mk(3)
-        with torch.cuda.device(dev):
-            rc = lib.sr_post_forward(W, H, tanx, tany, depth_ratio, allmap.data_ptr(), wvt.data_ptr(), acc.data_ptr(),
-                                     rn.data_ptr(), dist.data_ptr(), med.data_ptr(), ex.data_ptr(), sd.data_ptr(),
-                                     sn.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-        _capi.check(rc, "sr_post_forward")
+        _capi.call("sr_post_forward", dev, W, H, tanx, tany, depth_ratio, allmap, wvt, acc, rn, dist, med, ex, sd, sn)
         ctx.save_for_backward(allmap, wvt, sd)
         ctx.cfg = (W, H, tanx, tany, depth_ratio)
         return acc, rn, dist, med, ex, sd, sn
@@ -281,19 +276,14 @@ class _RenderPost(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_acc, g_rn, g_dist, g_med, g_ex, g_sd, g_sn):
         from . import _capi
-        lib = _capi.load()
         allmap, wvt, sd = ctx.saved_tensors
         W, H, tanx, tany, depth_ratio = ctx.cfg
         dev = allmap.device
         z = lambda g, c: torch.zeros((c, H, W), dtype=torch.float32, device=dev) if g is None else g.contiguous()  # noqa: E731
         g_acc, g_rn, g_dist, g_med, g_ex, g_sd, g_sn = z(g_acc, 1), z(g_rn, 3), z(g_dist, 1), z(g_med, 1), z(g_ex, 1), z(g_sd, 1), z(g_sn, 3)
         g_allmap = torch.empty_like(allmap)
-        with torch.cuda.device(dev):
-            rc = lib.sr_post_backward(W, H, tanx, tany, depth_ratio, allmap.data_ptr(), wvt.data_ptr(), sd.data_ptr(),
-                                      g_acc.data_ptr(), g_rn.data_ptr(), g_dist.data_ptr(), g_med.data_ptr(), g_ex.data_ptr(),
-                                      g_sd.data_ptr(), g_sn.data_ptr(), g_allmap.data_ptr(),
-                                      torch.cuda.current_stream(dev).cuda_stream)
-        _capi.check(rc, "sr_post_backward")
+        _capi.call("sr_post_backward", dev, W, H, tanx, tany, depth_ratio, allmap, wvt, sd, g_acc, g_rn, g_dist, g_med, g_ex, g_sd,
+                   g_sn, g_allmap)
         return g_allmap, None, None, None, None
 
 
@@ -381,7 +371,6 @@ class _RasterLossBatch(torch.autograd.Function):
     def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, bkgd, cfg, features=None, feature_loss=None):
         from . import _capi
         from .rasterizer import _C
-        lib = _capi.load()
         cams, bg, sh_degree, target, vis, mask, mask_wt, depth_ratio, w_rgb, w_mask, lam_n, lam_d, tanx, tany, target_stream = cfg
         M, H, W = len(cams), cams.image_height, cams.image_width
         dev = means3D.device
@@ -397,20 +386,14 @@ class _RasterLossBatch(torch.autograd.Function):
         dLa = torch.empty_like(allmap)
         dLb = torch.empty((M, 3), dtype=torch.float32, device=dev) if bkgd is not None else None
         scratch = torch.empty((M, H, W), dtype=torch.float32, device=dev)
-        ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
         f32 = lambda t: None if t is None else t.to(dtype=torch.float32).contiguous()  # noqa: E731
         target, vis, mask, mask_wt = f32(target), f32(vis), f32(mask), f32(mask_wt)
         bk = f32(bkgd.detach()) if bkgd is not None else None
         wvt = f32(cams.world_view_transform)         # (M,4,4) packed: callers may hand in a strided view
         if target_stream is not None:       # the targets are still being uploaded on another stream: join it only now,
             torch.cuda.current_stream(dev).wait_stream(target_stream)   # after the rasterizer forward has been queued
-        with torch.cuda.device(dev):
-            rc = lib.sr_render_loss_batch(M, W, H, tanx, tany, float(depth_ratio), color.data_ptr(), allmap.data_ptr(),
-                                          wvt.data_ptr(), target.data_ptr(), ptr(vis), ptr(mask), ptr(mask_wt),
-                                          ptr(bk), float(w_rgb), float(w_mask), float(lam_n), float(lam_d), terms.data_ptr(),
-                                          dLc.data_ptr(), dLa.data_ptr(), ptr(dLb), scratch.data_ptr(),
-                                          torch.cuda.current_stream(dev).cuda_stream)
-        _capi.check(rc, "sr_render_loss_batch")
+        _capi.call("sr_render_loss_batch", dev, M, W, H, tanx, tany, float(depth_ratio), color, allmap, wvt, target, vis, mask,
+                   mask_wt, bk, float(w_rgb), float(w_mask), float(lam_n), float(lam_d), terms, dLc, dLa, dLb, scratch)
         total = terms.sum()
         dLf = None
         if feature_loss is not None:        # the losses on the feature planes: csrc/loss.cu, sr_feature_loss_batch
@@ -420,12 +403,8 @@ class _RasterLossBatch(torch.autograd.Function):
             counts = torch.empty((M, 2), dtype=torch.int32, device=dev)
             dLf = torch.empty_like(feat)
             ftarget, is_det = f32(ftarget), f32(is_det)
-            with torch.cuda.device(dev):
-                rc = lib.sr_feature_loss_batch(M, W, H, F, 0 if ftarget is None else int(ftarget.shape[1]), gm,
-                                               feat.data_ptr(), ptr(ftarget), ptr(mask), ptr(is_det), allmap.data_ptr(),
-                                               weights.data_ptr(), fterms.data_ptr(), counts.data_ptr(), dLf.data_ptr(),
-                                               torch.cuda.current_stream(dev).cuda_stream)
-            _capi.check(rc, "sr_feature_loss_batch")
+            _capi.call("sr_feature_loss_batch", dev, M, W, H, F, 0 if ftarget is None else int(ftarget.shape[1]), gm, feat, ftarget,
+                       mask, is_det, allmap, weights, fterms, counts, dLf)
             total = total + fterms.sum()
         ctx.cfg = (cams, bg, sh_degree, tanx, tany)
         ctx.has_bkgd = bkgd is not None

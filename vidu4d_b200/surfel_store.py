@@ -115,16 +115,12 @@ class FlatSurfelModel(torch.nn.Module):
 
     # ---- one-kernel Adam (trainer.py:253 + 585-586) ---------------------------------------------------------------
     def adam_step(self, grad_scale: float = 1.0):
-        lib = _capi.load()
         off, total = self._offsets(self.P)
         begin = (C.c_int64 * (len(self.groups) + 1))(*off, total)
         lr = (C.c_float * len(self.groups))(*[self.lrs[n] for n, _ in self.groups])
         self.step_count += 1
-        with torch.cuda.device(self.flat.device):
-            rc = lib.sr_adam_flat(len(self.groups), begin, lr, self.betas[0], self.betas[1], self.eps, self.step_count, float(grad_scale),
-                                  self.flat.data_ptr(), self.grad_flat.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(),
-                                  torch.cuda.current_stream(self.flat.device).cuda_stream)
-        _capi.check(rc, "sr_adam_flat")
+        _capi.call("sr_adam_flat", self.flat.device, len(self.groups), begin, lr, self.betas[0], self.betas[1], self.eps,
+                   self.step_count, float(grad_scale), self.flat, self.grad_flat, self.exp_avg, self.exp_avg_sq)
 
     # ---- densification statistics (gaussian_model.py:450-452, trainer.py:553-560) ----------------------------------
     @torch.no_grad()
@@ -141,7 +137,6 @@ class FlatSurfelModel(torch.nn.Module):
     @torch.no_grad()
     def _compact(self, src, kind, child_slot=None, child_xyz=None, child_scaling=None):
         """New model = rows `src` of the old one.  kind 0: survivor (Adam state kept), 1: clone, 2: split child."""
-        lib = _capi.load()
         dev = self.flat.device
         P_new = int(src.numel())
         old_off, _ = self._offsets(self.P)
@@ -152,14 +147,10 @@ class FlatSurfelModel(torch.nn.Module):
         width = (C.c_int32 * n)(*[k for _, k in self.groups])
         ob, nb = (C.c_int64 * n)(*old_off), (C.c_int64 * n)(*new_off)
         src = src.to(torch.int32).contiguous(); kind = kind.to(torch.uint8).contiguous()
-        ptr = lambda t: None if t is None else t.contiguous().data_ptr()  # noqa: E731
         if child_slot is not None:
             child_slot = child_slot.to(torch.int32).contiguous(); child_xyz = child_xyz.float().contiguous(); child_scaling = child_scaling.float().contiguous()
-        with torch.cuda.device(dev):
-            rc = lib.sr_surfel_compact(n, width, ob, nb, 0, 4, P_new, src.data_ptr(), kind.data_ptr(), ptr(child_slot), ptr(child_xyz),
-                                       ptr(child_scaling), self.flat.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(),
-                                       p_new.data_ptr(), m_new.data_ptr(), v_new.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-        _capi.check(rc, "sr_surfel_compact")
+        _capi.call("sr_surfel_compact", dev, n, width, ob, nb, 0, 4, P_new, src, kind, child_slot, child_xyz, child_scaling, self.flat,
+                   self.exp_avg, self.exp_avg_sq, p_new, m_new, v_new)
         self.flat, self.exp_avg, self.exp_avg_sq, self.P = p_new, m_new, v_new, P_new
         self._bind()
 

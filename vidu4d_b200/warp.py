@@ -14,6 +14,8 @@ import torch
 
 from . import _capi
 
+B_MAX = 64                    # bones per call (the warp, reprojection, cycle and feature-row kernels)
+TABLE_SMEM_MAX = 200 * 1024   # bytes of shared memory the bone / frame tables may take (SR_TABLE_SMEM_MAX)
 
 # Hamilton product as ONE gather + two multiplies + one sum (out_i = sum_j SGN[i][j] * a[IDX[i][j]] * b[j]) instead of the
 # 28 elementwise kernels (and ~60 in the backward) of the unbind / stack formulation: the bone tables are tens of floats, so
@@ -45,7 +47,6 @@ def _qconj(q):
 class _BobWarp(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, rot, o2b_q, o2b_t, inv_gauss, se3_r, se3_d, cam_q, cam_t, delta):
-        lib = _capi.load()
         f = lambda t: None if t is None else t.detach().to(torch.float32).contiguous()  # noqa: E731
         xyz, rot, o2b_q, o2b_t, inv_gauss, se3_r, se3_d, cam_q, cam_t, delta = map(f, (xyz, rot, o2b_q, o2b_t, inv_gauss, se3_r,
                                                                                       se3_d, cam_q, cam_t, delta))
@@ -56,12 +57,8 @@ class _BobWarp(torch.autograd.Function):
         xyz_cam = torch.empty((M, P, 3), dtype=torch.float32, device=dev)
         rot_cam = torch.empty((M, P, 4), dtype=torch.float32, device=dev)
         ent = torch.empty((P,), dtype=torch.float32, device=dev)
-        ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
-        with torch.cuda.device(dev):
-            rc = lib.sr_bob_warp_forward(P, B, M, ptr(xyz), ptr(rot), ptr(o2b_q), ptr(o2b_t), ptr(inv_gauss), ptr(delta), ptr(se3_r),
-                                         ptr(se3_d), ptr(cam_q), ptr(cam_t), ptr(xyz_cam), ptr(rot_cam), ptr(ent),
-                                         torch.cuda.current_stream(dev).cuda_stream)
-        _capi.check(rc, "sr_bob_warp_forward")
+        _capi.call("sr_bob_warp_forward", dev, P, B, M, xyz, rot, o2b_q, o2b_t, inv_gauss, delta, se3_r, se3_d, cam_q, cam_t,
+                   xyz_cam, rot_cam, ent)
         ctx.dims = (P, B, M)
         ctx.has_delta = delta is not None
         ctx.save_for_backward(xyz, rot, o2b_q, o2b_t, inv_gauss, se3_r, se3_d, cam_q, cam_t,
@@ -70,7 +67,6 @@ class _BobWarp(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_xyz_cam, g_rot_cam, g_ent):
-        lib = _capi.load()
         P, B, M = ctx.dims
         xyz, rot, o2b_q, o2b_t, inv_gauss, se3_r, se3_d, cam_q, cam_t, delta = ctx.saved_tensors
         dev = xyz.device
@@ -80,30 +76,42 @@ class _BobWarp(torch.autograd.Function):
         g_xyz = torch.empty((P, 3), dtype=torch.float32, device=dev)
         g_rot = torch.empty((P, 4), dtype=torch.float32, device=dev)
         g_delta = torch.empty((P, B), dtype=torch.float32, device=dev) if ctx.has_delta else None
-        nt = int(lib.sr_bob_warp_table_floats(B, M))
-        g_tab = torch.empty((nt,), dtype=torch.float32, device=dev)
-        ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
-        with torch.cuda.device(dev):
-            rc = lib.sr_bob_warp_backward(P, B, M, ptr(xyz), ptr(rot), ptr(o2b_q), ptr(o2b_t), ptr(inv_gauss),
-                                          ptr(delta) if ctx.has_delta else None, ptr(se3_r), ptr(se3_d), ptr(cam_q), ptr(cam_t),
-                                          ptr(g_xyz_cam), ptr(g_rot_cam), ptr(g_ent), ptr(g_xyz), ptr(g_rot), ptr(g_delta),
-                                          ptr(g_tab), torch.cuda.current_stream(dev).cuda_stream)
-        _capi.check(rc, "sr_bob_warp_backward")
+        g_tab = torch.empty((int(_capi.load().sr_bob_warp_table_floats(B, M)),), dtype=torch.float32, device=dev)
+        _capi.call("sr_bob_warp_backward", dev, P, B, M, xyz, rot, o2b_q, o2b_t, inv_gauss, delta if ctx.has_delta else None,
+                   se3_r, se3_d, cam_q, cam_t, g_xyz_cam, g_rot_cam, g_ent, g_xyz, g_rot, g_delta, g_tab)
         g_oq, g_ot, g_ig, g_sr, g_sd, g_cq, g_ct = split_table_grads(g_tab, B, M)
         return g_xyz, g_rot, g_oq, g_ot, g_ig, g_sr, g_sd, g_cq, g_ct, g_delta
+
+
+def table_views(flat, shapes):
+    """Consecutive views of the flat buffer `flat`, one per shape, from its start."""
+    views, o = [], 0
+    for shape in shapes:
+        n = 1
+        for s_ in shape:
+            n *= s_
+        views.append(flat[o:o + n].view(shape)); o += n
+    return views
 
 
 def split_table_grads(g_tab, B, M):
     """Views of a flat g_tables buffer (sr_bob_warp_table_floats order): g_o2b_q, g_o2b_t, g_inv_gauss, g_se3_r, g_se3_d,
     g_cam_q, g_cam_t."""
-    o = 0
-    outs = []
-    for shape in ((B, 4), (B, 3), (B, 3), (M, B, 4), (M, B, 4), (M, 4), (M, 3)):
-        n = 1
-        for s_ in shape:
-            n *= s_
-        outs.append(g_tab[o:o + n].view(shape)); o += n
-    return outs
+    return table_views(g_tab, ((B, 4), (B, 3), (B, 3), (M, B, 4), (M, B, 4), (M, 4), (M, 3)))
+
+
+def check_pairs(named):
+    """Raise RuntimeError unless every (name, pair, shapes) has two tensors of the two given shapes."""
+    for name, pair, shapes in named:
+        if len(pair) != 2 or tuple(pair[0].shape) != shapes[0] or tuple(pair[1].shape) != shapes[1]:
+            raise RuntimeError(f"{name} must be tensors of shapes {shapes}, got {[tuple(t.shape) for t in pair]}")
+
+
+def check_articulations(B, M, rest_articulation, t_articulation, field2cam):
+    """The shapes of the warp's articulation and camera arguments: ((B,4),(B,4)), ((M,B,4),(M,B,4)), ((M,4),(M,3))."""
+    check_pairs((("rest_articulation", rest_articulation, ((B, 4), (B, 4))),
+                 ("t_articulation", t_articulation, ((M, B, 4), (M, B, 4))),
+                 ("field2cam", field2cam, ((M, 4), (M, 3)))))
 
 
 def bob_warp_tables(xyz, rot, o2b_q, o2b_t, inv_gauss, se3, field2cam, delta=None):
@@ -142,7 +150,6 @@ def warp_tables(rest_articulation, t_articulation, log_gauss):
 # Deformation-cycle regulariser (csrc/cycle.cu): the backward warp of every frame's warped surfels back to the canonical
 # space, with the backward warp's skin-entropy and delta-skin terms.
 
-B_MAX = 64
 CYCLE_TERMS = ("reg_deform_cyc", "reg_delta_skin", "reg_skin_entropy")
 
 
@@ -170,11 +177,7 @@ def _check_cycle(xyz, xyz_cam, rest_articulation, t_articulation, log_gauss, fie
     B = int(log_gauss.shape[0]) if log_gauss.dim() == 2 else -1
     if not 1 <= B <= B_MAX or tuple(log_gauss.shape) != (B, 3):
         raise RuntimeError(f"log_gauss must be (B,3) with 1 <= B <= {B_MAX}, got {tuple(log_gauss.shape)}")
-    for name, pair, shapes in (("rest_articulation", rest_articulation, ((B, 4), (B, 4))),
-                               ("t_articulation", t_articulation, ((M, B, 4), (M, B, 4))),
-                               ("field2cam", field2cam, ((M, 4), (M, 3)))):
-        if len(pair) != 2 or tuple(pair[0].shape) != shapes[0] or tuple(pair[1].shape) != shapes[1]:
-            raise RuntimeError(f"{name} must be tensors of shapes {shapes}, got {[tuple(t.shape) for t in pair]}")
+    check_articulations(B, M, rest_articulation, t_articulation, field2cam)
     if delta is not None and tuple(delta.shape) != (M, P, B):
         raise RuntimeError(f"delta must be (M,P,B) = ({M},{P},{B}), got {tuple(delta.shape)}")
     if torch.is_tensor(weights):
@@ -182,19 +185,13 @@ def _check_cycle(xyz, xyz_cam, rest_articulation, t_articulation, log_gauss, fie
             raise RuntimeError(f"weights must be 3 floats or a (3,) float32 tensor, got {tuple(weights.shape)} {weights.dtype}")
     elif len(weights) != 3:
         raise RuntimeError(f"weights must be 3 floats (reg_deform_cyc, reg_delta_skin, reg_skin_entropy), got {weights!r}")
-    if 2 * 4 * (M * B * 15 + B * 3 + M * 7) > 200 * 1024:        # sr_cycle_loss_table_floats, twice, in shared memory
+    if 2 * 4 * (M * B * 15 + B * 3 + M * 7) > TABLE_SMEM_MAX:    # sr_cycle_loss_table_floats, twice, in shared memory
         raise RuntimeError(f"the bone / frame tables of B = {B}, M = {M} frames do not fit in shared memory: split the frames")
     named = [("xyz", xyz), ("xyz_cam", xyz_cam), ("log_gauss", log_gauss), ("rest_articulation", rest_articulation[0]),
              ("rest_articulation", rest_articulation[1]), ("t_articulation", t_articulation[0]),
              ("t_articulation", t_articulation[1]), ("field2cam", field2cam[0]), ("field2cam", field2cam[1])]
     named += [(n, t) for n, t in (("delta", delta), ("weights", weights)) if torch.is_tensor(t)]
-    for name, t in named:
-        if t.dtype != torch.float32:
-            raise RuntimeError(f"{name} must be float32, got {t.dtype}")
-        if not t.is_cuda:
-            raise RuntimeError(f"{name} must be a CUDA tensor (there is no CPU fallback)")
-        if t.device != xyz.device:
-            raise RuntimeError(f"{name} is on {t.device}, xyz on {xyz.device}")
+    _capi.check_tensors(named, "xyz", xyz)
     return P, B, M
 
 
@@ -202,7 +199,6 @@ class _CycleLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, xyz_cam, o2b_q, o2b_t, inv_gauss, se3_r, se3_d, cam_q, cam_t, delta, weights, dims):
         P, B, M = dims
-        lib = _capi.load()
         f = lambda t: None if t is None else t.detach().contiguous()  # noqa: E731
         ins = tuple(map(f, (xyz, xyz_cam, o2b_q, o2b_t, inv_gauss, delta, se3_r, se3_d, cam_q, cam_t)))
         dev = xyz.device
@@ -210,11 +206,7 @@ class _CycleLoss(torch.autograd.Function):
         counts = torch.empty((M, 3), dtype=torch.int32, device=dev)
         scale = torch.empty((3,), dtype=torch.float32, device=dev)
         loss = torch.empty((), dtype=torch.float32, device=dev)
-        ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
-        with torch.cuda.device(dev):
-            rc = lib.sr_cycle_loss_forward(P, B, M, *map(ptr, ins), ptr(weights.detach()), ptr(terms), ptr(counts), ptr(scale),
-                                           ptr(loss), torch.cuda.current_stream(dev).cuda_stream)
-        _capi.check(rc, "sr_cycle_loss_forward")
+        _capi.call("sr_cycle_loss_forward", dev, P, B, M, *ins, weights, terms, counts, scale, loss)
         ctx.dims = dims
         ctx.ins = ins
         ctx.scale = scale
@@ -233,21 +225,10 @@ class _CycleLoss(torch.autograd.Function):
         g_xyz = torch.empty((P, 3), dtype=torch.float32, device=dev)
         g_xyz_cam = torch.empty((M, P, 3), dtype=torch.float32, device=dev)
         g_delta = torch.empty((M, P, B), dtype=torch.float32, device=dev) if delta is not None else None
-        lib = _capi.load()
-        g_tab = torch.empty((int(lib.sr_cycle_loss_table_floats(B, M)),), dtype=torch.float32, device=dev)
-        ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
-        with torch.cuda.device(dev):
-            rc = lib.sr_cycle_loss_backward(P, B, M, *map(ptr, ins), ptr(ctx.scale), ptr(g_loss), ptr(g_xyz_cam), ptr(g_xyz),
-                                            ptr(g_delta), ptr(g_tab), torch.cuda.current_stream(dev).cuda_stream)
-        _capi.check(rc, "sr_cycle_loss_backward")
-        o = 0
-        g = []
-        for shape in ((M, B, 4), (M, B, 3), (B, 3), (M, B, 4), (M, B, 4), (M, 4), (M, 3)):
-            n = 1
-            for s_ in shape:
-                n *= s_
-            g.append(g_tab[o:o + n].view(shape)); o += n
-        g_oq, g_ot, g_ig, g_sr, g_sd, g_cq, g_ct = g
+        g_tab = torch.empty((int(_capi.load().sr_cycle_loss_table_floats(B, M)),), dtype=torch.float32, device=dev)
+        _capi.call("sr_cycle_loss_backward", dev, P, B, M, *ins, ctx.scale, g_loss, g_xyz_cam, g_xyz, g_delta, g_tab)
+        g_oq, g_ot, g_ig, g_sr, g_sd, g_cq, g_ct = table_views(g_tab, ((M, B, 4), (M, B, 3), (B, 3), (M, B, 4), (M, B, 4), (M, 4),
+                                                                      (M, 3)))
         return g_xyz, g_xyz_cam, g_oq, g_ot, g_ig, g_sr, g_sd, g_cq, g_ct, g_delta, None, None
 
 
@@ -283,15 +264,12 @@ def cycle_loss(xyz, xyz_cam, rest_articulation, t_articulation, log_gauss, field
 # Per-surfel feature rows (csrc/feature_rows.cu): [regist | flow / s | normal | Gaussian-bone density] per frame, the
 # (M,P,Cf+6) channels render_loss_batch(features=) composites next to the colour.
 
-FEATURE_ROWS_MAX = 32
-
-
 def _check_feature_rows(regist_feat, xyz, scaling, xyz_cam, rot_cam, Kmat, field2cam, rest_articulation, logibeta):
     if xyz.dim() != 2 or xyz.shape[1] != 3:
         raise RuntimeError(f"xyz must be (P,3), got {tuple(xyz.shape)}")
     P = int(xyz.shape[0])
-    if regist_feat.dim() != 2 or regist_feat.shape[0] != P or regist_feat.shape[1] + 6 > FEATURE_ROWS_MAX:
-        raise RuntimeError(f"regist_feat must be (P,Cf) with P = {P} and Cf + 6 <= {FEATURE_ROWS_MAX}, got {tuple(regist_feat.shape)}")
+    if regist_feat.dim() != 2 or regist_feat.shape[0] != P or regist_feat.shape[1] + 6 > _capi.FEATURES_MAX:
+        raise RuntimeError(f"regist_feat must be (P,Cf) with P = {P} and Cf + 6 <= {_capi.FEATURES_MAX}, got {tuple(regist_feat.shape)}")
     Cf = int(regist_feat.shape[1])
     if tuple(scaling.shape) != (P, 2):
         raise RuntimeError(f"scaling must be (P,2) (the two tangent scales) with P = {P}, got {tuple(scaling.shape)}")
@@ -318,14 +296,7 @@ def _check_feature_rows(regist_feat, xyz, scaling, xyz_cam, rot_cam, Kmat, field
     named = [("regist_feat", regist_feat), ("xyz", xyz), ("scaling", scaling), ("xyz_cam", xyz_cam), ("rot_cam", rot_cam),
              ("Kmat", Kmat), ("field2cam", field2cam[0]), ("rest_articulation", rest_articulation[0]),
              ("rest_articulation", rest_articulation[1]), ("logibeta", logibeta)]
-    for name, t in named:
-        if t.dtype != torch.float32:
-            raise RuntimeError(f"{name} must be float32, got {t.dtype}")
-    for name, t in named:
-        if not t.is_cuda:
-            raise RuntimeError(f"{name} must be a CUDA tensor (there is no CPU fallback)")
-        if t.device != xyz.device:
-            raise RuntimeError(f"{name} is on {t.device}, xyz on {xyz.device}")
+    _capi.check_tensors(named, "xyz", xyz)
     return P, M, B, Cf
 
 
@@ -333,7 +304,6 @@ class _FeatureRows(torch.autograd.Function):
     @staticmethod
     def forward(ctx, regist, xyz, xyz_cam, rot_cam, cam_q, centres, beta, scaling, Kmat, dims):
         P, M, B, Cf = dims
-        lib = _capi.load()
         f = lambda t: t.detach().contiguous()  # noqa: E731
         regist, xyz, xyz_cam, rot_cam, cam_q, centres, beta, scaling, Kmat = map(f, (regist, xyz, xyz_cam, rot_cam, cam_q, centres,
                                                                                     beta, scaling, Kmat))
@@ -342,12 +312,8 @@ class _FeatureRows(torch.autograd.Function):
         density = torch.empty((P, 1), dtype=torch.float32, device=dev)
         s = torch.empty((), dtype=torch.float32, device=dev)
         aux = torch.empty((3,), dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            rc = lib.sr_feature_rows_forward(P, M, B, Cf, regist.data_ptr() if Cf else None, xyz.data_ptr(), scaling.data_ptr(),
-                                             xyz_cam.data_ptr(), rot_cam.data_ptr(), Kmat.data_ptr(), cam_q.data_ptr(),
-                                             centres.data_ptr(), beta.data_ptr(), rows.data_ptr(), density.data_ptr(), s.data_ptr(),
-                                             aux.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-        _capi.check(rc, "sr_feature_rows_forward")
+        _capi.call("sr_feature_rows_forward", dev, P, M, B, Cf, regist if Cf else None, xyz, scaling, xyz_cam, rot_cam, Kmat, cam_q,
+                   centres, beta, rows, density, s, aux)
         ctx.dims = dims
         ctx.save_for_backward(xyz, scaling, xyz_cam, rot_cam, Kmat, cam_q, centres, beta, s, aux)
         return rows, s, density
@@ -365,17 +331,9 @@ class _FeatureRows(torch.autograd.Function):
         g_xyz_cam = torch.empty((M, P, 3), dtype=torch.float32, device=dev)
         g_rot_cam = torch.empty((M, P, 4), dtype=torch.float32, device=dev)
         g_tab = torch.empty((M * 4 + B * 3 + 2,), dtype=torch.float32, device=dev)
-        ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
-        lib = _capi.load()
-        with torch.cuda.device(dev):
-            rc = lib.sr_feature_rows_backward(P, M, B, Cf, ptr(xyz), ptr(scaling), ptr(xyz_cam), ptr(rot_cam), ptr(Kmat), ptr(cam_q),
-                                              ptr(centres), ptr(beta), ptr(s), ptr(aux), ptr(g_rows), ptr(g_density), ptr(g_s),
-                                              ptr(g_regist) if Cf else None, ptr(g_xyz), ptr(g_xyz_cam), ptr(g_rot_cam), ptr(g_tab),
-                                              torch.cuda.current_stream(dev).cuda_stream)
-        _capi.check(rc, "sr_feature_rows_backward")
-        g_cq = g_tab[:M * 4].view(M, 4)
-        g_cen = g_tab[M * 4:M * 4 + B * 3].view(B, 3)
-        g_beta = g_tab[M * 4 + B * 3:M * 4 + B * 3 + 1]
+        _capi.call("sr_feature_rows_backward", dev, P, M, B, Cf, xyz, scaling, xyz_cam, rot_cam, Kmat, cam_q, centres, beta, s, aux,
+                   g_rows, g_density, g_s, g_regist if Cf else None, g_xyz, g_xyz_cam, g_rot_cam, g_tab)
+        g_cq, g_cen, g_beta = table_views(g_tab, ((M, 4), (B, 3), (1,)))
         return g_regist, g_xyz, g_xyz_cam, g_rot_cam, g_cq, g_cen, g_beta, None, None, None
 
 
