@@ -26,11 +26,21 @@ frame, forward + backward with seeded upstream gradients, at 300 K surfels, B = 
 graph, L2 flushed between steps, fused (csrc/feature_rows.cu) against the reference's statements in fp32 torch
 (tests/feature_rows_model.py), alternating in one process.
 
+--ssim times the fused SSIM op (csrc/ssim.cu), forward + backward of 1 - ssim(img1, img2), one CUDA graph, L2 flushed
+between steps, against an independently written torch expression of the same formula (conv2d with the 11x11 window and
+groups=C), alternating in one process, at 1x3x512^2, 8x3x512^2 and 1x3x1080x1920; then a render_loss_batch step (300 K
+surfels, 512x512, 8 frames) with w_ssim = 0 and 0.2.  The op's algorithmic bound, per channel-pixel: the forward reads
+x and y (8 B) and writes the three gradient maps (12 B); the backward reads the maps, x and y (20 B) and writes dL/dx
+(4 B), so 44 B in all; about 400 FLOP (five 11-tap passes each way, two for each of the five forward and three backward
+quantities, plus the per-pixel formula).  Printed with each size: the bytes / 3.35 TB/s and FLOP / 67 TFLOP/s bounds
+(H100 SXM data sheet) and the measured share of the larger.
+
     python tools/bench_features.py --features 4 22 32 [--steps 20 --warmup 5]
     python tools/bench_features.py --losses [--steps 20 --warmup 5]
     python tools/bench_features.py --reproj [--steps 20 --warmup 5]
     python tools/bench_features.py --cycle [--steps 20 --warmup 5]
     python tools/bench_features.py --rows [--steps 20 --warmup 5]
+    python tools/bench_features.py --ssim [--steps 20 --warmup 5]
 """
 import argparse
 import json
@@ -57,7 +67,10 @@ def main():
     ap.add_argument("--reproj", action="store_true")
     ap.add_argument("--cycle", action="store_true")
     ap.add_argument("--rows", action="store_true")
+    ap.add_argument("--ssim", action="store_true")
     args = ap.parse_args()
+    if args.ssim:
+        return bench_ssim(args)
     if args.rows:
         return bench_rows(args)
     if args.cycle:
@@ -610,6 +623,134 @@ def bench_rows(args):
                           "steps": args.steps, "statistic": "median step time", "gpu": gpu}), flush=True)
         del steps, bodies, d
         torch.cuda.empty_cache()
+    RZ.set_sync_mode(True)
+    RZ._pending.clear()
+
+
+SSIM_BYTES_PER_PX, SSIM_FLOP_PER_PX = 44, 400
+
+
+def _torch_window(C, dev):
+    """The 11x11 Gaussian window (sigma 1.5) of a depthwise conv2d over C channels."""
+    import math
+    g = torch.tensor([math.exp(-(i - 5) ** 2 / (2 * 1.5 ** 2)) for i in range(11)], dtype=torch.float32)
+    g = g / g.sum()
+    return (g[:, None] @ g[None, :]).expand(C, 1, 11, 11).contiguous().to(dev)
+
+
+def _torch_ssim(img1, img2, win):
+    """1 - SSIM in plain torch, written from the formula: depthwise conv2d with the window, groups = C."""
+    C = img1.shape[1]
+    f = lambda t: torch.nn.functional.conv2d(t, win, padding=5, groups=C)  # noqa: E731
+    mu1, mu2 = f(img1), f(img2)
+    s11, s22, s12 = f(img1 * img1) - mu1 * mu1, f(img2 * img2) - mu2 * mu2, f(img1 * img2) - mu1 * mu2
+    m = ((2 * mu1 * mu2 + 0.01 ** 2) * (2 * s12 + 0.03 ** 2)) / ((mu1 * mu1 + mu2 * mu2 + 0.01 ** 2) * (s11 + s22 + 0.03 ** 2) + 1e-10)
+    return 1.0 - m.mean()
+
+
+def _alternate(bodies, args, flush):
+    """Captures each body in a CUDA graph and replays them alternately, L2 flushed before each; median ms per body."""
+    from vidu4d_b200.graph import GraphedStep
+    steps = {k: GraphedStep(b, device=flush.device) for k, b in bodies.items()}
+    for s_ in steps.values():
+        s_()
+        for _ in range(args.warmup):
+            s_(check=False)
+    torch.cuda.synchronize()
+    ms = {k: [] for k in steps}
+    for i in range(args.steps):
+        for k, s_ in steps.items():
+            flush.fill_(i & 255)
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record(); s_.graph.replay(); b.record()
+            b.synchronize()
+            ms[k].append(a.elapsed_time(b))
+    return {k: float(np.median(v)) for k, v in ms.items()}, steps
+
+
+def bench_ssim(args):
+    from vidu4d_b200 import _capi, rasterizer as RZ
+    from vidu4d_b200.renderer import PipelineParams, make_camera, render_loss_batch, stack_cameras
+    from vidu4d_b200.ssim import ssim
+    from vidu4d_b200.synthetic import SurfelCloud, object_scene, orbit_view
+    assert torch.cuda.is_available(), "this measurement needs a GPU"
+    dev = torch.device("cuda:0")
+    _capi.load()
+    gpu = _gpu_name()
+    flush = torch.empty((256 << 20,), dtype=torch.uint8, device=dev)
+    for shape in ((1, 3, 512, 512), (8, 3, 512, 512), (1, 3, 1080, 1920)):
+        g = torch.Generator(device=dev).manual_seed(1)
+        x = torch.rand(shape, device=dev, generator=g).requires_grad_(True)
+        y = (x.detach() + 0.1 * torch.randn(shape, device=dev, generator=g)).clamp(0, 1)
+        win = _torch_window(shape[1], dev)
+        fns = {"fused": lambda: 1.0 - ssim(x, y), "torch": lambda: _torch_ssim(x, y, win)}
+
+        def make_body(fn):
+            def body():
+                x.grad = None
+                fn().backward()
+            return body
+        bodies = {k: make_body(f) for k, f in fns.items()}
+        peak, vals, grads = {}, {}, {}
+        for k, b in bodies.items():
+            torch.cuda.synchronize()
+            base = torch.cuda.memory_allocated()
+            torch.cuda.reset_peak_memory_stats()
+            b()
+            torch.cuda.synchronize()
+            peak[k] = round((torch.cuda.max_memory_allocated() - base) / 2**20, 1)
+            grads[k] = x.grad.clone()
+            with torch.no_grad():
+                vals[k] = float(fns[k]())
+        med, _ = _alternate(bodies, args, flush)
+        RZ.set_sync_mode(True)
+        RZ._pending.clear()
+        torch.cuda.synchronize()
+        _capi.get_profile()
+        _capi.set_profiling(True)
+        for _ in range(5):
+            bodies["fused"]()
+        prof = _capi.get_profile()
+        _capi.set_profiling(False)
+        kern = {k: round(v["ms"] / max(v["count"], 1), 4) for k, v in prof.items() if k.startswith("ssim")}
+        px = int(np.prod(shape))
+        t_bytes, t_flop = px * SSIM_BYTES_PER_PX / 3.35e12 * 1e3, px * SSIM_FLOP_PER_PX / 67e12 * 1e3
+        kms = sum(kern.values())
+        print(json.dumps({"workload": "1 - ssim, fwd + bwd", "shape": list(shape), "ms_per_step": {k: round(v, 4) for k, v in med.items()},
+                          "peak_mem_mb_above_inputs": peak, "kernel_ms_per_launch": kern,
+                          "bound_ms": {"bytes": round(t_bytes, 4), "flop": round(t_flop, 4)},
+                          "kernel_share_of_bound": round(max(t_bytes, t_flop) / kms, 3) if kms else None,
+                          "loss_abs_diff": abs(vals["fused"] - vals["torch"]),
+                          "grad_max_abs_diff_over_max": float((grads["fused"] - grads["torch"]).abs().max() / grads["torch"].abs().max()),
+                          "steps": args.steps, "statistic": "median step time", "gpu": gpu}), flush=True)
+        del bodies, fns, x, y, grads, win
+        torch.cuda.empty_cache()
+    # the term's cost inside a Stage-3 step
+    P, RES, M = args.surfels, 512, 8
+    scene = object_scene(P, seed=0, opacity="trained", center=(0.0, 0.0, 0.0))
+    cams = []
+    for f in range(M):
+        R, t = orbit_view(f, 64)
+        cams.append(make_camera(RES, RES, 2 * np.arctan(0.5), 2 * np.arctan(0.5), R=R.T, T=t, device=dev))
+    bc = stack_cameras(cams)
+    g = torch.Generator(device=dev).manual_seed(99)
+    rgb = torch.rand((M, 3, RES, RES), device=dev, generator=g)
+    cloud = SurfelCloud(scene, dev)
+    bkgd = torch.tensor([0.2, 0.3, 0.4], device=dev, requires_grad=True)
+    pipe, bg = PipelineParams(), torch.zeros(3, device=dev)
+
+    def make_step(w):
+        def body():
+            out = render_loss_batch(bc, cloud, pipe, bg, rgb, learnable_bkgd=bkgd, w_rgb=1.0 - w, w_ssim=w, lambda_dist=10.0)
+            out["loss"].backward()
+        return body
+    med, steps = _alternate({"w_ssim_0": make_step(0.0), "w_ssim_0.2": make_step(0.2)}, args, flush)
+    for s_ in steps.values():
+        s_.arm(); RZ.check_overflow(keep=True)
+    print(json.dumps({"workload": "render_loss_batch step (fwd + bwd)", "surfels": P, "resolution": RES, "frames": M,
+                      "ms_per_step": {k: round(v, 4) for k, v in med.items()},
+                      "library_launches_per_step": {k: s_.launches for k, s_ in steps.items()},
+                      "steps": args.steps, "statistic": "median step time", "gpu": gpu}), flush=True)
     RZ.set_sync_mode(True)
     RZ._pending.clear()
 

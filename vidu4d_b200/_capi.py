@@ -91,6 +91,15 @@ PROTOTYPES = {
 }
 SYMBOLS = tuple(PROTOTYPES)
 
+# the fused SSIM loss, declared in include/surfel_ssim.h: same library, same error path, its own header (and so its own
+# table) because surfel_raster.h is the rasterizer's drop-in boundary
+SSIM_PROTOTYPES = {
+    "sr_ssim_scratch_bytes": (C.c_int64, [_i32] * 4),
+    "sr_ssim_forward": (C.c_int, [_i32] * 4 + [_p] * 3 + [_i64] + [_p] * 5 + [_i64, _p]),
+    "sr_ssim_backward": (C.c_int, [_i32] * 4 + [_p] * 3 + [_i64] + [_p] * 3 + [_i32, _p, _i32] + [_p] * 3 + [_i64, _p]),
+}
+SSIM_SYMBOLS = tuple(SSIM_PROTOTYPES)
+
 
 _lib = None
 
@@ -105,10 +114,10 @@ def load():
             f"{LIB_PATH} not found: the CUDA extension is not built. Run `python -m vidu4d_b200.build` "
             "(or __graft_entry__.build()). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for s in SYMBOLS:
+    for s in SYMBOLS + SSIM_SYMBOLS:
         if not hasattr(lib, s):
             raise SurfelRasterError(f"{LIB_PATH} does not export {s}")
-    for name, (restype, argtypes) in PROTOTYPES.items():
+    for name, (restype, argtypes) in list(PROTOTYPES.items()) + list(SSIM_PROTOTYPES.items()):
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.sr_abi_version() != ABI_VERSION:

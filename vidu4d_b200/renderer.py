@@ -371,7 +371,8 @@ class _RasterLossBatch(torch.autograd.Function):
     def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, bkgd, cfg, features=None, feature_loss=None):
         from . import _capi
         from .rasterizer import _C
-        cams, bg, sh_degree, target, vis, mask, mask_wt, depth_ratio, w_rgb, w_mask, lam_n, lam_d, tanx, tany, target_stream = cfg
+        (cams, bg, sh_degree, target, vis, mask, mask_wt, depth_ratio, w_rgb, w_mask, lam_n, lam_d, tanx, tany, target_stream,
+         w_ssim) = cfg
         M, H, W = len(cams), cams.image_height, cams.image_width
         dev = means3D.device
         e = torch.empty((0,), dtype=torch.float32, device=dev)
@@ -395,6 +396,10 @@ class _RasterLossBatch(torch.autograd.Function):
         _capi.call("sr_render_loss_batch", dev, M, W, H, tanx, tany, float(depth_ratio), color, allmap, wvt, target, vis, mask,
                    mask_wt, bk, float(w_rgb), float(w_mask), float(lam_n), float(lam_d), terms, dLc, dLa, dLb, scratch)
         total = terms.sum()
+        sterms = None
+        if w_ssim > 0.0:                    # D-SSIM on the final colour: csrc/ssim.cu, its gradient added into dLc / dLa / dLb
+            sterms = _ssim_term(M, H, W, color, allmap, target, bk, w_ssim, dLc, dLa, dLb)
+            total = total + sterms.sum()
         dLf = None
         if feature_loss is not None:        # the losses on the feature planes: csrc/loss.cu, sr_feature_loss_batch
             ftarget, is_det, gm, weights = feature_loss
@@ -412,7 +417,8 @@ class _RasterLossBatch(torch.autograd.Function):
                               dLb if dLb is not None else e, features, dLf)
         ctx.has_features = features is not None
         outs = (total, terms, color, allmap, radii) + (() if feat is None else (feat,)) + (() if dLf is None else (fterms, counts))
-        ctx.mark_non_differentiable(terms, color, allmap, radii, *outs[6:])
+        outs = outs + (() if sterms is None else (sterms,))
+        ctx.mark_non_differentiable(terms, color, allmap, radii, *(o for o in outs[5:] if o is not feat))
         return outs
 
     @staticmethod
@@ -440,6 +446,25 @@ class _RasterLossBatch(torch.autograd.Function):
         return (_reduce_like(g3d, means3D), g2d, _reduce_like(gsh, sh), _reduce_like(gop, opacities),
                 _reduce_like(gsc, scales), _reduce_like(grot, rotations), g_bk, None,
                 _reduce_like(grads[8], features) if ctx.has_features else None, None)
+
+
+def _ssim_term(M, H, W, color, allmap, target, bkgd, w_ssim, dLc, dLa, dLb):
+    """Each frame's w_ssim * (1 - SSIM(color + (1 - alpha) * bkgd, target)), (M,), with its gradient ADDED into dL/dcolor,
+    dL/dalpha (allmap plane 1) and dL/dbkgd -- unscaled, like the other terms' (the backward applies the upstream scalar)."""
+    from . import _capi
+    dev = color.device
+    nbytes = int(_capi.load().sr_ssim_scratch_bytes(M, 3, H, W))
+    scratch = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+    per_frame = torch.empty((M,), dtype=torch.float32, device=dev)
+    mean = torch.empty((1,), dtype=torch.float32, device=dev)
+    maps = torch.empty((3, M, 3, H, W), dtype=torch.float32, device=dev)
+    alpha, d_alpha = (allmap[:, 1], dLa[:, 1]) if bkgd is not None else (None, None)
+    stride = 8 * H * W
+    _capi.call("sr_ssim_forward", dev, M, 3, H, W, color, target, alpha, stride, bkgd, per_frame, mean, maps, scratch, nbytes)
+    g = torch.full((M,), -float(w_ssim), dtype=torch.float32, device=dev)      # d(w (1 - ssim_f)) / d ssim_f
+    _capi.call("sr_ssim_backward", dev, M, 3, H, W, color, target, alpha, stride, bkgd, maps, g, 1, dLc, 1, d_alpha, dLb,
+               scratch, nbytes)
+    return (1.0 - per_frame) * float(w_ssim)
 
 
 def _check_feature_losses(M, H, W, features, feature_target, mask_gt, is_detected, gauss_mask_channel, feature_loss_weights):
@@ -495,7 +520,8 @@ def _check_loss_inputs(M, H, W, device, target_rgb, vis2d, mask_gt, mask_wt, lea
 
 def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_gt=None, mask_wt=None, learnable_bkgd=None,
                       w_rgb=1.0, w_mask=0.0, lambda_normal=0.0, lambda_dist=0.0, means3D=None, rotations=None, target_stream=None,
-                      features=None, feature_target=None, is_detected=None, gauss_mask_channel=None, feature_loss_weights=None):
+                      features=None, feature_target=None, is_detected=None, gauss_mask_channel=None, feature_loss_weights=None,
+                      w_ssim=0.0):
     """The Stage-3 inner loop for M frames in one call: rasterize every frame (batched launch set), post-process and
     evaluate the image losses in one fused kernel, and hand autograd a single scalar.
 
@@ -522,7 +548,11 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
     "viewspace_points": (M,P,3) whose .grad receives the densification proxy}; with features also "features": (M,F,H,W),
     differentiable, so that a caller's own losses on the planes backpropagate through the same rasterizer backward; with
     the fused feature losses also "feature_terms": (M,2) each frame's share of the weighted feature / reg_gauss_mask
-    terms (detached, included in "loss") and "feature_counts": (M,2) int32, each frame's number of positive values."""
+    terms (detached, included in "loss") and "feature_counts": (M,2) int32, each frame's number of positive values.
+
+    w_ssim > 0 adds, per frame, w_ssim * (1 - SSIM(final colour, target_rgb)) to "loss" (csrc/ssim.cu; gs/train.py's D-SSIM
+    term): the final colour includes learnable_bkgd, and SSIM is unmasked.  "ssim_terms": (M,) each frame's share
+    (detached).  Stage 3's setting is w_rgb = 1 - lambda_dssim, w_ssim = lambda_dssim.  w_ssim = 0 launches nothing more."""
     if not isinstance(cameras, BatchCameras):
         cameras = stack_cameras(cameras)
     M = len(cameras)
@@ -538,7 +568,7 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
     screenspace_points = torch.zeros((M, P, 3), dtype=xyz.dtype, requires_grad=True, device=xyz.device)
     tanx, tany = _cam_tans(cameras)
     cfg = (cameras, bg_color, pc.active_sh_degree, target_rgb, vis2d, mask_gt, mask_wt, float(pipe.depth_ratio),
-           w_rgb, w_mask, lambda_normal, lambda_dist, tanx, tany, target_stream)
+           w_rgb, w_mask, lambda_normal, lambda_dist, tanx, tany, target_stream, float(w_ssim))
     outs = _RasterLossBatch.apply(xyz, screenspace_points, pc.get_features, pc.get_opacity, pc.get_scaling, rot,
                                   learnable_bkgd, cfg, features, feature_loss)
     total, terms, color, allmap, radii = outs[:5]
@@ -548,4 +578,6 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
         out["features"] = outs[5]
     if feature_loss is not None:
         out["feature_terms"], out["feature_counts"] = outs[6], outs[7]
+    if w_ssim > 0.0:
+        out["ssim_terms"] = outs[-1]
     return out
