@@ -30,6 +30,8 @@ import numpy as np
 import pytest
 import torch
 
+from .error_bound import _E, _where
+
 pytestmark = pytest.mark.gpu
 
 U = 2.0 ** -24
@@ -45,71 +47,6 @@ def dev(built):
     from vidu4d_b200 import _capi
     _capi.load()
     return torch.device("cuda:0")
-
-
-# ------------------------------------------------------------------------------------------------ running error bound
-def _rnd(v, exact):
-    """The rounding of one fp32 operation whose exact result is v: none where the operands are exact and v is a float."""
-    r = np.abs(v)
-    return np.where(exact & (v.astype(np.float32).astype(np.float64) == v), 0.0, r)
-
-
-class _E:
-    """A float64 value and a bound (in units of u) on the absolute error of its fp32 evaluation, to first order."""
-    __slots__ = ("v", "b")
-
-    def __init__(self, v, b=None):
-        self.v = np.asarray(v, np.float64)
-        self.b = np.zeros_like(self.v) if b is None else np.asarray(b, np.float64)
-
-    @staticmethod
-    def const(c):
-        """The exact value c of a constant the kernel rounds to fp32 (1.0f / 3.0f, 1e12f, 1e-12f): one rounding."""
-        return _E(c, _rnd(np.asarray(c, np.float64), True))
-
-    def __add__(s, o):
-        o = _c(o)
-        v = s.v + o.v
-        return _E(v, s.b + o.b + _rnd(v, (s.b == 0) & (o.b == 0)))
-
-    def __sub__(s, o):
-        return s + (-_c(o))
-
-    def __neg__(s):
-        return _E(-s.v, s.b)
-
-    def __mul__(s, o):
-        o = _c(o)
-        v = s.v * o.v
-        return _E(v, np.abs(s.v) * o.b + np.abs(o.v) * s.b + _rnd(v, (s.b == 0) & (o.b == 0)))
-
-    def __truediv__(s, o):
-        o = _c(o)
-        with np.errstate(divide="ignore", invalid="ignore"):
-            v = s.v / o.v
-            b = s.b / np.abs(o.v) + np.abs(v) * o.b / np.abs(o.v)
-        return _E(v, b + _rnd(v, (s.b == 0) & (o.b == 0)))
-
-    def __getitem__(s, i):
-        return _E(s.v[i], s.b[i])
-
-    def abs(s):
-        return _E(np.abs(s.v), s.b)
-
-    def sqrt(s):
-        v = np.sqrt(s.v)
-        with np.errstate(divide="ignore", invalid="ignore"):
-            b = np.where(s.b > 0, s.b / (2.0 * v), 0.0)
-        return _E(v, b + _rnd(v, s.b == 0))
-
-
-def _c(x):
-    return x if isinstance(x, _E) else _E(x)
-
-
-def _where(c, a, b):
-    a, b = _c(a), _c(b)
-    return _E(np.where(c, a.v, b.v), np.where(c, a.b, b.b))
 
 
 def _full(inner, H, W):
