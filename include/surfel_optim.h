@@ -1,0 +1,60 @@
+/*
+ * surfel_optim.h -- C ABI of the optimizer step whose per-step state lives on the device: gradient-norm clipping over
+ * the flat surfel gradient buffer, and an Adam pass that reads its step count, learning rates and clip coefficient from
+ * device memory.
+ *
+ * The same library as surfel_raster.h (libsurfel_raster.so), the same SR_API visibility, SR_E* codes and
+ * sr_last_error() message path.  It lives in its own header because surfel_raster.h is the drop-in boundary of the
+ * reference rasterizer; sr_adam_flat there takes its step count and rates as launch arguments, which a CUDA graph
+ * freezes at capture.
+ *
+ * The flat buffer holds n_groups parameter groups back to back: group g is elements [begin[g], begin[g+1]), with
+ * begin a HOST int64 array of n_groups + 1 entries, begin[0] = 0, non-decreasing, 1 <= n_groups <= 8.  Groups may start
+ * at any element offset; the buffers themselves are 16-byte aligned.
+ *
+ * Together the two calls do what torch.nn.utils.clip_grad_norm_(params, max_norm) followed by torch.optim.Adam.step()
+ * does (lab4d/engine/trainer.py:547, 589-591):
+ *   S_g   = sum over group g of (grads * grad_scale)^2, in float64, per CTA and group, then a fixed-order one-CTA sum;
+ *   total = (float) sqrt(S_0 + ... + S_{n-1} + n_0^2 + ... + n_{e-1}^2), the n_i the fp32 norms of other gradients;
+ *   coef  = min((1 / (total + 1e-6f)) * max_norm, 1) in fp32, NaN passing through, as torch evaluates it;
+ *   Adam on (grads * grad_scale) * coef with bias corrections of the device step count.
+ * The launch shapes depend on the buffer size only, so equal inputs give equal bits on every device and stream.
+ * Neither call allocates memory or synchronises with the host, so both can be captured in a CUDA graph.
+ * Every function returns 0 on success or a negative SR_E* code; bad arguments return SR_EINVAL before any device work.
+ */
+#ifndef SURFEL_OPTIM_H_
+#define SURFEL_OPTIM_H_
+
+#include "surfel_raster.h"
+
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+/* bytes of DEVICE scratch sr_grad_norm_flat needs for n_groups groups, whatever their size (-1: bad n_groups) */
+SR_API int64_t sr_grad_norm_scratch_bytes(int32_t n_groups);
+
+/*
+ * total_norm[1], clip_coef[1]: DEVICE float, written.  group_sumsq (nullable): DEVICE double [n_groups], gets S_g.
+ * extra_norms: DEVICE float [n_extra] (n_extra >= 0; NULL allowed when 0).  scratch: DEVICE, at least
+ * sr_grad_norm_scratch_bytes(n_groups) bytes, 8-byte aligned.
+ */
+SR_API int sr_grad_norm_flat(int32_t n_groups, const int64_t* begin, const float* grads, float grad_scale,
+                             const float* extra_norms, int32_t n_extra, float max_norm, float* total_norm, float* clip_coef,
+                             double* group_sumsq, void* scratch, int64_t scratch_bytes, void* stream);
+
+/*
+ * One Adam step (torch.optim.Adam: amsgrad off, weight_decay 0) over params / exp_avg / exp_avg_sq, DEVICE float.
+ * lr: DEVICE float [n_groups].  step: DEVICE int64, incremented first; the step runs with t = the new value and the
+ * bias corrections (float)(1 - pow(beta1, t)) and (float)sqrt(1 - pow(beta2, t)) evaluated in double, as sr_adam_flat
+ * does on the host.  clip_coef: DEVICE float, or NULL for 1.  The step count advances also when the buffer is empty.
+ */
+SR_API int sr_adam_flat_state(int32_t n_groups, const int64_t* begin, const float* lr, float beta1, float beta2, float eps,
+                              int64_t* step, float grad_scale, const float* clip_coef, float* params, const float* grads,
+                              float* exp_avg, float* exp_avg_sq, void* stream);
+
+#ifdef __cplusplus
+}
+#endif
+
+#endif /* SURFEL_OPTIM_H_ */

@@ -100,6 +100,15 @@ SSIM_PROTOTYPES = {
 }
 SSIM_SYMBOLS = tuple(SSIM_PROTOTYPES)
 
+# gradient-norm clipping and the Adam step with its state on the device, declared in include/surfel_optim.h (own header
+# and table for the same reason)
+OPTIM_PROTOTYPES = {
+    "sr_grad_norm_scratch_bytes": (C.c_int64, [_i32]),
+    "sr_grad_norm_flat": (C.c_int, [_i32, _p, _p, _f32, _p, _i32, _f32] + [_p] * 4 + [_i64, _p]),
+    "sr_adam_flat_state": (C.c_int, [_i32, _p, _p, _f32, _f32, _f32, _p, _f32] + [_p] * 6),
+}
+OPTIM_SYMBOLS = tuple(OPTIM_PROTOTYPES)
+
 
 _lib = None
 
@@ -114,10 +123,10 @@ def load():
             f"{LIB_PATH} not found: the CUDA extension is not built. Run `python -m vidu4d_b200.build` "
             "(or __graft_entry__.build()). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for s in SYMBOLS + SSIM_SYMBOLS:
+    for s in SYMBOLS + SSIM_SYMBOLS + OPTIM_SYMBOLS:
         if not hasattr(lib, s):
             raise SurfelRasterError(f"{LIB_PATH} does not export {s}")
-    for name, (restype, argtypes) in list(PROTOTYPES.items()) + list(SSIM_PROTOTYPES.items()):
+    for name, (restype, argtypes) in list(PROTOTYPES.items()) + list(SSIM_PROTOTYPES.items()) + list(OPTIM_PROTOTYPES.items()):
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.sr_abi_version() != ABI_VERSION:

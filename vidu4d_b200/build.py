@@ -19,7 +19,8 @@ SOURCES = ["api.cu", "preprocess.cu", "sort.cu", "composite_fwd.cu", "composite_
            "postprocess.cu", "loss.cu", "warp.cu", "match.cu", "cycle.cu", "feature_rows.cu", "optim.cu", "knn.cu", "outlier.cu", "ssim.cu"]
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "composite_common.cuh"), os.path.join(CSRC, "post_common.cuh"),
            os.path.join(CSRC, "warp_common.cuh"),
-           os.path.join(HERE, "..", "include", "surfel_raster.h"), os.path.join(HERE, "..", "include", "surfel_ssim.h")]
+           os.path.join(HERE, "..", "include", "surfel_raster.h"), os.path.join(HERE, "..", "include", "surfel_ssim.h"),
+           os.path.join(HERE, "..", "include", "surfel_optim.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",

@@ -11,7 +11,13 @@
 //     new parameter, exp_avg and exp_avg_sq buffers from a source-index list, instead of ~60 torch cat / index /
 //     nn.Parameter re-creations per call.
 // Semantics are torch.optim.Adam's (amsgrad off, no weight decay) and the reference's row-wise copy rules, bit for bit.
+//
+// The per-step optimizer state can also live on the device (include/surfel_optim.h): a group-wise float64 sum of squares
+// of the gradient buffer gives torch.nn.utils.clip_grad_norm_'s coefficient in a one-CTA finish, and the Adam pass reads
+// its step count, learning rates and that coefficient from device memory, so a replayed CUDA graph steps as the
+// reference does (lab4d/engine/trainer.py:547, 589-591) without a re-capture.
 #include "common.cuh"
+#include "../../include/surfel_optim.h"
 
 namespace {
 
@@ -22,9 +28,38 @@ struct AdamGroups {
     float lr[MAXG];
 };
 
+// sr_adam_flat_state's device state; unused (all NULL) in sr_adam_flat's instantiation
+struct AdamDeviceState {
+    const float* lr;               // [n_groups]
+    const long long* step;         // already incremented: the 1-based number of this step
+    const float* coef;             // clip coefficient, or NULL for 1
+};
+
+// Bias corrections exactly as sr_adam_flat forms them on the host
+__device__ __forceinline__ void adam_bias_corrections(float beta1, float beta2, long long step, float& bc1, float& sqrt_bc2) {
+    bc1 = (float)(1.0 - pow((double)beta1, (double)step));
+    sqrt_bc2 = (float)sqrt(1.0 - pow((double)beta2, (double)step));
+}
+
+// DEVICE_STATE = false: sr_adam_flat, every scalar a launch argument.  DEVICE_STATE = true: sr_adam_flat_state, the step,
+// rates and clip coefficient read from S (bc1 / sqrt_bc2 / G.lr are then ignored).
+template <bool DEVICE_STATE>
 __global__ void __launch_bounds__(256)
 adam_flat_kernel(const AdamGroups G, float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                 float* __restrict__ v, float beta1, float beta2, float eps, float bc1, float sqrt_bc2, float grad_scale) {
+                 float* __restrict__ v, float beta1, float beta2, float eps, float bc1, float sqrt_bc2, float grad_scale,
+                 const AdamDeviceState S) {
+    float lrs[MAXG], coef = 1.0f;
+    if constexpr (DEVICE_STATE) {
+        // one thread per CTA forms the scalars (two float64 pow), the rest read them from shared memory
+        __shared__ float sc[2 + MAXG + 1];
+        if (threadIdx.x == 0) adam_bias_corrections(beta1, beta2, *S.step, sc[0], sc[1]);
+        if (threadIdx.x < MAXG) sc[2 + threadIdx.x] = threadIdx.x < G.n ? S.lr[threadIdx.x] : 0.0f;
+        if (threadIdx.x == MAXG) sc[2 + MAXG] = S.coef ? *S.coef : 1.0f;
+        __syncthreads();
+        bc1 = sc[0]; sqrt_bc2 = sc[1]; coef = sc[2 + MAXG];
+#pragma unroll
+        for (int q = 0; q < MAXG; q++) lrs[q] = sc[2 + q];
+    }
     const long long total = G.begin[G.n];
     for (long long i = (long long)blockIdx.x * 1024 + threadIdx.x * 4; i < total; i += (long long)gridDim.x * 1024) {
         // four consecutive elements; a group boundary can fall inside them, so the rate is looked up per element
@@ -43,10 +78,11 @@ adam_flat_kernel(const AdamGroups G, float* __restrict__ p, const float* __restr
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             const long long e = i + k;
-            float lr = G.lr[0];
+            float lr = DEVICE_STATE ? lrs[0] : G.lr[0];
 #pragma unroll
-            for (int q = 1; q < MAXG; q++) if (q < G.n && e >= G.begin[q]) lr = G.lr[q];
-            const float gr = G4[k] * grad_scale;
+            for (int q = 1; q < MAXG; q++) if (q < G.n && e >= G.begin[q]) lr = DEVICE_STATE ? lrs[q] : G.lr[q];
+            // (g * grad_scale) * coef, each product rounded: the averaging, then clip_grad_norm_'s in-place multiply
+            const float gr = DEVICE_STATE ? __fmul_rn(G4[k] * grad_scale, coef) : G4[k] * grad_scale;
             // torch/optim/adam.py _single_tensor_adam: exp_avg.lerp_(grad, 1 - beta1); exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2);
             // denom = exp_avg_sq.sqrt() / sqrt(bias_correction2) + eps; param.addcdiv_(exp_avg, denom, value=-lr / bias_correction1)
             M4[k] = M4[k] + (gr - M4[k]) * (1.0f - beta1);
@@ -101,6 +137,126 @@ compact_kernel(const CompactGroups G, int P_new, const int* __restrict__ src, co
     }
 }
 
+// ---- gradient norm (clip_grad_norm_) ----------------------------------------------------------------------------------
+// The grid is a function of the buffer size alone (never of the device), so every rank of a multi-GPU run, holding the
+// same all-reduced bytes, gets the same partials, the same sums and the same coefficient.
+constexpr int NORM_THREADS = 256, NORM_MAX_CTAS = 1024;
+struct GroupBounds {
+    int n;
+    long long begin[MAXG + 1];
+};
+
+int norm_ctas(long long total) {
+    const long long c = (total + NORM_THREADS * 4 - 1) / (NORM_THREADS * 4);
+    return (int)(c < NORM_MAX_CTAS ? c : NORM_MAX_CTAS);
+}
+
+// partials[q * gridDim.x + cta] = this CTA's float64 sum over group q of (g * grad_scale)^2.  The square of an fp32 value
+// is exact in float64, so the only roundings are the float64 additions, each in an order fixed by the launch shape.
+__global__ void __launch_bounds__(NORM_THREADS)
+grad_sumsq_kernel(const GroupBounds G, const float* __restrict__ g, float grad_scale, double* __restrict__ partials) {
+    const long long total = G.begin[G.n];
+    double acc[MAXG];
+#pragma unroll
+    for (int q = 0; q < MAXG; q++) acc[q] = 0.0;
+    // a thread's elements only move forward, so it runs one sum for the current group and banks it when a group ends
+    int cq = 0;
+    long long cend = G.begin[1];
+    double run = 0.0;
+    for (long long i = (long long)blockIdx.x * (NORM_THREADS * 4) + threadIdx.x * 4; i < total;
+         i += (long long)gridDim.x * (NORM_THREADS * 4)) {
+        float4 x4;
+        if (i + 3 < total) {
+            x4 = *reinterpret_cast<const float4*>(g + i);
+        } else {
+            float t[4] = {};
+            for (int k = 0; k < 4 && i + k < total; k++) t[k] = g[i + k];
+            x4 = make_float4(t[0], t[1], t[2], t[3]);
+        }
+        const float* X = &x4.x;
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const long long e = i + k;
+            if (e >= total) break;
+            while (e >= cend) {           // groups may be empty and may start inside a float4
+#pragma unroll
+                for (int q = 0; q < MAXG; q++) if (q == cq) acc[q] += run;
+                run = 0.0; cq++; cend = G.begin[cq + 1];
+            }
+            const double y = (double)(X[k] * grad_scale);
+            run += y * y;
+        }
+    }
+#pragma unroll
+    for (int q = 0; q < MAXG; q++) if (q == cq) acc[q] += run;
+
+    __shared__ double red[MAXG][NORM_THREADS / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int q = 0; q < MAXG; q++) {
+        if (q >= G.n) break;
+        double a = acc[q];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+        if (lane == 0) red[q][warp] = a;
+    }
+    __syncthreads();
+    if (threadIdx.x < G.n) {
+        double t = 0.0;
+#pragma unroll
+        for (int w = 0; w < NORM_THREADS / 32; w++) t += red[threadIdx.x][w];
+        partials[(size_t)threadIdx.x * gridDim.x + blockIdx.x] = t;
+    }
+}
+
+// One CTA: each group's partials summed in a fixed order, then the norm and torch's clip coefficient.
+__global__ void __launch_bounds__(NORM_THREADS)
+grad_norm_finish_kernel(int n, int parts, const double* __restrict__ partials, const float* __restrict__ extra_norms, int n_extra,
+                        float max_norm, float* __restrict__ total_norm, float* __restrict__ clip_coef,
+                        double* __restrict__ group_sumsq) {
+    __shared__ double S[MAXG];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int q = warp; q < n; q += NORM_THREADS / 32) {
+        double a = 0.0;
+        for (int i = lane; i < parts; i += 32) a += partials[(size_t)q * parts + i];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+        if (lane == 0) S[q] = a;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int q = 0; q < n; q++) {
+            t += S[q];
+            if (group_sumsq) group_sumsq[q] = S[q];
+        }
+        for (int e = 0; e < n_extra; e++) {
+            const double x = extra_norms[e];
+            t += x * x;
+        }
+        const float tot = (float)sqrt(t);
+        // torch: max_norm / (total + 1e-6) is (total + 1e-6).reciprocal() * max_norm (Tensor.__rdiv__), all in fp32;
+        // clamp(max=1) passes a NaN through
+        const float c = (1.0f / (tot + 1e-6f)) * max_norm;
+        *total_norm = tot;
+        *clip_coef = c > 1.0f ? 1.0f : c;
+    }
+}
+
+__global__ void adam_step_count_kernel(long long* step) { *step += 1; }
+
+// the group table both device-state entry points take: n_groups in [1, MAXG], begin[0] = 0, begin non-decreasing
+int check_groups(const char* fn, int32_t n_groups, const int64_t* begin) {
+    if (n_groups < 1 || n_groups > MAXG) return sr_fail(SR_EINVAL, "%s: n_groups must be in [1, %d], got %d", fn, MAXG, n_groups);
+    if (!begin) return sr_fail(SR_EINVAL, "%s: begin is NULL", fn);
+    if (begin[0] != 0) return sr_fail(SR_EINVAL, "%s: begin[0] must be 0, got %lld", fn, (long long)begin[0]);
+    for (int i = 0; i < n_groups; i++)
+        if (begin[i + 1] < begin[i])
+            return sr_fail(SR_EINVAL, "%s: begin must be non-decreasing (begin[%d] = %lld > begin[%d] = %lld)", fn, i,
+                           (long long)begin[i], i + 1, (long long)begin[i + 1]);
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -129,9 +285,73 @@ SR_API int sr_adam_flat(int32_t n_groups, const int64_t* begin /* host, n_groups
     const long long blocks = (total + 1023) / 1024;
     ProfileScope ps("adam_flat", s);
     // grid-stride: at most 16 CTAs per SM of an H100 SXM (132 SMs)
-    adam_flat_kernel<<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, s>>>(G, params, grads, exp_avg, exp_avg_sq, beta1,
-                                                                                       beta2, eps, bc1, sqrt_bc2, grad_scale);
+    adam_flat_kernel<false><<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, s>>>(
+        G, params, grads, exp_avg, exp_avg_sq, beta1, beta2, eps, bc1, sqrt_bc2, grad_scale, AdamDeviceState{});
     return sr_launched(1, "sr_adam_flat");
+}
+
+SR_API int64_t sr_grad_norm_scratch_bytes(int32_t n_groups) {
+    if (n_groups < 1 || n_groups > MAXG) return -1;
+    return (int64_t)NORM_MAX_CTAS * n_groups * (int64_t)sizeof(double);
+}
+
+SR_API int sr_grad_norm_flat(int32_t n_groups, const int64_t* begin, const float* grads, float grad_scale, const float* extra_norms,
+                             int32_t n_extra, float max_norm, float* total_norm, float* clip_coef, double* group_sumsq,
+                             void* scratch, int64_t scratch_bytes, void* stream_) {
+    int rc = check_groups("sr_grad_norm_flat", n_groups, begin);
+    if (rc) return rc;
+    if (!grads || !total_norm || !clip_coef || !scratch)
+        return sr_fail(SR_EINVAL, "sr_grad_norm_flat: grads, total_norm, clip_coef and scratch must not be NULL");
+    if ((uintptr_t)grads & 15) return sr_fail(SR_EINVAL, "sr_grad_norm_flat: grads must be 16-byte aligned");
+    if ((uintptr_t)scratch & 7) return sr_fail(SR_EINVAL, "sr_grad_norm_flat: scratch must be 8-byte aligned");
+    if (n_extra < 0) return sr_fail(SR_EINVAL, "sr_grad_norm_flat: n_extra must be >= 0, got %d", n_extra);
+    if (n_extra > 0 && !extra_norms) return sr_fail(SR_EINVAL, "sr_grad_norm_flat: extra_norms is NULL but n_extra = %d", n_extra);
+    if (scratch_bytes < sr_grad_norm_scratch_bytes(n_groups))
+        return sr_fail(SR_EINVAL, "sr_grad_norm_flat: scratch holds fewer bytes than sr_grad_norm_scratch_bytes(%d)", n_groups);
+    GroupBounds G{};
+    G.n = n_groups;
+    for (int i = 0; i <= n_groups; i++) G.begin[i] = begin[i];
+    const int parts = norm_ctas(begin[n_groups]);
+    double* partials = (double*)scratch;
+    cudaStream_t s = (cudaStream_t)stream_;
+    if (parts > 0) {
+        ProfileScope ps("grad_sumsq", s);
+        grad_sumsq_kernel<<<parts, NORM_THREADS, 0, s>>>(G, grads, grad_scale, partials);
+    }
+    {
+        ProfileScope ps("grad_norm_finish", s);
+        grad_norm_finish_kernel<<<1, NORM_THREADS, 0, s>>>(n_groups, parts, partials, extra_norms, n_extra, max_norm, total_norm,
+                                                          clip_coef, group_sumsq);
+    }
+    return sr_launched(parts > 0 ? 2 : 1, "sr_grad_norm_flat");
+}
+
+SR_API int sr_adam_flat_state(int32_t n_groups, const int64_t* begin, const float* lr, float beta1, float beta2, float eps,
+                              int64_t* step, float grad_scale, const float* clip_coef, float* params, const float* grads,
+                              float* exp_avg, float* exp_avg_sq, void* stream_) {
+    int rc = check_groups("sr_adam_flat_state", n_groups, begin);
+    if (rc) return rc;
+    if (!lr || !step || !params || !grads || !exp_avg || !exp_avg_sq)
+        return sr_fail(SR_EINVAL, "sr_adam_flat_state: a required pointer is NULL");
+    if (((uintptr_t)params | (uintptr_t)grads | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) & 15)
+        return sr_fail(SR_EINVAL, "sr_adam_flat_state: params, grads, exp_avg and exp_avg_sq must be 16-byte aligned");
+    if ((uintptr_t)step & 7) return sr_fail(SR_EINVAL, "sr_adam_flat_state: step must be 8-byte aligned");
+    AdamGroups G{};
+    G.n = n_groups;
+    for (int i = 0; i <= n_groups; i++) G.begin[i] = begin[i];
+    const long long total = begin[n_groups];
+    cudaStream_t s = (cudaStream_t)stream_;
+    {
+        ProfileScope ps("adam_step_count", s);
+        adam_step_count_kernel<<<1, 1, 0, s>>>(reinterpret_cast<long long*>(step));
+    }
+    if (total == 0) return sr_launched(1, "sr_adam_flat_state");
+    const long long blocks = (total + 1023) / 1024;
+    ProfileScope ps("adam_flat_state", s);
+    adam_flat_kernel<true><<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, s>>>(
+        G, params, grads, exp_avg, exp_avg_sq, beta1, beta2, eps, 1.0f, 1.0f, grad_scale,
+        AdamDeviceState{lr, reinterpret_cast<const long long*>(step), clip_coef});
+    return sr_launched(2, "sr_adam_flat_state");
 }
 
 /* Gather the surfel rows of every parameter group (and both Adam moments) into new flat buffers: new row s = old row

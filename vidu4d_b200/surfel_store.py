@@ -61,6 +61,13 @@ class FlatSurfelModel(torch.nn.Module):
         self._install(tensors + ([] if regist_feat is None else [regist_feat]), dev)
         self.exp_avg = torch.zeros_like(self.flat)
         self.exp_avg_sq = torch.zeros_like(self.flat)
+        # step()'s state, on the device at fixed addresses so that a captured step reads the current values on every
+        # replay: the step count (shared by the groups, kept across densification and reset_opacity as the reference
+        # keeps each group's `step`), the per-group rates, and the coefficient clip_grad_norm_ leaves for step()
+        self.device_step = torch.zeros((), dtype=torch.int64, device=dev)
+        self.device_lr = torch.tensor([self.lrs[n] for n, _ in self.groups], dtype=torch.float32, device=dev)
+        self.clip_coef = torch.ones((), dtype=torch.float32, device=dev)
+        self._clip_pending = False
         self._reset_stats()
 
     # ---- layout -------------------------------------------------------------------------------------------------
@@ -93,6 +100,7 @@ class FlatSurfelModel(torch.nn.Module):
             p = torch.nn.Parameter(self.flat[o:o + P * k].view(shapes[name]))
             p.grad = self.grad_flat[o:o + P * k].view(shapes[name])
             setattr(self, _ATTR[name], p)
+        self._clip_pending = False            # a clip coefficient belongs to the gradients it was computed from
 
     def _reset_stats(self):
         dev = self.flat.device
@@ -112,6 +120,7 @@ class FlatSurfelModel(torch.nn.Module):
 
     def zero_grad_flat(self):
         self.grad_flat.zero_()
+        self._clip_pending = False
 
     # ---- one-kernel Adam (trainer.py:253 + 585-586) ---------------------------------------------------------------
     def adam_step(self, grad_scale: float = 1.0):
@@ -121,6 +130,49 @@ class FlatSurfelModel(torch.nn.Module):
         self.step_count += 1
         _capi.call("sr_adam_flat", self.flat.device, len(self.groups), begin, lr, self.betas[0], self.betas[1], self.eps,
                    self.step_count, float(grad_scale), self.flat, self.grad_flat, self.exp_avg, self.exp_avg_sq)
+
+    # ---- clip + Adam with the per-step state on the device (trainer.py:547, 589-591) -----------------------------------
+    def _begin(self):
+        off, total = self._offsets(self.P)
+        return (C.c_int64 * (len(self.groups) + 1))(*off, total)
+
+    def set_lr(self, name: str, value: float):
+        """Set group `name`'s learning rate for step() (written in place: a captured step picks it up) and adam_step()."""
+        i = [n for n, _ in self.groups].index(name)
+        self.lrs[name] = float(value)
+        self.device_lr[i].fill_(float(value))
+
+    @torch.no_grad()
+    def clip_grad_norm_(self, max_norm: float, extra_params=(), grad_scale: float = 1.0):
+        """torch.nn.utils.clip_grad_norm_(self.flat_params() + extra_params, max_norm) (trainer.py:547, check_grad) for a
+        step whose surfel gradients are grad_flat * grad_scale.  The extras' gradients (None ones skipped) are scaled
+        here, with torch._foreach_mul_; the surfel gradients are scaled inside the next step(), which must get the same
+        grad_scale.  Returns the total norm as a device tensor, without a host synchronisation."""
+        dev = self.flat.device
+        grads = [p.grad for p in extra_params if p.grad is not None]
+        _capi.check_tensors([(f"extra_params[{i}].grad", g) for i, g in enumerate(grads)], "the surfel buffer", self.flat)
+        norms = torch.stack(torch._foreach_norm(grads)) if grads else None
+        n = len(self.groups)
+        scratch = torch.empty((int(_capi.load().sr_grad_norm_scratch_bytes(n)),), dtype=torch.uint8, device=dev)
+        total = torch.empty((), dtype=torch.float32, device=dev)
+        _capi.call("sr_grad_norm_flat", dev, n, self._begin(), self.grad_flat, float(grad_scale), norms, len(grads),
+                   float(max_norm), total, self.clip_coef, None, scratch, scratch.numel())
+        if grads:
+            torch._foreach_mul_(grads, self.clip_coef)
+        self._clip_pending = True
+        return total
+
+    @torch.no_grad()
+    def step(self, grad_scale: float = 1.0):
+        """One Adam step (the gs_optimizer.step() of trainer.py:589-591) with its step count and rates read from the
+        device, and the surfel gradients multiplied by grad_scale, then by the coefficient of a clip_grad_norm_ made
+        since the last zero_grad_flat() / step().  device_step advances by one, also with no surfels.  Capturable: each
+        replay of a graph holding this call steps with the current count and rates.  step_count is adam_step()'s."""
+        coef = self.clip_coef if self._clip_pending else None
+        self._clip_pending = False
+        _capi.call("sr_adam_flat_state", self.flat.device, len(self.groups), self._begin(), self.device_lr, self.betas[0],
+                   self.betas[1], self.eps, self.device_step, float(grad_scale), coef, self.flat, self.grad_flat,
+                   self.exp_avg, self.exp_avg_sq)
 
     # ---- densification statistics (gaussian_model.py:450-452, trainer.py:553-560) ----------------------------------
     @torch.no_grad()
