@@ -109,6 +109,14 @@ OPTIM_PROTOTYPES = {
 }
 OPTIM_SYMBOLS = tuple(OPTIM_PROTOTYPES)
 
+# the fused delta-skinning MLP, declared in include/surfel_skin_mlp.h (own header and table for the same reason)
+SKIN_MLP_PROTOTYPES = {
+    "sr_delta_skin_scratch_bytes": (C.c_int64, [_i32] * 3),
+    "sr_delta_skin_forward": (C.c_int, [_i32] * 6 + [_p] * 8),
+    "sr_delta_skin_backward": (C.c_int, [_i32] * 6 + [_p] * 14 + [_i64, _p]),
+}
+SKIN_MLP_SYMBOLS = tuple(SKIN_MLP_PROTOTYPES)
+
 
 _lib = None
 
@@ -123,10 +131,11 @@ def load():
             f"{LIB_PATH} not found: the CUDA extension is not built. Run `python -m vidu4d_b200.build` "
             "(or __graft_entry__.build()). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for s in SYMBOLS + SSIM_SYMBOLS + OPTIM_SYMBOLS:
+    for s in SYMBOLS + SSIM_SYMBOLS + OPTIM_SYMBOLS + SKIN_MLP_SYMBOLS:
         if not hasattr(lib, s):
             raise SurfelRasterError(f"{LIB_PATH} does not export {s}")
-    for name, (restype, argtypes) in list(PROTOTYPES.items()) + list(SSIM_PROTOTYPES.items()) + list(OPTIM_PROTOTYPES.items()):
+    for name, (restype, argtypes) in (list(PROTOTYPES.items()) + list(SSIM_PROTOTYPES.items()) + list(OPTIM_PROTOTYPES.items())
+                                      + list(SKIN_MLP_PROTOTYPES.items())):
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.sr_abi_version() != ABI_VERSION:

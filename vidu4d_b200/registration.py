@@ -9,7 +9,7 @@ in two autograd functions, because the caller's delta-skinning MLP runs on the m
 
     cand = draw_candidates(M, P, 2048, device=dev)
     xyz_m = global_match(feat_px, model._regist_feat, model._xyz, cand, logsigma, num_grad=8)      # (M,H,W,3)
-    delta = delta_mlp(xyz_m)                                                                      # (M,H,W,B) or None
+    delta = delta_skin(xyz_m, rest_articulation, log_gauss, mlp, cond_mean)         # warp.delta_skin: (M,H,W,B); or None
     out = reproj_loss(xyz_m, hxy, Kmat, rest_articulation, t_articulation, log_gauss, field2cam, mask_fg, is_detected,
                       weight=wt, train_res=256, delta=delta)
 

@@ -125,7 +125,7 @@ def bob_warp(xyz, rot, rest_articulation, t_articulation, log_gauss, field2cam, 
 
     xyz (P,3), rot (P,4): canonical surfels.  rest_articulation ((B,4),(B,4)) and t_articulation ((M,B,4),(M,B,4)): bone-to-
     object dual quaternions.  log_gauss (B,3).  field2cam ((M,4),(M,3)).  delta (P,B): optional delta skinning term
-    (relu(mlp) * 0.1 of skinning.py:104-119; the MLP itself stays in PyTorch).
+    (relu(mlp) * 0.1 of skinning.py:104-119: delta_skin(xyz, rest_articulation, log_gauss, mlp, cond)).
     Returns xyz_cam (M,P,3), rot_cam (M,P,4), skin_entropy (P,)."""
     o2b_q, o2b_t, inv_gauss, se3_r, se3_d = warp_tables(rest_articulation, t_articulation, log_gauss)
     return _BobWarp.apply(xyz, rot, o2b_q, o2b_t, inv_gauss, se3_r, se3_d, field2cam[0], field2cam[1], delta)
@@ -239,7 +239,8 @@ def cycle_loss(xyz, xyz_cam, rest_articulation, t_articulation, log_gauss, field
     xyz (P,3): canonical surfels.  xyz_cam (M,P,3): bob_warp's output for the same surfels, so autograd chains through
     both kernels.  rest_articulation ((B,4),(B,4)), t_articulation ((M,B,4),(M,B,4)), log_gauss (B,3), field2cam
     ((M,4),(M,3)): as for bob_warp.  delta (M,P,B) or None: the frame-conditioned delta skinning term (relu(mlp) * 0.1 of
-    skinning.py:104-119) that the caller evaluates on the surfels in object space at time t.  weights: the weights of
+    skinning.py:104-119) evaluated on the surfels in object space at time t: delta_skin(xyz_t, t_articulation, log_gauss, mlp,
+    cond) with xyz_t (M,P,3) and the frames' cond (M,C).  weights: the weights of
     {reg_deform_cyc, reg_delta_skin, reg_skin_entropy}, 3 floats or a (3,) float32 CUDA tensor read at run time (refill it
     in place between CUDA-graph replays).
 
@@ -368,3 +369,139 @@ def feature_rows(regist_feat, xyz, scaling, xyz_cam, rot_cam, Kmat, field2cam, r
     rows, s, density = _FeatureRows.apply(regist_feat, xyz, xyz_cam, rot_cam, field2cam[0], centres, beta, scaling, Kmat,
                                           (P, M, B, Cf))
     return {"rows": rows, "flow_scale": s, "gauss_density": density}
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Delta-skinning MLP (csrc/skin_mlp.cu): delta = relu(delta_field([xyz_bone | t_embed | inst_code])) * 0.1 of
+# skinning.py:104-119, the `delta=` argument of bob_warp, cycle_loss and reproj_loss.
+
+SKIN_MLP_WIDTH = 64           # hidden units of the reference's delta_field (CondMLP(D=2, W=64), skinning.py:74-85)
+SKIN_MLP_DEPTH = 2
+
+
+class DeltaSkinMLP(torch.nn.Module):
+    """The reference's `SkinningField.delta_field` (CondMLP(D=2, W=64), base.py:17-150) with the fused op as its forward.
+
+    Parameters carry the reference's names and shapes -- linear_1.0.weight (64, 3B+C), linear_1.0.bias, linear_2.0.weight
+    (64,64), linear_2.0.bias, linear_final.weight (B,64), linear_final.bias -- so load_state_dict of the reference's
+    delta_field state (without its inst_embedding entries) works.  cond_channels C = 128 time + 32 instance channels."""
+
+    def __init__(self, num_bones, cond_channels=160):
+        super().__init__()
+        if not 1 <= num_bones <= B_MAX:
+            raise RuntimeError(f"num_bones must be in [1, {B_MAX}], got {num_bones}")
+        if cond_channels < 0:
+            raise RuntimeError(f"cond_channels must be >= 0, got {cond_channels}")
+        self.num_bones, self.cond_channels = int(num_bones), int(cond_channels)
+        relu = torch.nn.ReLU(True)
+        self.linear_1 = torch.nn.Sequential(torch.nn.Linear(3 * num_bones + cond_channels, SKIN_MLP_WIDTH), relu)
+        self.linear_2 = torch.nn.Sequential(torch.nn.Linear(SKIN_MLP_WIDTH, SKIN_MLP_WIDTH), relu)
+        self.linear_final = torch.nn.Linear(SKIN_MLP_WIDTH, num_bones)
+
+    def forward(self, points, articulation, log_gauss, cond):
+        return delta_skin(points, articulation, log_gauss, self, cond)
+
+
+def delta_skin_tables(articulation, log_gauss, W1, b1, cond):
+    """The first layer folded per frame: F (Mt,64,4) float32 with W1 [xyz_bone | cond] + b1 = F [x; 1], Mt = 1 when the
+    bones and cond are shared and M when either is per frame.  xyz_bone[b] = (R_b x + t_b) exp(-log_gauss[b]) with
+    (R_b, t_b) the inverse of bone b's articulation (transforms.py:9-25, skinning.py:126-142), so the product with W1's
+    first 3B columns is a (64,3) matrix and a 64-vector; W1's other columns times cond, and b1, join that vector.  Built
+    in float64 with differentiable torch ops and rounded once."""
+    r, d = articulation[0].double(), articulation[1].double()
+    if r.dim() == 2:
+        r, d = r[None], d[None]
+    q = _qconj(r)                                               # object -> bone, as warp_tables / cycle_tables
+    t = 2.0 * _qmul(_qconj(d), r)[..., 1:]                      # (Mb,B,3)
+    w, x, y, z = q.unbind(-1)
+    R = torch.stack((w * w + x * x - y * y - z * z, 2 * (x * y - w * z), 2 * (x * z + w * y),
+                     2 * (x * y + w * z), w * w - x * x + y * y - z * z, 2 * (y * z - w * x),
+                     2 * (x * z - w * y), 2 * (y * z + w * x), w * w - x * x - y * y + z * z), -1)
+    B = int(log_gauss.shape[0])
+    R = R.view(R.shape[0], B, 3, 3)                             # q v q* as a matrix, q not normalised (nor is it there)
+    ig = torch.exp(-log_gauss.double())                         # (B,3)
+    W1 = W1.double()
+    Wx = W1[:, :3 * B].view(1, -1, B, 3) * ig                   # (1,64,B,3)
+    # tens of thousands of products: plain broadcast sums, no GEMM call
+    A = (Wx[..., None] * R[:, None]).sum((2, 3))                # (Mb,64,3)
+    c = (Wx * t[:, None]).sum((2, 3))                           # (Mb,64)
+    cond = cond.double()
+    if cond.dim() == 1:
+        cond = cond[None]
+    c = c + (cond[:, None, :] * W1[None, :, 3 * B:]).sum(-1) + b1.double()      # (Mt,64): (1 | M) broadcast with (1 | M)
+    A = A.expand(c.shape[0], -1, -1)
+    return torch.cat((A, c[..., None]), -1).to(torch.float32)
+
+
+def _check_delta_skin(points, articulation, log_gauss, mlp, cond):
+    if points.dim() not in (2, 3, 4) or points.shape[-1] != 3 or any(s_ < 1 for s_ in points.shape):
+        raise RuntimeError(f"points must be (N,3), (M,N,3) or (M,H,W,3) with every dimension >= 1, got {tuple(points.shape)}")
+    M = int(points.shape[0]) if points.dim() > 2 else 1
+    B = int(log_gauss.shape[0]) if log_gauss.dim() == 2 else -1
+    if not 1 <= B <= B_MAX or tuple(log_gauss.shape) != (B, 3):
+        raise RuntimeError(f"log_gauss must be (B,3) with 1 <= B <= {B_MAX}, got {tuple(log_gauss.shape)}")
+    if not isinstance(mlp, DeltaSkinMLP):
+        raise RuntimeError(f"mlp must be a DeltaSkinMLP, got {type(mlp).__name__}")
+    if mlp.num_bones != B:
+        raise RuntimeError(f"mlp has {mlp.num_bones} bones, log_gauss {B}")
+    shapes = [tuple(t.shape) for t in articulation] if len(articulation) == 2 else None
+    if shapes not in ([(B, 4)] * 2, [(M, B, 4)] * 2):
+        raise RuntimeError(f"articulation must be ((B,4),(B,4)) or ((M,B,4),(M,B,4)) with B = {B}, M = {M}, got {shapes}")
+    C = mlp.cond_channels
+    if tuple(cond.shape) not in ((C,), (M, C)):
+        raise RuntimeError(f"cond must be (C,) or (M,C) with C = {C}, M = {M}, got {tuple(cond.shape)}")
+    named = [("points", points), ("articulation", articulation[0]), ("articulation", articulation[1]), ("log_gauss", log_gauss),
+             ("cond", cond)] + [("mlp." + n, p) for n, p in mlp.named_parameters()]
+    _capi.check_tensors(named, "points", points)
+    return M, B
+
+
+class _DeltaSkin(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, points, F, W2, b2, W3, b3, dims):
+        M, N, B = dims
+        ins = tuple(t.detach().contiguous() for t in (points, F, W2, b2, W3, b3))
+        dev = points.device
+        delta = torch.empty((M, N, B), dtype=torch.float32, device=dev)
+        _capi.call("sr_delta_skin_forward", dev, M, N, B, int(F.shape[0]), SKIN_MLP_WIDTH, SKIN_MLP_DEPTH, *ins, delta)
+        ctx.dims = dims
+        ctx.save_for_backward(*ins)
+        return delta
+
+    @staticmethod
+    def backward(ctx, g_delta):
+        M, N, B = ctx.dims
+        ins = ctx.saved_tensors
+        F, W2, b2, W3, b3 = ins[1:]
+        dev = F.device
+        g_delta = g_delta.to(torch.float32).contiguous()
+        g_points = torch.empty((M, N, 3), dtype=torch.float32, device=dev)
+        grads = tuple(torch.empty_like(t) for t in (F, W2, b2, W3, b3))
+        nbytes = int(_capi.load().sr_delta_skin_scratch_bytes(M, N, B))
+        scratch = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+        _capi.call("sr_delta_skin_backward", dev, M, N, B, int(F.shape[0]), SKIN_MLP_WIDTH, SKIN_MLP_DEPTH, *ins, g_delta, g_points,
+                   *grads, scratch, nbytes)
+        return (g_points,) + grads + (None,)
+
+
+def delta_skin(points, articulation, log_gauss, mlp, cond):
+    """The delta skinning term of skinning.py:104-119, delta = relu(delta_field([xyz_bone | cond])) * 0.1, as one fused
+    CUDA op each way (csrc/skin_mlp.cu) -- the `delta=` of bob_warp, cycle_loss and reproj_loss.
+
+    points (N,3), (M,N,3) or (M,H,W,3): object-space points.  articulation ((B,4),(B,4)) shared by every frame or
+    ((M,B,4),(M,B,4)) per frame: the bones the skinning is evaluated on as dual quaternions (rest_articulation for the
+    forward warps, t_articulation for the cycle's backward warp).  log_gauss (B,3).  mlp: a DeltaSkinMLP.  cond (C,)
+    shared or (M,C) per frame: cat(t_embed, inst_code), the time code (the mean embedding, or the frame's) and the instance
+    code, which stay the caller's few torch ops.
+
+    Returns delta of shape points.shape[:-1] + (B,), differentiable in points, both halves of articulation, log_gauss,
+    cond and the MLP's six parameters.  The first layer is folded per frame into a (64,4) table in float64 (see
+    delta_skin_tables); the kernels never form xyz_bone, the (…,3B+C) input or a stored activation.  The backward holds
+    sr_delta_skin_scratch_bytes of scratch (a few MB) for the fixed-order sum of the weight gradients: results are
+    bit-identical from run to run.  No host synchronisation."""
+    M, B = _check_delta_skin(points, articulation, log_gauss, mlp, cond)
+    F = delta_skin_tables(articulation, log_gauss, mlp.linear_1[0].weight, mlp.linear_1[0].bias, cond)
+    N = points.numel() // (3 * M)
+    delta = _DeltaSkin.apply(points.reshape(M, N, 3), F, mlp.linear_2[0].weight, mlp.linear_2[0].bias, mlp.linear_final.weight,
+                             mlp.linear_final.bias, (M, N, B))
+    return delta.view(tuple(points.shape[:-1]) + (B,))
