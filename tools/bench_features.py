@@ -35,12 +35,21 @@ x and y (8 B) and writes the three gradient maps (12 B); the backward reads the 
 quantities, plus the per-pixel formula).  Printed with each size: the bytes / 3.35 TB/s and FLOP / 67 TFLOP/s bounds
 (H100 SXM data sheet) and the measured share of the larger.
 
+--mask times a Stage-3 training step -- render_loss_batch over 300 K surfels, forward + backward -- with the silhouette
+term as the reference weighs it (batch balance weights, vis2d and is_detected masks, positive mean over the batch): fused
+(csrc/mask_loss.cu, mask_loss_weight=) with the whole step captured in one CUDA graph, against the reference's torch
+statements on out["allmap"][:, 1] run eagerly (they synchronise with the host, so that step cannot be captured),
+alternating in one process, at 256x256 x 2 frames (Stage-3 training) and 512x512 x 8 frames (headline).  Reports step
+times from CUDA events, the three kernels' times (sr_set_profiling), peak memory above the inputs, the torch-level host
+synchronisations of one eager step (torch.cuda.set_sync_debug_mode), and the two paths' loss and gradients.
+
     python tools/bench_features.py --features 4 22 32 [--steps 20 --warmup 5]
     python tools/bench_features.py --losses [--steps 20 --warmup 5]
     python tools/bench_features.py --reproj [--steps 20 --warmup 5]
     python tools/bench_features.py --cycle [--steps 20 --warmup 5]
     python tools/bench_features.py --rows [--steps 20 --warmup 5]
     python tools/bench_features.py --ssim [--steps 20 --warmup 5]
+    python tools/bench_features.py --mask [--steps 20 --warmup 5]
 """
 import argparse
 import json
@@ -68,7 +77,10 @@ def main():
     ap.add_argument("--cycle", action="store_true")
     ap.add_argument("--rows", action="store_true")
     ap.add_argument("--ssim", action="store_true")
+    ap.add_argument("--mask", action="store_true")
     args = ap.parse_args()
+    if args.mask:
+        return bench_mask(args)
     if args.ssim:
         return bench_ssim(args)
     if args.rows:
@@ -751,6 +763,143 @@ def bench_ssim(args):
                       "ms_per_step": {k: round(v, 4) for k, v in med.items()},
                       "library_launches_per_step": {k: s_.launches for k, s_ in steps.items()},
                       "steps": args.steps, "statistic": "median step time", "gpu": gpu}), flush=True)
+    RZ.set_sync_mode(True)
+    RZ._pending.clear()
+
+
+def _torch_mask_term(acc, mask, vis, det, w):
+    """lab4d/engine/model.py:587-611,648-650,950-967,1000-1012 as the reference writes them, on (M,H,W) planes."""
+    vd = vis * det[:, None, None]
+    if mask.sum() > 0 and (1 - mask).sum() > 0:
+        pos_wt = vd.sum() / mask[vd > 0].sum()
+        neg_wt = vd.sum() / (1 - mask[vd > 0]).sum()
+        bw = 0.5 * pos_wt * mask + 0.5 * neg_wt * (1 - mask)
+    else:
+        bw = 1
+    v = (acc - mask).pow(2) * bw * vis * det[:, None, None]
+    v = v.mean() if (v > 0).sum() == 0 else v[v > 0].mean()
+    return v * w
+
+
+def _count_syncs(fn):
+    """torch-level host synchronisations of one call of fn (torch.cuda.set_sync_debug_mode)."""
+    import warnings
+    with warnings.catch_warnings(record=True) as rec:
+        warnings.simplefilter("always")
+        torch.cuda.set_sync_debug_mode("warn")
+        try:
+            fn()
+        finally:
+            torch.cuda.set_sync_debug_mode("default")
+    return sum("synchroniz" in str(r.message) for r in rec)
+
+
+def bench_mask(args):
+    from vidu4d_b200 import _capi, rasterizer as RZ
+    from vidu4d_b200.graph import GraphedStep
+    from vidu4d_b200.renderer import PipelineParams, make_camera, render_loss_batch, stack_cameras
+    from vidu4d_b200.synthetic import SurfelCloud, object_scene, orbit_view
+    assert torch.cuda.is_available(), "this measurement needs a GPU"
+    dev = torch.device("cuda:0")
+    _capi.load()
+    gpu = _gpu_name()
+    P = args.surfels
+    scene = object_scene(P, seed=0, opacity="trained", center=(0.0, 0.0, 0.0))
+    flush = torch.empty((256 << 20,), dtype=torch.uint8, device=dev)
+    pipe, bg = PipelineParams(), torch.zeros(3, device=dev)
+    for RES, M in ((256, 2), (512, 8)):
+        cams = []
+        for f in range(M):
+            R, t = orbit_view(f, 64)
+            cams.append(make_camera(RES, RES, 2 * np.arctan(0.5), 2 * np.arctan(0.5), R=R.T, T=t, device=dev))
+        bc = stack_cameras(cams)
+        g = torch.Generator(device=dev).manual_seed(99)
+        rgb = torch.rand((M, 3, RES, RES), device=dev, generator=g)
+        mask = (torch.rand((M, RES, RES), device=dev, generator=g) > 0.6).float()
+        vis = (torch.rand((M, RES, RES), device=dev, generator=g) > 0.1).float()
+        det = torch.ones(M, device=dev)
+        w = torch.tensor([0.1], device=dev)
+        cloud = SurfelCloud(scene, dev)
+        kw = dict(vis2d=vis, mask_gt=mask, lambda_normal=0.05, lambda_dist=10.0)
+
+        def fused():
+            out = render_loss_batch(bc, cloud, pipe, bg, rgb, is_detected=det, mask_loss_weight=w, **kw)
+            out["loss"].backward()
+            return out["loss"]
+
+        def eager():
+            # the statements' own forward and autograd backward to dL/dalpha; the rasterizer backward that dL/dalpha feeds
+            # runs for the other terms either way, at a cost independent of the values it is handed
+            out = render_loss_batch(bc, cloud, pipe, bg, rgb, **kw)
+            alpha = out["allmap"][:, 1].detach().requires_grad_(True)
+            loss = out["loss"] + _torch_mask_term(alpha, mask, vis, det, w[0])
+            loss.backward()
+            eager.alpha = alpha
+            return loss
+        RZ.set_sync_mode(True)
+        fused(); eager()                                               # warm-up: learns the instance capacity
+        torch.cuda.synchronize()
+        peak, loss = {}, {}
+        for k, b in (("fused", fused), ("torch", eager)):
+            torch.cuda.synchronize()
+            base = torch.cuda.memory_allocated()
+            torch.cuda.reset_peak_memory_stats()
+            cloud.zero_grad()
+            loss[k] = float(b().detach())
+            torch.cuda.synchronize()
+            peak[k] = round((torch.cuda.max_memory_allocated() - base) / 2**20, 1)
+        # dL/dalpha of the term: the fused kernels on the torch arm's alpha against its autograd gradient
+        from vidu4d_b200.renderer import _mask_term
+        am = torch.zeros((M, 8, RES, RES), device=dev)
+        am[:, 1] = eager.alpha.detach()
+        dla = torch.zeros_like(am)
+        _mask_term(M, RES, RES, am, mask, vis, det, w, dla)
+        ga = eager.alpha.grad
+        compare = {"loss_rel_diff": abs(loss["fused"] - loss["torch"]) / abs(loss["torch"]),
+                   "dL_dalpha_max_abs_diff_over_max": float((dla[:, 1] - ga).abs().max() / ga.abs().max())}
+        RZ.set_sync_mode(False)
+        syncs = {"fused": _count_syncs(fused), "torch": _count_syncs(eager)}
+        torch.cuda.synchronize()
+        RZ._pending.clear()
+        step = GraphedStep(fused, device=dev)
+        step()
+        for _ in range(args.warmup):
+            step(check=False)
+            eager()
+        torch.cuda.synchronize()
+        RZ._pending.clear()
+        ms = {"fused": [], "torch": []}
+        for i in range(args.steps):
+            for k in ("fused", "torch"):
+                flush.fill_(i & 255)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record()
+                step.graph.replay() if k == "fused" else eager()
+                b.record()
+                b.synchronize()
+                RZ._pending.clear()
+                ms[k].append(a.elapsed_time(b))
+        step.arm(); RZ.check_overflow(keep=True)
+        RZ._pending.clear()
+        RZ.set_sync_mode(True)
+        fused()
+        torch.cuda.synchronize()
+        _capi.get_profile()
+        _capi.set_profiling(True)
+        for _ in range(5):
+            fused()
+        prof = _capi.get_profile()
+        _capi.set_profiling(False)
+        kern = {k: round(v["ms"] / max(v["count"], 1), 4) for k, v in prof.items()
+                if k in ("mask_stats", "mask_loss", "mask_loss_scale", "loss_grad")}
+        print(json.dumps({"workload": "render_loss_batch step with the silhouette term (fwd + bwd)", "surfels": P,
+                          "resolution": RES, "frames": M, "ms_per_step": {k: round(float(np.median(v)), 4) for k, v in ms.items()},
+                          "capture": {"fused": "one CUDA graph", "torch": "eager"}, "peak_mem_mb_above_inputs": peak,
+                          "kernel_ms_per_launch": kern, "torch_host_syncs_per_eager_step": syncs,
+                          "library_launches_per_step_fused": step.launches, "outputs": compare, "steps": args.steps,
+                          "statistic": "median step time", "gpu": gpu}), flush=True)
+        del step
+        torch.cuda.empty_cache()
     RZ.set_sync_mode(True)
     RZ._pending.clear()
 

@@ -117,6 +117,14 @@ SKIN_MLP_PROTOTYPES = {
 }
 SKIN_MLP_SYMBOLS = tuple(SKIN_MLP_PROTOTYPES)
 
+# Stage 3's silhouette loss with the reference's balance weights, declared in include/surfel_mask_loss.h (own header and
+# table for the same reason)
+MASK_LOSS_PROTOTYPES = {
+    "sr_mask_loss_scratch_bytes": (C.c_int64, [_i32] * 3),
+    "sr_mask_loss_batch": (C.c_int, [_i32] * 3 + [_p, _i64] + [_p] * 9 + [_i64, _p]),
+}
+MASK_LOSS_SYMBOLS = tuple(MASK_LOSS_PROTOTYPES)
+
 
 _lib = None
 
@@ -131,11 +139,11 @@ def load():
             f"{LIB_PATH} not found: the CUDA extension is not built. Run `python -m vidu4d_b200.build` "
             "(or __graft_entry__.build()). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for s in SYMBOLS + SSIM_SYMBOLS + OPTIM_SYMBOLS + SKIN_MLP_SYMBOLS:
+    for s in SYMBOLS + SSIM_SYMBOLS + OPTIM_SYMBOLS + SKIN_MLP_SYMBOLS + MASK_LOSS_SYMBOLS:
         if not hasattr(lib, s):
             raise SurfelRasterError(f"{LIB_PATH} does not export {s}")
     for name, (restype, argtypes) in (list(PROTOTYPES.items()) + list(SSIM_PROTOTYPES.items()) + list(OPTIM_PROTOTYPES.items())
-                                      + list(SKIN_MLP_PROTOTYPES.items())):
+                                      + list(SKIN_MLP_PROTOTYPES.items()) + list(MASK_LOSS_PROTOTYPES.items())):
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.sr_abi_version() != ABI_VERSION:

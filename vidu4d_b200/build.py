@@ -17,11 +17,12 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libsurfel_raster.so")
 SOURCES = ["api.cu", "preprocess.cu", "sort.cu", "composite_fwd.cu", "composite_tile.cu", "composite_feat.cu", "surfel_bwd.cu",
            "postprocess.cu", "loss.cu", "warp.cu", "match.cu", "cycle.cu", "feature_rows.cu", "optim.cu", "knn.cu", "outlier.cu", "ssim.cu",
-           "skin_mlp.cu"]
+           "skin_mlp.cu", "mask_loss.cu"]
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "composite_common.cuh"), os.path.join(CSRC, "post_common.cuh"),
            os.path.join(CSRC, "warp_common.cuh"),
            os.path.join(HERE, "..", "include", "surfel_raster.h"), os.path.join(HERE, "..", "include", "surfel_ssim.h"),
-           os.path.join(HERE, "..", "include", "surfel_optim.h"), os.path.join(HERE, "..", "include", "surfel_skin_mlp.h")]
+           os.path.join(HERE, "..", "include", "surfel_optim.h"), os.path.join(HERE, "..", "include", "surfel_skin_mlp.h"),
+           os.path.join(HERE, "..", "include", "surfel_mask_loss.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",

@@ -368,7 +368,8 @@ class _RasterLossBatch(torch.autograd.Function):
     further differentiable output; their incoming gradient (already scaled) goes to the same rasterizer backward."""
 
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, bkgd, cfg, features=None, feature_loss=None):
+    def forward(ctx, means3D, means2D, sh, opacities, scales, rotations, bkgd, cfg, features=None, feature_loss=None,
+                mask_loss=None):
         from . import _capi
         from .rasterizer import _C
         (cams, bg, sh_degree, target, vis, mask, mask_wt, depth_ratio, w_rgb, w_mask, lam_n, lam_d, tanx, tany, target_stream,
@@ -400,6 +401,11 @@ class _RasterLossBatch(torch.autograd.Function):
         if w_ssim > 0.0:                    # D-SSIM on the final colour: csrc/ssim.cu, its gradient added into dLc / dLa / dLb
             sterms = _ssim_term(M, H, W, color, allmap, target, bk, w_ssim, dLc, dLa, dLb)
             total = total + sterms.sum()
+        mterms = None
+        if mask_loss is not None:           # after SSIM: the silhouette term's gradient is the last addend of dL/dalpha
+            is_det, weight = mask_loss
+            mterms, mcounts = _mask_term(M, H, W, allmap, mask, vis, f32(is_det), weight, dLa)
+            total = total + mterms.sum()
         dLf = None
         if feature_loss is not None:        # the losses on the feature planes: csrc/loss.cu, sr_feature_loss_batch
             ftarget, is_det, gm, weights = feature_loss
@@ -417,7 +423,7 @@ class _RasterLossBatch(torch.autograd.Function):
                               dLb if dLb is not None else e, features, dLf)
         ctx.has_features = features is not None
         outs = (total, terms, color, allmap, radii) + (() if feat is None else (feat,)) + (() if dLf is None else (fterms, counts))
-        outs = outs + (() if sterms is None else (sterms,))
+        outs = outs + (() if sterms is None else (sterms,)) + (() if mterms is None else (mterms, mcounts))
         ctx.mark_non_differentiable(terms, color, allmap, radii, *(o for o in outs[5:] if o is not feat))
         return outs
 
@@ -445,7 +451,7 @@ class _RasterLossBatch(torch.autograd.Function):
         g_bk = (dLb.sum(0) * g_total) if ctx.has_bkgd else None
         return (_reduce_like(g3d, means3D), g2d, _reduce_like(gsh, sh), _reduce_like(gop, opacities),
                 _reduce_like(gsc, scales), _reduce_like(grot, rotations), g_bk, None,
-                _reduce_like(grads[8], features) if ctx.has_features else None, None)
+                _reduce_like(grads[8], features) if ctx.has_features else None, None, None)
 
 
 def _ssim_term(M, H, W, color, allmap, target, bkgd, w_ssim, dLc, dLa, dLb):
@@ -465,6 +471,39 @@ def _ssim_term(M, H, W, color, allmap, target, bkgd, w_ssim, dLc, dLa, dLb):
     _capi.call("sr_ssim_backward", dev, M, 3, H, W, color, target, alpha, stride, bkgd, maps, g, 1, dLc, 1, d_alpha, dLb,
                scratch, nbytes)
     return (1.0 - per_frame) * float(w_ssim)
+
+
+def _mask_term(M, H, W, allmap, mask, vis, is_detected, weight, dLa):
+    """Stage 3's silhouette term as the reference weighs it (csrc/mask_loss.cu): returns each frame's share (M,) and count of
+    positive values (M,) int32, and ADDS its gradient into dL/dalpha (allmap plane 1) -- unscaled, like the other terms'."""
+    from . import _capi
+    dev = allmap.device
+    nbytes = int(_capi.load().sr_mask_loss_scratch_bytes(M, W, H))
+    scratch = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+    terms = torch.empty((M,), dtype=torch.float32, device=dev)
+    counts = torch.empty((M,), dtype=torch.int32, device=dev)
+    balance = torch.empty((3,), dtype=torch.float32, device=dev)
+    _capi.call("sr_mask_loss_batch", dev, M, W, H, allmap[:, 1], 8 * H * W, mask, vis, is_detected, weight, terms, counts,
+               balance, dLa[:, 1], scratch, nbytes)
+    return terms, counts
+
+
+def _check_mask_loss(M, device, mask_gt, mask_wt, w_mask, is_detected, mask_loss_weight):
+    """Validate the fused silhouette term's arguments of render_loss_batch before anything runs on the device; returns
+    (is_detected, weight)."""
+    if mask_gt is None:
+        raise RuntimeError("mask_loss_weight needs mask_gt")
+    if mask_wt is not None or w_mask != 0.0:
+        raise RuntimeError("mask_loss_weight replaces the plain mask term: pass neither mask_wt nor w_mask != 0 with it")
+    if tuple(mask_loss_weight.shape) != (1,) or mask_loss_weight.dtype != torch.float32:
+        raise RuntimeError(f"mask_loss_weight must be a float32 (1,) tensor, got {mask_loss_weight.dtype} "
+                           f"{tuple(mask_loss_weight.shape)}")
+    if is_detected is not None and tuple(is_detected.shape) != (M,):
+        raise RuntimeError(f"is_detected must be (M,) = ({M},), got {tuple(is_detected.shape)}")
+    for name, t in (("mask_loss_weight", mask_loss_weight), ("is_detected", is_detected)):
+        if t is not None and (not t.is_cuda or t.device != device):
+            raise RuntimeError(f"{name} must be a CUDA tensor on the rasterizer's device {device}, got {t.device}")
+    return is_detected, mask_loss_weight.contiguous()
 
 
 def _check_feature_losses(M, H, W, features, feature_target, mask_gt, is_detected, gauss_mask_channel, feature_loss_weights):
@@ -521,7 +560,7 @@ def _check_loss_inputs(M, H, W, device, target_rgb, vis2d, mask_gt, mask_wt, lea
 def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_gt=None, mask_wt=None, learnable_bkgd=None,
                       w_rgb=1.0, w_mask=0.0, lambda_normal=0.0, lambda_dist=0.0, means3D=None, rotations=None, target_stream=None,
                       features=None, feature_target=None, is_detected=None, gauss_mask_channel=None, feature_loss_weights=None,
-                      w_ssim=0.0):
+                      w_ssim=0.0, mask_loss_weight=None):
     """The Stage-3 inner loop for M frames in one call: rasterize every frame (batched launch set), post-process and
     evaluate the image losses in one fused kernel, and hand autograd a single scalar.
 
@@ -552,7 +591,15 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
 
     w_ssim > 0 adds, per frame, w_ssim * (1 - SSIM(final colour, target_rgb)) to "loss" (csrc/ssim.cu; gs/train.py's D-SSIM
     term): the final colour includes learnable_bkgd, and SSIM is unmasked.  "ssim_terms": (M,) each frame's share
-    (detached).  Stage 3's setting is w_rgb = 1 - lambda_dssim, w_ssim = lambda_dssim.  w_ssim = 0 launches nothing more."""
+    (detached).  Stage 3's setting is w_rgb = 1 - lambda_dssim, w_ssim = lambda_dssim.  w_ssim = 0 launches nothing more.
+
+    mask_loss_weight: (1,) float32 DEVICE tensor mask_wt (read at run time, like feature_loss_weights) turns on Stage 3's
+    silhouette term as the reference weighs it (csrc/mask_loss.cu, lab4d/engine/model.py:587-611,648-650,950-967,
+    1000-1012): mask_wt * mean over the batch's positive values of (alpha - mask_gt)^2 * bw * vis2d * is_detected[frame],
+    with the batch's class-balance weights bw of get_mask_balance_wt (or v.mean() if no value is positive).  Needs
+    mask_gt; excludes mask_wt and w_mask != 0 (the plain per-frame mask term).  "mask_terms": (M,) each frame's share
+    (detached, included in "loss"); "mask_counts": (M,) int32, each frame's number of positive values.  Its gradient is
+    added into dL/dalpha after the SSIM term's.  None launches nothing more."""
     if not isinstance(cameras, BatchCameras):
         cameras = stack_cameras(cameras)
     M = len(cameras)
@@ -563,6 +610,9 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
     if feature_target is not None or gauss_mask_channel is not None:
         feature_loss = _check_feature_losses(M, cameras.image_height, cameras.image_width, features, feature_target, mask_gt,
                                              is_detected, gauss_mask_channel, feature_loss_weights)
+    mask_loss = None
+    if mask_loss_weight is not None:
+        mask_loss = _check_mask_loss(M, xyz.device, mask_gt, mask_wt, w_mask, is_detected, mask_loss_weight)
     rot = pc.get_rotation if rotations is None else rotations
     P = int(xyz.shape[-2])
     screenspace_points = torch.zeros((M, P, 3), dtype=xyz.dtype, requires_grad=True, device=xyz.device)
@@ -570,7 +620,7 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
     cfg = (cameras, bg_color, pc.active_sh_degree, target_rgb, vis2d, mask_gt, mask_wt, float(pipe.depth_ratio),
            w_rgb, w_mask, lambda_normal, lambda_dist, tanx, tany, target_stream, float(w_ssim))
     outs = _RasterLossBatch.apply(xyz, screenspace_points, pc.get_features, pc.get_opacity, pc.get_scaling, rot,
-                                  learnable_bkgd, cfg, features, feature_loss)
+                                  learnable_bkgd, cfg, features, feature_loss, mask_loss)
     total, terms, color, allmap, radii = outs[:5]
     out = {"loss": total, "terms": terms, "render": color, "allmap": allmap, "radii": radii,
            "visibility_filter": radii > 0, "viewspace_points": screenspace_points}
@@ -578,6 +628,10 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
         out["features"] = outs[5]
     if feature_loss is not None:
         out["feature_terms"], out["feature_counts"] = outs[6], outs[7]
+    k = 5 + (features is not None) + 2 * (feature_loss is not None)
     if w_ssim > 0.0:
-        out["ssim_terms"] = outs[-1]
+        out["ssim_terms"] = outs[k]
+        k += 1
+    if mask_loss is not None:
+        out["mask_terms"], out["mask_counts"] = outs[k], outs[k + 1]
     return out
