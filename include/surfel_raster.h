@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SR_ABI_VERSION 10
+#define SR_ABI_VERSION 11
 
 #if defined(__GNUC__)
 #define SR_API __attribute__((visibility("default")))
@@ -70,7 +70,7 @@ typedef struct sr_frame {
     float   scale_modifier;  /* accepted and ignored, exactly like the reference (forward.cu:95) */
     int32_t prefiltered;     /* if set, a culled surfel is an error in the reference (__trap); we report it via status bit 2 */
     int32_t debug;           /* if set, synchronise + check after every launch (auxiliary.h:271-278) */
-    uint32_t flags;          /* reserved, must be 0 */
+    uint32_t flags;          /* 0, or SR_FRAME_CAMERAS (surfel_camera.h): per-frame intrinsics from a device table; other bits reserved, must be 0 */
 } sr_frame;
 
 /* ---- buffer sizing (replaces required<GeometryState/ImageState/BinningState>, rasterizer_impl.h:66-72) */

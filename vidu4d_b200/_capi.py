@@ -11,10 +11,11 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libsurfel_raster.so")
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 SR_STATUS_OVERFLOW = 1
 SR_STATUS_PREFILTER = 4
 SR_BATCH_SUM_SHARED = 1
+SR_FRAME_CAMERAS = 1        # sr_frame.flags bit (include/surfel_camera.h): per-frame intrinsics from a device table
 FEATURES_MAX = 32          # channels per call (SR_FEAT_MAX); also the widest feature row sr_feature_rows_* writes
 
 
@@ -25,6 +26,11 @@ class SrFrame(C.Structure):
         ("tan_fovx", C.c_float), ("tan_fovy", C.c_float), ("scale_modifier", C.c_float),
         ("prefiltered", C.c_int32), ("debug", C.c_int32), ("flags", C.c_uint32),
     ]
+
+
+class SrFrameCameras(C.Structure):
+    """sr_frame_cameras (include/surfel_camera.h): an sr_frame with SR_FRAME_CAMERAS set, and its DEVICE [M*4] table."""
+    _fields_ = [("frame", SrFrame), ("cameras", C.c_void_p)]
 
 
 class SrBatch(C.Structure):
@@ -125,6 +131,13 @@ MASK_LOSS_PROTOTYPES = {
 }
 MASK_LOSS_SYMBOLS = tuple(MASK_LOSS_PROTOTYPES)
 
+# per-frame intrinsics (the loss pass's entry point; the rasterizer reads the table through sr_frame_cameras), declared in
+# include/surfel_camera.h (own header and table for the same reason)
+CAMERA_PROTOTYPES = {
+    "sr_render_loss_batch_cameras": (C.c_int, [_i32, _i32, _i32, _p, _f32] + [_p] * 8 + [_f32] * 4 + [_p] * 6),
+}
+CAMERA_SYMBOLS = tuple(CAMERA_PROTOTYPES)
+
 
 _lib = None
 
@@ -139,11 +152,12 @@ def load():
             f"{LIB_PATH} not found: the CUDA extension is not built. Run `python -m vidu4d_b200.build` "
             "(or __graft_entry__.build()). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for s in SYMBOLS + SSIM_SYMBOLS + OPTIM_SYMBOLS + SKIN_MLP_SYMBOLS + MASK_LOSS_SYMBOLS:
+    for s in SYMBOLS + SSIM_SYMBOLS + OPTIM_SYMBOLS + SKIN_MLP_SYMBOLS + MASK_LOSS_SYMBOLS + CAMERA_SYMBOLS:
         if not hasattr(lib, s):
             raise SurfelRasterError(f"{LIB_PATH} does not export {s}")
     for name, (restype, argtypes) in (list(PROTOTYPES.items()) + list(SSIM_PROTOTYPES.items()) + list(OPTIM_PROTOTYPES.items())
-                                      + list(SKIN_MLP_PROTOTYPES.items()) + list(MASK_LOSS_PROTOTYPES.items())):
+                                      + list(SKIN_MLP_PROTOTYPES.items()) + list(MASK_LOSS_PROTOTYPES.items())
+                                      + list(CAMERA_PROTOTYPES.items())):
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.sr_abi_version() != ABI_VERSION:

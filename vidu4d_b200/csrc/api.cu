@@ -14,6 +14,7 @@
 #include <cstring>
 
 #include "common.cuh"
+#include "../../include/surfel_camera.h"
 
 namespace {
 thread_local char g_err[512] = "";
@@ -40,6 +41,9 @@ CamParams make_cam(const sr_frame* f, const float* vm, const float* campos, cons
     // backward.cu:570 / 683-684
     c.bcx = c.focal_x * f->tan_fovx;
     c.bcy = c.focal_y * f->tan_fovy;
+    c.kcx = c.bcx; c.kcy = c.bcy;
+    // SR_FRAME_CAMERAS: the kernels replace the intrinsics above with each frame's row (common.cuh cam_of_frame)
+    c.cams = (f->flags & SR_FRAME_CAMERAS) ? reinterpret_cast<const sr_frame_cameras*>(f)->cameras : nullptr;
     return c;
 }
 
@@ -50,6 +54,8 @@ int check_frame(const sr_frame* f) {
     if (f->width > 65535 || f->height > 65535) return sr_fail(SR_EINVAL, "image side must be < 65536");
     if (f->sh_degree < 0 || f->sh_degree > 3) return sr_fail(SR_EINVAL, "sh_degree must be 0..3");
     if (f->sh_coeffs < 0) return sr_fail(SR_EINVAL, "sh_coeffs must be >= 0");
+    if ((f->flags & SR_FRAME_CAMERAS) && !reinterpret_cast<const sr_frame_cameras*>(f)->cameras)
+        return sr_fail(SR_EINVAL, "SR_FRAME_CAMERAS is set but the per-frame camera table is NULL");
     if (f->sh_coeffs > 0 && (f->sh_degree + 1) * (f->sh_degree + 1) > f->sh_coeffs)
         return sr_fail(SR_EINVAL, "sh_degree %d needs %d coefficients, shs has %d", f->sh_degree,
                        (f->sh_degree + 1) * (f->sh_degree + 1), f->sh_coeffs);

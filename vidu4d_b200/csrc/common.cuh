@@ -128,8 +128,10 @@ struct CamParams {
     const float* vm;       // DEVICE viewmatrix[16] as passed (column-major 4x4 in glm terms)
     const float* campos;   // DEVICE [3]
     const float* bg;       // DEVICE [3]
-    float focal_x, focal_y, cx, cy;     // forward intrinsics: cx = W/2, cy = H/2 (forward.cu:208)
-    float bcx, bcy;                     // backward intrinsics: focal*tanfov (backward.cu:570)
+    const float* cams;     // DEVICE [frames*4] per-frame (tan_x, tan_y, cx_off, cy_off), or nullptr: the scalars below
+    float focal_x, focal_y, cx, cy;     // forward intrinsics: cx = W/2 + cx_off, cy = H/2 + cy_off (forward.cu:208)
+    float bcx, bcy;                     // backward intrinsics: focal*tanfov (backward.cu:570), the mean2D proxy's scale
+    float kcx, kcy;                     // backward K's principal point: bcx + cx_off, bcy + cy_off
     int W, H, tiles_x, tiles_y;
     int P, D, M;
 };
@@ -261,9 +263,25 @@ template <class T>
 __device__ __forceinline__ T* fr(T* p, long long stride_bytes, int f) {
     return p ? reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(p) + (uintptr_t)((long long)f * stride_bytes)) : p;
 }
+// Frame f's camera.  With a per-frame table (c.cams), its intrinsics come from row f by make_cam's own operations (each
+// one rounded on its own, as the host rounds them), then the principal-point offset is added: a row holding the launch's
+// tangents and zero offsets reproduces the scalar intrinsics bit for bit.  The row is read as four scalar loads, so the
+// table needs no more than float alignment.  Its values are not checked.
 __device__ __forceinline__ CamParams cam_of_frame(CamParams c, const FrameStrides& fs, int f) {
     c.vm = fr(c.vm, fs.vm, f);
     c.campos = fr(c.campos, fs.campos, f);
+    if (c.cams) {
+        const float* r = c.cams + 4 * (size_t)f;
+        const float tx = __ldg(r), ty = __ldg(r + 1), ox = __ldg(r + 2), oy = __ldg(r + 3);
+        c.focal_y = __fdiv_rn((float)c.H, __fmul_rn(2.0f, ty));
+        c.focal_x = __fdiv_rn((float)c.W, __fmul_rn(2.0f, tx));
+        c.cx = __fadd_rn(__fmul_rn((float)c.W, 0.5f), ox);
+        c.cy = __fadd_rn(__fmul_rn((float)c.H, 0.5f), oy);
+        c.bcx = __fmul_rn(c.focal_x, tx);
+        c.bcy = __fmul_rn(c.focal_y, ty);
+        c.kcx = __fadd_rn(c.bcx, ox);
+        c.kcy = __fadd_rn(c.bcy, oy);
+    }
     return c;
 }
 __device__ __forceinline__ float4 ld_nc_f4(const float4* p) {

@@ -16,13 +16,15 @@
 // and every pixel picks up its four neighbours' results, so there are no atomics on image data and the result is
 // deterministic.  Batched: blockIdx.z = frame.
 #include "post_common.cuh"
+#include "../../include/surfel_camera.h"
 
 namespace {
 using namespace post;
 
 struct LossCfg {
     int W, H;
-    float tanx, tany, depth_ratio;
+    const float* cams;             // DEVICE [M*4] per-frame (tan_x, tan_y, cx_off, cy_off) (surfel_camera.h), or nullptr
+    float tanx, tany, depth_ratio; // tanx / tany: every frame's, when cams is nullptr
     float w_rgb, w_mask, lambda_normal, lambda_dist;
 };
 
@@ -100,7 +102,11 @@ loss_grad_kernel(const LossCfg g, const float* __restrict__ color, const float* 
     // pixel) and its neighbours pick the result up from shared memory -- no atomics on image data, deterministic
     __shared__ float sg[6][10][34];
     __shared__ PostCam cam_s;
-    if (threadIdx.x == 0) cam_s = load_cam(wvt + (size_t)f * 16, W, H, g.tanx, g.tany);
+    if (threadIdx.x == 0) {
+        const float* r = g.cams + 4 * (size_t)f;
+        cam_s = g.cams ? load_cam(wvt + (size_t)f * 16, W, H, __ldg(r), __ldg(r + 1), __ldg(r + 2), __ldg(r + 3))
+                       : load_cam(wvt + (size_t)f * 16, W, H, g.tanx, g.tany);
+    }
     __syncthreads();
     const PostCam& c = cam_s;
     float s0 = 0.f, s1 = 0.f, s2 = 0.f;               // surf_normal at this pixel
@@ -299,21 +305,18 @@ feat_loss_scale_kernel(const FeatLossCfg g, const float* __restrict__ weights, c
     if (g.gm >= 0) gf[g.gm * N] *= s[1];
 }
 
-}  // namespace
-
-extern "C" {
-
-SR_API int sr_render_loss_batch(int32_t M, int32_t W, int32_t H, float tanx, float tany, float depth_ratio,
-                                const float* color, const float* allmap, const float* world_view_transform,
-                                const float* target_rgb, const float* vis2d, const float* mask_gt, const float* mask_wt,
-                                const float* learnable_bkgd, float w_rgb, float w_mask, float lambda_normal, float lambda_dist,
-                                float* loss_terms, float* dL_dcolor, float* dL_dallmap, float* dL_dbkgd, float* surf_depth_scratch,
-                                void* stream_) {
-    if (M < 1 || W <= 0 || H <= 0) return sr_fail(SR_EINVAL, "sr_render_loss_batch: M, W and H must be positive");
+// sr_render_loss_batch and sr_render_loss_batch_cameras: `cams` (nullptr = the shared tanx / tany) is the only difference
+int render_loss_batch(const char* name, int32_t M, int32_t W, int32_t H, const float* cams, float tanx, float tany,
+                             float depth_ratio, const float* color, const float* allmap, const float* world_view_transform,
+                             const float* target_rgb, const float* vis2d, const float* mask_gt, const float* mask_wt,
+                             const float* learnable_bkgd, float w_rgb, float w_mask, float lambda_normal, float lambda_dist,
+                             float* loss_terms, float* dL_dcolor, float* dL_dallmap, float* dL_dbkgd, float* surf_depth_scratch,
+                             void* stream_) {
+    if (M < 1 || W <= 0 || H <= 0) return sr_fail(SR_EINVAL, "%s: M, W and H must be positive", name);
     if (!color || !allmap || !world_view_transform || !target_rgb || !loss_terms || !dL_dcolor || !dL_dallmap || !surf_depth_scratch)
-        return sr_fail(SR_EINVAL, "sr_render_loss_batch: a required pointer is NULL");
+        return sr_fail(SR_EINVAL, "%s: a required pointer is NULL", name);
     cudaStream_t s = (cudaStream_t)stream_;
-    LossCfg g{W, H, tanx, tany, depth_ratio, w_rgb, w_mask, lambda_normal, lambda_dist};
+    LossCfg g{W, H, cams, tanx, tany, depth_ratio, w_rgb, w_mask, lambda_normal, lambda_dist};
     dim3 grid((W + 31) / 32, (H + 7) / 8, M);
     CK(cudaMemsetAsync(loss_terms, 0, (size_t)M * 4 * sizeof(float), s), "sr_render_loss_batch: memset(loss_terms)");
     if (dL_dbkgd) CK(cudaMemsetAsync(dL_dbkgd, 0, (size_t)M * 3 * sizeof(float), s), "sr_render_loss_batch: memset(dL_dbkgd)");
@@ -326,7 +329,34 @@ SR_API int sr_render_loss_batch(int32_t M, int32_t W, int32_t H, float tanx, flo
         loss_grad_kernel<<<grid, 256, 0, s>>>(g, color, allmap, world_view_transform, target_rgb, vis2d, mask_gt, mask_wt,
                                              learnable_bkgd, surf_depth_scratch, loss_terms, dL_dcolor, dL_dallmap, dL_dbkgd);
     }
-    return sr_launched(2, "sr_render_loss_batch");
+    return sr_launched(2, name);
+}
+
+}  // namespace
+
+extern "C" {
+
+SR_API int sr_render_loss_batch(int32_t M, int32_t W, int32_t H, float tanx, float tany, float depth_ratio,
+                                const float* color, const float* allmap, const float* world_view_transform,
+                                const float* target_rgb, const float* vis2d, const float* mask_gt, const float* mask_wt,
+                                const float* learnable_bkgd, float w_rgb, float w_mask, float lambda_normal, float lambda_dist,
+                                float* loss_terms, float* dL_dcolor, float* dL_dallmap, float* dL_dbkgd, float* surf_depth_scratch,
+                                void* stream_) {
+    return render_loss_batch("sr_render_loss_batch", M, W, H, nullptr, tanx, tany, depth_ratio, color, allmap,
+                             world_view_transform, target_rgb, vis2d, mask_gt, mask_wt, learnable_bkgd, w_rgb, w_mask,
+                             lambda_normal, lambda_dist, loss_terms, dL_dcolor, dL_dallmap, dL_dbkgd, surf_depth_scratch, stream_);
+}
+
+SR_API int sr_render_loss_batch_cameras(int32_t M, int32_t W, int32_t H, const float* cameras, float depth_ratio,
+                                        const float* color, const float* allmap, const float* world_view_transform,
+                                        const float* target_rgb, const float* vis2d, const float* mask_gt,
+                                        const float* mask_wt, const float* learnable_bkgd, float w_rgb, float w_mask,
+                                        float lambda_normal, float lambda_dist, float* loss_terms, float* dL_dcolor,
+                                        float* dL_dallmap, float* dL_dbkgd, float* surf_depth_scratch, void* stream_) {
+    if (!cameras) return sr_fail(SR_EINVAL, "sr_render_loss_batch_cameras: the per-frame camera table is NULL");
+    return render_loss_batch("sr_render_loss_batch_cameras", M, W, H, cameras, 0.f, 0.f, depth_ratio, color, allmap,
+                             world_view_transform, target_rgb, vis2d, mask_gt, mask_wt, learnable_bkgd, w_rgb, w_mask,
+                             lambda_normal, lambda_dist, loss_terms, dL_dcolor, dL_dallmap, dL_dbkgd, surf_depth_scratch, stream_);
 }
 
 SR_API int sr_feature_loss_batch(int32_t M, int32_t W, int32_t H, int32_t F, int32_t Cf, int32_t gauss_mask_channel,

@@ -12,8 +12,10 @@ struct PostCam {
     float fx, fy, cx, cy;
 };
 
-// world_view_transform is W2C^T (row-vector convention).  c2w = inverse(W2C) by the adjugate formula.
-__device__ __forceinline__ PostCam load_cam(const float* __restrict__ wvt, int W, int H, float tanx, float tany) {
+// world_view_transform is W2C^T (row-vector convention).  c2w = inverse(W2C) by the adjugate formula.  ox, oy: the
+// principal point minus (W/2, H/2) in pixels (0 = the image centre, as point_utils.py:12-13 builds K).
+__device__ __forceinline__ PostCam load_cam(const float* __restrict__ wvt, int W, int H, float tanx, float tany, float ox = 0.f,
+                                            float oy = 0.f) {
     PostCam c;
     float m[16];
 #pragma unroll
@@ -40,7 +42,7 @@ __device__ __forceinline__ PostCam load_cam(const float* __restrict__ wvt, int W
     c.o[0] = -(c.A[0] * t0 + c.A[1] * t1 + c.A[2] * t2);
     c.o[1] = -(c.A[3] * t0 + c.A[4] * t1 + c.A[5] * t2);
     c.o[2] = -(c.A[6] * t0 + c.A[7] * t1 + c.A[8] * t2);
-    c.fx = W / (2.0f * tanx); c.fy = H / (2.0f * tany); c.cx = W * 0.5f; c.cy = H * 0.5f;
+    c.fx = W / (2.0f * tanx); c.fy = H / (2.0f * tany); c.cx = W * 0.5f + ox; c.cy = H * 0.5f + oy;
     return c;
 }
 

@@ -82,7 +82,9 @@ __device__ __forceinline__ void stage_rows_out(float* __restrict__ gdst, const f
     }
 }
 
-__global__ void __launch_bounds__(SB)
+// 5 blocks per SM (at most 102 registers): without the bound, the per-frame intrinsics of a camera table (common.cuh
+// cam_of_frame) take the kernel to 112 registers and 4 blocks whenever shared memory does not limit it first
+__global__ void __launch_bounds__(SB, 5)
 surfel_bwd_kernel(const CamParams c_, const FrameStrides fs, const float* __restrict__ means3D, const float* __restrict__ shs,
                   const float2* __restrict__ scales, const float4* __restrict__ rotations, const int* __restrict__ radii,
                   const float4* __restrict__ srec, const uint8_t* __restrict__ clamped, const float4* __restrict__ sgrad,
@@ -230,13 +232,13 @@ surfel_bwd_body(const CamParams& c, const int idx, const int M, const float* shv
     const V3 p = {__ldg(means3D + 3 * (size_t)idx), __ldg(means3D + 3 * (size_t)idx + 1), __ldg(means3D + 3 * (size_t)idx + 2)};
     V3 pv = wmul(vm, p);
     pv.x += vm[12]; pv.y += vm[13]; pv.z += vm[14];
-    // dL_dM column j = K^T (dTu[j], dTv[j], dTw[j]) with the BACKWARD intrinsics (cx = focal*tanfov)
+    // dL_dM column j = K^T (dTu[j], dTv[j], dTw[j]) with the BACKWARD intrinsics (cx = focal*tanfov + cx_off)
     V3 dM[3];
 #pragma unroll
     for (int j = 0; j < 3; j++) {
         dM[j].x = c.focal_x * dT[j];
         dM[j].y = c.focal_y * dT[3 + j];
-        dM[j].z = c.bcx * dT[j] + c.bcy * dT[3 + j] + dT[6 + j];
+        dM[j].z = c.kcx * dT[j] + c.kcy * dT[3 + j] + dT[6 + j];
     }
     const V3 dRS0 = wtmul(vm, dM[0]), dRS1 = wtmul(vm, dM[1]), dpw = wtmul(vm, dM[2]);
     V3 dtn = wtmul(vm, V3{dnr[0], dnr[1], dnr[2]});

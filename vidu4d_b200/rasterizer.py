@@ -19,7 +19,7 @@ PyTorch is plumbing here: it owns device memory and streams; every kernel is in 
 from __future__ import annotations
 
 import ctypes as C
-from typing import NamedTuple
+from typing import NamedTuple, Optional
 
 import torch
 import torch.nn as nn
@@ -221,11 +221,37 @@ def _as_float(x) -> float:
 _STRIDED = ("means3D", "sh", "colors", "opacity", "scales", "rotations")     # sr_batch's per-surfel strides, in its order
 
 
+def _check_intrinsics(intrinsics, M: int, ref):
+    """The (M,4) per-frame camera table (tan_fovx, tan_fovy, cx_off, cy_off) of include/surfel_camera.h: float32, contiguous,
+    on ref's device.  Only its shape is checked -- its values stay on the device."""
+    if intrinsics is None:
+        return None
+    if not torch.is_tensor(intrinsics) or intrinsics.dtype != torch.float32 or tuple(intrinsics.shape) != (M, 4):
+        raise RuntimeError(f"intrinsics must be a float32 (M,4) = {(M, 4)} tensor of (tan_fovx, tan_fovy, cx_off, cy_off)")
+    if not intrinsics.is_cuda or intrinsics.device != ref.device:
+        raise RuntimeError(f"intrinsics must be a CUDA tensor on {ref.device}")
+    return intrinsics.contiguous()
+
+
+def _frame(P, degree, Msh, W, H, tan_fovx, tan_fovy, scale_modifier, prefiltered, debug, intrinsics):
+    """sr_frame, or with a camera table sr_frame_cameras (whose tangents are not read, so nothing is read back from the
+    device).  Returns (the struct to keep alive, the sr_frame pointer to pass)."""
+    if intrinsics is None:
+        fr = _capi.SrFrame(P, int(degree), Msh, W, H, _as_float(tan_fovx), _as_float(tan_fovy), float(scale_modifier),
+                           int(bool(prefiltered)), int(bool(debug)), 0)
+        return fr, C.byref(fr)
+    fc = _capi.SrFrameCameras(_capi.SrFrame(P, int(degree), Msh, W, H, 0.0, 0.0, float(scale_modifier), int(bool(prefiltered)),
+                                            int(bool(debug)), _capi.SR_FRAME_CAMERAS), intrinsics.data_ptr())
+    return fc, C.byref(fc.frame)
+
+
 def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, scales, rotations, features, viewmatrix,
-             projmatrix, campos, H, W, degree, tan_fovx, tan_fovy, scale_modifier, prefiltered, debug, concat=True):
+             projmatrix, campos, H, W, degree, tan_fovx, tan_fovy, scale_modifier, prefiltered, debug, concat=True,
+             intrinsics=None):
     """The one sr_forward call behind every _C forward: M frames, F = 0 without features.  The caller has validated the
     inputs and made them contiguous float32 CUDA tensors; `strides` gives the floats between consecutive frames of each
-    per-surfel input (absent = shared).  The outputs get a leading frame dimension iff frame_dim.  In sync mode an
+    per-surfel input (absent = shared).  intrinsics: the checked (M,4) camera table, which replaces tan_fovx / tan_fovy,
+    or None.  The outputs get a leading frame dimension iff frame_dim.  In sync mode an
     overflowed call is re-run with a larger instance buffer; in nosync mode the status words join _pending.
     Returns (num_rendered (list of M ints, or -1 in nosync mode), out_color, out_others, radii, geom, binning, img,
     out_feat): with concat, out_color holds 3+F planes per frame and out_feat is the view of the last F; None when F = 0."""
@@ -235,8 +261,7 @@ def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, sc
     Msh = int(sh.shape[-2]) if sh is not None and sh.numel() != 0 else 0
     F = int(features.shape[-1]) if features is not None else 0
     lead = (M,) if frame_dim else ()
-    fr = _capi.SrFrame(P, int(degree), Msh, W, H, _as_float(tan_fovx), _as_float(tan_fovy), float(scale_modifier),
-                       int(bool(prefiltered)), int(bool(debug)), 0)
+    fr, frp = _frame(P, degree, Msh, W, H, tan_fovx, tan_fovy, scale_modifier, prefiltered, debug, intrinsics)
     bt = _capi.SrBatch(M, 0, *(strides.get(k, 0) for k in _STRIDED))
     with torch.cuda.device(dev):
         if F and concat:
@@ -260,7 +285,7 @@ def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, sc
             nosync = (not _sync_mode) and key in _cap_hint
             host = _host_slot(M) if nosync else torch.empty((M, 2), dtype=torch.int32, pin_memory=True)
             # an overflow re-run below re-runs the feature pass too
-            _capi.call("sr_forward", dev, C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh),
+            _capi.call("sr_forward", dev, frp, C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh),
                        _ptr(colors), _ptr(opacity), _ptr(scales), _ptr(rotations), _ptr(features), F, strides.get("features", 0),
                        _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), out_color, cstride, _ptr(out_feat), fstride, out_others,
                        _ptr(radii), geom, binning, img, cap, nr_dev, host)
@@ -289,7 +314,7 @@ def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, sc
 def _backward(M, frame_dim, strides, background, means3D, sh, colors, scales, rotations, features, viewmatrix, projmatrix,
               campos, radii, dL_dout_color, dL_dout_features, dL_dout_others, geomBuffer, binningBuffer, imageBuffer, degree,
               tan_fovx, tan_fovy, scale_modifier, debug, grad_scale=None, features_grad_scale=None, sum_shared=False,
-              want_transmat=True, outs=None):
+              want_transmat=True, outs=None, intrinsics=None):
     """The one sr_backward call behind every _C backward; none when P = 0, whose gradients are zero-filled.  Inputs as
     for _forward; strides["opacity"] is the forward's opacity stride.  The feature planes' gradient is dL_dout_features,
     or the tail of dL_dout_color when that is None.  Each gradient is (M,P,.), or (P,.) without frame_dim and, under
@@ -325,15 +350,14 @@ def _backward(M, frame_dim, strides, background, means3D, sh, colors, scales, ro
         dL_dfeatures = mk("features", F) if F else None
         if P > 0:
             cap = _capacity_from_bytes(int(binningBuffer.numel()) // M, W, H)
-            fr = _capi.SrFrame(P, int(degree), Msh, W, H, _as_float(tan_fovx), _as_float(tan_fovy),
-                               float(scale_modifier), 0, int(bool(debug)), 0)
+            fr, frp = _frame(P, degree, Msh, W, H, tan_fovx, tan_fovy, scale_modifier, False, debug, intrinsics)
             bt = _capi.SrBatch(M, _capi.SR_BATCH_SUM_SHARED if sum_shared else 0, *(strides.get(k, 0) for k in _STRIDED))
             gs = fgs = None
             if grad_scale is not None:
                 gs = grad_scale.to(device=dev, dtype=torch.float32).reshape(()).contiguous()
             if F and features_grad_scale is not None:
                 fgs = features_grad_scale.to(device=dev, dtype=torch.float32).reshape(()).contiguous()
-            _capi.call("sr_backward", dev, C.byref(fr), C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D),
+            _capi.call("sr_backward", dev, frp, C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D),
                        _ptr(sh), _ptr(colors), _ptr(scales), _ptr(rotations), _ptr(features), F, strides.get("features", 0),
                        _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), _ptr(radii), _ptr(dL_dout_color), cstride, dfeat_ptr,
                        fstride, _ptr(dL_dout_others), _ptr(gs), _ptr(fgs), geomBuffer, binningBuffer, imageBuffer, cap,
@@ -421,14 +445,18 @@ class _CNamespace:
     @staticmethod
     def rasterize_gaussians_batch(background, means3D, colors, opacity, scales, rotations, scale_modifier, viewmatrix,
                                   projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
-                                  prefiltered=False, debug=False, features=None, concat=True):
+                                  prefiltered=False, debug=False, features=None, concat=True, intrinsics=None):
         """M frames at once.  viewmatrix / projmatrix (M,4,4), campos (M,3).  Every per-surfel input is either shared by
         all frames -- the single-frame shape, e.g. means3D (P,3) -- or per frame with a leading M, e.g. (M,P,3) (Stage 3:
         each frame rasterizes its own warped copy of the surfels).  Returns (num_rendered (list of M ints, or -1 in nosync
         mode), out_color (M,3,H,W), out_others (M,8,H,W), radii (M,P), geomBuffer, binningBuffer, imgBuffer).
         features (P,F) shared or (M,P,F) per frame, 1 <= F <= 32: an eighth element, the (M,F,H,W) feature planes, is
         returned; with concat=True out_color is (M,3+F,H,W) and the feature planes are its view [:, 3:], with concat=False
-        the two are separate tensors."""
+        the two are separate tensors.
+        intrinsics: optional (M,4) float32 CUDA table, frame m's row (tan_fovx, tan_fovy, cx_off, cy_off) with the principal
+        point at (W/2 + cx_off, H/2 + cy_off) (include/surfel_camera.h; renderer.camera_table builds it from K).  The kernels
+        read it from device memory, so tan_fovx / tan_fovy are not read, nothing synchronises, and a captured call renders
+        with what the table holds at replay."""
         M = int(viewmatrix.shape[0])
         if viewmatrix.ndim != 3 or viewmatrix.shape[1:] != (4, 4) or campos.shape != (M, 3):
             raise RuntimeError("batched cameras: viewmatrix must be (M,4,4) and campos (M,3)")
@@ -436,11 +464,12 @@ class _CNamespace:
         projmatrix = _f32c(projmatrix, "projmatrix"); campos = _f32c(campos, "campos")
         if features is not None:
             _check_features(features, int(means3D.shape[-2]), background, batched=True)
+        intrinsics = _check_intrinsics(intrinsics, M, means3D)
         ins, strides = _batch_inputs(M, means3D=(means3D, (3,)), sh=(sh, None), colors=(colors, (3,)), opacity=(opacity, (1,)),
                                      scales=(scales, (2,)), rotations=(rotations, (4,)), features=(features, None))
         out = _forward(M, True, strides, background, ins["means3D"], ins["sh"], ins["colors"], ins["opacity"], ins["scales"],
                        ins["rotations"], ins["features"], viewmatrix, projmatrix, campos, int(image_height),
-                       int(image_width), degree, tan_fovx, tan_fovy, scale_modifier, prefiltered, debug, concat)
+                       int(image_width), degree, tan_fovx, tan_fovy, scale_modifier, prefiltered, debug, concat, intrinsics)
         return out if features is not None else out[:7]
 
     @staticmethod
@@ -448,7 +477,7 @@ class _CNamespace:
                                            projmatrix, tan_fovx, tan_fovy, dL_dout_color, dL_dout_others, sh, degree, campos,
                                            geomBuffer, binningBuffer, imageBuffer, grad_scale=None, debug=False,
                                            sum_shared=False, opacity_shared=True, want_transmat=True, outs=None,
-                                           features=None, dL_dout_features=None, features_grad_scale=None):
+                                           features=None, dL_dout_features=None, features_grad_scale=None, intrinsics=None):
         """Backward of rasterize_gaussians_batch.  dL_dout_color (M,3,H,W), dL_dout_others (M,8,H,W); grad_scale: optional
         0-d device tensor multiplying both (the upstream scalar of a fused loss).  Returns the eight gradient tensors
         (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dtransMat, dL_dsh, dL_dscales, dL_drotations), each with a
@@ -461,7 +490,7 @@ class _CNamespace:
         features (P,F) or (M,P,F): the gradient of the feature planes is either the tail of dL_dout_color (M,3+F,H,W) or a
         separate dL_dout_features (M,F,H,W) (then dL_dout_color is (M,3,H,W)); features_grad_scale (optional 0-d device
         tensor) multiplies it instead of grad_scale.  A ninth gradient, dL_dfeatures, is returned: (M,P,F), or (P,F) for
-        shared features with sum_shared=True."""
+        shared features with sum_shared=True.  intrinsics: the forward's (M,4) camera table, or None."""
         M = int(viewmatrix.shape[0])
         H, W = int(dL_dout_color.shape[-2]), int(dL_dout_color.shape[-1])
         background = _f32c(background, "background"); viewmatrix = _f32c(viewmatrix, "viewmatrix")
@@ -476,13 +505,15 @@ class _CNamespace:
                 dL_dout_features = _f32c(dL_dout_features, "dL_dout_features")
                 if tuple(dL_dout_features.shape) != (M, F, H, W) or tuple(dL_dout_color.shape) != (M, 3, H, W):
                     raise RuntimeError("dL_dout_color must be (M,3,H,W) and dL_dout_features (M,F,H,W)")
+        intrinsics = _check_intrinsics(intrinsics, M, means3D)
         ins, strides = _batch_inputs(M, means3D=(means3D, (3,)), sh=(sh, None), colors=(colors, (3,)),
                                      scales=(scales, (2,)), rotations=(rotations, (4,)), features=(features, None))
         strides["opacity"] = 0 if (opacity_shared or M == 1) else int(ins["means3D"].shape[-2])
         return _backward(M, True, strides, background, ins["means3D"], ins["sh"], ins["colors"], ins["scales"],
                          ins["rotations"], ins["features"], viewmatrix, projmatrix, campos, radii, dL_dout_color,
                          dL_dout_features, dL_dout_others, geomBuffer, binningBuffer, imageBuffer, degree, tan_fovx,
-                         tan_fovy, scale_modifier, debug, grad_scale, features_grad_scale, sum_shared, want_transmat, outs)
+                         tan_fovy, scale_modifier, debug, grad_scale, features_grad_scale, sum_shared, want_transmat, outs,
+                         intrinsics)
 
     @staticmethod
     def mark_visible(means3D, viewmatrix, projmatrix):
@@ -586,7 +617,9 @@ class _RasterizeGaussians(torch.autograd.Function):
 
 
 class BatchRasterizationSettings(NamedTuple):
-    """GaussianRasterizationSettings for M frames: viewmatrix / projmatrix are (M,4,4), campos is (M,3)."""
+    """GaussianRasterizationSettings for M frames: viewmatrix / projmatrix are (M,4,4), campos is (M,3).  intrinsics:
+    optional (M,4) float32 CUDA table of per-frame (tan_fovx, tan_fovy, cx_off, cy_off); when set, tanfovx / tanfovy are
+    not read (see _C.rasterize_gaussians_batch)."""
     image_height: int
     image_width: int
     tanfovx: float
@@ -599,6 +632,7 @@ class BatchRasterizationSettings(NamedTuple):
     campos: torch.Tensor
     prefiltered: bool = False
     debug: bool = False
+    intrinsics: Optional[torch.Tensor] = None
 
 
 def _reduce_like(grad, inp):
@@ -617,6 +651,8 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, rs, features=None):
         kw = {} if features is None else {"features": features}
+        if getattr(rs, "intrinsics", None) is not None:     # settings without the field (GaussianRasterizationSettings) work too
+            kw["intrinsics"] = rs.intrinsics
         num_rendered, color, allmap, radii, geomBuffer, binningBuffer, imgBuffer = _C.rasterize_gaussians_batch(
             rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, rs.viewmatrix, rs.projmatrix,
             rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh, rs.sh_degree, rs.campos, rs.prefiltered, rs.debug,
@@ -641,6 +677,8 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
         if grad_allmap is None:
             grad_allmap = torch.zeros((M, 8, H, W), dtype=torch.float32, device=means3D.device)
         kw = {"features": features} if F else {}
+        if getattr(rs, "intrinsics", None) is not None:     # settings without the field (GaussianRasterizationSettings) work too
+            kw["intrinsics"] = rs.intrinsics
         grads = _C.rasterize_gaussians_backward_batch(
             rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, rs.viewmatrix, rs.projmatrix,
             rs.tanfovx, rs.tanfovy, grad_color, grad_allmap, sh, rs.sh_degree, rs.campos, geomBuffer, binningBuffer, imgBuffer,

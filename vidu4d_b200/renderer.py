@@ -20,11 +20,12 @@ point_utils.py:9-18): the per-camera ray table is built once and cached.
 from __future__ import annotations
 
 import math
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
+from typing import Optional
 
 import torch
 
-from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer
+from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer, _check_intrinsics
 
 
 def _tan_half(fov) -> float:
@@ -341,7 +342,11 @@ class PipelineParams:
 # ---------------------------------------------------------------------------------------------
 @dataclass
 class BatchCameras:
-    """M cameras sharing resolution and field of view (Stage 3: gs/scene/cameras.py:72-162 builds them per frame)."""
+    """M cameras sharing resolution (Stage 3: gs/scene/cameras.py:72-162 builds them per frame).  Without `intrinsics` they
+    also share the field of view FoVx / FoVy, with the principal point at the image centre.  intrinsics: optional (M,4)
+    float32 CUDA table of each frame's (tan_fovx, tan_fovy, cx_off, cy_off) -- see camera_table() -- that the rasterizer
+    and the loss pass read on the device instead: FoVx / FoVy are then not read at all (no host synchronisation), and a
+    captured step renders with whatever the table holds at replay."""
     image_width: int
     image_height: int
     FoVx: float
@@ -349,9 +354,29 @@ class BatchCameras:
     world_view_transform: torch.Tensor   # (M,4,4), each W2C transposed
     full_proj_transform: torch.Tensor    # (M,4,4)
     camera_center: torch.Tensor          # (M,3)
+    intrinsics: Optional[torch.Tensor] = None   # (M,4) per-frame camera table, or None
 
     def __len__(self):
         return int(self.world_view_transform.shape[0])
+
+
+def camera_table(width, height, K) -> torch.Tensor:
+    """The (M,4) per-frame camera table (tan_fovx, tan_fovy, cx_off, cy_off) of BatchCameras.intrinsics from pinhole
+    intrinsics K (M,3,3), the same K feature_rows and reproj_loss project with:
+        tan_fovx = W / (2 K[:,0,0]),  tan_fovy = H / (2 K[:,1,1]),  cx_off = K[:,0,2] - W/2,  cy_off = K[:,1,2] - H/2.
+    float32 torch ops on K's device, with no host synchronisation, so it can sit inside a captured step; K gets no
+    gradient through it (nothing differentiates the rasterizer with respect to its camera).  The reference's KCamera
+    derives its FoV from the focal length with arctan and the rasterizer takes tan of half of it again, so its tangent may
+    differ from this one in the last bit."""
+    if K.ndim != 3 or tuple(K.shape[1:]) != (3, 3):
+        raise RuntimeError(f"K must be (M,3,3), got {tuple(K.shape)}")
+    K = K.detach().to(torch.float32)
+    W, H = float(width), float(height)
+    fx, fy = K[:, 0, 0], K[:, 1, 1]
+    # tensor / tensor: a Python number over a tensor would multiply by the reciprocal, which is not the IEEE quotient
+    tan_x = torch.full_like(fx, W) / (2.0 * fx)
+    tan_y = torch.full_like(fy, H) / (2.0 * fy)
+    return torch.stack((tan_x, tan_y, K[:, 0, 2] - 0.5 * W, K[:, 1, 2] - 0.5 * H), dim=1).contiguous()
 
 
 def stack_cameras(cams) -> BatchCameras:
@@ -378,6 +403,8 @@ class _RasterLossBatch(torch.autograd.Function):
         dev = means3D.device
         e = torch.empty((0,), dtype=torch.float32, device=dev)
         kw = {} if features is None else {"features": features, "concat": False}
+        if cams.intrinsics is not None:
+            kw["intrinsics"] = cams.intrinsics
         out = _C.rasterize_gaussians_batch(
             bg, means3D, e, opacities, scales, rotations, 1.0, cams.world_view_transform, cams.full_proj_transform, tanx, tany,
             H, W, sh, sh_degree, cams.camera_center, **kw)
@@ -394,8 +421,13 @@ class _RasterLossBatch(torch.autograd.Function):
         wvt = f32(cams.world_view_transform)         # (M,4,4) packed: callers may hand in a strided view
         if target_stream is not None:       # the targets are still being uploaded on another stream: join it only now,
             torch.cuda.current_stream(dev).wait_stream(target_stream)   # after the rasterizer forward has been queued
-        _capi.call("sr_render_loss_batch", dev, M, W, H, tanx, tany, float(depth_ratio), color, allmap, wvt, target, vis, mask,
-                   mask_wt, bk, float(w_rgb), float(w_mask), float(lam_n), float(lam_d), terms, dLc, dLa, dLb, scratch)
+        if cams.intrinsics is None:
+            _capi.call("sr_render_loss_batch", dev, M, W, H, tanx, tany, float(depth_ratio), color, allmap, wvt, target, vis,
+                       mask, mask_wt, bk, float(w_rgb), float(w_mask), float(lam_n), float(lam_d), terms, dLc, dLa, dLb, scratch)
+        else:
+            _capi.call("sr_render_loss_batch_cameras", dev, M, W, H, cams.intrinsics, float(depth_ratio), color, allmap, wvt,
+                       target, vis, mask, mask_wt, bk, float(w_rgb), float(w_mask), float(lam_n), float(lam_d), terms, dLc, dLa,
+                       dLb, scratch)
         total = terms.sum()
         sterms = None
         if w_ssim > 0.0:                    # D-SSIM on the final colour: csrc/ssim.cu, its gradient added into dLc / dLa / dLb
@@ -443,6 +475,8 @@ class _RasterLossBatch(torch.autograd.Function):
                 g_feat = torch.zeros((dLc.shape[0], features.shape[-1]) + tuple(dLc.shape[2:]), dtype=torch.float32,
                                      device=means3D.device)
             kw = {"features": features, "dL_dout_features": g_feat}
+        if cams.intrinsics is not None:
+            kw["intrinsics"] = cams.intrinsics
         grads = _C.rasterize_gaussians_backward_batch(
             bg, means3D, radii, e, scales, rotations, 1.0, cams.world_view_transform, cams.full_proj_transform, tanx, tany,
             dLc, dLa, sh, sh_degree, cams.camera_center, gb, bb, ib, grad_scale=g_total, sum_shared=True,
@@ -564,7 +598,8 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
     """The Stage-3 inner loop for M frames in one call: rasterize every frame (batched launch set), post-process and
     evaluate the image losses in one fused kernel, and hand autograd a single scalar.
 
-    cameras: BatchCameras (or a list of cameras, stacked here).  pc: as in render().  means3D (M,P,3) / rotations (M,P,4):
+    cameras: BatchCameras (or a list of cameras, stacked here); with cameras.intrinsics every frame is rendered, and its
+    normals are derived, with its own focal length and principal point.  pc: as in render().  means3D (M,P,3) / rotations (M,P,4):
     optional per-frame overrides -- the bob-warped surfels of each frame (DeformableGaussian._override_xyz/_rotation,
     lab4d/nnutils/deformable_gaussian.py:163-176); default = pc.get_xyz / pc.get_rotation shared by all frames.
     target_rgb (M,3,H,W); vis2d / mask_gt / mask_wt (M,H,W) or None; learnable_bkgd (3,) or None.
@@ -616,7 +651,11 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
     rot = pc.get_rotation if rotations is None else rotations
     P = int(xyz.shape[-2])
     screenspace_points = torch.zeros((M, P, 3), dtype=xyz.dtype, requires_grad=True, device=xyz.device)
-    tanx, tany = _cam_tans(cameras)
+    if cameras.intrinsics is not None:
+        cameras = replace(cameras, intrinsics=_check_intrinsics(cameras.intrinsics, M, xyz))
+        tanx = tany = None                  # not read: the table replaces them
+    else:
+        tanx, tany = _cam_tans(cameras)
     cfg = (cameras, bg_color, pc.active_sh_degree, target_rgb, vis2d, mask_gt, mask_wt, float(pipe.depth_ratio),
            w_rgb, w_mask, lambda_normal, lambda_dist, tanx, tany, target_stream, float(w_ssim))
     outs = _RasterLossBatch.apply(xyz, screenspace_points, pc.get_features, pc.get_opacity, pc.get_scaling, rot,
