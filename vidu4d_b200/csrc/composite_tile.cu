@@ -255,11 +255,12 @@ composite_tile_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ range
 //      pair (BwdPixel::pair_scalars) that go to a shared pair buffer.  A pair's slot is its pixel's base -- a CTA-wide
 //      exclusive scan of the per-pixel pair counts of the chunk -- plus its rank in the pixel's back-to-front list.
 //   2. instance phase (thread = instance of the chunk; warp w = stage w): the instance's pixel set is the transpose of
-//      its stage's 32 x 32 (pixel x instance) masks.  For each of its pixels the thread recomputes the pair geometry
-//      (pair_alpha: the same arithmetic on the same inputs, so the same alpha and the same low-pass branch), runs
-//      pair_geom_vjp and sums the 16 + 2 components in registers; one red.v4 x 4 (+ one v2) per instance leaves.
+//      its stage's 32 x 32 (pixel x instance) masks.  For each of its pixels the thread runs pair_geom_vjp_stored on
+//      the stored scalars -- G dL/dalpha, and the low-pass branch in the sign of alpha T, so neither G nor alpha is
+//      evaluated again -- and sums the 16 + 2 components in registers; one red.v4 x 4 (+ one v2) per instance leaves.
 // A pair whose slot lies beyond the buffer (a dense chunk) takes the direct path in phase 1 -- full VJP and per-pair
-// reductions -- and phase 2 skips it: the capacity changes the order of the float sums, never what is summed.
+// reductions -- and phase 2 skips it: the capacity changes the order of the float sums and the rounding of a pair's
+// terms (the direct path keeps the correctly rounded quotients), never which terms are summed.
 constexpr int BWD_CH = 256;        // instances per chunk == threads per CTA (one instance per thread in phase 2)
 constexpr int BWD_NSLOT = 2;
 constexpr int BWD_CAP = 4608;      // pair-buffer slots, 12 B each; headline chunks: 2,200 pairs average, 5,500 p99
@@ -294,9 +295,9 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
     uint32_t* cm_all = reinterpret_cast<uint32_t*>(smem_raw + SM::masks);
     float4* pd4 = reinterpret_cast<float4*>(smem_raw + SM::pd4);
     float2* pd2 = reinterpret_cast<float2*>(smem_raw + SM::pd2);
-    float* buf_a = reinterpret_cast<float*>(smem_raw + SM::buf);     // dL/dalpha (times T, with the background term)
+    float* buf_a = reinterpret_cast<float*>(smem_raw + SM::buf);     // G times dL/dalpha (times T, with the background term)
     float* buf_z = buf_a + BWD_CAP;                                   // dL/dz
-    float* buf_t = buf_z + BWD_CAP;                                   // alpha T
+    float* buf_t = buf_z + BWD_CAP;                                   // alpha T, negated on the low-pass branch
     uint16_t* sfx = reinterpret_cast<uint16_t*>(smem_raw + SM::sfx);  // first slot of (stage, pixel)'s pairs
     uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + SM::full);
     uint32_t* wsum = reinterpret_cast<uint32_t*>(smem_raw + SM::wsum);
@@ -405,7 +406,9 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                 float dL_dalpha, dL_dz, aT;
                 px.pair_scalars(S + idx * REC4, c * CH + idx, q, dL_dalpha, dL_dz, aT);
                 if (slot < BWD_CAP) {
-                    buf_a[slot] = dL_dalpha; buf_z[slot] = dL_dz; buf_t[slot] = aT;
+                    // aT > 0: a recorded contributor has alpha >= 1/255, and T >= T_final >= 1e-4 (the walk back
+                    // multiplies T by 1/(1 - alpha) > 1), so aT's sign bit is free to carry the low-pass branch
+                    buf_a[slot] = q.G_ * dL_dalpha; buf_z[slot] = dL_dz; buf_t[slot] = (q.rho3d <= q.rho2d) ? aT : -aT;
                 } else {
                     float v[16];
 #pragma unroll
@@ -459,22 +462,14 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                     if (slot >= BWD_CAP) continue;          // went out directly in phase 1
                     const int px_ = tile_x * SR_TILE + (sw & 1) * 8 + (l & 7), py_ = tile_y * SR_TILE + (sw >> 1) * 4 + (l >> 3);
                     const float pixx = (float)px_ + 0.5f, pixy = (float)py_ + 0.5f;
-                    PairAlpha q;
-                    pair_alpha(r0, r1, r2, pixx, pixy, q);
-                    float v[16];
-#pragma unroll
-                    for (int i = 0; i < 10; i++) v[i] = 0.f;
-                    float m2x = 0.f, m2y = 0.f;
-                    bool lowpass = false;
-                    pair_geom_vjp(q, r1, r2.w, pixx, pixy, buf_a[slot], buf_z[slot], v, m2x, m2y, lowpass);
-                    const float aT = buf_t[slot];
+                    const float t = buf_t[slot];
+                    const bool lowpass = t < 0.f;
+                    pair_geom_vjp_stored(r0, r1, r2, pixx, pixy, buf_a[slot], buf_z[slot], lowpass, acc, a2x, a2y);
+                    const float aT = fabsf(t);
                     const float4 d4 = pd4[p];
                     const float2 d2 = pd2[p];
-                    v[10] = aT * d4.x; v[11] = aT * d4.y; v[12] = aT * d4.z;
-                    v[13] = aT * d4.w; v[14] = aT * d2.x; v[15] = aT * d2.y;
-#pragma unroll
-                    for (int i = 0; i < 16; i++) acc[i] += v[i];
-                    a2x += m2x; a2y += m2y;
+                    acc[10] += aT * d4.x; acc[11] += aT * d4.y; acc[12] += aT * d4.z;
+                    acc[13] += aT * d4.w; acc[14] += aT * d2.x; acc[15] += aT * d2.y;
                     lowpass_any |= lowpass;
                     any_in = true;
                 }
