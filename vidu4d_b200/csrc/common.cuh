@@ -112,7 +112,7 @@ static inline __host__ __device__ BinLayout bin_layout(int64_t capacity, int til
     L.values[1] = o; o = sr_align_up(o + C * 4);
     L.inst_rec = o;  o = sr_align_up(o + C * SR_REC_FLOATS * 4);
     // contribution masks: per (32-instance stage of a tile list, 8x4 sub-tile, pixel) the instances that
-    // contributed to the pixel -- written by the forward composite, walked by the backward.
+    // contributed to the pixel -- written by the forward composite, walked by the backward (contrib_word).
     // Stage s of tile t lives at index (range.x >> 5) + t + s  (<= capacity/32 + tiles in total).
     L.contrib = o;   o = sr_align_up(o + ((C >> 5) + (size_t)(tiles > 0 ? tiles : 0) + 1) * SR_CONTRIB_STAGE_WORDS * 4);
     // the three below are zeroed together by one memset at the start of every forward
@@ -121,6 +121,12 @@ static inline __host__ __device__ BinLayout bin_layout(int64_t capacity, int til
     L.status = o;    o = sr_align_up(o + (size_t)SR_SORT_MAX_PASSES * L.sort_tiles * SR_SORT_BINS * 4);
     L.total = o;
     return L;
+}
+// Index, in words from L.contrib, of the contribution mask of slot `slot` (pixel ly * 8 + lx) of 8x4 sub-tile `sub` in
+// stage 0 of tile `tile`, whose sorted list starts at instance range_x.  Stage s of the tile is
+// s * SR_CONTRIB_STAGE_WORDS words further.
+static inline __host__ __device__ size_t contrib_word(uint32_t range_x, int tile, int sub, int slot) {
+    return (((size_t)(range_x >> 5) + tile) * 8 + sub) * 32 + slot;
 }
 
 // Host-side uniform parameters shared by the per-surfel kernels.

@@ -10,8 +10,8 @@
 //   * a separate pass after the composite forward / backward; the pinned composite kernels are untouched.  It reads
 //     what either composite forward leaves behind: the instance records, the per-(stage, pixel) contribution masks,
 //     final_T and each 8x4 sub-tile's deepest contributor (sub_last);
-//   * work item = (tile, 8x4 sub-tile) = one warp = one CTA, lane = pixel; the tile's records stream through a private
-//     2-stage ring of 32 records with cp.async.bulk on mbarriers, as in composite_fwd.cu.  Every lane
+//   * work item = (tile, 8x4 sub-tile) = one warp = one CTA, lane = pixel; the tile's records stream through the
+//     warp-private 2-stage ring of 32 records that composite_fwd.cu uses (comp::Ring).  Every lane
 //     walks only its own recorded contributors -- no cull or alpha test is repeated -- and re-evaluates alpha with the
 //     forward's arithmetic (comp::pair_alpha), so each plane is bit-identical to a colour plane of the same values;
 //   * a CTA owns SR_FEAT_CHUNK = 8 channels (gridDim.y = ceil(F/8)): 8 accumulators (forward) or 8 accumulators + 8
@@ -64,20 +64,6 @@ __device__ __forceinline__ void red_chunk(float* row, int c0, int F, const float
     }
 }
 
-// The warp's record ring: stage k of the walk (k = 0, 1, ..) holds list batch order(k); lane 0 issues.
-struct Ring {
-    float4 (*st)[WB * REC4];
-    uint64_t* bar;
-    const float4* src;
-    int len;
-    __device__ __forceinline__ void issue(int k, int b) {
-        const int s = k % NST;
-        const uint32_t bytes = (uint32_t)min(WB, len - b * WB) * 80u;
-        mbar_expect_tx(&bar[s], bytes);
-        bulk_g2s(st[s], src + (size_t)b * WB * REC4, bytes, &bar[s]);
-    }
-};
-
 // ------------------------------------------------------------------------------------------------ forward
 template <int V>
 __global__ void __launch_bounds__(32, 32)
@@ -102,15 +88,11 @@ feature_fwd_kernel(const FrameStrides fs, const FeatArgs ft, const uint2* __rest
     const uint2 range = ranges[tile];
     const int len = min((int)(range.y - range.x), (int)sub_last[tile * 8 + warp]);   // nothing deeper contributed
     const int nb = (len + WB - 1) / WB;
-    const int sx0 = (warp & 1) * 8, sy0 = (warp >> 1) * 4;
-    const int pix_x = tile_x * SR_TILE + sx0 + (lane & 7), pix_y = tile_y * SR_TILE + sy0 + (lane >> 3);
-    const float pixx = (float)pix_x + 0.5f, pixy = (float)pix_y + 0.5f;
+    const SubPixel sp = sub_pixel(tile_x, tile_y, warp, lane);
 
     Ring ring{st, bar, irec + (size_t)range.x * REC4, len};
     if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < NST; s++) mbar_init(&bar[s], 1);
-        fence_mbar_init();
+        ring.init();
         for (int b = 0; b < NST && b < nb; b++) ring.issue(b, b);
     }
     __syncwarp();
@@ -118,33 +100,30 @@ feature_fwd_kernel(const FrameStrides fs, const FeatArgs ft, const uint2* __rest
     float T = 1.0f, acc[FC];
 #pragma unroll
     for (int k = 0; k < FC; k++) acc[k] = 0.f;
-    // slot = pixel index inside the 8x4 sub-tile (composite_fwd.cu writes one word per stage and pixel)
-    const uint32_t* cm_in = contrib_masks + (((size_t)(range.x >> 5) + tile) * 8 + warp) * 32 + lane;
+    const uint32_t* cm_in = contrib_masks + contrib_word(range.x, tile, warp, lane);
     uint32_t next = nb > 0 ? __ldg(cm_in) : 0u;
     for (int b = 0; b < nb; b++) {
         uint32_t own = next;
         if (b + 1 < nb) next = __ldg(cm_in + (size_t)(b + 1) * SR_CONTRIB_STAGE_WORDS);
-        const int s = b % NST;
-        mbar_wait(&bar[s], (uint32_t)((b / NST) & 1));
-        const float4* S = st[s];
+        const float4* S = ring.wait(b);
         while (own != 0u) {                               // front to back over this pixel's contributors only
             const int jj = __ffs(own) - 1;
             own &= own - 1u;
             const float4* R = S + jj * REC4;
             PairAlpha q;
-            pair_alpha(R[0], R[1], R[2], pixx, pixy, q);
+            pair_alpha(R[0], R[1], R[2], sp.pixx, sp.pixy, q);
             float x[FC];
             load_chunk<V>(feat + (size_t)__float_as_uint(R[4].z) * F, c0, F, x);
 #pragma unroll
             for (int k = 0; k < FC; k++) acc[k] = ff(T, fm(q.alpha, x[k]), acc[k]);   // == the colour planes' update
             T = fm(T, fa(1.0f, -q.alpha));
         }
-        __syncwarp();                                     // every lane is done reading stage s
+        __syncwarp();                                     // every lane is done reading stage b
         if (lane == 0 && b + NST < nb) ring.issue(b + NST, b + NST);
     }
 
-    if (pix_x < W && pix_y < H) {
-        const size_t N = (size_t)W * H, pid = (size_t)W * pix_y + pix_x;
+    if (sp.inside(W, H)) {
+        const size_t N = (size_t)W * H, pid = (size_t)W * sp.pix_y + sp.pix_x;
 #pragma unroll
         for (int k = 0; k < FC; k++)
             if (c0 + k < F) out[(size_t)(c0 + k) * N + pid] = ft.bg ? ff(T, __ldg(ft.bg + c0 + k), acc[k]) : ff(T, 0.0f, acc[k]);
@@ -179,23 +158,19 @@ feature_bwd_kernel(const FrameStrides fs, const FeatArgs ft, const uint2* __rest
     const int len = min((int)(range.y - range.x), (int)sub_last[tile * 8 + warp]);
     const int nb = (len + WB - 1) / WB;
     if (nb == 0) return;
-    const int sx0 = (warp & 1) * 8, sy0 = (warp >> 1) * 4;
-    const int pix_x = tile_x * SR_TILE + sx0 + (lane & 7), pix_y = tile_y * SR_TILE + sy0 + (lane >> 3);
-    const float pixx = (float)pix_x + 0.5f, pixy = (float)pix_y + 0.5f;
+    const SubPixel sp = sub_pixel(tile_x, tile_y, warp, lane);
 
     // the k-th consumed batch is b = nb-1-k
     Ring ring{st, bar, irec + (size_t)range.x * REC4, len};
     if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < NST; s++) mbar_init(&bar[s], 1);
-        fence_mbar_init();
+        ring.init();
         for (int k = 0; k < NST && k < nb; k++) ring.issue(k, nb - 1 - k);
     }
     __syncwarp();
 
     // per-pixel state (comp::BwdPixel::load, feature planes only)
-    const bool inside = pix_x < W && pix_y < H;
-    const size_t N = (size_t)W * H, pid = (size_t)W * pix_y + pix_x;
+    const bool inside = sp.inside(W, H);
+    const size_t N = (size_t)W * H, pid = (size_t)W * sp.pix_y + sp.pix_x;
     const float T_final = inside ? final_Ts[pid] : 0.f;
     float T = T_final, g[FC], accum[FC], bg_dot = 0.f;
     const float gs = ft.grad_scale ? __ldg(ft.grad_scale) : 1.0f;
@@ -206,21 +181,20 @@ feature_bwd_kernel(const FrameStrides fs, const FeatArgs ft, const uint2* __rest
         accum[k] = 0.f;
     }
 
-    const uint32_t* cm_in = contrib_masks + (((size_t)(range.x >> 5) + tile) * 8 + warp) * 32 + lane;
+    const uint32_t* cm_in = contrib_masks + contrib_word(range.x, tile, warp, lane);
     uint32_t next = __ldg(cm_in + (size_t)(nb - 1) * SR_CONTRIB_STAGE_WORDS);
     for (int k = 0; k < nb; k++) {
-        const int b = nb - 1 - k, s = k % NST;
+        const int b = nb - 1 - k;
         uint32_t own = next;
         if (b > 0) next = __ldg(cm_in + (size_t)(b - 1) * SR_CONTRIB_STAGE_WORDS);
-        mbar_wait(&bar[s], (uint32_t)((k / NST) & 1));
-        const float4* S = st[s];
+        const float4* S = ring.wait(k);
         while (own != 0u) {                               // back to front over this pixel's contributors only
             const int jj = 31 - __clz(own);
             own &= ~(1u << jj);
             const float4* R = S + jj * REC4;
             const float4 r1 = R[1], r2 = R[2];
             PairAlpha q;
-            pair_alpha(R[0], r1, r2, pixx, pixy, q);
+            pair_alpha(R[0], r1, r2, sp.pixx, sp.pixy, q);
             const float alpha = q.alpha;
             const float r1ma = rcp_approx(1.f - alpha);   // as comp::BwdPixel::pair_scalars
             T = T * r1ma;
@@ -242,7 +216,7 @@ feature_bwd_kernel(const FrameStrides fs, const FeatArgs ft, const uint2* __rest
             float v[16];
             float m2x = 0.f, m2y = 0.f;
             bool lowpass = false;
-            pair_geom_vjp(q, r1, r2.w, pixx, pixy, dL_dalpha, 0.f, v, m2x, m2y, lowpass);
+            pair_geom_vjp(q, r1, r2.w, sp.pixx, sp.pixy, dL_dalpha, 0.f, v, m2x, m2y, lowpass);
             float* gp = sgrad + (size_t)id * SR_GRAD_FLOATS;
             if (!lowpass) {
                 asm volatile("red.global.v4.f32.add [%0], {%1, %2, %3, %4};" :: "l"(gp + SR_G_T), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]) : "memory");

@@ -5,7 +5,7 @@
 // Design (DESIGN.md "composite"):
 //   * work item = (tile, 8x4 sub-tile) = one warp = one CTA, launched longest-tile-first; each warp streams the
 //     tile's sorted instance records (80 B each, contiguous) through its own double-buffered shared-memory ring
-//     with cp.async.bulk (TMA 1-D) on its own mbarriers -- no CTA-wide synchronisation;
+//     (comp::Ring: cp.async.bulk, TMA 1-D, on its own mbarriers) -- no CTA-wide synchronisation;
 //   * one pixel per lane.  Per 32-record stage, lane = instance turns the instance's conservative cull rectangle into
 //     column and row masks of the sub-tile (group_survivors); then each lane walks its own survivor list, so up to 32
 //     different instances are evaluated per warp iteration.  With ~5x5-pixel footprints a whole-warp 8x4 block
@@ -13,8 +13,8 @@
 //   * per stage and pixel the kernel records which instances contributed (one 128-B store per warp): the backward
 //     walks exactly those;
 //   * culling and the rho_cut early-out never change a result: a skipped pair provably has alpha < 1/255;
-//   * per-pair arithmetic uses explicit-rounding intrinsics in the contraction pattern of the reference's
-//     sm_100a SASS, so colour/depth/alpha/normal/median planes are bit-identical to the reference build.
+//   * the per-pixel state, per-pair arithmetic and output words are comp::FwdPixel's, shared with the tile forward
+//     (composite_tile.cu): the two differ only in how records reach the lanes and how they stop early.
 #include "composite_common.cuh"
 
 namespace {
@@ -49,47 +49,29 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
     const uint2 range = ranges[tile];
     const int len = (int)(range.y - range.x);
     const int nb = (len + WB - 1) / WB;
+    const SubPixel sp = sub_pixel(tile_x, tile_y, warp, lane);     // warp -> 8x4 sub-tile, lane -> pixel
 
-    // warp -> 8x4 sub-tile, lane -> pixel (slot lane = ly * 8 + lx of the contribution-mask layout)
-    const int sx0 = (warp & 1) * 8, sy0 = (warp >> 1) * 4;
-    const int bx0 = sx0 + lane % 8, by0 = sy0 + lane / 8;      // tile-local pixel
-    const int pix_x = tile_x * SR_TILE + bx0, pix_y = tile_y * SR_TILE + by0;
-    const bool inside = pix_x < W && pix_y < H;
-    const float pixx = (float)pix_x + 0.5f, pixy = (float)pix_y + 0.5f;
-
-    const float4* src = irec + (size_t)range.x * REC4;
-    auto issue = [&](int b) {   // lane 0 only
-        const int s = b % NST;
-        const uint32_t bytes = (uint32_t)min(WB, len - b * WB) * 80u;
-        mbar_expect_tx(&bar[s], bytes);
-        bulk_g2s(st[s], src + (size_t)b * WB * REC4, bytes, &bar[s]);
-    };
+    Ring ring{st, bar, irec + (size_t)range.x * REC4, len};
     if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < NST; s++) mbar_init(&bar[s], 1);
-        fence_mbar_init();
-        for (int b = 0; b < NST && b < nb; b++) issue(b);
+        ring.init();
+        for (int b = 0; b < NST && b < nb; b++) ring.issue(b, b);
     }
     __syncwarp();
 
-    float T = 1.0f, C0 = 0.f, C1 = 0.f, C2 = 0.f, D = 0.f, N0 = 0.f, N1 = 0.f, N2 = 0.f;
-    float dist1 = 0.f, dist2 = 0.f, distortion = 0.f, median_depth = 0.f, median_weight = 0.f;
-    uint32_t median_contributor = 0, last_contributor = 0;
-    bool done = !inside;
-    // instances of the current stage that contributed to this lane's pixel, kept for the backward (common.cuh
-    // bin_layout: contrib); slot = pixel index inside the 8x4 sub-tile, so a warp's 32 words are one 128-B store
+    FwdPixel px;
+    bool done = !sp.inside(W, H);
+    // instances of the current stage that contributed to this lane's pixel, kept for the backward: a warp's 32 words
+    // are one 128-B store
     uint32_t cmask = 0u;
-    uint32_t* cm_out = contrib_masks + (((size_t)(range.x >> 5) + tile) * 8 + warp) * 32 + ((by0 - sy0) * 8 + (bx0 - sx0));
+    uint32_t* cm_out = contrib_masks + contrib_word(range.x, tile, warp, lane);
 
     for (int b = 0; b < nb; b++) {
-        const int s = b % NST;
-        mbar_wait(&bar[s], (uint32_t)((b / NST) & 1));
+        const float4* S = ring.wait(b);
         const int cnt = min(WB, len - b * WB);
-        const float4* S = st[s];
         uint32_t cull = 0;
         if (lane < cnt) cull = __float_as_uint(S[lane * REC4 + 4].w);
         // lane = instance: which pixels does this instance's cull rectangle touch?
-        uint32_t mym = group_survivors(cull, sx0, sy0, lane);
+        uint32_t mym = group_survivors(cull, sp.sx0, sp.sy0, lane);
         {   // a finished pixel must not keep the warp iterating over its survivors
             const uint32_t db = __ballot_sync(0xffffffffu, done);
             if ((db >> lane) & 1u) mym = 0u;
@@ -100,87 +82,25 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
             mym &= mym - 1;                              // no-op when mym == 0
             const float rho_cut = cull_rho_cut(__shfl_sync(0xffffffffu, cull, jj));   // before any divergence
             if (!act || done) continue;
-            const float4 r0 = S[jj * REC4], r1 = S[jj * REC4 + 1], r2 = S[jj * REC4 + 2];
-            // T rows: Tu=(r0.x,r0.y,r0.z) Tv=(r0.w,r1.x,r1.y) Tw=(r1.z,r1.w,r2.x); xy=(r2.y,r2.z); opac=r2.w
-            const float kx = ff(pixx, r1.z, -r0.x), ky = ff(pixx, r1.w, -r0.y), kz = ff(pixx, r2.x, -r0.z);
-            const float lx_ = ff(pixy, r1.z, -r0.w), ly_ = ff(pixy, r1.w, -r1.x), lz_ = ff(pixy, r2.x, -r1.y);
-            const float pz = ff(kx, ly_, -fm(ky, lx_));
-            if (pz == 0.0f) continue;
-            const float ppx = ff(ky, lz_, -fm(kz, ly_));
-            const float ppy = ff(kz, lx_, -fm(kx, lz_));
-            float sx, sy;
-            div2_rn(ppx, ppy, pz, sx, sy);
-            const float rho3d = ff(sx, sx, fm(sy, sy));
-            const float dx = fa(r2.y, -pixx), dy = fa(r2.z, -pixy);
-            const float q2 = ff(dx, dx, fm(dy, dy));
-            const float rho2d = fa(q2, q2);
-            const float rho = fminf(rho3d, rho2d);
-            if (rho > rho_cut) continue;                 // alpha < 1/255 guaranteed: same outcome as below, no expf
-            const float depth = (rho3d <= rho2d) ? fa(r2.x, ff(r1.z, sx, fm(r1.w, sy))) : r2.x;
-            if (depth < 0.2f) continue;
-            const float power = fm(rho, -0.5f);
-            if (power > 0.0f) continue;
-            const float alpha = fminf(0.99f, fm(r2.w, expf(power)));
-            if (alpha < 1.0f / 255.0f) continue;
-            const float test_T = fm(T, fa(1.0f, -alpha));
-            if (test_T < 0.0001f) { done = true; continue; }
-            const float4 r3 = S[jj * REC4 + 3], r4 = S[jj * REC4 + 4];
-            const uint32_t contributor = (uint32_t)(b * WB + jj + 1);
-            const float A = fa(1.0f, -T);
-            const float mdep = map_depth(depth);
-            const float mm = fm(mdep, mdep);
-            const float error = ff(-dist1, fa(mdep, mdep), ff(A, mm, dist2));
-            distortion = ff(T, fm(alpha, error), distortion);
-            if (T > 0.5f) { median_depth = depth; median_weight = fm(T, alpha); median_contributor = contributor; }
-            N0 = ff(T, fm(r3.x, alpha), N0);
-            N1 = ff(T, fm(r3.y, alpha), N1);
-            N2 = ff(T, fm(r3.z, alpha), N2);
-            D = ff(T, fm(depth, alpha), D);
-            dist1 = ff(T, fm(alpha, mdep), dist1);
-            dist2 = ff(T, fm(alpha, mm), dist2);
-            C0 = ff(T, fm(alpha, r3.w), C0);
-            C1 = ff(T, fm(alpha, r4.x), C1);
-            C2 = ff(T, fm(alpha, r4.y), C2);
-            T = test_T;
-            last_contributor = contributor;
-            cmask |= 1u << jj;
+            if (px.blend(S + jj * REC4, sp.pixx, sp.pixy, rho_cut, b * WB, jj, cmask)) done = true;
         }
-        __syncwarp();                                   // every lane is done reading stage s
+        __syncwarp();                                   // every lane is done reading stage b
         cm_out[(size_t)b * SR_CONTRIB_STAGE_WORDS] = cmask;
         cmask = 0u;
         if (__all_sync(0xffffffffu, done)) {
             // drain the copies still in flight before this warp (and its CTA's smem) goes away
-            for (int b2 = b + 1; b2 < nb && b2 < b + NST; b2++) mbar_wait(&bar[b2 % NST], (uint32_t)((b2 / NST) & 1));
+            for (int b2 = b + 1; b2 < nb && b2 < b + NST; b2++) ring.wait(b2);
             break;
         }
-        if (lane == 0 && b + NST < nb) issue(b + NST);
+        if (lane == 0 && b + NST < nb) ring.issue(b + NST, b + NST);
     }
 
     // deepest list position any pixel of this sub-tile used: the backward starts its reverse walk there
-    uint32_t wmax = last_contributor;
+    uint32_t wmax = px.last_contributor;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
     if (lane == 0) sub_last[tile * 8 + warp] = wmax;
-
-    if (inside) {
-        const size_t N = (size_t)W * H, pid = (size_t)W * pix_y + pix_x;
-        final_T[pid] = T;
-        final_T[pid + N] = dist1;
-        final_T[pid + 2 * N] = dist2;
-        n_contrib[pid] = last_contributor;
-        n_contrib[pid + N] = median_contributor;
-        out_color[pid] = ff(T, __ldg(bg), C0);
-        out_color[pid + N] = ff(T, __ldg(bg + 1), C1);
-        out_color[pid + 2 * N] = ff(T, __ldg(bg + 2), C2);
-        out_others[pid] = D;
-        out_others[pid + N] = fa(1.0f, -T);
-        out_others[pid + 2 * N] = N0;
-        out_others[pid + 3 * N] = N1;
-        out_others[pid + 4 * N] = N2;
-        out_others[pid + 5 * N] = median_depth;
-        out_others[pid + 6 * N] = distortion;
-        out_others[pid + 7 * N] = median_weight;
-    }
+    px.store(sp, W, H, bg, final_T, n_contrib, out_color, out_others);
 }
 
 }  // namespace

@@ -2,8 +2,9 @@
 //
 // Replaces (behaviour, not code) of the reference's renderCUDA forward / backward,
 // RAST/cuda_rasterizer/forward.cu:265-463 and backward.cu:143-449.  The backward here is the only one; the forward is
-// an alternative to composite_fwd.cu (the one-warp-per-CTA forward, the default) with the same per-pair arithmetic,
-// contribution masks and outputs.  What changes is how the instance list reaches the lanes:
+// an alternative to composite_fwd.cu (the one-warp-per-CTA forward, the default) with the same per-pixel state,
+// per-pair arithmetic and outputs (comp::FwdPixel) and contribution masks.  What changes is how the instance list
+// reaches the lanes and how the kernel stops early:
 //
 //   * CTA = one tile = 8 warps (one per 8x4 sub-tile, lane = pixel).  The tile's sorted 80-byte instance records
 //     stream through ONE ring of NSLOT chunks of CH instances, filled by cp.async.bulk (TMA 1-D) and shared by the 8
@@ -76,12 +77,7 @@ composite_tile_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ range
     const uint2 range = ranges[tile];
     const int len = (int)(range.y - range.x);
     const int nchunks = (len + CH - 1) / CH;
-
-    // warp -> 8x4 sub-tile, lane -> pixel (slot lane = ly * 8 + lx of the contribution-mask layout)
-    const int sx0 = (warp & 1) * 8, sy0 = (warp >> 1) * 4;
-    const int pix_x = tile_x * SR_TILE + sx0 + (lane & 7), pix_y = tile_y * SR_TILE + sy0 + (lane >> 3);
-    const bool inside = pix_x < W && pix_y < H;
-    const float pixx = (float)pix_x + 0.5f, pixy = (float)pix_y + 0.5f;
+    const SubPixel sp = sub_pixel(tile_x, tile_y, warp, lane);     // warp -> 8x4 sub-tile, lane -> pixel
 
     const float4* src = irec + (size_t)range.x * REC4;
     auto issue = [&](int c) {   // one thread
@@ -100,13 +96,11 @@ composite_tile_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ range
     }
     __syncthreads();                               // the only CTA-wide barrier
 
-    float T = 1.0f, C0 = 0.f, C1 = 0.f, C2 = 0.f, D = 0.f, N0 = 0.f, N1 = 0.f, N2 = 0.f;
-    float dist1 = 0.f, dist2 = 0.f, distortion = 0.f, median_depth = 0.f, median_weight = 0.f;
-    uint32_t median_contributor = 0, last_contributor = 0;
-    bool done = !inside;
+    FwdPixel px;
+    bool done = !sp.inside(W, H);
     bool counted = false;                          // (warp-uniform) this warp is in ctl[0]
     uint32_t* cm = cm_all + warp * NSTG * 32 + lane;          // this lane's column: cm[st * 32]
-    uint32_t* cm_out = contrib_masks + (((size_t)(range.x >> 5) + tile) * 8 + warp) * 32 + lane;
+    uint32_t* cm_out = contrib_masks + contrib_word(range.x, tile, warp, lane);
 
     for (int c = 0; c < nchunks; c++) {
         const int s = c % NSLOT;
@@ -131,7 +125,7 @@ composite_tile_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ range
                 if (st < nst) {
                     const int i = st * 32 + lane;
                     const uint32_t cull = i < cnt ? __float_as_uint(S[i * REC4 + 4].w) : 0u;
-                    const uint32_t m = group_survivors(cull, sx0, sy0, lane);
+                    const uint32_t m = group_survivors(cull, sp.sx0, sp.sy0, lane);
                     cm[st * 32] = m;
                     if (m) nz |= 1u << st;
                 }
@@ -151,50 +145,9 @@ composite_tile_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ range
                 const int jj = __ffs(mym) - 1;
                 mym &= mym - 1u;
                 const float4* R = S + (st * 32 + jj) * REC4;
-                const float4 r0 = R[0], r1 = R[1], r2 = R[2], r4 = R[4];
-                // T rows: Tu=(r0.x,r0.y,r0.z) Tv=(r0.w,r1.x,r1.y) Tw=(r1.z,r1.w,r2.x); xy=(r2.y,r2.z); opac=r2.w
-                const float kx = ff(pixx, r1.z, -r0.x), ky = ff(pixx, r1.w, -r0.y), kz = ff(pixx, r2.x, -r0.z);
-                const float lx_ = ff(pixy, r1.z, -r0.w), ly_ = ff(pixy, r1.w, -r1.x), lz_ = ff(pixy, r2.x, -r1.y);
-                const float pz = ff(kx, ly_, -fm(ky, lx_));
-                if (pz == 0.0f) continue;
-                const float ppx = ff(ky, lz_, -fm(kz, ly_));
-                const float ppy = ff(kz, lx_, -fm(kx, lz_));
-                float sx, sy;
-                div2_rn(ppx, ppy, pz, sx, sy);
-                const float rho3d = ff(sx, sx, fm(sy, sy));
-                const float dx = fa(r2.y, -pixx), dy = fa(r2.z, -pixy);
-                const float q2 = ff(dx, dx, fm(dy, dy));
-                const float rho2d = fa(q2, q2);
-                const float rho = fminf(rho3d, rho2d);
-                if (rho > cull_rho_cut(__float_as_uint(r4.w))) continue;   // alpha < 1/255 guaranteed: no expf
-                const float depth = (rho3d <= rho2d) ? fa(r2.x, ff(r1.z, sx, fm(r1.w, sy))) : r2.x;
-                if (depth < 0.2f) continue;
-                const float power = fm(rho, -0.5f);
-                if (power > 0.0f) continue;
-                const float alpha = fminf(0.99f, fm(r2.w, expf(power)));
-                if (alpha < 1.0f / 255.0f) continue;
-                const float test_T = fm(T, fa(1.0f, -alpha));
-                if (test_T < 0.0001f) { done = true; mym = 0u; nz = 0u; continue; }
-                const float4 r3 = R[3];
-                const uint32_t contributor = (uint32_t)(c * CH + st * 32 + jj + 1);
-                const float A = fa(1.0f, -T);
-                const float mdep = map_depth(depth);
-                const float mm = fm(mdep, mdep);
-                const float error = ff(-dist1, fa(mdep, mdep), ff(A, mm, dist2));
-                distortion = ff(T, fm(alpha, error), distortion);
-                if (T > 0.5f) { median_depth = depth; median_weight = fm(T, alpha); median_contributor = contributor; }
-                N0 = ff(T, fm(r3.x, alpha), N0);
-                N1 = ff(T, fm(r3.y, alpha), N1);
-                N2 = ff(T, fm(r3.z, alpha), N2);
-                D = ff(T, fm(depth, alpha), D);
-                dist1 = ff(T, fm(alpha, mdep), dist1);
-                dist2 = ff(T, fm(alpha, mm), dist2);
-                C0 = ff(T, fm(alpha, r3.w), C0);
-                C1 = ff(T, fm(alpha, r4.x), C1);
-                C2 = ff(T, fm(alpha, r4.y), C2);
-                T = test_T;
-                last_contributor = contributor;
-                cmask |= 1u << jj;
+                if (px.blend(R, sp.pixx, sp.pixy, cull_rho_cut(__float_as_uint(R[4].w)), c * CH + st * 32, jj, cmask)) {
+                    done = true; mym = 0u; nz = 0u;
+                }
             }
             // contribution masks of the chunk (zero for the stages this pixel never reached): one 128-B store per stage
 #pragma unroll
@@ -221,30 +174,11 @@ composite_tile_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ range
     }
 
     // deepest list position any pixel of this sub-tile used: the backward starts its reverse walk there
-    uint32_t wmax = last_contributor;
+    uint32_t wmax = px.last_contributor;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
     if (lane == 0) sub_last[tile * 8 + warp] = wmax;
-
-    if (inside) {
-        const size_t N = (size_t)W * H, pid = (size_t)W * pix_y + pix_x;
-        final_T[pid] = T;
-        final_T[pid + N] = dist1;
-        final_T[pid + 2 * N] = dist2;
-        n_contrib[pid] = last_contributor;
-        n_contrib[pid + N] = median_contributor;
-        out_color[pid] = ff(T, __ldg(bg), C0);
-        out_color[pid + N] = ff(T, __ldg(bg + 1), C1);
-        out_color[pid + 2 * N] = ff(T, __ldg(bg + 2), C2);
-        out_others[pid] = D;
-        out_others[pid + N] = fa(1.0f, -T);
-        out_others[pid + 2 * N] = N0;
-        out_others[pid + 3 * N] = N1;
-        out_others[pid + 4 * N] = N2;
-        out_others[pid + 5 * N] = median_depth;
-        out_others[pid + 6 * N] = distortion;
-        out_others[pid + 7 * N] = median_weight;
-    }
+    px.store(sp, W, H, bg, final_T, n_contrib, out_color, out_others);
 }
 
 // ------------------------------------------------------------------------------------------------ backward
@@ -323,7 +257,6 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
     if (nchunks == 0) return;                      // CTA-uniform
     const int nb_w = (len_w + 31) >> 5;            // stages this sub-tile reads
 
-    const int sx0 = (warp & 1) * 8, sy0 = (warp >> 1) * 4;
     const float4* src = irec + (size_t)range.x * REC4;
     // the k-th consumed chunk (k = 0, 1, ..) is c = nchunks-1-k; it lives in slot k % NSLOT
     auto issue = [&](int k) {   // one thread
@@ -341,13 +274,12 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
     }
 
     BwdPixel px;
-    px.load(tile_x * SR_TILE + sx0 + (lane & 7), tile_y * SR_TILE + sy0 + (lane >> 3), W, H, bg, final_Ts, n_contrib,
-            dL_dpixels, dL_dothers, grad_scale);
+    px.load(sub_pixel(tile_x, tile_y, warp, lane), W, H, bg, final_Ts, n_contrib, dL_dpixels, dL_dothers, grad_scale);
     pd4[threadIdx.x] = make_float4(px.dpix0, px.dpix1, px.dpix2, px.dn0);      // thread == pixel == warp * 32 + lane
     pd2[threadIdx.x] = make_float2(px.dn1, px.dn2);
 
     uint32_t* cm = cm_all + warp * NSTG * 32 + lane;
-    const uint32_t* cm_in = contrib_masks + (((size_t)(range.x >> 5) + tile) * 8 + warp) * 32 + lane;
+    const uint32_t* cm_in = contrib_masks + contrib_word(range.x, tile, warp, lane);
     uint32_t pre[NSTG];                            // the next chunk's masks, in flight while this one is walked
     auto fetch = [&](int c) {
 #pragma unroll
@@ -460,11 +392,10 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                     const uint32_t pm = cm_all[(sw * NSTG + warp) * 32 + l];
                     const int slot = (int)sfx[warp * NPIX + p] + __popc((pm >> lane) >> 1);
                     if (slot >= BWD_CAP) continue;          // went out directly in phase 1
-                    const int px_ = tile_x * SR_TILE + (sw & 1) * 8 + (l & 7), py_ = tile_y * SR_TILE + (sw >> 1) * 4 + (l >> 3);
-                    const float pixx = (float)px_ + 0.5f, pixy = (float)py_ + 0.5f;
+                    const SubPixel pp = sub_pixel(tile_x, tile_y, sw, l);
                     const float t = buf_t[slot];
                     const bool lowpass = t < 0.f;
-                    pair_geom_vjp_stored(r0, r1, r2, pixx, pixy, buf_a[slot], buf_z[slot], lowpass, acc, a2x, a2y);
+                    pair_geom_vjp_stored(r0, r1, r2, pp.pixx, pp.pixy, buf_a[slot], buf_z[slot], lowpass, acc, a2x, a2y);
                     const float aT = fabsf(t);
                     const float4 d4 = pd4[p];
                     const float2 d2 = pd2[p];
