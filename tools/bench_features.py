@@ -394,7 +394,7 @@ def bench_reproj(args):
         prof = _capi.get_profile()
         _capi.set_profiling(False)
         kern = {k: round(v["ms"] / max(v["count"], 1), 4) for k, v in prof.items()
-                if k in ("match_fwd", "match_bwd", "match_scatter", "reproj_fwd", "reproj_scale", "reproj_bwd")}
+                if k in ("match_fwd", "match_bwd", "match_bwd_global", "match_scatter", "reproj_fwd", "reproj_scale", "reproj_bwd")}
         print(json.dumps({"workload": "feat_reproj step (match + warp + projection + loss, fwd + bwd)", "surfels": P,
                           "resolution": RES, "frames": M, "candidates": 2048, "num_grad": 8, "bones": B,
                           "ms_per_step": {k: round(float(np.median(v)), 4) for k, v in ms.items()},

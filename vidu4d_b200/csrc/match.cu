@@ -17,7 +17,8 @@
 //             candidate position first (a later candidate never displaces an equal earlier one).  Candidate indices
 //             outside [0, M*P) are skipped (their rows are staged as NaN, which never enters the top-K).
 // match_bwd   one thread per pixel over the saved top-K; dL/dfeat_cand and dL/dxyz_cand go to a (C,19) shared-memory
-//             accumulator per CTA, flushed once per CTA (persistent grid); dL/dlogsigma is block-reduced.
+//             accumulator per CTA, flushed once per CTA (persistent grid); dL/dlogsigma is block-reduced.  When (C,19)
+//             floats exceed the device's opt-in shared memory, a second instantiation adds them to g_cand directly.
 // match_scatter adds the (C,19) candidate rows into g_regist_feat (P,16) / g_xyz (P,3) at cand[c] mod P (duplicates sum).
 // reproj_fwd  one thread per pixel: skinning weights of the matched point, frame m's dual-quaternion blend, field2cam,
 //             the frame's K; per-frame sums and integer counts of v > 0 (block reduction + per-frame atomics).
@@ -145,15 +146,21 @@ match_fwd_kernel(const MatchDims d, const float* __restrict__ feat_px, const flo
     xyz_matched[3 * n] = ox; xyz_matched[3 * n + 1] = oy; xyz_matched[3 * n + 2] = oz;
 }
 
+// SMEM: the (C,19) rows are summed in shared memory and flushed once per CTA.  Without it (C * 19 floats beyond the
+// device's opt-in shared memory) every product goes straight to g_cand with a global atomic.
+template <bool SMEM>
 __global__ void __launch_bounds__(BWD_THREADS)
 match_bwd_kernel(const MatchDims d, const float* __restrict__ feat_px, const float* __restrict__ xyz,
                  const int32_t* __restrict__ cand, const float* __restrict__ logsigma, const int32_t* __restrict__ top_idx,
                  const float* __restrict__ top_prob, const float* __restrict__ top_score,
                  const float* __restrict__ g_xyz_matched, float* __restrict__ g_cand, float* __restrict__ g_logsigma) {
-    extern __shared__ float acc[];                                   // (C,19) candidate gradient rows of this CTA
+    extern __shared__ float acc_smem[];                              // (C,19) candidate gradient rows of this CTA
     __shared__ float red[BWD_THREADS / 32];
-    for (int i = threadIdx.x; i < d.C * ROW; i += blockDim.x) acc[i] = 0.f;
-    __syncthreads();
+    float* const acc = SMEM ? acc_smem : g_cand;
+    if constexpr (SMEM) {
+        for (int i = threadIdx.x; i < d.C * ROW; i += blockDim.x) acc[i] = 0.f;
+        __syncthreads();
+    }
     const float tau = expf(__ldg(logsigma));
     float glog = 0.f;
     for (long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x; n < d.N; n += (long long)gridDim.x * blockDim.x) {
@@ -197,8 +204,10 @@ match_bwd_kernel(const MatchDims d, const float* __restrict__ feat_px, const flo
         for (int w = 0; w < (int)(blockDim.x >> 5); w++) t += red[w];
         if (t != 0.f) atomicAdd(g_logsigma, t);
     }
-    for (int i = threadIdx.x; i < d.C * ROW; i += blockDim.x)
-        if (acc[i] != 0.f) atomicAdd(g_cand + i, acc[i]);
+    if constexpr (SMEM) {
+        for (int i = threadIdx.x; i < d.C * ROW; i += blockDim.x)
+            if (acc[i] != 0.f) atomicAdd(g_cand + i, acc[i]);
+    }
 }
 
 __global__ void __launch_bounds__(256)
@@ -414,19 +423,25 @@ SR_API int sr_global_match_backward(int32_t M, int32_t H, int32_t W, int32_t P, 
     CK(cudaMemsetAsync(g_regist_feat, 0, (size_t)P * FEAT * sizeof(float), s), "sr_global_match_backward: memset(g_regist_feat)");
     CK(cudaMemsetAsync(g_xyz, 0, (size_t)P * 3 * sizeof(float), s), "sr_global_match_backward: memset(g_xyz)");
     CK(cudaMemsetAsync(g_logsigma, 0, sizeof(float), s), "sr_global_match_backward: memset(g_logsigma)");
-    const size_t smem = (size_t)C * ROW * sizeof(float);
-    CK(sr_opt_in_smem(match_bwd_kernel, smem), "sr_global_match_backward: shared-memory opt-in");
-    int dev = 0, sms = 132, per_sm = 1;
-    cudaGetDevice(&dev);
+    int dev = 0, sms = 132, per_sm = 1, optin = 0;
+    CK(cudaGetDevice(&dev), "sr_global_match_backward: cudaGetDevice");
+    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev), "sr_global_match_backward: opt-in limit");
+    cudaFuncAttributes fa{};
+    CK(cudaFuncGetAttributes(&fa, match_bwd_kernel<true>), "sr_global_match_backward: cudaFuncGetAttributes");
+    // the (C,19) rows fit beside the kernel's static shared memory up to C = (optin - static) / 76 (3056 on an H100)
+    const bool in_smem = (size_t)C * ROW * sizeof(float) + fa.sharedSizeBytes <= (size_t)optin;
+    const size_t smem = in_smem ? (size_t)C * ROW * sizeof(float) : 0;
+    auto kern = in_smem ? match_bwd_kernel<true> : match_bwd_kernel<false>;
+    CK(sr_opt_in_smem(kern, smem), "sr_global_match_backward: shared-memory opt-in");
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, match_bwd_kernel, BWD_THREADS, smem);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, BWD_THREADS, smem);
     // persistent grid: each CTA flushes its (C,19) rows once, so fewer, fuller CTAs mean fewer global reductions
     const long long want = (d.N + BWD_THREADS - 1) / BWD_THREADS;
     const int grid = (int)std::max(1LL, std::min(want, (long long)sms * std::max(per_sm, 1)));
     {
-        ProfileScope ps("match_bwd", s);
-        match_bwd_kernel<<<grid, BWD_THREADS, smem, s>>>(d, feat_px, xyz, cand, logsigma, top_idx, top_prob, top_score,
-                                                         g_xyz_matched, g_cand, g_logsigma);
+        ProfileScope ps(in_smem ? "match_bwd" : "match_bwd_global", s);   // the profile names the path taken
+        kern<<<grid, BWD_THREADS, smem, s>>>(d, feat_px, xyz, cand, logsigma, top_idx, top_prob, top_score, g_xyz_matched,
+                                             g_cand, g_logsigma);
     }
     {
         ProfileScope ps("match_scatter", s);
