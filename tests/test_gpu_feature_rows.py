@@ -13,7 +13,11 @@ Tolerances, each relative to the largest magnitude of the tensor compared (so a 
   * against the fp32 fixtures both sides carry their own fp32 rounding, and the chain through bob_warp adds the warp's
     (tests/test_gpu_warp.py uses 1e-4 for it): FIX_TOL = 3e-4.
 The density's arg-max bone is a knife edge only if two bones score within fp32 rounding of each other; the seeded inputs
-have none (a swap would show up as a 100% error in that surfel's centre gradient)."""
+have none (a swap would show up as a 100% error in that surfel's centre gradient).
+
+These tolerances are relative to each tensor's largest element, so they cannot see an error confined to small elements.
+tests/test_gpu_feature_rows_bounds.py holds every element, the raw g_tables and aux included, to an a-priori
+rounding-error bound, on both row paths, at the flow-scale ties, at the density's edges and up to M = 1024."""
 import os
 
 import numpy as np
