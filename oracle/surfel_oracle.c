@@ -290,6 +290,7 @@ typedef struct {
     uint8_t *knife;   /* N: 1 = some pair's expf-dependent decision lies within its margin of the threshold */
     double *walk_S;   /* N: S over every contributor of the pixel (see above) */
     double *fbound;   /* 14*N: per plane, sum over terms of (weight in u) * |term| for colour 3, allmap 8, final_T 3 */
+    uint32_t *nblend; /* N: pairs blended into the pixel (without culling: every pair of the tile's list is evaluated) */
 } so_fwd_ext;
 
 static inline int so_near(double v, double thr, double rel) { return fabs(v - thr) <= rel * fabs(thr); }
@@ -305,6 +306,7 @@ static void composite_pixel(const so_state *s, const float *feat, const float *b
     /* ext: S over the contributors so far, knife flag, bound sums (colour 0-2, allmap 3-10, final_T 11-13) */
     double S = 0.0, fb[14] = {0}, ra[14] = {0};
     int knife = 0;
+    uint32_t nblend = 0;
     for (uint32_t i = r0; i < r1; i++) {
         contributor++;
         uint32_t id = s->point_list[i];
@@ -369,6 +371,7 @@ static void composite_pixel(const so_state *s, const float *feat, const float *b
         for (int ch = 0; ch < 3; ch++) C[ch] = FMA(T, alpha * feat[3 * (size_t)id + ch], C[ch]);
         T = test_T;
         last_contributor = contributor;
+        nblend++;
     }
     s->final_T[pid] = T; s->final_T[pid + N] = dist1; s->final_T[pid + 2 * N] = dist2;
     s->n_contrib[pid] = last_contributor;
@@ -389,18 +392,20 @@ static void composite_pixel(const so_state *s, const float *feat, const float *b
         fb[11 + 0] = wT;
         if (ext->knife) ext->knife[pid] = (uint8_t)knife;
         if (ext->walk_S) ext->walk_S[pid] = S;
+        if (ext->nblend) ext->nblend[pid] = nblend;
         if (ext->fbound)
             for (int k = 0; k < 14; k++) ext->fbound[k * N + pid] = fb[k];
     }
 }
 
 /* The composite alone, over a state whose per-surfel records (transMat, means2D, normal_opacity), point_list and ranges
- * are given -- e.g. the GPU's own -- into its final_T, n_contrib, out_color and out_others.  knife / walk_S / fbound:
- * optional outputs (NULL = not wanted), see so_fwd_ext. */
-void so_composite(so_state *s, const float *feat, const float *bg, uint8_t *knife, double *walk_S, double *fbound) {
+ * are given -- e.g. the GPU's own -- into its final_T, n_contrib, out_color and out_others.  knife / walk_S / fbound /
+ * nblend: optional outputs (NULL = not wanted), see so_fwd_ext. */
+void so_composite(so_state *s, const float *feat, const float *bg, uint8_t *knife, double *walk_S, double *fbound,
+                  uint32_t *nblend) {
     const int tiles = s->tiles_x * s->tiles_y, W = s->W, H = s->H;
-    so_fwd_ext e = {knife, walk_S, fbound};
-    const so_fwd_ext *ext = (knife || walk_S || fbound) ? &e : NULL;
+    so_fwd_ext e = {knife, walk_S, fbound, nblend};
+    const so_fwd_ext *ext = (knife || walk_S || fbound || nblend) ? &e : NULL;
 #pragma omp parallel for schedule(dynamic, 1)
     for (int t = 0; t < tiles; t++) {
         int tx = t % s->tiles_x, ty = t / s->tiles_x;
@@ -494,7 +499,7 @@ so_state *so_forward(const so_params *p) {
         if (i == R - 1) s->ranges[2 * cur + 1] = (uint32_t)R;
     }
     /* ---- composite, forward.cu:265-463 ---- */
-    so_composite(s, p->colors_precomp ? p->colors_precomp : s->rgb, p->bg, NULL, NULL, NULL);
+    so_composite(s, p->colors_precomp ? p->colors_precomp : s->rgb, p->bg, NULL, NULL, NULL, NULL);
     return s;
 }
 

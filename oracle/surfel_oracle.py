@@ -14,7 +14,8 @@ API (numpy in, numpy out):
 Rounding-error bounds (see the error analysis in surfel_oracle.c):
     st, ext = from_records(inputs, transMat=, means2D=, normal_opacity=, rgb=, radii=, clamped=, point_list=, ranges=)
         composite only, from given per-surfel records (e.g. the GPU's); ext = composite_ext(st)
-    ext = composite_ext(st) -> dict(knife (H,W) bool, walk_S (H,W), fbound (14,H,W)); also refreshes st's planes
+    ext = composite_ext(st) -> dict(knife (H,W) bool, walk_S (H,W), fbound (14,H,W), nblend (H,W)); also refreshes
+        st's planes
     grads = backward(st, dL_dcolor, dL_dallmap, bounds=True) -> adds "acc", "bound", "asum" (P,18), SO_A_* order
     chain(st, acc) -> the gradient dict from given (P,18) accumulators
     chain_bound(st, B) -> per output element sum_j |d out / d acc_j| B_j
@@ -81,7 +82,8 @@ def lib():
         _lib.so_free.argtypes = [C.POINTER(_State)]
         _lib.so_backward.argtypes = [C.POINTER(_Params), C.POINTER(_State)] + [f32p] * 11
         _lib.so_backward_ex.argtypes = [C.POINTER(_Params), C.POINTER(_State)] + [f32p] * 11 + [f64p] * 4
-        _lib.so_composite.argtypes = [C.POINTER(_State), f32p, f32p, C.POINTER(C.c_uint8), f64p, f64p]
+        _lib.so_composite.argtypes = [C.POINTER(_State), f32p, f32p, C.POINTER(C.c_uint8), f64p, f64p,
+                                      C.POINTER(C.c_uint32)]
         _lib.so_chain.argtypes = [C.POINTER(_Params), C.POINTER(_State), f32p] + [f32p] * 9
         _lib.so_chain_bound.argtypes = [C.POINTER(_Params), C.POINTER(_State), f64p] + [f64p] * 9
         _lib.so_mark_visible.argtypes = [C.c_int, f32p, f32p, C.POINTER(C.c_uint8)]
@@ -258,8 +260,10 @@ def backward(st: OracleState, dL_dcolor, dL_dallmap, bounds=False):
 
 def composite_ext(st: OracleState):
     """Re-runs the composite on st's records (in place: color, allmap, final_T, n_contrib) and returns its optional
-    outputs: knife (H,W) bool, walk_S (H,W) and fbound (14,H,W) -- per plane (colour 3, allmap 8, final_T 3) the sum
-    over terms of (weight in units of 2^-24) * |term|.  Also stores walk_S on st for backward(bounds=True)."""
+    outputs: knife (H,W) bool, walk_S (H,W), fbound (14,H,W) -- per plane (colour 3, allmap 8, final_T 3) the sum
+    over terms of (weight in units of 2^-24) * |term| -- and nblend (H,W), the pairs blended into each pixel (the
+    composite evaluates every pair of the tile's list: it does not cull).  Also stores walk_S on st for
+    backward(bounds=True)."""
     W, H, N = st.W, st.H, st.W * st.H
     keep = []
     st.final_T = np.zeros((3, H, W), np.float32)
@@ -268,14 +272,17 @@ def composite_ext(st: OracleState):
     color = np.zeros(3 * N, np.float32); others = np.zeros(8 * N, np.float32)
     s.out_color = color.ctypes.data_as(f32p); s.out_others = others.ctypes.data_as(f32p)
     knife = np.zeros(N, np.uint8); walk_S = np.zeros(N, np.float64); fbound = np.zeros(14 * N, np.float64)
+    nblend = np.zeros(N, np.uint32)
     inp = st._inputs
     feat = inp["colors_precomp"] if inp["colors_precomp"] is not None else np.ascontiguousarray(st.rgb, np.float32)
     keep.append(feat)
     lib().so_composite(C.byref(s), _ptr(feat), _ptr(inp["bg"]), knife.ctypes.data_as(C.POINTER(C.c_uint8)),
-                       walk_S.ctypes.data_as(f64p), fbound.ctypes.data_as(f64p))
+                       walk_S.ctypes.data_as(f64p), fbound.ctypes.data_as(f64p),
+                       nblend.ctypes.data_as(C.POINTER(C.c_uint32)))
     st.color = color.reshape(3, H, W); st.allmap = others.reshape(8, H, W)
     st.walk_S = walk_S.reshape(H, W)
-    return dict(knife=knife.reshape(H, W).astype(bool), walk_S=st.walk_S, fbound=fbound.reshape(14, H, W))
+    return dict(knife=knife.reshape(H, W).astype(bool), walk_S=st.walk_S, fbound=fbound.reshape(14, H, W),
+                nblend=nblend.reshape(H, W))
 
 
 def from_records(means3D, opacities, scales, rotations, shs=None, colors_precomp=None, *, sh_degree=0, W, H, tanfovx,

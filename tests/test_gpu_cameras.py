@@ -338,11 +338,17 @@ def test_captured_step_follows_table_refilled_in_place(dev):
         res.update(terms=o["terms"], render=o["render"], allmap=o["allmap"], radii=o["radii"],
                    grads=[p.grad for p in cloud.flat_params()])
 
+    from vidu4d_b200 import rasterizer as RZ
     step = GraphedStep(body, device=dev)
-    step()
-    bc.intrinsics.copy_(camera_table(W, H, K2))                    # in place: the graph reads the same memory
-    step()
-    got = {k: ([g.clone() for g in v] if k == "grads" else v.clone()) for k, v in res.items()}
+    try:
+        step()
+        bc.intrinsics.copy_(camera_table(W, H, K2))                # in place: the graph reads the same memory
+        step()
+        got = {k: ([g.clone() for g in v] if k == "grads" else v.clone()) for k, v in res.items()}
+    finally:
+        # GraphedStep leaves the host in nosync mode (num_rendered = -1); later tests read num_rendered back
+        RZ.set_sync_mode(True)
+        RZ._pending.clear()
     cloud2 = SurfelCloud(scene, dev)
     bc2 = stack_cameras(cams)
     bc2.intrinsics = camera_table(W, H, K2)

@@ -244,6 +244,13 @@ def case_constructed(name, dev):
     return frame, grads, {}
 
 
+def case_cull(name, dev):
+    """A scene of tests/test_gpu_cull_bounds.py: the tile forward reads the same cull words."""
+    from .test_gpu_cull_bounds import SINGLE, scene_single
+    frame, grads, _ = _single(scene_single(**SINGLE[name])[0], dev)
+    return frame, grads, {}
+
+
 def case_features_single(F, dev):
     from tests.golden.make_golden import build_case
     frame, grads, _ = _single(build_case(6000, 96, 80, 90 + F, bg=(0.2, 0.1, 0.3)), dev, F=F, seed=F)
@@ -357,6 +364,8 @@ CASES["ragged_200x116"] = (case_build, dict(P=12000, W=200, H=116, seed=82, cent
 for _n in CONSTRUCTED:
     CASES[_n] = (case_constructed, _n)
 CASES["long_lists"] = (case_build, dict(P=50000, W=32, H=32, seed=72))
+for _n in ("cull_mix_72x52", "cull_mix_37x23"):
+    CASES[_n] = (case_cull, _n)
 CASES["batch8_512"] = (case_batch8, None)
 CASES["batch5_edges"] = (case_batch5, None)
 for _f in FEATURE_COUNTS:

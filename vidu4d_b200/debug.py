@@ -44,8 +44,8 @@ def decode(geomBuffer, binningBuffer, imgBuffer, P: int, W: int, H: int, num_ren
     return out
 
 
-def contributing_pairs(dec: dict) -> int:
-    """Number of (pixel, instance) pairs that contributed to the frame = population count of the contribution masks the
+def _lane_counts(dec: dict) -> torch.Tensor:
+    """(tiles, 8, 32) int64: per tile, 8 x 4 sub-tile and lane, the population count of the contribution masks the
     forward recorded, over the stages the backward reads (stage s of tile t is row (range.x >> 5) + t + s; a sub-tile's
     stages end at its deepest contributor)."""
     rg = dec["ranges"].to(torch.int64)
@@ -55,7 +55,7 @@ def contributing_pairs(dec: dict) -> int:
     nb = (torch.minimum(sl, (rg[:, 1] - rg[:, 0])[:, None]) + 31) >> 5            # (tiles, 8) stages per sub-tile
     base = (rg[:, 0] >> 5) + torch.arange(tiles, device=rg.device)
     maxnb = int(nb.max().item()) if tiles else 0
-    total = 0
+    total = torch.zeros((tiles, 8, 32), dtype=torch.int64, device=rg.device)
     for s in range(maxnb):
         live = nb > s                                                             # (tiles, 8)
         rows = (base + s).clamp_(max=m.shape[0] - 1)
@@ -65,5 +65,21 @@ def contributing_pairs(dec: dict) -> int:
         w = (w & 0x33333333) + ((w >> 2) & 0x33333333)
         w = (w + (w >> 4)) & 0x0F0F0F0F
         cnt = ((w * 0x01010101) & 0xFFFFFFFF) >> 24
-        total += int((cnt.sum(dim=2) * live).sum().item())
+        total += cnt * live[:, :, None]
     return total
+
+
+def contributing_pairs(dec: dict) -> int:
+    """Number of (pixel, instance) pairs that contributed to the frame = population count of the contribution masks the
+    forward recorded, over the stages the backward reads (_lane_counts)."""
+    return int(_lane_counts(dec).sum().item())
+
+
+def contributing_pairs_per_pixel(dec: dict, W: int, H: int) -> torch.Tensor:
+    """(counts, outside): contributing_pairs split by pixel, an (H, W) int64 tensor, and the number of pairs recorded for
+    lanes outside the image (none, if the cull rectangles hold).  Lane l of sub-tile w of tile t is pixel
+    (16 (t % tiles_x) + 8 (w & 1) + (l & 7), 16 (t // tiles_x) + 4 (w >> 1) + (l >> 3))."""
+    c = _lane_counts(dec)
+    tx, ty = (W + 15) // 16, (H + 15) // 16
+    img = c.view(ty, tx, 4, 2, 4, 8).permute(0, 2, 4, 1, 3, 5).reshape(ty * 16, tx * 16)
+    return img[:H, :W], int(img.sum().item()) - int(img[:H, :W].sum().item())
