@@ -175,6 +175,7 @@ def test_off_centre_principal_point_against_oracle(dev):
     from oracle import surfel_oracle as so
     from vidu4d_b200.synthetic import object_scene
     from . import camera_model as cm
+    from . import preprocess_bounds as pb
     from .test_gpu_grad_bounds import (CHAIN, GRADS, K, U, _check_all, _check_forward, _check_knife, _fallback_pairs, _np,
                                        _print)
     M, P, W, H = 3, 20000, 136, 88
@@ -205,15 +206,14 @@ def test_off_centre_principal_point_against_oracle(dev):
                                   normal_opacity=rec[:, [12, 13, 14, 11]], rgb=rec[:, 15:18], radii=dec["radii"],
                                   clamped=(cl[:, None] >> np.arange(3)) & 1, point_list=_np(dec["point_list"]).view(np.uint32),
                                   ranges=_np(dec["ranges"]).view(np.uint32))
-        # the GPU's own records are the oracle's input above: pin them to the oracle's preprocess, moved by the offsets
-        full = so.forward(_np(means[f]), sc.opacities, sc.scales, sc.rotations, shs=sc.shs, sh_degree=3, W=W, H=H, tanfovx=tx,
-                          tanfovy=ty, bg=bg, viewmatrix=_np(vms[f]), projmatrix=_np(pms[f]), campos=_np(cps[f]))
-        T_ref, c_ref = cm.offset_records(full, ox, oy)
-        vis = (dec["radii"] > 0) & (full.radii > 0)
-        assert vis.sum() > 0.3 * P, f
-        tm = rec[vis, 0:9]
-        assert np.abs(T_ref[vis] - tm).max() <= 1e-5 * np.abs(tm).max(), f
-        assert np.abs(c_ref[vis] - rec[vis, 9:11]).max() <= 1e-3, f
+        # the GPU's own records are the oracle's input above: pin them to the model of the preprocess with this frame's
+        # table row (tests/preprocess_bounds.py), every field under its rounding-error bound
+        inp_f = dict(means3D=_np(means[f]), rotations=sc.rotations, scales=sc.scales, opacities=sc.opacities, shs=sc.shs,
+                     colors_precomp=None, deg=3)
+        rep = pb.check_records(dec, inp_f, pb.camera(_np(vms[f]), _np(cps[f]), W, H, (tx, ty), (ox, oy)), "sh",
+                               f"off-centre frame {f}")
+        pb.print_report(f"off-centre frame {f} records", rep)
+        assert rep["visible"] > 0.3 * P, f
         fwd = _check_forward(f"off-centre frame {f}", st, ext, _np(color[f]), _np(allmap[f]), dec, W, H)
         keep = torch.from_numpy((~ext["knife"]).astype(np.float32)).to(dev)
         dLc[f] *= keep

@@ -253,7 +253,7 @@ def test_single_frame(name, dev):
     r["radii"] = _np(r["radii"])
     _check_lists(name, r, P, W, H)
     st, ext = _oracle_frame(r, P, W, H, inp["means3D"], inp["opacities"], inp["scales"], inp["rotations"], None,
-                            inp["colors_precomp"], 0, inp["bg"], inp["viewmatrix"], inp["projmatrix"], inp["campos"])
+                            inp["colors_precomp"], 0, inp["bg"], inp["viewmatrix"], inp["projmatrix"], inp["campos"], name=name)
     fwd = _check_forward(name, st, ext, _np(r["color"]), _np(r["allmap"]), r, W, H)
     _check_knife(name, int(ext["knife"].sum()))
     _check_cull(name, r, ext, P, W, H, label)
@@ -273,8 +273,13 @@ def test_single_frame(name, dev):
 
 
 # ------------------------------------------------------------------------------------------------ batches
-def _oracle_from_dec(so, dec, sc, means, W, H, tx, ty):
+def _oracle_from_dec(so, dec, sc, means, W, H, tx, ty, ox, oy, name):
+    from . import preprocess_bounds as pb
     P = sc.opacities.shape[0]
+    cam = pb.camera(np.eye(4, dtype=np.float32), np.zeros(3, np.float32), W, H, (tx, ty), (ox, oy))
+    inp = dict(means3D=_np(means), rotations=sc.rotations, scales=sc.scales, opacities=sc.opacities, shs=sc.shs,
+               colors_precomp=None, deg=3)
+    pb.print_report(f"{name} records", pb.check_records(dec, inp, cam, "sh", name))
     rec = _np(dec["surfel_rec"]).reshape(P, 20)
     cl = _np(dec["clamped"]).astype(np.uint8).reshape(P)
     return so.from_records(_np(means), sc.opacities, sc.scales, sc.rotations, shs=sc.shs, sh_degree=3, W=W, H=H,
@@ -312,7 +317,7 @@ def _run_batch(name, dev, sc, label, means, W, H, rows, edge_frames):
         dec["radii"] = _np(radii[f])
         dec["num_rendered"] = nr[f]
         _check_lists(f"{name} frame {f}", dec, P, W, H)
-        st, ext = _oracle_from_dec(so, dec, sc, means[f], W, H, tx, ty)
+        st, ext = _oracle_from_dec(so, dec, sc, means[f], W, H, tx, ty, ox, oy, f"{name} frame {f}")
         fwd = _check_forward(f"{name} frame {f}", st, ext, _np(color[f]), _np(allmap[f]), dec, W, H)
         _check_cull(f"{name} frame {f}", dec, ext, P, W, H, label, edges=f in edge_frames)
         keep = torch.from_numpy((~ext["knife"]).astype(np.float32)).to(dev)

@@ -228,13 +228,15 @@ def _oracle_fwd(name, dec, inp, means3D, feat, bgf, color, allmap, dev=None, s=N
     tan = (float(inp["tanfov"][0]), float(inp["tanfov"][1]))
     geo = (means3D, inp["opacities"], inp["scales"], inp["rotations"])
     st, ext = _oracle_frame(dec, P, W, H, *geo, None if pre else inp["shs"], inp["colors_precomp"] if pre else None, deg,
-                            inp["bg"], inp["viewmatrix"], inp["projmatrix"], inp["campos"], tan)
+                            inp["bg"], inp["viewmatrix"], inp["projmatrix"], inp["campos"], tan, name=name)
     fwd = _check_forward(name, st, ext, _np(color[:3]), _np(allmap), dec, W, H)
     ok = ~ext["knife"]
     planes = _np(color[3:])
     groups = []
     for k, (cols, b3, n) in enumerate(_groups(feat, bgf)):
-        sg, eg = _oracle_frame(dec, P, W, H, *geo, None, cols, 0, b3, inp["viewmatrix"], inp["projmatrix"], inp["campos"], tan)
+        # the records hold the colour forward's rgb, not the group's: their geometry only
+        sg, eg = _oracle_frame(dec, P, W, H, *geo, None, cols, 0, b3, inp["viewmatrix"], inp["projmatrix"], inp["campos"], tan,
+                               records=None, name=f"{name} group {k}")
         assert np.array_equal(eg["knife"], ext["knife"]), (name, "group", k, "knife mask differs from the colour's")
         for c in range(n):
             err = np.abs(planes[3 * k + c].astype(np.float64) - sg.color[c])

@@ -65,9 +65,20 @@ def _np(x):
 
 
 # ------------------------------------------------------------------------------------------------ oracle side
-def _oracle_frame(dec, P, W, H, means3D, opacities, scales, rotations, shs, colors, deg, bg, vm, pm, cp, tan=(TAN, TAN)):
-    """The oracle's state composited from one frame's decoded GPU buffers, and its knife mask / bounds."""
+def _oracle_frame(dec, P, W, H, means3D, opacities, scales, rotations, shs, colors, deg, bg, vm, pm, cp, tan=(TAN, TAN),
+                  off=None, records="auto", name=""):
+    """The oracle's state composited from one frame's decoded GPU buffers, and its knife mask / bounds.  The records it
+    composites are first held to tests/preprocess_bounds.py's model of the preprocess (check_records) for this frame's
+    inputs and camera (off: the principal-point offsets of an intrinsics-table row): records="auto" checks rgb and the
+    clamp bits against the SH evaluation or as a copy of `colors`, None the geometry only."""
     from oracle import surfel_oracle as so
+    from . import preprocess_bounds as pb
+    if records is not False:
+        src = ("precomp" if colors is not None else "sh") if records == "auto" else None
+        inp = dict(means3D=means3D, rotations=rotations, scales=scales, opacities=opacities, shs=shs,
+                   colors_precomp=colors, deg=deg)
+        rep = pb.check_records(dec, inp, pb.camera(vm, cp, W, H, tan, off), src, name)
+        pb.print_report(f"{name} records", rep)
     rec = _np(dec["surfel_rec"]).reshape(P, 20)
     cl = _np(dec["clamped"]).astype(np.uint8).reshape(P)
     radii = dec["radii"]
@@ -216,7 +227,7 @@ def _run_single(name, inp, dev):
     shs = None if pre else inp["shs"]
     col = inp["colors_precomp"] if pre else None
     st, ext = _oracle_frame(r, P, W, H, inp["means3D"], inp["opacities"], inp["scales"], inp["rotations"], shs, col, deg,
-                            inp["bg"], inp["viewmatrix"], inp["projmatrix"], inp["campos"], tan)
+                            inp["bg"], inp["viewmatrix"], inp["projmatrix"], inp["campos"], tan, name=name)
     fwd = _check_forward(name, st, ext, _np(r["color"]), _np(r["allmap"]), r, W, H)
     _check_knife(name, int(ext["knife"].sum()))
     keep = (~ext["knife"]).astype(np.float32)
@@ -347,7 +358,7 @@ def _batch(name, dev, sc, means, cams, W, H, seed):
         dec["radii"] = _np(radii[f])
         dec["num_rendered"] = nr[f]
         st, ext = _oracle_frame(dec, P, W, H, _np(means[f]), sc.opacities, sc.scales, sc.rotations, sc.shs, None, 3,
-                                _np(bg), _np(vms[f]), _np(pms[f]), _np(cps[f]))
+                                _np(bg), _np(vms[f]), _np(pms[f]), _np(cps[f]), name=f"{name} frame {f}")
         fwd = _check_forward(f"{name} frame {f}", st, ext, _np(color[f]), _np(allmap[f]), dec, W, H)
         keep = torch.from_numpy((~ext["knife"]).astype(np.float32)).to(dev)
         dLc[f] *= keep
