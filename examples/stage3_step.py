@@ -208,9 +208,8 @@ def run_full(surfels, res, frames, steps, bones, warm=5, seed=0, densify_at=None
         out = render_loss_batch(bc, model, pipe, bg, targets.index_select(0, fr), w_rgb=1.0, lambda_normal=0.05, lambda_dist=0.01,
                                 means3D=xc, rotations=torch.nn.functional.normalize(rc, dim=-1))
         out["loss"].backward()
-        # densification statistics (trainer.py:553-560), inside the graph: per frame, on device
-        for m in range(M):
-            model.add_densification_stats(out["viewspace_points"].grad[m], out["visibility_filter"][m], out["radii"][m])
+        # densification statistics (trainer.py:553-560), inside the graph: all M frames in one kernel, on device
+        model.add_densification_stats(out["viewspace_points"].grad, out["visibility_filter"], out["radii"])
         model.adam_step()
         opt.step()
         loss_out.copy_(out["loss"].detach())

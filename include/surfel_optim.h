@@ -1,7 +1,7 @@
 /*
  * surfel_optim.h -- C ABI of the optimizer step whose per-step state lives on the device: gradient-norm clipping over
- * the flat surfel gradient buffer, and an Adam pass that reads its step count, learning rates and clip coefficient from
- * device memory.
+ * the flat surfel gradient buffer, an Adam pass that reads its step count, learning rates and clip coefficient from
+ * device memory, and the batched densification statistics.
  *
  * The same library as surfel_raster.h (libsurfel_raster.so), the same SR_API visibility, SR_E* codes and
  * sr_last_error() message path.  It lives in its own header because surfel_raster.h is the drop-in boundary of the
@@ -52,6 +52,19 @@ SR_API int sr_grad_norm_flat(int32_t n_groups, const int64_t* begin, const float
 SR_API int sr_adam_flat_state(int32_t n_groups, const int64_t* begin, const float* lr, float beta1, float beta2, float eps,
                               int64_t* step, float grad_scale, const float* clip_coef, float* params, const float* grads,
                               float* exp_avg, float* exp_avg_sq, void* stream);
+
+/*
+ * Densification statistics of a batch of M frames (gaussian_model.py add_densification_stats, trainer.py:553-560).
+ * viewspace_grad: DEVICE float (M,P,3), the screen-space proxy gradient of the batched backward.  radii: DEVICE int32
+ * (M,P); frame m sees surfel i iff radii[m,i] > 0.  accum, denom, max_radii: DEVICE float [P], updated in place: for
+ * m = 0 .. M-1 in order, where frame m sees surfel i,
+ *   accum[i] += ||grad_scale * viewspace_grad[m,i]||,  denom[i] += 1,  max_radii[i] = max(max_radii[i], radii[m,i]),
+ * each step rounded to float as torch's per-frame update rounds it (the norm: fl(fl(fl(x^2) + fl(z^2)) + fl(y^2)),
+ * then a correctly rounded sqrt).  One thread per surfel, no atomics: equal inputs give equal bits.  M = 0 or P = 0
+ * launches nothing.  Arrays 4-byte aligned.
+ */
+SR_API int sr_densify_stats(int32_t M, int32_t P, const float* viewspace_grad, const int32_t* radii, float grad_scale,
+                            float* accum, float* denom, float* max_radii, void* stream);
 
 #ifdef __cplusplus
 }

@@ -112,6 +112,7 @@ OPTIM_PROTOTYPES = {
     "sr_grad_norm_scratch_bytes": (C.c_int64, [_i32]),
     "sr_grad_norm_flat": (C.c_int, [_i32, _p, _p, _f32, _p, _i32, _f32] + [_p] * 4 + [_i64, _p]),
     "sr_adam_flat_state": (C.c_int, [_i32, _p, _p, _f32, _f32, _f32, _p, _f32] + [_p] * 6),
+    "sr_densify_stats": (C.c_int, [_i32, _i32, _p, _p, _f32] + [_p] * 4),
 }
 OPTIM_SYMBOLS = tuple(OPTIM_PROTOTYPES)
 

@@ -16,6 +16,9 @@
 // of the gradient buffer gives torch.nn.utils.clip_grad_norm_'s coefficient in a one-CTA finish, and the Adam pass reads
 // its step count, learning rates and that coefficient from device memory, so a replayed CUDA graph steps as the
 // reference does (lab4d/engine/trainer.py:547, 589-591) without a re-capture.
+//
+// The densification statistics of a batch of M frames (trainer.py:553-560, gaussian_model.py:450-452) are one kernel
+// too: sr_densify_stats reads the batched backward's (M,P,3) screen-space proxy gradient and (M,P) radii once.
 #include "common.cuh"
 #include "../../include/surfel_optim.h"
 
@@ -245,6 +248,31 @@ grad_norm_finish_kernel(int n, int parts, const double* __restrict__ partials, c
 
 __global__ void adam_step_count_kernel(long long* step) { *step += 1; }
 
+// ---- densification statistics (sr_densify_stats) ----------------------------------------------------------------------
+// One thread per surfel walks the M frames in order, so each statistic is updated frame after frame exactly as M
+// successive calls of the per-frame torch update would (no atomics: the bits depend on the inputs alone).
+__global__ void __launch_bounds__(256)
+densify_stats_kernel(int M, int P, const float* __restrict__ g, const int* __restrict__ radii, float grad_scale,
+                     float* __restrict__ accum, float* __restrict__ denom, float* __restrict__ max_radii) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P) return;
+    float a = accum[i], d = denom[i], r = max_radii[i];
+    for (int m = 0; m < M; m++) {
+        const long long e = (long long)m * P + i;
+        const int rad = radii[e];
+        if (rad <= 0) continue;
+        const float x = __fmul_rn(g[e * 3 + 0], grad_scale), y = __fmul_rn(g[e * 3 + 1], grad_scale),
+                    z = __fmul_rn(g[e * 3 + 2], grad_scale);
+        // torch.norm(dim=-1) over a row of 3 (ATen's NormTwoOps through gpu_reduce_kernel): two lanes share the row,
+        // lane 0 sums elements 0 and 2, lane 1 holds element 1, then the lanes combine -- every square and sum rounded
+        const float sq = __fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(z, z)), __fmul_rn(y, y));
+        a = __fadd_rn(a, sqrtf(sq));
+        d = __fadd_rn(d, 1.0f);
+        r = fmaxf(r, (float)rad);
+    }
+    accum[i] = a; denom[i] = d; max_radii[i] = r;
+}
+
 // the group table both device-state entry points take: n_groups in [1, MAXG], begin[0] = 0, begin non-decreasing
 int check_groups(const char* fn, int32_t n_groups, const int64_t* begin) {
     if (n_groups < 1 || n_groups > MAXG) return sr_fail(SR_EINVAL, "%s: n_groups must be in [1, %d], got %d", fn, MAXG, n_groups);
@@ -352,6 +380,20 @@ SR_API int sr_adam_flat_state(int32_t n_groups, const int64_t* begin, const floa
         G, params, grads, exp_avg, exp_avg_sq, beta1, beta2, eps, 1.0f, 1.0f, grad_scale,
         AdamDeviceState{lr, reinterpret_cast<const long long*>(step), clip_coef});
     return sr_launched(2, "sr_adam_flat_state");
+}
+
+SR_API int sr_densify_stats(int32_t M, int32_t P, const float* viewspace_grad, const int32_t* radii, float grad_scale,
+                            float* accum, float* denom, float* max_radii, void* stream_) {
+    if (M < 0 || P < 0) return sr_fail(SR_EINVAL, "sr_densify_stats: M and P must be >= 0, got M = %d, P = %d", M, P);
+    if (M == 0 || P == 0) return 0;
+    if (!viewspace_grad || !radii || !accum || !denom || !max_radii)
+        return sr_fail(SR_EINVAL, "sr_densify_stats: viewspace_grad, radii, accum, denom and max_radii must not be NULL");
+    if (((uintptr_t)viewspace_grad | (uintptr_t)radii | (uintptr_t)accum | (uintptr_t)denom | (uintptr_t)max_radii) & 3)
+        return sr_fail(SR_EINVAL, "sr_densify_stats: every array must be 4-byte aligned");
+    cudaStream_t s = (cudaStream_t)stream_;
+    ProfileScope ps("densify_stats", s);
+    densify_stats_kernel<<<(P + 255) / 256, 256, 0, s>>>(M, P, viewspace_grad, radii, grad_scale, accum, denom, max_radii);
+    return sr_launched(1, "sr_densify_stats");
 }
 
 /* Gather the surfel rows of every parameter group (and both Adam moments) into new flat buffers: new row s = old row

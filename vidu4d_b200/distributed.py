@@ -8,6 +8,9 @@ backward) and the canonical-surfel gradients are summed across ranks once per op
     shard_frames()   which global frame indices this rank renders (rank r takes r, r+G, ...)
     FlatGrads        one flat fp32 buffer that *is* the .grad of every surfel parameter, so the exchange is a
                      single NCCL all-reduce over NVLink (gloo on CPU in the tests), no per-tensor buckets.
+                     A FlatSurfelModel, whose size changes with densification, uses its own allreduce_grads_.
+    shared_generator()   the same random stream on every rank (densify_and_prune's split noise)
+    check_replicas()     raise if the ranks' copies of some tensors differ in any bit (a debugging and test aid)
 """
 from __future__ import annotations
 
@@ -46,6 +49,68 @@ def init_distributed(backend: str | None = None, device: torch.device | None = N
 def shard_frames(num_frames: int, rank: int, world: int) -> List[int]:
     """Round-robin frame assignment: rank r renders frames r, r+world, ... (SURVEY.md section 8(e))."""
     return list(range(rank, num_frames, world))
+
+
+def _multi_rank(group) -> bool:
+    return dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1
+
+
+def shared_generator(device, seed: int | None = None, group=None) -> torch.Generator:
+    """A generator on `device` seeded with the group's rank 0's seed (its `seed`, or a fresh random one), so that every
+    rank draws the same numbers.  Pass it to FlatSurfelModel.densify_and_prune(generator=).  On one rank: seeded with
+    `seed` (or a fresh one)."""
+    device = torch.device(device)
+    if seed is None:
+        seed = int.from_bytes(os.urandom(8), "little") >> 1
+    if _multi_rank(group):
+        t = torch.tensor([int(seed)], dtype=torch.int64, device=device)
+        dist.broadcast(t, src=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
+        seed = int(t.item())
+    return torch.Generator(device=device).manual_seed(int(seed))
+
+
+_P31 = (1 << 31) - 1
+
+
+def _checksum(t: torch.Tensor) -> torch.Tensor:
+    """A 64-bit checksum of t's raw bits, on t's device, as a 0-d int64 tensor: the low 31 bits of the sum of its 32-bit
+    words (any single changed word shows) in the high half, and the position-weighted sum of the words modulo 2^31 - 1
+    (moved words show) in the low half.  Every intermediate stays below 2^63 for tensors of up to 2^31 words."""
+    b = t.detach().contiguous().reshape(-1).view(torch.uint8)
+    if b.numel() % 4:
+        b = torch.cat([b, b.new_zeros(4 - b.numel() % 4)])
+    w = b.view(torch.int32).to(torch.int64) & 0xFFFFFFFF
+    pos = torch.arange(1, w.numel() + 1, dtype=torch.int64, device=w.device) % _P31
+    weighted = (w % _P31) * pos % _P31
+    return (w.sum() & 0x7FFFFFFF) * (1 << 32) + weighted.sum() % _P31
+
+
+def check_replicas(named_tensors: dict, group=None) -> None:
+    """Raise RuntimeError unless every rank holds the same bits in each tensor of `named_tensors` (name -> tensor, or
+    name -> int such as the surfel count P), naming the first entry that differs and the ranks whose copy differs from
+    the group's rank 0.  All-gathers one checksum and one size per entry (a debugging and test aid: one host sync; not
+    meant for the step).  No-op on one rank."""
+    if not _multi_rank(group):
+        return
+    names = list(named_tensors)
+    dev = next((v.device for v in named_tensors.values() if isinstance(v, torch.Tensor)), torch.device("cpu"))
+    rows = []
+    for name in names:
+        v = named_tensors[name]
+        if isinstance(v, torch.Tensor):
+            rows.append(torch.stack([torch.tensor(v.numel(), device=dev), _checksum(v.to(dev))]))
+        else:
+            rows.append(torch.tensor([int(v), 0], dtype=torch.int64, device=dev))
+    mine = torch.stack(rows)
+    world = dist.get_world_size(group)
+    got = [torch.empty_like(mine) for _ in range(world)]
+    dist.all_gather(got, mine, group=group)
+    got = torch.stack(got).cpu()
+    for k, name in enumerate(names):
+        bad = [r for r in range(1, world) if not torch.equal(got[r, k], got[0, k])]
+        if bad:
+            what = "value or size" if int(got[bad[0], k, 0]) != int(got[0, k, 0]) else "bits"
+            raise RuntimeError(f"replicas differ in {name!r} ({what}): ranks {bad} of the group differ from its rank 0")
 
 
 class FlatGrads:

@@ -8,7 +8,7 @@ Mirrors the slice of the reference the Stage-3 loop uses (same names and argumen
     gs/scene/gaussian_model.py:450-452     add_densification_stats
     lab4d/engine/trainer.py:243-253        the gs_optimizer: torch.optim.Adam, one param group per tensor, eps = 1e-15
     lab4d/engine/trainer.py:550-568        max_radii2D bookkeeping + when densify_and_prune is called
-The layout is the one the gradient all-reduce uses (distributed.FlatGrads): groups back to back, each (P, k) row-major.
+The layout is the one the gradient all-reduce uses (allreduce_grads_): groups back to back, each (P, k) row-major.
 """
 from __future__ import annotations
 
@@ -104,9 +104,21 @@ class FlatSurfelModel(torch.nn.Module):
 
     def _reset_stats(self):
         dev = self.flat.device
-        self.xyz_gradient_accum = torch.zeros((self.P, 1), device=dev)
-        self.denom = torch.zeros((self.P, 1), device=dev)
+        # xyz_gradient_accum and denom are the two rows of one buffer, so that one SUM all-reduce covers both
+        self.densify_stats = torch.zeros((2, self.P), device=dev)
         self.max_radii2D = torch.zeros((self.P,), device=dev)
+
+    # (P,1) views of densify_stats' rows; assigning one copies into the row (`accum += x` stays in place)
+    def _stats_row(i):
+        def get(self):
+            return self.densify_stats[i].unsqueeze(-1)
+
+        def set_(self, value):
+            self.densify_stats[i].copy_(value.reshape(self.P))
+        return property(get, set_)
+    xyz_gradient_accum = _stats_row(0)
+    denom = _stats_row(1)
+    del _stats_row
 
     # ---- what render() reads (gaussian_model.py:98-118) -------------------------------------------------------------
     get_xyz = property(lambda s: s._xyz)
@@ -176,14 +188,83 @@ class FlatSurfelModel(torch.nn.Module):
 
     # ---- densification statistics (gaussian_model.py:450-452, trainer.py:553-560) ----------------------------------
     @torch.no_grad()
-    def add_densification_stats(self, viewspace_grad, update_filter, radii=None):
+    def add_densification_stats(self, viewspace_grad, update_filter, radii=None, grad_scale: float = 1.0):
         """Same values as the reference's boolean-mask updates, written with masks and in-place ops: fixed shapes and
-        stable addresses, so the call can sit inside a captured CUDA graph (a boolean index would need a host sync)."""
+        stable addresses, so the call can sit inside a captured CUDA graph (a boolean index would need a host sync).
+
+        One frame: viewspace_grad (P,3), update_filter (P,) bool, radii (P,) or None -- torch ops.
+        A batch of M frames: viewspace_grad (M,P,3) float32 (render_loss_batch's out["viewspace_points"].grad),
+        update_filter (M,P) or None, radii (M,P) int32 -- one kernel (sr_densify_stats) that applies the frames in order,
+        with the same bits as M one-frame calls.  A frame sees a surfel where radii > 0; update_filter, when given, must
+        be that mask (render_loss_batch's visibility_filter is).
+        The norm is taken of grad_scale * viewspace_grad: the per-frame gradient of a loss that sums its frames, scaled
+        as the step scales the parameter gradients (1 / frames, over all ranks)."""
+        if viewspace_grad.dim() == 3:
+            self._add_densification_stats_batch(viewspace_grad, update_filter, radii, grad_scale)
+            return
+        if grad_scale != 1.0:
+            viewspace_grad = viewspace_grad * grad_scale
         f = update_filter.unsqueeze(-1).to(torch.float32)
         self.xyz_gradient_accum.add_(torch.norm(viewspace_grad, dim=-1, keepdim=True) * f)
         self.denom.add_(f)
         if radii is not None:
             self.max_radii2D.copy_(torch.where(update_filter, torch.max(self.max_radii2D, radii.float()), self.max_radii2D))
+
+    def _add_densification_stats_batch(self, viewspace_grad, update_filter, radii, grad_scale):
+        M, P = int(viewspace_grad.shape[0]), self.P
+        if tuple(viewspace_grad.shape) != (M, P, 3):
+            raise RuntimeError(f"viewspace_grad must be (M,P,3) with P = {P}, got {tuple(viewspace_grad.shape)}")
+        if radii is None or tuple(radii.shape) != (M, P):
+            raise RuntimeError(f"the batched form needs radii (M,P) = ({M},{P}), got "
+                               f"{None if radii is None else tuple(radii.shape)}")
+        if update_filter is not None and tuple(update_filter.shape) != (M, P):
+            raise RuntimeError(f"update_filter must be (M,P) = ({M},{P}) or None, got {tuple(update_filter.shape)}")
+        if viewspace_grad.dtype != torch.float32:
+            raise RuntimeError(f"viewspace_grad must be float32, got {viewspace_grad.dtype}")
+        if radii.dtype != torch.int32:
+            raise RuntimeError(f"radii must be int32, got {radii.dtype}")
+        ref = self.densify_stats
+        _capi.check_tensors([("viewspace_grad", viewspace_grad), ("radii", radii), ("the statistics", ref)],
+                            "the surfel buffer", self.flat, floats=[])
+        if not math.isfinite(grad_scale):
+            raise RuntimeError(f"grad_scale must be finite, got {grad_scale}")
+        _capi.call("sr_densify_stats", self.flat.device, M, P, viewspace_grad.contiguous(), radii.contiguous(),
+                   float(grad_scale), ref[0], ref[1], self.max_radii2D)
+
+    # ---- multi-GPU: every rank keeps the same surfels (DESIGN.md section 4) -----------------------------------------
+    @staticmethod
+    def _world(group):
+        import torch.distributed as dist
+        if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+            return None
+        return dist
+
+    @torch.no_grad()
+    def sync_densification_stats(self, group=None):
+        """Make every rank's statistics those of all the ranks' frames: SUM over densify_stats (accum and denom, one
+        collective), MAX over max_radii2D.  Call it right before densify_and_prune.  No-op on one rank."""
+        dist = self._world(group)
+        if dist is None:
+            return
+        dist.all_reduce(self.densify_stats, op=dist.ReduceOp.SUM, group=group)
+        dist.all_reduce(self.max_radii2D, op=dist.ReduceOp.MAX, group=group)
+
+    @torch.no_grad()
+    def allreduce_grads_(self, average_over: int | None = None, group=None):
+        """Sum grad_flat over the ranks (one collective), then multiply by 1 / average_over if given.  Reads the current
+        buffer, so it stays right after densification re-binds the gradients.  Returns grad_flat."""
+        dist = self._world(group)
+        if dist is not None:
+            dist.all_reduce(self.grad_flat, op=dist.ReduceOp.SUM, group=group)
+        if average_over:
+            self.grad_flat.mul_(1.0 / float(average_over))
+        return self.grad_flat
+
+    def replica_state(self) -> dict:
+        """What must be equal on every rank between steps, by name (distributed.check_replicas' argument).  The
+        statistics are each rank's own until sync_densification_stats."""
+        return {"P": self.P, "flat": self.flat, "exp_avg": self.exp_avg, "exp_avg_sq": self.exp_avg_sq,
+                "device_step": self.device_step, "densify_stats": self.densify_stats, "max_radii2D": self.max_radii2D}
 
     # ---- densify / prune in one gather (gaussian_model.py:376-446) ------------------------------------------------
     @torch.no_grad()
@@ -209,9 +290,9 @@ class FlatSurfelModel(torch.nn.Module):
     @torch.no_grad()
     def prune_points(self, mask):
         keep = torch.nonzero(~mask, as_tuple=False).squeeze(1)
-        stats = (self.xyz_gradient_accum[keep], self.denom[keep], self.max_radii2D[keep])
+        stats = (self.densify_stats[:, keep], self.max_radii2D[keep])
         self._compact(keep, torch.zeros_like(keep, dtype=torch.uint8))
-        self.xyz_gradient_accum, self.denom, self.max_radii2D = stats
+        self.densify_stats, self.max_radii2D = stats
 
     @torch.no_grad()
     def remove_radius_outliers(self, nb_points: int = 20, radius: float = 0.004) -> int:
