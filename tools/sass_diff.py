@@ -1,0 +1,106 @@
+"""Check that the default rasterizer backward kernels compile to the same SASS as at another commit.
+
+The deterministic backward adds instantiations next to the default composite, feature and per-surfel backward kernels;
+the default ones must not change by a single instruction.  This script compiles composite_tile.cu, composite_feat.cu
+and surfel_bwd.cu -- and preprocess.cu, whose tile-rectangle code the deterministic backward now shares -- for sm_90a,
+from the working tree and from BASE, with the library's own nvcc flags, and compares the disassembly of every default
+kernel after removing addresses, encodings and the kernel's mangled name (a template parameter changes the name, not
+the code).
+
+BASE is the commit before the deterministic backward, feb2f64; with the change committed on top of it, HEAD^ names it
+too.  --base HEAD checks uncommitted work against the last commit.
+
+Usage: python tools/sass_diff.py [--base REV]      exit status 0 = identical, 1 = a kernel differs or is missing
+"""
+from __future__ import annotations
+
+import argparse
+import os
+import re
+import subprocess
+import sys
+import tarfile
+import tempfile
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+from vidu4d_b200.build import NVCC_FLAGS, _nvcc  # noqa: E402
+
+SOURCES = ["composite_tile.cu", "composite_feat.cu", "surfel_bwd.cu", "preprocess.cu"]
+# (demangled-name pattern in the base build, pattern of the same kernel in the working tree)
+KERNELS = [
+    (r"composite_tile_bwd_kernel(<\(bool\)0>)?\(", r"composite_tile_bwd_kernel(<\(bool\)0>)?\("),
+    (r"composite_tile_fwd_kernel\(", r"composite_tile_fwd_kernel\("),       # shares the chunk wait with the backward
+    (r"feature_bwd_kernel<\(int\)4>\(", r"feature_bwd_kernel<\(int\)4>\("),
+    (r"feature_bwd_kernel<\(int\)2>\(", r"feature_bwd_kernel<\(int\)2>\("),
+    (r"feature_bwd_kernel<\(int\)1>\(", r"feature_bwd_kernel<\(int\)1>\("),
+    (r"surfel_bwd_kernel\(", r"surfel_bwd_kernel\("),
+    (r"preprocess_fwd_kernel\(", r"preprocess_fwd_kernel\("),
+    (r"emit_keys_kernel\(", r"emit_keys_kernel\("),
+    (r"scan_block_sums_kernel\(", r"scan_block_sums_kernel\("),
+    (r"mark_visible_kernel\(", r"mark_visible_kernel\("),
+]
+
+
+def _sass(tree: str, src: str, out: str) -> dict:
+    """{demangled kernel name: normalised instruction list} of one translation unit."""
+    obj = os.path.join(out, src.replace(".cu", ".o"))
+    subprocess.run([_nvcc()] + NVCC_FLAGS + ["-c", os.path.join(tree, "vidu4d_b200", "csrc", src), "-o", obj], check=True)
+    text = subprocess.run(["cuobjdump", "-sass", obj], check=True, capture_output=True, text=True).stdout
+    names = subprocess.run(["cu++filt"], input="\n".join(re.findall(r"Function : (\S+)", text)), capture_output=True,
+                           text=True).stdout.split("\n")
+    kernels, cur, i = {}, None, 0
+    for line in text.split("\n"):
+        m = re.search(r"Function : (\S+)", line)
+        if m:
+            cur = names[i] if i < len(names) and names[i] else m.group(1)
+            i += 1
+            kernels[cur] = []
+            continue
+        m = re.match(r"\s*/\*[0-9a-f]{4,}\*/\s+(.*?)\s*;", line)
+        if cur and m:
+            ins = re.sub(r"\b_Z\w+", "<sym>", m.group(1))              # branch targets / calls carry the mangled name
+            kernels[cur].append(ins)
+    return kernels
+
+
+def _find(kernels: dict, pattern: str):
+    hits = [k for k in kernels if re.search(pattern, k)]
+    return hits[0] if len(hits) == 1 else None
+
+
+def main() -> int:
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--base", default="feb2f64", help="commit to compare with (default: the one before the change)")
+    args = ap.parse_args()
+    with tempfile.TemporaryDirectory() as tmp:
+        base = os.path.join(tmp, "base")
+        os.makedirs(base)
+        tarpath = os.path.join(tmp, "base.tar")
+        subprocess.run(["git", "-C", ROOT, "archive", "-o", tarpath, args.base, "vidu4d_b200/csrc", "include"], check=True)
+        with tarfile.open(tarpath) as t:
+            t.extractall(base)
+        ok = True
+        for src in SOURCES:
+            old = _sass(base, src, os.path.join(tmp, "base"))
+            os.makedirs(os.path.join(tmp, "new"), exist_ok=True)
+            new = _sass(ROOT, src, os.path.join(tmp, "new"))
+            for pat_old, pat_new in KERNELS:
+                ko = _find(old, pat_old)
+                if ko is None:
+                    continue                                        # not in this translation unit
+                kn = _find(new, pat_new)
+                if kn is None:
+                    print(f"MISSING  {ko}: no kernel matching {pat_new!r} in the working tree")
+                    ok = False
+                elif old[ko] != new[kn]:
+                    diff = sum(a != b for a, b in zip(old[ko], new[kn])) + abs(len(old[ko]) - len(new[kn]))
+                    print(f"DIFFERS  {ko} -> {kn}: {len(old[ko])} vs {len(new[kn])} instructions, {diff} differ")
+                    ok = False
+                else:
+                    print(f"same     {kn}: {len(new[kn])} instructions")
+    return 0 if ok else 1
+
+
+if __name__ == "__main__":
+    sys.exit(main())

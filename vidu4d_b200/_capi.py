@@ -15,6 +15,7 @@ ABI_VERSION = 11
 SR_STATUS_OVERFLOW = 1
 SR_STATUS_PREFILTER = 4
 SR_BATCH_SUM_SHARED = 1
+SR_BATCH_DETERMINISTIC = 2  # sr_batch.flags bit (include/surfel_deterministic.h): fixed-order backward in a scratch
 SR_FRAME_CAMERAS = 1        # sr_frame.flags bit (include/surfel_camera.h): per-frame intrinsics from a device table
 FEATURES_MAX = 32          # channels per call (SR_FEAT_MAX); also the widest feature row sr_feature_rows_* writes
 
@@ -37,6 +38,11 @@ class SrBatch(C.Structure):
     """sr_batch: frames + per-frame strides (in floats; 0 = shared by all frames) of the per-surfel inputs."""
     _fields_ = [("frames", C.c_int32), ("flags", C.c_uint32), ("means3D", C.c_int64), ("shs", C.c_int64), ("colors_precomp", C.c_int64),
                 ("opacities", C.c_int64), ("scales", C.c_int64), ("rotations", C.c_int64)]
+
+
+class SrBatchDet(C.Structure):
+    """sr_batch_det (include/surfel_deterministic.h): an sr_batch with SR_BATCH_DETERMINISTIC set, and its DEVICE scratch."""
+    _fields_ = [("batch", SrBatch), ("scratch", C.c_void_p), ("scratch_bytes", C.c_int64)]
 
 
 class SrDebugLayout(C.Structure):
@@ -139,6 +145,13 @@ CAMERA_PROTOTYPES = {
 }
 CAMERA_SYMBOLS = tuple(CAMERA_PROTOTYPES)
 
+# the deterministic backward's scratch size (sr_backward takes the mode through sr_batch_det), declared in
+# include/surfel_deterministic.h (own header and table for the same reason)
+DET_PROTOTYPES = {
+    "sr_backward_det_bytes": (C.c_size_t, [_i64, _i32]),
+}
+DET_SYMBOLS = tuple(DET_PROTOTYPES)
+
 
 _lib = None
 
@@ -153,12 +166,12 @@ def load():
             f"{LIB_PATH} not found: the CUDA extension is not built. Run `python -m vidu4d_b200.build` "
             "(or __graft_entry__.build()). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for s in SYMBOLS + SSIM_SYMBOLS + OPTIM_SYMBOLS + SKIN_MLP_SYMBOLS + MASK_LOSS_SYMBOLS + CAMERA_SYMBOLS:
+    for s in SYMBOLS + SSIM_SYMBOLS + OPTIM_SYMBOLS + SKIN_MLP_SYMBOLS + MASK_LOSS_SYMBOLS + CAMERA_SYMBOLS + DET_SYMBOLS:
         if not hasattr(lib, s):
             raise SurfelRasterError(f"{LIB_PATH} does not export {s}")
     for name, (restype, argtypes) in (list(PROTOTYPES.items()) + list(SSIM_PROTOTYPES.items()) + list(OPTIM_PROTOTYPES.items())
                                       + list(SKIN_MLP_PROTOTYPES.items()) + list(MASK_LOSS_PROTOTYPES.items())
-                                      + list(CAMERA_PROTOTYPES.items())):
+                                      + list(CAMERA_PROTOTYPES.items()) + list(DET_PROTOTYPES.items())):
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.sr_abi_version() != ABI_VERSION:

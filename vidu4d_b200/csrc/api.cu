@@ -15,6 +15,7 @@
 
 #include "common.cuh"
 #include "../../include/surfel_camera.h"
+#include "../../include/surfel_deterministic.h"
 
 namespace {
 thread_local char g_err[512] = "";
@@ -143,6 +144,7 @@ const char* sr_get_profile(void) {
 }
 
 size_t sr_geom_bytes(int32_t P) { return geom_layout(P).total; }
+size_t sr_backward_det_bytes(int64_t capacity, int32_t F) { return det_slot_bytes(capacity) + det_fslot_bytes(capacity, F); }
 size_t sr_image_bytes(int32_t width, int32_t height) { return image_layout(width, height).total; }
 size_t sr_binning_bytes(int64_t capacity, int32_t width, int32_t height) {
     return bin_layout(capacity, image_layout(width > 0 ? width : 0, height > 0 ? height : 0).tiles).total;
@@ -319,6 +321,17 @@ static int backward_batch(const sr_frame* f, const sr_batch* b, const float* bac
     if (!dL_dtransMat && b->frames == 1 && !(b->flags & SR_BATCH_SUM_SHARED)) return sr_fail(SR_EINVAL, "dL_dtransMat is NULL");
     if (shs && !dL_dsh) return sr_fail(SR_EINVAL, "dL_dsh is NULL");
     if (capacity <= 0) return sr_fail(SR_EINVAL, "capacity must be positive");
+    // SR_BATCH_DETERMINISTIC: b is the batch member of an sr_batch_det whose scratch holds M frames' slots
+    const bool det = (b->flags & SR_BATCH_DETERMINISTIC) != 0;
+    const sr_batch_det* bd = reinterpret_cast<const sr_batch_det*>(b);
+    if (det) {
+        const size_t need = sr_backward_det_bytes(capacity, ft ? ft->F : 0) * (size_t)b->frames;
+        if (!bd->scratch) return sr_fail(SR_EINVAL, "SR_BATCH_DETERMINISTIC is set but the scratch pointer is NULL");
+        if (bd->scratch_bytes < 0 || (size_t)bd->scratch_bytes < need)
+            return sr_fail(SR_EINVAL, "deterministic backward: scratch has %lld bytes, needs %zu (sr_backward_det_bytes x frames)",
+                           (long long)bd->scratch_bytes, need);
+        if ((uintptr_t)bd->scratch & 15) return sr_fail(SR_EINVAL, "deterministic backward: scratch must be 16-byte aligned");
+    }
     if (ft) {
         const long long N = (long long)f->width * f->height;
         if (dcolor_stride < 3 * N) return sr_fail(SR_EINVAL, "dL_dout_color frame stride must be >= 3*H*W");
@@ -367,7 +380,21 @@ static int backward_batch(const sr_frame* f, const sr_batch* b, const float* bac
         // else (M,P,F); zeroed here, the feature pass adds into it
         ft->dfeat_stride = (sum && ft->feat_stride == 0) ? 0 : Pl * ft->F * 4;
         const size_t rows = ft->dfeat_stride == 0 ? 1 : (size_t)M;
-        CK(cudaMemsetAsync(ft->dfeat, 0, rows * (size_t)Pl * ft->F * sizeof(float), stream), "memset(dL_dfeatures)");
+        if (!det) CK(cudaMemsetAsync(ft->dfeat, 0, rows * (size_t)Pl * ft->F * sizeof(float), stream), "memset(dL_dfeatures)");
+    }
+    if (det) {
+        // per frame: [slots of capacity instances | feature slots]; det_gather writes the accumulator and dL/dfeatures whole
+        DetArgs d{};
+        const size_t sb = det_slot_bytes(capacity), per = sr_backward_det_bytes(capacity, ft ? ft->F : 0);
+        d.slots = (float*)bd->scratch; d.slots_stride = (long long)per;
+        d.fslots = ft ? (float*)((char*)bd->scratch + sb) : nullptr; d.fslots_stride = (long long)per;
+        d.point_offsets = (const uint32_t*)(a.geom + a.gl.point_offsets); d.radii = radii; d.tiles_y = a.il.tiles_y;
+        CK(launch_det_zero(a, d, ft ? ft->F : 0), "det_zero"); DBG("det_zero");
+        CK(launch_composite_tile_bwd_det(a, d), "composite_bwd_det"); DBG("composite_bwd_det");
+        if (ft) { CK(launch_feature_bwd_det(a, *ft, d), "feature_bwd_det"); DBG("feature_bwd_det"); }
+        CK(launch_det_gather(a, d, ft), "det_gather"); DBG("det_gather");
+        CK(launch_surfel_bwd(a), "surfel_bwd"); DBG("surfel_bwd");
+        return 0;
     }
     CK(launch_composite_tile_bwd(a), "composite_bwd"); DBG("composite_bwd");
     // after composite_bwd (which zeroes the per-surfel accumulator), before surfel_bwd (which reads it)

@@ -220,6 +220,22 @@ cudaError_t launch_composite_tile_bwd(const BwdArgs& a);  // composite_tile.cu
 bool sr_composite_tile_fwd();                             // SURFEL_COMPOSITE[_FWD]=tile|warp
 cudaError_t launch_feature_fwd(const FwdArgs& a, const FeatArgs& ft);   // composite_feat.cu (after the composite forward)
 cudaError_t launch_feature_bwd(const BwdArgs& a, const FeatArgs& ft);   // composite_feat.cu (after the composite backward)
+// Deterministic backward (include/surfel_deterministic.h): per frame, one 20-float slot per instance (the geometry /
+// colour gradient of one (instance, tile), accumulator layout SR_G_*) and F floats per instance (its dL/dfeatures), both
+// indexed by the instance's emission index.  Strides in BYTES between consecutive frames.
+struct DetArgs {
+    float* slots;  long long slots_stride;
+    float* fslots; long long fslots_stride;         // nullptr when F = 0
+    const uint32_t* point_offsets;                  // the geometry buffer's (frame stride FrameStrides::geom)
+    const int* radii;                               // (frame stride FrameStrides::radii)
+    int tiles_y;
+};
+static inline size_t det_slot_bytes(int64_t capacity) { return sr_align_up((size_t)(capacity > 0 ? capacity : 1) * SR_GRAD_FLOATS * 4); }
+static inline size_t det_fslot_bytes(int64_t capacity, int F) { return sr_align_up((size_t)(capacity > 0 ? capacity : 1) * (F > 0 ? F : 0) * 4); }
+cudaError_t launch_det_zero(const BwdArgs& a, const DetArgs& d, int F);                      // composite_det.cu
+cudaError_t launch_composite_tile_bwd_det(const BwdArgs& a, const DetArgs& d);              // composite_tile.cu
+cudaError_t launch_feature_bwd_det(const BwdArgs& a, const FeatArgs& ft, const DetArgs& d); // composite_det.cu
+cudaError_t launch_det_gather(const BwdArgs& a, const DetArgs& d, const FeatArgs* ft);     // composite_det.cu
 cudaError_t launch_mark_visible(int P, const float* means3D, const float* vm, uint8_t* present, cudaStream_t s);
 // clears `bytes` at p + f * pitch for every frame f of the batch (one 2-D memset)
 cudaError_t sr_memset_frames(void* p, size_t pitch, size_t bytes, int frames, cudaStream_t s);
@@ -289,6 +305,28 @@ __device__ __forceinline__ CamParams cam_of_frame(CamParams c, const FrameStride
         c.kcy = __fadd_rn(c.bcy, oy);
     }
     return c;
+}
+// The tile rectangle [rmin, rmax) of a surfel centred at (px, py) with radius max_radius (getRect, auxiliary.h:64-74).
+// The float operations are exact by construction (adds and power-of-two scaling).  emit_keys emits a surfel's instances
+// row-major over this rectangle; the deterministic backward recomputes it to find an instance's emission index.
+__device__ __forceinline__ void sr_tile_rect(float px, float py, int max_radius, int gx, int gy, uint2& rmin, uint2& rmax) {
+    const float r = (float)max_radius;
+    int x0 = (int)__fmul_rn(__fadd_rn(px, -r), 0.0625f), y0 = (int)__fmul_rn(__fadd_rn(py, -r), 0.0625f);
+    int x1 = (int)__fmul_rn(__fadd_rn(__fadd_rn(__fadd_rn(px, r), 16.f), -1.f), 0.0625f);
+    int y1 = (int)__fmul_rn(__fadd_rn(__fadd_rn(__fadd_rn(py, r), 16.f), -1.f), 0.0625f);
+    rmin.x = min((unsigned)gx, (unsigned)max(0, x0));
+    rmin.y = min((unsigned)gy, (unsigned)max(0, y0));
+    rmax.x = min((unsigned)gx, (unsigned)max(0, x1));
+    rmax.y = min((unsigned)gy, (unsigned)max(0, y1));
+}
+// Emission index of surfel id's instance on tile (tx, ty): the surfel's first index (point_offsets is the inclusive scan
+// of tiles_touched) plus the tile's row-major position in its rectangle
+__device__ __forceinline__ uint32_t sr_emission_index(const uint32_t* __restrict__ point_offsets, const int* __restrict__ radii,
+                                                      uint32_t id, float px, float py, int tx, int ty, int gx, int gy) {
+    uint2 rmin, rmax;
+    sr_tile_rect(px, py, __ldg(radii + id), gx, gy, rmin, rmax);
+    const uint32_t first = id == 0 ? 0u : __ldg(point_offsets + id - 1);
+    return first + ((uint32_t)ty - rmin.y) * (rmax.x - rmin.x) + ((uint32_t)tx - rmin.x);
 }
 __device__ __forceinline__ float4 ld_nc_f4(const float4* p) {
     float4 r;

@@ -30,17 +30,6 @@ using namespace comp;
 
 constexpr int TWARPS = 8;      // 8x4 sub-tiles of a 16x16 tile
 
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n"     // suspend-time hint: the warp sleeps in hardware
-        "selp.u32 %0, 1, 0, p;\n"                                          // instead of spinning (r2a ncu: 8 % of the
-        "}\n" : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity), "r"(20000u) : "memory");   // forward's issue slots were the spin loop)
-    return ok != 0;
-}
-
 // ------------------------------------------------------------------------------------------------ forward
 constexpr int FWD_CH = 256;        // instances per chunk
 constexpr int FWD_NSLOT = 2;       // ring slots
@@ -213,7 +202,17 @@ struct BwdSmem {
 static_assert(BWD_CH == 32 * TWARPS, "phase 2 gives every instance of a chunk its own thread");
 static_assert(BwdSmem::full % 8 == 0, "mbarrier alignment");
 static_assert(2 * (BwdSmem::total + 1024) <= 233472, "two CTAs per SM (228 KB, 1 KB reserved per CTA)");
+// Deterministic instantiation (DET = true, include/surfel_deterministic.h):
+//   * the (instance, tile) sum is STORED into the instance's slot det.slots[emission index] instead of reduced into the
+//     per-surfel accumulator; launch_det_gather sums a surfel's slots in emission order;
+//   * there is no direct path: a chunk with more pairs than BWD_CAP runs phases 1 and 2 in passes.  Pass k takes the
+//     pixels whose slot base lies in [k DET_PASS, (k+1) DET_PASS) -- whole pixels, in scan order, and a pixel has at
+//     most BWD_CH pairs in a chunk, so its pairs fit the buffer at offset k DET_PASS (comp::DetPasses, DET_PASS =
+//     BWD_CAP - BWD_CH).  Phase 2 of pass k > 0 resumes
+//     from the partial sum pass k-1 stored in the slot.  Phase 2 adds an instance's pixels in ascending pixel order
+//     whatever the passes, so the sum is the one a single pass would form, and no pair takes the full VJP.
 
+template <bool DET>
 __global__ void __launch_bounds__(32 * TWARPS, 2)
 composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_scale, const uint2* __restrict__ ranges,
                           const uint32_t* __restrict__ tile_order, int tiles_x,
@@ -221,7 +220,7 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                           const float* __restrict__ final_Ts, const uint32_t* __restrict__ n_contrib,
                           const uint32_t* __restrict__ sub_last, const float* __restrict__ dL_dpixels,
                           const float* __restrict__ dL_dothers, const uint32_t* __restrict__ contrib_masks,
-                          float* __restrict__ sgrad) {
+                          float* __restrict__ sgrad, const DetArgs det) {
     using SM = BwdSmem;
     constexpr int CH = BWD_CH, NSLOT = BWD_NSLOT, NSTG = SM::NSTG, NPIX = 32 * TWARPS;
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -242,6 +241,12 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
     final_Ts = fr(final_Ts, fs.img, f); n_contrib = fr(n_contrib, fs.img, f); sub_last = fr(sub_last, fs.img, f);
     dL_dpixels = fr(dL_dpixels, fs.dcolor, f); dL_dothers = fr(dL_dothers, fs.dothers, f);
     contrib_masks = fr(contrib_masks, fs.bin, f); sgrad = fr(sgrad, fs.geom, f);
+    float* slots = nullptr;
+    const uint32_t* point_offsets = nullptr;
+    const int* radii = nullptr;
+    if constexpr (DET) {
+        slots = fr(det.slots, det.slots_stride, f); point_offsets = fr(det.point_offsets, fs.geom, f); radii = fr(det.radii, fs.radii, f);
+    }
     const int tile = (int)tile_order[blockIdx.x / (unsigned)fs.frames];
     const int tile_x = tile % tiles_x, tile_y = tile / tiles_x;
     const uint2 range = ranges[tile];
@@ -307,6 +312,14 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
         __syncthreads();                           // masks and warp totals are in; the previous chunk is finished
         int base = incl - np;
         for (int w = 0; w < warp; w++) base += (int)wsum[w];
+        int npass = 1, my_pass = 0;                // DET: passes over the chunk, and this pixel's
+        DetPasses dp(0, BWD_CAP, CH);
+        if constexpr (DET) {
+            int total = 0;
+            for (int w = 0; w < TWARPS; w++) total += (int)wsum[w];
+            dp = DetPasses(total, BWD_CAP, CH);
+            npass = dp.npass; my_pass = dp.of(base);
+        }
         {
             int run = base;                        // pairs of this pixel in later stages come first (back to front)
 #pragma unroll
@@ -322,12 +335,17 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
         }
         const float4* S = ring + (size_t)s * CH * REC4;
 
+        for (int pass = 0; pass < npass; pass++) {
+        if constexpr (DET) { if (pass > 0) __syncthreads(); }     // the previous pass's phase 2 is done with the buffer
+        const int off = DET ? dp.offset(pass) : 0;
+        uint32_t nzp = nz;
+        if constexpr (DET) nzp = my_pass == pass ? nz : 0u;
         // ---- phase 1: lane = pixel, back to front over its contributors
-        if (__any_sync(0xffffffffu, nz != 0u)) {
+        if (__any_sync(0xffffffffu, nzp != 0u)) {
             int st = 0, slot = base;
             uint32_t mym = 0u;
             for (;;) {
-                if (mym == 0u && nz) { st = 31 - __clz(nz); nz &= ~(1u << st); mym = cm[st * 32]; }
+                if (mym == 0u && nzp) { st = 31 - __clz(nzp); nzp &= ~(1u << st); mym = cm[st * 32]; }
                 const bool act = mym != 0u;
                 if (!__any_sync(0xffffffffu, act)) break;
                 if (!act) continue;
@@ -337,10 +355,11 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                 PairAlpha q;
                 float dL_dalpha, dL_dz, aT;
                 px.pair_scalars(S + idx * REC4, c * CH + idx, q, dL_dalpha, dL_dz, aT);
-                if (slot < BWD_CAP) {
+                if (DET || slot < BWD_CAP) {
                     // aT > 0: a recorded contributor has alpha >= 1/255, and T >= T_final >= 1e-4 (the walk back
                     // multiplies T by 1/(1 - alpha) > 1), so aT's sign bit is free to carry the low-pass branch
-                    buf_a[slot] = q.G_ * dL_dalpha; buf_z[slot] = dL_dz; buf_t[slot] = (q.rho3d <= q.rho2d) ? aT : -aT;
+                    const int b = slot - off;
+                    buf_a[b] = q.G_ * dL_dalpha; buf_z[b] = dL_dz; buf_t[b] = (q.rho3d <= q.rho2d) ? aT : -aT;
                 } else {
                     float v[16];
 #pragma unroll
@@ -372,6 +391,21 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                 for (int i = 0; i < 16; i++) acc[i] = 0.f;
                 float a2x = 0.f, a2y = 0.f;
                 bool lowpass_any = false, any_in = false;
+                float* gslot = nullptr;
+                if constexpr (DET) {
+                    gslot = slots + (size_t)sr_emission_index(point_offsets, radii, __float_as_uint(R[4].z), r2.y, r2.z, tile_x,
+                                                              tile_y, tiles_x, det.tiles_y) * SR_GRAD_FLOATS;
+                    if (pass > 0) {                // resume the partial sum of the earlier passes
+                        const float4* g4 = reinterpret_cast<const float4*>(gslot);
+#pragma unroll
+                        for (int q = 0; q < 4; q++) {
+                            const float4 t = g4[q];
+                            acc[4 * q] = t.x; acc[4 * q + 1] = t.y; acc[4 * q + 2] = t.z; acc[4 * q + 3] = t.w;
+                        }
+                        const float4 t = g4[4];
+                        a2x = t.x; a2y = t.y;
+                    }
+                }
                 // one flat walk over the instance's pixels: the warp iterates max over lanes of the pair count
                 uint32_t nzw = 0u;
 #pragma unroll
@@ -390,8 +424,14 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                     w &= w - 1u;
                     const int p = sw * 32 + l;
                     const uint32_t pm = cm_all[(sw * NSTG + warp) * 32 + l];
-                    const int slot = (int)sfx[warp * NPIX + p] + __popc((pm >> lane) >> 1);
-                    if (slot >= BWD_CAP) continue;          // went out directly in phase 1
+                    int slot = (int)sfx[warp * NPIX + p] + __popc((pm >> lane) >> 1);
+                    if constexpr (DET) {
+                        // pixel p's pass: its slot base is the first stage's entry of the slot table
+                        if (dp.of((int)sfx[(NSTG - 1) * NPIX + p]) != pass) continue;
+                        slot -= off;
+                    } else {
+                        if (slot >= BWD_CAP) continue;      // went out directly in phase 1
+                    }
                     const SubPixel pp = sub_pixel(tile_x, tile_y, sw, l);
                     const float t = buf_t[slot];
                     const bool lowpass = t < 0.f;
@@ -404,7 +444,14 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                     lowpass_any |= lowpass;
                     any_in = true;
                 }
-                if (any_in) {
+                if constexpr (DET) {
+                    if (any_in) {
+                        float4* g4 = reinterpret_cast<float4*>(gslot);
+#pragma unroll
+                        for (int q = 0; q < 4; q++) g4[q] = make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
+                        g4[4] = make_float4(a2x, a2y, 0.f, 0.f);
+                    }
+                } else if (any_in) {
                     float* gp = sgrad + (size_t)__float_as_uint(R[4].z) * SR_GRAD_FLOATS;
                     red_add<16>(gp, acc);
                     if (lowpass_any) {
@@ -414,6 +461,7 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                 }
             }
         }
+        }                                          // passes
         __syncthreads();                           // ring slot, masks, pair buffer and slot table are free again
         if (threadIdx.x == 0 && k + NSLOT < nchunks) issue(k + NSLOT);
     }
@@ -446,19 +494,25 @@ cudaError_t launch_composite_tile_fwd(const FwdArgs& a) {
     return cudaGetLastError();
 }
 
-cudaError_t launch_composite_tile_bwd(const BwdArgs& a) {
-    cudaError_t e = sr_memset_frames(a.geom + a.gl.sgrad, (size_t)a.fs.geom, (size_t)(a.cam.P > 0 ? a.cam.P : 1) * SR_GRAD_FLOATS * 4,
-                                     a.fs.frames, a.stream);
+template <bool DET>
+static cudaError_t launch_tile_bwd(const BwdArgs& a, const DetArgs& d) {
+    if (!DET) {
+        cudaError_t e = sr_memset_frames(a.geom + a.gl.sgrad, (size_t)a.fs.geom, (size_t)(a.cam.P > 0 ? a.cam.P : 1) * SR_GRAD_FLOATS * 4,
+                                         a.fs.frames, a.stream);
+        if (e != cudaSuccess) return e;
+    }
+    ProfileScope ps(DET ? "composite_bwd_det" : "composite_bwd", a.stream);
+    cudaError_t e = sr_opt_in_smem(composite_tile_bwd_kernel<DET>, BwdSmem::total);
     if (e != cudaSuccess) return e;
-    ProfileScope ps("composite_bwd", a.stream);
-    e = sr_opt_in_smem(composite_tile_bwd_kernel, BwdSmem::total);
-    if (e != cudaSuccess) return e;
-    composite_tile_bwd_kernel<<<a.il.tiles * a.fs.frames, 32 * TWARPS, BwdSmem::total, a.stream>>>(
+    composite_tile_bwd_kernel<DET><<<a.il.tiles * a.fs.frames, 32 * TWARPS, BwdSmem::total, a.stream>>>(
         a.fs, a.grad_scale, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles_x,
         (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, a.cam.bg,
         (const float*)(a.img + a.il.final_T), (const uint32_t*)(a.img + a.il.n_contrib),
         (const uint32_t*)(a.img + a.il.tile_last), a.dL_dcolor, a.dL_dothers,
-        (const uint32_t*)(a.bin + a.bl.contrib), (float*)(a.geom + a.gl.sgrad));
+        (const uint32_t*)(a.bin + a.bl.contrib), (float*)(a.geom + a.gl.sgrad), d);
     sr_count_launch();
     return cudaGetLastError();
 }
+
+cudaError_t launch_composite_tile_bwd(const BwdArgs& a) { return launch_tile_bwd<false>(a, DetArgs{}); }
+cudaError_t launch_composite_tile_bwd_det(const BwdArgs& a, const DetArgs& d) { return launch_tile_bwd<true>(a, d); }

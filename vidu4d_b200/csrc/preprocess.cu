@@ -49,16 +49,9 @@ __device__ __forceinline__ float3 w_mul(const View& c, float3 v) {
                        ff(v.z, c.m[10], ff(v.x, c.m[2], fm(v.y, c.m[6]))));
 }
 
-// auxiliary.h:64-74 (float ops are exact-by-construction here: adds and power-of-two scaling)
+// auxiliary.h:64-74: one copy in common.cuh, shared with the deterministic backward's emission index
 __device__ __forceinline__ void get_rect(float px, float py, int max_radius, int gx, int gy, uint2& rmin, uint2& rmax) {
-    const float r = (float)max_radius;
-    int x0 = (int)fm(fa(px, -r), 0.0625f), y0 = (int)fm(fa(py, -r), 0.0625f);
-    int x1 = (int)fm(fa(fa(fa(px, r), 16.f), -1.f), 0.0625f);
-    int y1 = (int)fm(fa(fa(fa(py, r), 16.f), -1.f), 0.0625f);
-    rmin.x = min((unsigned)gx, (unsigned)max(0, x0));
-    rmin.y = min((unsigned)gy, (unsigned)max(0, y0));
-    rmax.x = min((unsigned)gx, (unsigned)max(0, x1));
-    rmax.y = min((unsigned)gy, (unsigned)max(0, y1));
+    sr_tile_rect(px, py, max_radius, gx, gy, rmin, rmax);
 }
 
 // forward.cu:20-71.  No binning decision depends on the colour, so this is not written with explicit-rounding

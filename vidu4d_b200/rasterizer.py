@@ -32,6 +32,7 @@ from . import _capi
 _CAP_ALIGN = 256           # capacities are multiples of this so that bytes -> capacity is invertible
 _cap_hint: dict = {}       # (device index, W, H) -> last seen num_rendered
 _sync_mode = True          # True: read num_rendered back after every forward (like the reference)
+_deterministic = False     # set_deterministic
 _pending: list = []        # nosync mode: (pinned host words (frames,2), key, capacity, stream) awaiting check_overflow()
 _MAX_PENDING = 4096        # nosync forwards that may accumulate before check_overflow() is forced
 _host_pool: list = []      # pinned (64,2) int32 status blocks, pre-allocated so that a forward never allocates pinned memory
@@ -46,6 +47,22 @@ def set_sync_mode(flag: bool):
     sync=False: no host<->device synchronisation at all; call check_overflow() once per step."""
     global _sync_mode
     _sync_mode = bool(flag)
+
+
+def set_deterministic(flag: bool):
+    """flag=True: every rasterizer backward runs the deterministic kernels (include/surfel_deterministic.h): no float
+    atomic touches a gradient and every sum has an order fixed by the data, so the same inputs give the same gradient
+    bits on every call, and each frame of a batch the bits of a one-frame call.  It costs one scratch of
+    sr_backward_det_bytes(capacity, F) per frame (from torch's allocator) and some time (BASELINE.md).  The mode is also
+    on while torch.are_deterministic_algorithms_enabled().  Process-wide, like set_sync_mode; the forward is unaffected."""
+    global _deterministic
+    _deterministic = bool(flag)
+
+
+def deterministic() -> bool:
+    """Whether the rasterizer backward runs deterministically: set_deterministic(True) or
+    torch.use_deterministic_algorithms(True)."""
+    return _deterministic or torch.are_deterministic_algorithms_enabled()
 
 
 def _round_cap(n: int) -> int:
@@ -351,7 +368,15 @@ def _backward(M, frame_dim, strides, background, means3D, sh, colors, scales, ro
         if P > 0:
             cap = _capacity_from_bytes(int(binningBuffer.numel()) // M, W, H)
             fr, frp = _frame(P, degree, Msh, W, H, tan_fovx, tan_fovy, scale_modifier, False, debug, intrinsics)
-            bt = _capi.SrBatch(M, _capi.SR_BATCH_SUM_SHARED if sum_shared else 0, *(strides.get(k, 0) for k in _STRIDED))
+            flags = _capi.SR_BATCH_SUM_SHARED if sum_shared else 0
+            if deterministic():
+                nbytes = M * int(_capi.load().sr_backward_det_bytes(cap, F))
+                scratch = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+                bd = _capi.SrBatchDet(_capi.SrBatch(M, flags | _capi.SR_BATCH_DETERMINISTIC, *(strides.get(k, 0) for k in _STRIDED)),
+                                      scratch.data_ptr(), nbytes)
+                bt = bd.batch
+            else:
+                bt = _capi.SrBatch(M, flags, *(strides.get(k, 0) for k in _STRIDED))
             gs = fgs = None
             if grad_scale is not None:
                 gs = grad_scale.to(device=dev, dtype=torch.float32).reshape(()).contiguous()
