@@ -174,6 +174,7 @@ typedef struct sr_debug_layout {
     size_t n_contrib;       /* uint32[2*N] last, median */
     size_t ranges;          /* uint32[tiles*2] */
     size_t sub_last;        /* uint32[tiles*8] deepest contributor (list position + 1) per 8x4 sub-tile */
+    size_t tile_order;      /* uint32[tiles] composite launch order: tiles by floor(log2(list length)), longest first */
 } sr_debug_layout;
 SR_API int sr_debug_view(int32_t P, int32_t width, int32_t height, int64_t capacity, sr_debug_layout* out);
 

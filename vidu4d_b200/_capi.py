@@ -52,6 +52,7 @@ class SrDebugLayout(C.Structure):
         ("keys", C.c_size_t * 2), ("values", C.c_size_t * 2), ("sort_ctl", C.c_size_t),
         ("inst_rec", C.c_size_t), ("contrib", C.c_size_t),
         ("final_T", C.c_size_t), ("n_contrib", C.c_size_t), ("ranges", C.c_size_t), ("sub_last", C.c_size_t),
+        ("tile_order", C.c_size_t),
     ]
 
 

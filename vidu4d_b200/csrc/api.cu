@@ -160,6 +160,7 @@ int sr_debug_view(int32_t P, int32_t width, int32_t height, int64_t capacity, sr
     out->keys[0] = b.keys[0]; out->keys[1] = b.keys[1]; out->values[0] = b.values[0]; out->values[1] = b.values[1];
     out->sort_ctl = b.sort_ctl; out->inst_rec = b.inst_rec; out->contrib = b.contrib;
     out->final_T = i.final_T; out->n_contrib = i.n_contrib; out->ranges = i.ranges; out->sub_last = i.tile_last;
+    out->tile_order = i.tile_order;
     return 0;
 }
 

@@ -40,6 +40,7 @@ def decode(geomBuffer, binningBuffer, imgBuffer, P: int, W: int, H: int, num_ren
         "ranges": view(imgBuffer, L.ranges, 2 * tiles, torch.int32).view(tiles, 2),
         "sub_last": view(imgBuffer, L.sub_last, 8 * tiles, torch.int32).view(tiles, 8),
         "contrib_masks": view(binningBuffer, L.contrib, ((cap >> 5) + tiles + 1) * 256, torch.int32).view(-1, 8, 32),
+        "tile_order": view(imgBuffer, L.tile_order, tiles, torch.int32),
     }
     return out
 
