@@ -1,14 +1,11 @@
-"""Check that the default rasterizer backward kernels compile to the same SASS as at another commit.
+"""Check that kernels compile to the same SASS as at another commit.
 
-The deterministic backward adds instantiations next to the default composite, feature and per-surfel backward kernels;
-the default ones must not change by a single instruction.  This script compiles composite_tile.cu, composite_feat.cu
-and surfel_bwd.cu -- and preprocess.cu, whose tile-rectangle code the deterministic backward now shares -- for sm_90a,
-from the working tree and from BASE, with the library's own nvcc flags, and compares the disassembly of every default
-kernel after removing addresses, encodings and the kernel's mangled name (a template parameter changes the name, not
-the code).
+A change that shares device code between kernels, or adds code next to them, can leave a kernel's instructions as they
+were; this script shows whether it did.  It compiles SOURCES for sm_90a, from the working tree and from BASE, with the
+library's own nvcc flags, and compares the disassembly of every kernel in KERNELS that BASE has, after removing
+addresses, encodings and the kernel's mangled name (a template parameter changes the name, not the code).
 
-BASE is the commit before the deterministic backward, feb2f64; with the change committed on top of it, HEAD^ names it
-too.  --base HEAD checks uncommitted work against the last commit.
+BASE defaults to HEAD, which checks uncommitted work against the last commit; HEAD^ checks the last commit.
 
 Usage: python tools/sass_diff.py [--base REV]      exit status 0 = identical, 1 = a kernel differs or is missing
 """
@@ -26,11 +23,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from vidu4d_b200.build import NVCC_FLAGS, _nvcc  # noqa: E402
 
-SOURCES = ["composite_tile.cu", "composite_feat.cu", "surfel_bwd.cu", "preprocess.cu"]
+SOURCES = ["composite_tile.cu", "composite_feat.cu", "composite_det.cu", "surfel_bwd.cu", "preprocess.cu"]
 # (demangled-name pattern in the base build, pattern of the same kernel in the working tree)
 KERNELS = [
     (r"composite_tile_bwd_kernel(<\(bool\)0>)?\(", r"composite_tile_bwd_kernel(<\(bool\)0>)?\("),
     (r"composite_tile_fwd_kernel\(", r"composite_tile_fwd_kernel\("),       # shares the chunk wait with the backward
+    (r"det_zero_kernel\(", r"det_zero_kernel\("),
+    (r"det_gather_kernel\(", r"det_gather_kernel\("),
     (r"feature_bwd_kernel<\(int\)4>\(", r"feature_bwd_kernel<\(int\)4>\("),
     (r"feature_bwd_kernel<\(int\)2>\(", r"feature_bwd_kernel<\(int\)2>\("),
     (r"feature_bwd_kernel<\(int\)1>\(", r"feature_bwd_kernel<\(int\)1>\("),
@@ -71,7 +70,7 @@ def _find(kernels: dict, pattern: str):
 
 def main() -> int:
     ap = argparse.ArgumentParser()
-    ap.add_argument("--base", default="feb2f64", help="commit to compare with (default: the one before the change)")
+    ap.add_argument("--base", default="HEAD", help="commit to compare with (default: HEAD)")
     args = ap.parse_args()
     with tempfile.TemporaryDirectory() as tmp:
         base = os.path.join(tmp, "base")

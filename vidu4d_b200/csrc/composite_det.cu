@@ -22,42 +22,33 @@
 namespace {
 using namespace comp;
 
-constexpr int DW = 8;              // warps per CTA = 8x4 sub-tiles of a tile
-constexpr int DCH = 256;           // instances per chunk == threads per CTA
-constexpr int DNSLOT = 2;
-constexpr int DNPIX = 32 * DW;
 constexpr int FCAP = 3072;         // pair-buffer slots, 8 B each
 struct FdSmem {
-    static constexpr int NSTG = DCH / 32;
-    static constexpr size_t masks = (size_t)DNSLOT * DCH * REC4 * sizeof(float4);
-    static constexpr size_t g = masks + (size_t)DW * NSTG * 32 * sizeof(uint32_t);              // dL/dplane [channel][pixel]
-    static constexpr size_t buf = g + (size_t)SR_FEAT_MAX * DNPIX * sizeof(float);               // pair buffer, 2 x FCAP
+    static constexpr size_t masks = (size_t)BWD_NSLOT * BWD_CH * REC4 * sizeof(float4);
+    static constexpr size_t g = masks + (size_t)BWD_NSTG * BWD_NPIX * sizeof(uint32_t);          // dL/dplane [channel][pixel]
+    static constexpr size_t buf = g + (size_t)SR_FEAT_MAX * BWD_NPIX * sizeof(float);            // pair buffer, 2 x FCAP
     static constexpr size_t sfx = buf + 2 * (size_t)FCAP * sizeof(float);                        // slot table [stage][pixel]
-    static constexpr size_t full = sfx + (size_t)NSTG * DNPIX * sizeof(uint16_t);
-    static constexpr size_t wsum = full + DNSLOT * sizeof(uint64_t);
-    static constexpr size_t total = wsum + DW * sizeof(uint32_t);
+    static constexpr size_t full = sfx + (size_t)BWD_NSTG * BWD_NPIX * sizeof(uint16_t);
+    static constexpr size_t wsum = full + BWD_NSLOT * sizeof(uint64_t);
+    static constexpr size_t total = wsum + BWD_WARPS * sizeof(uint32_t);
 };
 static_assert(FdSmem::full % 8 == 0, "mbarrier alignment");
 static_assert(2 * (FdSmem::total + 1024) <= 233472, "two CTAs per SM (228 KB, 1 KB reserved per CTA)");
-static_assert(DCH * DCH <= 65536, "a chunk's pair count fits the 16-bit slot table");
 
 // NCH = the channel count F rounded up to a multiple of SR_FEAT_CHUNK (register arrays of compile-time size)
 template <int NCH>
-__global__ void __launch_bounds__(DNPIX, 2)
+__global__ void __launch_bounds__(BWD_NPIX, 2)
 feature_bwd_det_kernel(const FrameStrides fs, const FeatArgs ft, const uint2* __restrict__ ranges,
                        const uint32_t* __restrict__ tile_order, int tiles_x, const float4* __restrict__ irec, int W, int H,
                        const float* __restrict__ final_Ts, const uint32_t* __restrict__ sub_last,
                        const uint32_t* __restrict__ contrib_masks, const DetArgs det) {
     using SM = FdSmem;
-    constexpr int CH = DCH, NSLOT = DNSLOT, NSTG = SM::NSTG, NPIX = DNPIX;
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    float4* ring = reinterpret_cast<float4*>(smem_raw);
     uint32_t* cm_all = reinterpret_cast<uint32_t*>(smem_raw + SM::masks);
     float* gsm = reinterpret_cast<float*>(smem_raw + SM::g);
     float* buf_a = reinterpret_cast<float*>(smem_raw + SM::buf);     // G times dL/dalpha (times T, with the background term)
     float* buf_t = buf_a + FCAP;                                      // alpha T, negated on the low-pass branch
     uint16_t* sfx = reinterpret_cast<uint16_t*>(smem_raw + SM::sfx);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + SM::full);
     uint32_t* wsum = reinterpret_cast<uint32_t*>(smem_raw + SM::wsum);
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -74,31 +65,12 @@ feature_bwd_det_kernel(const FrameStrides fs, const FeatArgs ft, const uint2* __
     const int tile = (int)tile_order[blockIdx.x / (unsigned)fs.frames];
     const int tile_x = tile % tiles_x, tile_y = tile / tiles_x;
     const uint2 range = ranges[tile];
-    const int rlen = (int)(range.y - range.x);
-    const uint32_t my_last = sub_last[tile * 8 + (lane & 7)];
-    uint32_t cta_last = my_last;
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) cta_last = max(cta_last, __shfl_xor_sync(0xffffffffu, cta_last, o));
-    const int len = min(rlen, (int)cta_last);
-    const int len_w = min(rlen, (int)__shfl_sync(0xffffffffu, my_last, warp));
-    const int nchunks = (len + CH - 1) / CH;
-    if (nchunks == 0) return;                      // CTA-uniform
-    const int nb_w = (len_w + 31) >> 5;
-
-    const float4* src = irec + (size_t)range.x * REC4;
-    auto issue = [&](int k) {   // one thread; the k-th consumed chunk is c = nchunks-1-k, in slot k % NSLOT
-        const int c = nchunks - 1 - k, s = k % NSLOT;
-        const uint32_t bytes = (uint32_t)min(CH, len - c * CH) * 80u;
-        fence_proxy_async();
-        mbar_expect_tx(&full[s], bytes);
-        bulk_g2s(ring + (size_t)s * CH * REC4, src + (size_t)c * CH * REC4, bytes, &full[s]);
-    };
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int s = 0; s < NSLOT; s++) mbar_init(&full[s], 1);
-        fence_mbar_init();
-        for (int k = 0; k < NSLOT && k < nchunks; k++) issue(k);
-    }
+    const BwdTile bt = bwd_tile(range, sub_last, tile);
+    if (bt.nchunks == 0) return;                   // CTA-uniform
+    const int nb_w = bt.nb_w();
+    const ChunkRing ring{reinterpret_cast<float4*>(smem_raw), reinterpret_cast<uint64_t*>(smem_raw + SM::full),
+                         irec + (size_t)range.x * REC4, bt.len, bt.nchunks};
+    if (threadIdx.x == 0) ring.init();
 
     // per-pixel state (as feature_bwd_kernel's, all channels at once); thread == pixel == warp * 32 + lane
     const SubPixel sp = sub_pixel(tile_x, tile_y, warp, lane);
@@ -112,66 +84,36 @@ feature_bwd_det_kernel(const FrameStrides fs, const FeatArgs ft, const uint2* __
         accum[c] = 0.f;
         if (c < F) {
             const float g = inside ? dout[(size_t)c * N + pid] * gs : 0.f;
-            gsm[c * NPIX + threadIdx.x] = g;
+            gsm[c * BWD_NPIX + threadIdx.x] = g;
             if (ft.bg) bg_dot += __ldg(ft.bg + c) * g;
         }
     }
 
-    uint32_t* cm = cm_all + warp * NSTG * 32 + lane;
-    const uint32_t* cm_in = contrib_masks + contrib_word(range.x, tile, warp, lane);
-    uint32_t pre[NSTG];
-    auto fetch = [&](int c) {
-#pragma unroll
-        for (int st = 0; st < NSTG; st++) {
-            const int g = c * NSTG + st;
-            pre[st] = g < nb_w ? __ldg(cm_in + (size_t)g * SR_CONTRIB_STAGE_WORDS) : 0u;
-        }
-    };
-    fetch(nchunks - 1);
+    PixelMasks masks{cm_all + warp * BWD_NSTG * 32 + lane, contrib_masks + contrib_word(range.x, tile, warp, lane),
+                     nb_w};
+    masks.fetch(bt.nchunks - 1);
 
-    for (int k = 0; k < nchunks; k++) {
-        const int c = nchunks - 1 - k, s = k % NSLOT;
-        uint32_t nz = 0u;
-        int np = 0;
-#pragma unroll
-        for (int st = 0; st < NSTG; st++) { cm[st * 32] = pre[st]; if (pre[st]) nz |= 1u << st; np += __popc(pre[st]); }
-        int incl = np;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int y = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += y;
-        }
-        if (lane == 31) wsum[warp] = (uint32_t)incl;
-        __syncthreads();                           // masks, warp totals and dL/dplane are in; the previous chunk is done
-        int base = incl - np, total = 0;
-        for (int w = 0; w < DW; w++) { if (w < warp) base += (int)wsum[w]; total += (int)wsum[w]; }
-        {
-            int run = base;
-#pragma unroll
-            for (int st = NSTG - 1; st >= 0; st--) {
-                sfx[st * NPIX + threadIdx.x] = (uint16_t)min(run, 0xffff);
-                run += __popc(pre[st]);
-            }
-        }
-        const DetPasses dp(total, FCAP, CH);
-        const int npass = dp.npass, my_pass = dp.of(base);
-        if (c > 0) fetch(c - 1);
-        {
-            const uint32_t parity = (uint32_t)((k / NSLOT) & 1);
-            while (!mbar_try_wait(&full[s], parity)) { }
-        }
-        const float4* S = ring + (size_t)s * CH * REC4;
+    for (int k = 0; k < bt.nchunks; k++) {
+        const int c = bt.nchunks - 1 - k, s = k % BWD_NSLOT;
+        int np, total = 0;
+        const uint32_t nz = masks.install(np);
+        const int base = masks.scan(np, wsum, sfx);            // its barrier also orders dL/dplane before the first chunk
+#pragma unroll 1                                               // rolled: fewer registers beside the channel arrays
+        for (int w = 0; w < BWD_WARPS; w++) total += (int)wsum[w];
+        const DetPasses dp(total, FCAP, BWD_CH);
+        if (c > 0) masks.fetch(c - 1);
+        const float4* S = ring.wait(k, s);
 
-        for (int pass = 0; pass < npass; pass++) {
+        for (int pass = 0; pass < dp.npass; pass++) {
             if (pass > 0) __syncthreads();         // the previous pass's phase 2 is done with the buffer
             const int off = dp.offset(pass);
             // ---- phase 1: lane = pixel, back to front over its contributors
-            uint32_t nzp = my_pass == pass ? nz : 0u;
+            uint32_t nzp = dp.of(base) == pass ? nz : 0u;
             if (__any_sync(0xffffffffu, nzp != 0u)) {
                 int st = 0, slot = base;
                 uint32_t mym = 0u;
                 for (;;) {
-                    if (mym == 0u && nzp) { st = 31 - __clz(nzp); nzp &= ~(1u << st); mym = cm[st * 32]; }
+                    if (mym == 0u && nzp) { st = 31 - __clz(nzp); nzp &= ~(1u << st); mym = masks.cm[st * 32]; }
                     const bool act = mym != 0u;
                     if (!__any_sync(0xffffffffu, act)) break;
                     if (!act) continue;
@@ -191,7 +133,7 @@ feature_bwd_det_kernel(const FrameStrides fs, const FeatArgs ft, const uint2* __
                     for (int ch = 0; ch < NCH; ch++) {
                         if (ch < F) {
                             const float x = __ldg(row + ch);
-                            dL_dalpha += (x - accum[ch]) * gsm[ch * NPIX + threadIdx.x];
+                            dL_dalpha += (x - accum[ch]) * gsm[ch * BWD_NPIX + threadIdx.x];
                             accum[ch] = alpha * x + oma * accum[ch];
                         }
                     }
@@ -205,14 +147,8 @@ feature_bwd_det_kernel(const FrameStrides fs, const FeatArgs ft, const uint2* __
             __syncthreads();                       // pair buffer complete
 
             // ---- phase 2: thread = instance warp * 32 + lane of the chunk
-            uint32_t pw[DW];
-            uint32_t anyw = 0u;
-#pragma unroll
-            for (int sw = 0; sw < DW; sw++) {
-                pw[sw] = transpose32(cm_all[(sw * NSTG + warp) * 32 + lane], lane);
-                anyw |= pw[sw];
-            }
-            if (anyw) {
+            const InstancePixels ip(cm_all);
+            if (ip.any) {
                 const float4* R = S + threadIdx.x * REC4;
                 const float4 r0 = R[0], r1 = R[1], r2 = R[2];
                 const uint32_t e = sr_emission_index(point_offsets, radii, __float_as_uint(R[4].z), r2.y, r2.z, tile_x, tile_y,
@@ -225,36 +161,11 @@ feature_bwd_det_kernel(const FrameStrides fs, const FeatArgs ft, const uint2* __
                 for (int i = 0; i < 16; i++) acc[i] = 0.f;
 #pragma unroll
                 for (int ch = 0; ch < NCH; ch++) df[ch] = 0.f;
-                uint32_t nzw = 0u;
-#pragma unroll
-                for (int sw = 0; sw < DW; sw++) if (pw[sw]) nzw |= 1u << sw;
-                int sw = 0;
-                uint32_t w = 0u;
-                for (;;) {
-                    if (w == 0u) {
-                        if (nzw == 0u) break;
-                        sw = __ffs(nzw) - 1;
-                        nzw &= nzw - 1u;
-#pragma unroll
-                        for (int qq = 0; qq < DW; qq++) if (qq == sw) w = pw[qq];
-                    }
-                    const int l = __ffs(w) - 1;
-                    w &= w - 1u;
-                    const int p = sw * 32 + l;
-                    if (dp.of((int)sfx[(NSTG - 1) * NPIX + p]) != pass) continue;
-                    const uint32_t pm = cm_all[(sw * NSTG + warp) * 32 + l];
-                    const int slot = (int)sfx[warp * NPIX + p] + __popc((pm >> lane) >> 1) - off;
+                ip.walk(cm_all, sfx, dp, pass, [&](int p, int sw, int l, int b) {
                     if (!any_in) {
                         // first pair of this pass: start from what the slot holds -- the colour pass's sum, and the
                         // partial sums of earlier passes
-                        const float4* g4 = reinterpret_cast<const float4*>(gslot);
-#pragma unroll
-                        for (int qq = 0; qq < 4; qq++) {
-                            const float4 t = g4[qq];
-                            acc[4 * qq] = t.x; acc[4 * qq + 1] = t.y; acc[4 * qq + 2] = t.z; acc[4 * qq + 3] = t.w;
-                        }
-                        const float4 t = g4[4];
-                        a2x = t.x; a2y = t.y;
+                        slot_load(gslot, acc, a2x, a2y);
                         if (pass > 0) {
 #pragma unroll
                             for (int ch = 0; ch < NCH; ch++) if (ch < F) df[ch] = fslot[ch];
@@ -262,24 +173,21 @@ feature_bwd_det_kernel(const FrameStrides fs, const FeatArgs ft, const uint2* __
                         any_in = true;
                     }
                     const SubPixel pp = sub_pixel(tile_x, tile_y, sw, l);
-                    const float t = buf_t[slot];
-                    pair_geom_vjp_stored(r0, r1, r2, pp.pixx, pp.pixy, buf_a[slot], 0.f, t < 0.f, acc, a2x, a2y);
+                    const float t = buf_t[b];
+                    pair_geom_vjp_stored(r0, r1, r2, pp.pixx, pp.pixy, buf_a[b], 0.f, t < 0.f, acc, a2x, a2y);
                     const float aT = fabsf(t);
 #pragma unroll
-                    for (int ch = 0; ch < NCH; ch++) if (ch < F) df[ch] += aT * gsm[ch * NPIX + p];
-                }
+                    for (int ch = 0; ch < NCH; ch++) if (ch < F) df[ch] += aT * gsm[ch * BWD_NPIX + p];
+                });
                 if (any_in) {
-                    float4* g4 = reinterpret_cast<float4*>(gslot);
-#pragma unroll
-                    for (int qq = 0; qq < 4; qq++) g4[qq] = make_float4(acc[4 * qq], acc[4 * qq + 1], acc[4 * qq + 2], acc[4 * qq + 3]);
-                    g4[4] = make_float4(a2x, a2y, 0.f, 0.f);
+                    slot_store(gslot, acc, a2x, a2y);
 #pragma unroll
                     for (int ch = 0; ch < NCH; ch++) if (ch < F) fslot[ch] = df[ch];
                 }
             }
         }
         __syncthreads();                           // ring slot, masks, pair buffer and slot table are free again
-        if (threadIdx.x == 0 && k + NSLOT < nchunks) issue(k + NSLOT);
+        if (threadIdx.x == 0 && k + BWD_NSLOT < bt.nchunks) ring.issue(k + BWD_NSLOT);
     }
 }
 
@@ -383,7 +291,7 @@ cudaError_t launch_feature_bwd_det(const BwdArgs& a, const FeatArgs& ft, const D
     ProfileScope ps("feature_bwd_det", a.stream);
     auto launch = [&](auto kern) -> cudaError_t {
         if (cudaError_t e = sr_opt_in_smem(kern, FdSmem::total)) return e;
-        kern<<<a.il.tiles * a.fs.frames, DNPIX, FdSmem::total, a.stream>>>(
+        kern<<<a.il.tiles * a.fs.frames, BWD_NPIX, FdSmem::total, a.stream>>>(
             a.fs, ft, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles_x,
             (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, (const float*)(a.img + a.il.final_T),
             (const uint32_t*)(a.img + a.il.tile_last), (const uint32_t*)(a.bin + a.bl.contrib), d);

@@ -184,36 +184,30 @@ composite_tile_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ range
 // A pair whose slot lies beyond the buffer (a dense chunk) takes the direct path in phase 1 -- full VJP and per-pair
 // reductions -- and phase 2 skips it: the capacity changes the order of the float sums and the rounding of a pair's
 // terms (the direct path keeps the correctly rounded quotients), never which terms are summed.
-constexpr int BWD_CH = 256;        // instances per chunk == threads per CTA (one instance per thread in phase 2)
-constexpr int BWD_NSLOT = 2;
 constexpr int BWD_CAP = 4608;      // pair-buffer slots, 12 B each; headline chunks: 2,200 pairs average, 5,500 p99
 struct BwdSmem {
-    static constexpr int NSTG = BWD_CH / 32;
     // offsets of the regions that follow the ring
     static constexpr size_t masks = (size_t)BWD_NSLOT * BWD_CH * REC4 * sizeof(float4);      // masks [warp][stage][lane]
-    static constexpr size_t pd4 = masks + (size_t)TWARPS * NSTG * 32 * sizeof(uint32_t);      // per pixel: dpix0..2, dn0
-    static constexpr size_t pd2 = pd4 + 32 * TWARPS * sizeof(float4);                           // per pixel: dn1, dn2
-    static constexpr size_t buf = pd2 + 32 * TWARPS * sizeof(float2);                           // pair buffer, 3 x BWD_CAP
+    static constexpr size_t pd4 = masks + (size_t)BWD_NSTG * BWD_NPIX * sizeof(uint32_t);     // per pixel: dpix0..2, dn0
+    static constexpr size_t pd2 = pd4 + BWD_NPIX * sizeof(float4);                              // per pixel: dn1, dn2
+    static constexpr size_t buf = pd2 + BWD_NPIX * sizeof(float2);                              // pair buffer, 3 x BWD_CAP
     static constexpr size_t sfx = buf + 3 * (size_t)BWD_CAP * sizeof(float);                   // slot table [stage][pixel]
-    static constexpr size_t full = sfx + (size_t)NSTG * 32 * TWARPS * sizeof(uint16_t);        // mbarriers
+    static constexpr size_t full = sfx + (size_t)BWD_NSTG * BWD_NPIX * sizeof(uint16_t);       // mbarriers
     static constexpr size_t wsum = full + BWD_NSLOT * sizeof(uint64_t);                         // pair count per warp
-    static constexpr size_t total = wsum + TWARPS * sizeof(uint32_t);
+    static constexpr size_t total = wsum + BWD_WARPS * sizeof(uint32_t);
 };
-static_assert(BWD_CH == 32 * TWARPS, "phase 2 gives every instance of a chunk its own thread");
 static_assert(BwdSmem::full % 8 == 0, "mbarrier alignment");
 static_assert(2 * (BwdSmem::total + 1024) <= 233472, "two CTAs per SM (228 KB, 1 KB reserved per CTA)");
 // Deterministic instantiation (DET = true, include/surfel_deterministic.h):
 //   * the (instance, tile) sum is STORED into the instance's slot det.slots[emission index] instead of reduced into the
 //     per-surfel accumulator; launch_det_gather sums a surfel's slots in emission order;
-//   * there is no direct path: a chunk with more pairs than BWD_CAP runs phases 1 and 2 in passes.  Pass k takes the
-//     pixels whose slot base lies in [k DET_PASS, (k+1) DET_PASS) -- whole pixels, in scan order, and a pixel has at
-//     most BWD_CH pairs in a chunk, so its pairs fit the buffer at offset k DET_PASS (comp::DetPasses, DET_PASS =
-//     BWD_CAP - BWD_CH).  Phase 2 of pass k > 0 resumes
-//     from the partial sum pass k-1 stored in the slot.  Phase 2 adds an instance's pixels in ascending pixel order
-//     whatever the passes, so the sum is the one a single pass would form, and no pair takes the full VJP.
+//   * there is no direct path: a chunk with more pairs than BWD_CAP runs phases 1 and 2 in passes of whole pixels
+//     (comp::DetPasses).  Phase 2 of pass k > 0 resumes from the partial sum pass k-1 stored in the slot.  Phase 2 adds
+//     an instance's pixels in ascending pixel order whatever the passes, so the sum is the one a single pass would
+//     form, and no pair takes the full VJP.
 
 template <bool DET>
-__global__ void __launch_bounds__(32 * TWARPS, 2)
+__global__ void __launch_bounds__(BWD_NPIX, 2)
 composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_scale, const uint2* __restrict__ ranges,
                           const uint32_t* __restrict__ tile_order, int tiles_x,
                           const float4* __restrict__ irec, int W, int H, const float* __restrict__ bg,
@@ -222,9 +216,7 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                           const float* __restrict__ dL_dothers, const uint32_t* __restrict__ contrib_masks,
                           float* __restrict__ sgrad, const DetArgs det) {
     using SM = BwdSmem;
-    constexpr int CH = BWD_CH, NSLOT = BWD_NSLOT, NSTG = SM::NSTG, NPIX = 32 * TWARPS;
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    float4* ring = reinterpret_cast<float4*>(smem_raw);
     uint32_t* cm_all = reinterpret_cast<uint32_t*>(smem_raw + SM::masks);
     float4* pd4 = reinterpret_cast<float4*>(smem_raw + SM::pd4);
     float2* pd2 = reinterpret_cast<float2*>(smem_raw + SM::pd2);
@@ -232,7 +224,6 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
     float* buf_z = buf_a + BWD_CAP;                                   // dL/dz
     float* buf_t = buf_z + BWD_CAP;                                   // alpha T, negated on the low-pass branch
     uint16_t* sfx = reinterpret_cast<uint16_t*>(smem_raw + SM::sfx);  // first slot of (stage, pixel)'s pairs
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + SM::full);
     uint32_t* wsum = reinterpret_cast<uint32_t*>(smem_raw + SM::wsum);
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -250,140 +241,74 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
     const int tile = (int)tile_order[blockIdx.x / (unsigned)fs.frames];
     const int tile_x = tile % tiles_x, tile_y = tile / tiles_x;
     const uint2 range = ranges[tile];
-    const int rlen = (int)(range.y - range.x);
-    // nothing beyond a sub-tile's deepest contributor matters to it; the CTA streams up to the deepest of the eight
-    const uint32_t my_last = sub_last[tile * 8 + (lane & 7)];
-    uint32_t cta_last = my_last;
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) cta_last = max(cta_last, __shfl_xor_sync(0xffffffffu, cta_last, o));
-    const int len = min(rlen, (int)cta_last);
-    const int len_w = min(rlen, (int)__shfl_sync(0xffffffffu, my_last, warp));
-    const int nchunks = (len + CH - 1) / CH;
-    if (nchunks == 0) return;                      // CTA-uniform
-    const int nb_w = (len_w + 31) >> 5;            // stages this sub-tile reads
-
-    const float4* src = irec + (size_t)range.x * REC4;
-    // the k-th consumed chunk (k = 0, 1, ..) is c = nchunks-1-k; it lives in slot k % NSLOT
-    auto issue = [&](int k) {   // one thread
-        const int c = nchunks - 1 - k, s = k % NSLOT;
-        const uint32_t bytes = (uint32_t)min(CH, len - c * CH) * 80u;
-        fence_proxy_async();                       // the slot's previous readers (generic proxy) passed a CTA barrier
-        mbar_expect_tx(&full[s], bytes);
-        bulk_g2s(ring + (size_t)s * CH * REC4, src + (size_t)c * CH * REC4, bytes, &full[s]);
-    };
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int s = 0; s < NSLOT; s++) mbar_init(&full[s], 1);
-        fence_mbar_init();
-        for (int k = 0; k < NSLOT && k < nchunks; k++) issue(k);
-    }
+    const BwdTile bt = bwd_tile(range, sub_last, tile);
+    if (bt.nchunks == 0) return;                   // CTA-uniform
+    const int nb_w = bt.nb_w();
+    const ChunkRing ring{reinterpret_cast<float4*>(smem_raw), reinterpret_cast<uint64_t*>(smem_raw + SM::full),
+                         irec + (size_t)range.x * REC4, bt.len, bt.nchunks};
+    if (threadIdx.x == 0) ring.init();
 
     BwdPixel px;
     px.load(sub_pixel(tile_x, tile_y, warp, lane), W, H, bg, final_Ts, n_contrib, dL_dpixels, dL_dothers, grad_scale);
     pd4[threadIdx.x] = make_float4(px.dpix0, px.dpix1, px.dpix2, px.dn0);      // thread == pixel == warp * 32 + lane
     pd2[threadIdx.x] = make_float2(px.dn1, px.dn2);
 
-    uint32_t* cm = cm_all + warp * NSTG * 32 + lane;
-    const uint32_t* cm_in = contrib_masks + contrib_word(range.x, tile, warp, lane);
-    uint32_t pre[NSTG];                            // the next chunk's masks, in flight while this one is walked
-    auto fetch = [&](int c) {
-#pragma unroll
-        for (int st = 0; st < NSTG; st++) {
-            const int g = c * NSTG + st;
-            pre[st] = g < nb_w ? __ldg(cm_in + (size_t)g * SR_CONTRIB_STAGE_WORDS) : 0u;
-        }
-    };
-    fetch(nchunks - 1);
+    PixelMasks masks{cm_all + warp * BWD_NSTG * 32 + lane, contrib_masks + contrib_word(range.x, tile, warp, lane),
+                     nb_w};
+    masks.fetch(bt.nchunks - 1);
 
-    for (int k = 0; k < nchunks; k++) {
-        const int c = nchunks - 1 - k, s = k % NSLOT;
-        uint32_t nz = 0u;
-        int np = 0;
-#pragma unroll
-        for (int st = 0; st < NSTG; st++) { cm[st * 32] = pre[st]; if (pre[st]) nz |= 1u << st; np += __popc(pre[st]); }
-        // slot base of this pixel = exclusive scan of the pair counts over the CTA's pixels
-        int incl = np;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int y = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += y;
-        }
-        if (lane == 31) wsum[warp] = (uint32_t)incl;
-        __syncthreads();                           // masks and warp totals are in; the previous chunk is finished
-        int base = incl - np;
-        for (int w = 0; w < warp; w++) base += (int)wsum[w];
-        int npass = 1, my_pass = 0;                // DET: passes over the chunk, and this pixel's
-        DetPasses dp(0, BWD_CAP, CH);
-        if constexpr (DET) {
-            int total = 0;
-            for (int w = 0; w < TWARPS; w++) total += (int)wsum[w];
-            dp = DetPasses(total, BWD_CAP, CH);
-            npass = dp.npass; my_pass = dp.of(base);
-        }
-        {
-            int run = base;                        // pairs of this pixel in later stages come first (back to front)
-#pragma unroll
-            for (int st = NSTG - 1; st >= 0; st--) {
-                sfx[st * NPIX + threadIdx.x] = (uint16_t)min(run, 0xffff);
-                run += __popc(pre[st]);
-            }
-        }
-        if (c > 0) fetch(c - 1);
-        {
-            const uint32_t parity = (uint32_t)((k / NSLOT) & 1);
-            while (!mbar_try_wait(&full[s], parity)) { }
-        }
-        const float4* S = ring + (size_t)s * CH * REC4;
+    for (int k = 0; k < bt.nchunks; k++) {
+        const int c = bt.nchunks - 1 - k, s = k % BWD_NSLOT;
+        int np, total = 0;
+        const uint32_t nz = masks.install(np);
+        const int base = masks.scan(np, wsum, sfx);
+        if constexpr (DET) for (int w = 0; w < BWD_WARPS; w++) total += (int)wsum[w];
+        const DetPasses dp(total, BWD_CAP, BWD_CH);                // one pass unless DET
+        const int my_pass = dp.of(base);
+        if (c > 0) masks.fetch(c - 1);
+        const float4* S = ring.wait(k, s);
 
-        for (int pass = 0; pass < npass; pass++) {
-        if constexpr (DET) { if (pass > 0) __syncthreads(); }     // the previous pass's phase 2 is done with the buffer
-        const int off = DET ? dp.offset(pass) : 0;
-        uint32_t nzp = nz;
-        if constexpr (DET) nzp = my_pass == pass ? nz : 0u;
-        // ---- phase 1: lane = pixel, back to front over its contributors
-        if (__any_sync(0xffffffffu, nzp != 0u)) {
-            int st = 0, slot = base;
-            uint32_t mym = 0u;
-            for (;;) {
-                if (mym == 0u && nzp) { st = 31 - __clz(nzp); nzp &= ~(1u << st); mym = cm[st * 32]; }
-                const bool act = mym != 0u;
-                if (!__any_sync(0xffffffffu, act)) break;
-                if (!act) continue;
-                const int jj = 31 - __clz(mym);
-                mym &= ~(1u << jj);
-                const int idx = st * 32 + jj;
-                PairAlpha q;
-                float dL_dalpha, dL_dz, aT;
-                px.pair_scalars(S + idx * REC4, c * CH + idx, q, dL_dalpha, dL_dz, aT);
-                if (DET || slot < BWD_CAP) {
-                    // aT > 0: a recorded contributor has alpha >= 1/255, and T >= T_final >= 1e-4 (the walk back
-                    // multiplies T by 1/(1 - alpha) > 1), so aT's sign bit is free to carry the low-pass branch
-                    const int b = slot - off;
-                    buf_a[b] = q.G_ * dL_dalpha; buf_z[b] = dL_dz; buf_t[b] = (q.rho3d <= q.rho2d) ? aT : -aT;
-                } else {
-                    float v[16];
+        for (int pass = 0; pass < dp.npass; pass++) {
+            if (pass > 0) __syncthreads();         // the previous pass's phase 2 is done with the buffer
+            const int off = dp.offset(pass);
+            // ---- phase 1: lane = pixel, back to front over its contributors
+            uint32_t nzp = my_pass == pass ? nz : 0u;
+            if (__any_sync(0xffffffffu, nzp != 0u)) {
+                int st = 0, slot = base;
+                uint32_t mym = 0u;
+                for (;;) {
+                    if (mym == 0u && nzp) { st = 31 - __clz(nzp); nzp &= ~(1u << st); mym = masks.cm[st * 32]; }
+                    const bool act = mym != 0u;
+                    if (!__any_sync(0xffffffffu, act)) break;
+                    if (!act) continue;
+                    const int jj = 31 - __clz(mym);
+                    mym &= ~(1u << jj);
+                    const int idx = st * 32 + jj;
+                    PairAlpha q;
+                    float dL_dalpha, dL_dz, aT;
+                    px.pair_scalars(S + idx * REC4, c * BWD_CH + idx, q, dL_dalpha, dL_dz, aT);
+                    if (DET || slot < BWD_CAP) {
+                        // aT > 0: a recorded contributor has alpha >= 1/255, and T >= T_final >= 1e-4 (the walk back
+                        // multiplies T by 1/(1 - alpha) > 1), so aT's sign bit is free to carry the low-pass branch
+                        const int b = slot - off;
+                        buf_a[b] = q.G_ * dL_dalpha; buf_z[b] = dL_dz; buf_t[b] = (q.rho3d <= q.rho2d) ? aT : -aT;
+                    } else {
+                        float v[16];
 #pragma unroll
-                    for (int i = 0; i < 10; i++) v[i] = 0.f;
-                    float m2x = 0.f, m2y = 0.f;
-                    bool lowpass = false;
-                    px.pair_vjp(S + idx * REC4, q, dL_dalpha, dL_dz, aT, v, m2x, m2y, lowpass);
-                    red_pixel(sgrad, S + idx * REC4, v, m2x, m2y, lowpass);
+                        for (int i = 0; i < 10; i++) v[i] = 0.f;
+                        float m2x = 0.f, m2y = 0.f;
+                        bool lowpass = false;
+                        px.pair_vjp(S + idx * REC4, q, dL_dalpha, dL_dz, aT, v, m2x, m2y, lowpass);
+                        red_pixel(sgrad, S + idx * REC4, v, m2x, m2y, lowpass);
+                    }
+                    slot++;
                 }
-                slot++;
             }
-        }
-        __syncthreads();                           // pair buffer and slot table complete
+            __syncthreads();                       // pair buffer and slot table complete
 
-        // ---- phase 2: thread = instance warp * 32 + lane of the chunk
-        {
-            uint32_t pw[TWARPS];                   // pw[sw] bit l: pixel l of sub-tile sw has this instance as a contributor
-            uint32_t anyw = 0u;
-#pragma unroll
-            for (int sw = 0; sw < TWARPS; sw++) {
-                pw[sw] = transpose32(cm_all[(sw * NSTG + warp) * 32 + lane], lane);
-                anyw |= pw[sw];
-            }
-            if (anyw) {
+            // ---- phase 2: thread = instance warp * 32 + lane of the chunk
+            const InstancePixels ip(cm_all);
+            if (ip.any) {
                 const float4* R = S + threadIdx.x * REC4;
                 const float4 r0 = R[0], r1 = R[1], r2 = R[2];
                 float acc[16];
@@ -395,47 +320,14 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                 if constexpr (DET) {
                     gslot = slots + (size_t)sr_emission_index(point_offsets, radii, __float_as_uint(R[4].z), r2.y, r2.z, tile_x,
                                                               tile_y, tiles_x, det.tiles_y) * SR_GRAD_FLOATS;
-                    if (pass > 0) {                // resume the partial sum of the earlier passes
-                        const float4* g4 = reinterpret_cast<const float4*>(gslot);
-#pragma unroll
-                        for (int q = 0; q < 4; q++) {
-                            const float4 t = g4[q];
-                            acc[4 * q] = t.x; acc[4 * q + 1] = t.y; acc[4 * q + 2] = t.z; acc[4 * q + 3] = t.w;
-                        }
-                        const float4 t = g4[4];
-                        a2x = t.x; a2y = t.y;
-                    }
+                    if (pass > 0) slot_load(gslot, acc, a2x, a2y);     // resume the partial sum of the earlier passes
                 }
-                // one flat walk over the instance's pixels: the warp iterates max over lanes of the pair count
-                uint32_t nzw = 0u;
-#pragma unroll
-                for (int sw = 0; sw < TWARPS; sw++) if (pw[sw]) nzw |= 1u << sw;
-                int sw = 0;
-                uint32_t w = 0u;
-                for (;;) {
-                    if (w == 0u) {
-                        if (nzw == 0u) break;
-                        sw = __ffs(nzw) - 1;
-                        nzw &= nzw - 1u;
-#pragma unroll
-                        for (int q = 0; q < TWARPS; q++) if (q == sw) w = pw[q];
-                    }
-                    const int l = __ffs(w) - 1;
-                    w &= w - 1u;
-                    const int p = sw * 32 + l;
-                    const uint32_t pm = cm_all[(sw * NSTG + warp) * 32 + l];
-                    int slot = (int)sfx[warp * NPIX + p] + __popc((pm >> lane) >> 1);
-                    if constexpr (DET) {
-                        // pixel p's pass: its slot base is the first stage's entry of the slot table
-                        if (dp.of((int)sfx[(NSTG - 1) * NPIX + p]) != pass) continue;
-                        slot -= off;
-                    } else {
-                        if (slot >= BWD_CAP) continue;      // went out directly in phase 1
-                    }
+                ip.walk(cm_all, sfx, dp, pass, [&](int p, int sw, int l, int b) {
+                    if (!DET && b >= BWD_CAP) return;      // went out directly in phase 1
                     const SubPixel pp = sub_pixel(tile_x, tile_y, sw, l);
-                    const float t = buf_t[slot];
+                    const float t = buf_t[b];
                     const bool lowpass = t < 0.f;
-                    pair_geom_vjp_stored(r0, r1, r2, pp.pixx, pp.pixy, buf_a[slot], buf_z[slot], lowpass, acc, a2x, a2y);
+                    pair_geom_vjp_stored(r0, r1, r2, pp.pixx, pp.pixy, buf_a[b], buf_z[b], lowpass, acc, a2x, a2y);
                     const float aT = fabsf(t);
                     const float4 d4 = pd4[p];
                     const float2 d2 = pd2[p];
@@ -443,14 +335,9 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                     acc[13] += aT * d4.w; acc[14] += aT * d2.x; acc[15] += aT * d2.y;
                     lowpass_any |= lowpass;
                     any_in = true;
-                }
+                });
                 if constexpr (DET) {
-                    if (any_in) {
-                        float4* g4 = reinterpret_cast<float4*>(gslot);
-#pragma unroll
-                        for (int q = 0; q < 4; q++) g4[q] = make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
-                        g4[4] = make_float4(a2x, a2y, 0.f, 0.f);
-                    }
+                    if (any_in) slot_store(gslot, acc, a2x, a2y);
                 } else if (any_in) {
                     float* gp = sgrad + (size_t)__float_as_uint(R[4].z) * SR_GRAD_FLOATS;
                     red_add<16>(gp, acc);
@@ -461,9 +348,8 @@ composite_tile_bwd_kernel(const FrameStrides fs, const float* __restrict__ grad_
                 }
             }
         }
-        }                                          // passes
         __syncthreads();                           // ring slot, masks, pair buffer and slot table are free again
-        if (threadIdx.x == 0 && k + NSLOT < nchunks) issue(k + NSLOT);
+        if (threadIdx.x == 0 && k + BWD_NSLOT < bt.nchunks) ring.issue(k + BWD_NSLOT);
     }
 }
 
@@ -504,7 +390,7 @@ static cudaError_t launch_tile_bwd(const BwdArgs& a, const DetArgs& d) {
     ProfileScope ps(DET ? "composite_bwd_det" : "composite_bwd", a.stream);
     cudaError_t e = sr_opt_in_smem(composite_tile_bwd_kernel<DET>, BwdSmem::total);
     if (e != cudaSuccess) return e;
-    composite_tile_bwd_kernel<DET><<<a.il.tiles * a.fs.frames, 32 * TWARPS, BwdSmem::total, a.stream>>>(
+    composite_tile_bwd_kernel<DET><<<a.il.tiles * a.fs.frames, BWD_NPIX, BwdSmem::total, a.stream>>>(
         a.fs, a.grad_scale, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles_x,
         (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, a.cam.bg,
         (const float*)(a.img + a.il.final_T), (const uint32_t*)(a.img + a.il.n_contrib),
