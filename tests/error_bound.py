@@ -3,7 +3,8 @@
 _E holds a float64 value v, a bound b (in units of u = 2^-24) on the absolute error of the fp32 evaluation of the same
 expression on the same fp32 inputs, and optionally f, that fp32 evaluation itself (the "shadow": float32 NumPy, the same
 operations in the same order).  Each operation adds |a| err(b) + |b| err(a) for a product, err(a) / |b| + |a/b| err(b) / |b|
-for a quotient, and so on, plus one rounding of its result unless that result is exact in fp32.  The shadow is carried
+for a quotient, and so on, plus one rounding of its result unless that result is exact in fp32 (a product with an exact 0
+is); a rounding is charged u |v| plus 2^-150, the most a result that underflows to a subnormal can lose.  The shadow is carried
 only where every operand has one (leaves made with _E.leaf); _c gives plain numbers one.
 
 The library functions are charged their CUDA accuracy without --use_fast_math: expf <= 2 ulp, logf <= 1 ulp,
@@ -13,10 +14,14 @@ a*b + c into one FMA, which rounds once: the two roundings charged for it still 
 import numpy as np
 
 
+TINY_U = 2.0 ** -126       # half the subnormal spacing 2^-149, in units of u: a result that underflows errs by up to 2^-150
+
+
 def _rnd(v, exact):
-    """The rounding of one fp32 operation whose exact result is v: none where the operands are exact and v is a float."""
+    """The rounding of one fp32 operation whose exact result is v: none where the operands are exact and v is a float;
+    otherwise u |v| for a normal result, and at most 2^-150 more where it is subnormal."""
     r = np.abs(v)
-    return np.where(exact & (v.astype(np.float32).astype(np.float64) == v), 0.0, r)
+    return np.where(exact & (v.astype(np.float32).astype(np.float64) == v), 0.0, r + TINY_U)
 
 
 def _sh(fn, *xs):
@@ -61,14 +66,15 @@ class _E:
     def __mul__(s, o):
         o = _c(o)
         v = s.v * o.v
-        return _E(v, np.abs(s.v) * o.b + np.abs(o.v) * s.b + _rnd(v, (s.b == 0) & (o.b == 0)), _sh(np.multiply, s, o))
+        ex = ((s.b == 0) & (o.b == 0)) | ((s.v == 0) & (s.b == 0)) | ((o.v == 0) & (o.b == 0))     # x * exact 0 = 0
+        return _E(v, np.abs(s.v) * o.b + np.abs(o.v) * s.b + _rnd(v, ex), _sh(np.multiply, s, o))
 
     def __truediv__(s, o):
         o = _c(o)
         with np.errstate(divide="ignore", invalid="ignore"):
             v = s.v / o.v
             b = s.b / np.abs(o.v) + np.abs(v) * o.b / np.abs(o.v)
-        return _E(v, b + _rnd(v, (s.b == 0) & (o.b == 0)), _sh(np.divide, s, o))
+        return _E(v, b + _rnd(v, ((s.b == 0) & (o.b == 0)) | ((s.v == 0) & (s.b == 0))), _sh(np.divide, s, o))
 
     def __getitem__(s, i):
         return _E(s.v[i], s.b[i], None if s.f is None else s.f[i])

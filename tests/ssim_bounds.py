@@ -174,7 +174,7 @@ def forward(img1, img2, alpha=None, bkgd=None):
 # ------------------------------------------------------------------------------------------------ backward
 def backward(img1, img2, maps, dL_dssim, per_image, alpha=None, bkgd=None, dimg1=None, dalpha=None, dbkgd=None):
     """ssim_bwd + ssim_bkgd_reduce.  maps (3,N,C,H,W): the forward's maps as fp32 leaves, or float64 (exact, no shadow) to
-    pin the values to ssim_model.  dL_dssim: the fp32 upstream array the kernel indexes ([n] with per_image, else [0]).
+    pin the values to ssim_model, or the forward's (A, B, Cm) _E values when the GPU's maps are not at hand.  dL_dssim: the fp32 upstream array the kernel indexes ([n] with per_image, else [0]).
     dimg1 (N,C,H,W): the prefill under accumulate = 1, or None.  dalpha (N,H,W) and dbkgd (N,3): the prefills the
     composite adds onto.  Returns dict of _E: dimg1, and with alpha dalpha and dbkgd."""
     N, C, H, W = img1.shape
@@ -183,7 +183,9 @@ def backward(img1, img2, maps, dL_dssim, per_image, alpha=None, bkgd=None, dimg1
     up = _E.leaf(np.asarray(dL_dssim, np.float32).reshape(-1))
     g = (up[np.arange(N)] if per_image else up[np.zeros(N, int)]) * inv_count
     g = g[:, None, None, None]
-    if np.asarray(maps).dtype == np.float32:
+    if isinstance(maps[0], _E):                  # the forward's running-error maps: their bound carries through
+        mp = list(maps)
+    elif np.asarray(maps).dtype == np.float32:
         mp = [_E.leaf(a) for a in maps]
     else:
         mp = [_E(np.asarray(a, np.float64)) for a in maps]

@@ -31,6 +31,7 @@ import pytest
 import torch
 
 from .error_bound import _E, _where
+from .feature_loss_bounds import CONFIGS as FEATURE_CONFIGS
 
 pytestmark = pytest.mark.gpu
 
@@ -57,8 +58,9 @@ def _full(inner, H, W):
     return _E(v, b)
 
 
-def _cam(wvt, W, H, tanx, tany):
-    """post_common.cuh load_cam: R, the adjugate inverse A, fx, fy, cx, cy."""
+def _cam(wvt, W, H, tanx, tany, ox=0.0, oy=0.0):
+    """post_common.cuh load_cam: R, the adjugate inverse A, fx, fy, cx = W * 0.5f + ox, cy = H * 0.5f + oy (tanx, tany,
+    ox, oy: the fp32 values of a per-frame camera row, or the shared tangents with no offset)."""
     m = [_E(float(x)) for x in np.asarray(wvt, np.float32).reshape(16)]
     R = [m[i * 4 + j] for i in range(3) for j in range(3)]
     B = [m[j * 4 + i] for i in range(3) for j in range(3)]
@@ -69,7 +71,9 @@ def _cam(wvt, W, H, tanx, tany):
     A = [c[k] * inv for k in range(3) for c in (c0, c1, c2)]
     fx = _E(float(W)) / _E(2.0 * float(np.float32(tanx)))
     fy = _E(float(H)) / _E(2.0 * float(np.float32(tany)))
-    return dict(R=R, A=A, fx=fx, fy=fy, cx=_E(W * 0.5), cy=_E(H * 0.5))
+    cx = _E(W * 0.5) + _E(float(np.float32(ox)))
+    cy = _E(H * 0.5) + _E(float(np.float32(oy)))
+    return dict(R=R, A=A, fx=fx, fy=fy, cx=cx, cy=cy)
 
 
 def _ray(c, X, Y):
@@ -154,11 +158,11 @@ def _stencil_knife(st, H, W):
     return own, nb
 
 
-def _loss_model(color, am, wvt, target, o, vis, mask, wt, bk):
+def _loss_model(color, am, wvt, target, o, vis, mask, wt, bk, cam=(TANX, TANY, 0.0, 0.0)):
     """loss_grad_kernel's expressions for one frame as _E values: dL/dcolor, dL/dallmap planes 0..6, the per-pixel loss
-    terms and dL/dbkgd parts, the rgb knife mask and the stencil knife masks."""
+    terms and dL/dbkgd parts, the rgb knife mask and the stencil knife masks.  cam: the frame's (tanx, tany, ox, oy)."""
     _, H, W = color.shape
-    c = _cam(wvt, W, H, TANX, TANY)
+    c = _cam(wvt, W, H, *cam)
     r = _E(float(np.float32(o["depth_ratio"])))
     invN = _E(1.0) / _E(float(H * W))
     sN = _E(float(np.float32(o["lambda_normal"]))) * invN
@@ -375,11 +379,26 @@ OPTS = {
                       depth_ratio=0.3),
     "mask_no_wt": dict(vis=True, mask=True, wt=False, bk=True, w_rgb=1.0, w_mask=0.5, lambda_normal=0.05, lambda_dist=0.01,
                        depth_ratio=1.0),
+    # every term, each frame with its own camera row (sr_render_loss_batch_cameras)
+    "cameras": dict(vis=True, mask=True, wt=True, bk=True, w_rgb=0.8, w_mask=0.1, lambda_normal=0.05, lambda_dist=100.0,
+                    depth_ratio=0.3, table=True),
 }
 
 
+def camera_rows(M, W, H):
+    """(M,4) fp32 per-frame (tan_x, tan_y, cx_off, cy_off): both tangents differ from frame to frame, the offsets are
+    non-integer, alternate in sign and move the principal point (W/2 + ox, H/2 + oy) by about a third of the image --
+    across a 32-column block seam from W = 97 up, across an 8-row seam from H = 17 up."""
+    f = np.arange(M)
+    sgn = np.where(f % 2, -1.0, 1.0)
+    rows = np.stack([0.5 - 0.021 * f, 0.35 + 0.017 * f, sgn * (0.34 * W + 0.625 + 0.25 * f),
+                     -sgn * (0.34 * H + 0.3125 + 0.125 * f)], 1)
+    return rows.astype(np.float32)
+
+
 # ------------------------------------------------------------------------------------------------ GPU calls
-def _loss_gpu(M, W, H, o, color, am, wvt, target, vis, mask, wt, bk, dev):
+def _loss_gpu(M, W, H, o, color, am, wvt, target, vis, mask, wt, bk, dev, table=None):
+    """sr_render_loss_batch with the shared TANX / TANY, or sr_render_loss_batch_cameras with the (M,4) device `table`."""
     from vidu4d_b200 import _capi
     lib = _capi.load()
     ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
@@ -388,11 +407,16 @@ def _loss_gpu(M, W, H, o, color, am, wvt, target, vis, mask, wt, bk, dev):
     dLa = torch.full((M, 8, H, W), NAN, device=dev)
     dLb = torch.full((M, 3), NAN, device=dev) if bk is not None else None
     sd = torch.full((M, H, W), NAN, device=dev)
-    rc = lib.sr_render_loss_batch(M, W, H, TANX, TANY, o["depth_ratio"], color.data_ptr(), am.data_ptr(), wvt.data_ptr(),
-                                  target.data_ptr(), ptr(vis), ptr(mask), ptr(wt), ptr(bk), o["w_rgb"], o["w_mask"],
-                                  o["lambda_normal"], o["lambda_dist"], terms.data_ptr(), dLc.data_ptr(), dLa.data_ptr(),
-                                  ptr(dLb), sd.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
-    _capi.check(rc, "sr_render_loss_batch")
+    rest = (o["depth_ratio"], color.data_ptr(), am.data_ptr(), wvt.data_ptr(), target.data_ptr(), ptr(vis), ptr(mask),
+            ptr(wt), ptr(bk), o["w_rgb"], o["w_mask"], o["lambda_normal"], o["lambda_dist"], terms.data_ptr(),
+            dLc.data_ptr(), dLa.data_ptr(), ptr(dLb), sd.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+    if table is None:
+        fn = "sr_render_loss_batch"
+        rc = lib.sr_render_loss_batch(M, W, H, TANX, TANY, *rest)
+    else:
+        fn = "sr_render_loss_batch_cameras"
+        rc = lib.sr_render_loss_batch_cameras(M, W, H, table.data_ptr(), *rest)
+    _capi.check(rc, fn)
     torch.cuda.synchronize(dev)
     return terms, dLc, dLa, dLb, sd
 
@@ -454,6 +478,7 @@ def _reached(H, W):
 
 def _run(name, M, W, H, opt, seed, dev, post=True):
     from oracle import post_oracle as po
+    from . import camera_model as cm
     o = dict(OPTS[opt])
     am, color, target, vis, planted = _frames(M, W, H, seed, o["vis"], o["bk"])
     mask = (np.random.default_rng(seed + 1).uniform(size=(M, H, W)) > 0.5).astype(np.float32) if o["mask"] else None
@@ -465,9 +490,10 @@ def _run(name, M, W, H, opt, seed, dev, post=True):
     wvt_np = wview.numpy().copy()
     T = lambda x: None if x is None else torch.from_numpy(np.ascontiguousarray(x)).to(dev)  # noqa: E731
     args = (T(color), T(am), wview.contiguous().to(dev), T(target), T(visn), T(mask), T(wt), T(bk))
-    terms, dLc, dLa, dLb, sd = _loss_gpu(M, W, H, o, *args, dev)
+    rows = camera_rows(M, W, H) if o.get("table") else None
+    terms, dLc, dLa, dLb, sd = _loss_gpu(M, W, H, o, *args, dev, table=T(rows))
     # no atomics on image data: bit for bit the same planes on a second call
-    _, dLc2, dLa2, _, _ = _loss_gpu(M, W, H, o, *args, dev)
+    _, dLc2, dLa2, _, _ = _loss_gpu(M, W, H, o, *args, dev, table=T(rows))
     assert torch.equal(dLc, dLc2) and torch.equal(dLa, dLa2), name
     terms, dLc, dLa, sd = terms.cpu().numpy(), dLc.cpu().numpy(), dLa.cpu().numpy(), sd.cpu().numpy()
     dLb = None if dLb is None else dLb.cpu().numpy()
@@ -484,13 +510,18 @@ def _run(name, M, W, H, opt, seed, dev, post=True):
         okw = dict(w_rgb=float(np.float32(o["w_rgb"])), w_mask=float(np.float32(o["w_mask"])) if mask is not None else 0.0,
                    lambda_normal=float(np.float32(o["lambda_normal"])), lambda_dist=float(np.float32(o["lambda_dist"])),
                    bkgd=bk)
-        oargs = (color[f], am[f], wvt_np[f], float(np.float32(TANX)), float(np.float32(TANY)),
+        cam = (TANX, TANY, 0.0, 0.0) if rows is None else tuple(float(x) for x in rows[f])
+        oargs = (color[f], am[f], wvt_np[f], float(np.float32(cam[0])), float(np.float32(cam[1])),
                  float(np.float32(o["depth_ratio"])), target[f], vf, mg, mw)
-        _, ot = po.stage3_losses(*oargs, **okw)
-        gr = po.stage3_losses_backward(*oargs, **okw)
+        if rows is None:
+            _, ot = po.stage3_losses(*oargs, **okw)
+            gr = po.stage3_losses_backward(*oargs, **okw)
+        else:                   # the centred oracle with the ray grid's principal point moved (tests/camera_model.py)
+            _, ot = cm.stage3_losses(cam[2], cam[3], *oargs, **okw)
+            gr = cm.stage3_losses_backward(cam[2], cam[3], *oargs, **okw)
         gcol, gall = gr[0], gr[1].copy()
         mdl = _loss_model(color[f], am[f], wvt_np[f], target[f], o, visn[f] if visn is not None else None,
-                          None if mask is None else mask[f], None if wt is None else wt[f], bk)
+                          None if mask is None else mask[f], None if wt is None else wt[f], bk, cam=cam)
         # rgb knife pixels: the GPU's sign must be one of the three; the oracle is re-evaluated at it
         kn = mdl["rgb_knife"]
         knives["rgb"] += int(kn.sum())
@@ -580,8 +611,12 @@ def _check_reach(name, W, H, planted, o, dLa):
 
 W_GRID = (1, 2, 3, 31, 32, 33, 63, 65, 97)
 H_GRID = (1, 2, 3, 7, 8, 9, 17)
-GRID = [(W, H, 1 + 2 * ((i + j) % 2), list(OPTS)[(i + 2 * j) % len(OPTS)])
+BASE_OPTS = ("bench", "all_bkgd", "no_normal", "mask_no_wt")
+GRID = [(W, H, 1 + 2 * ((i + j) % 2), BASE_OPTS[(i + 2 * j) % len(BASE_OPTS)])
         for i, W in enumerate(W_GRID) for j, H in enumerate(H_GRID)]
+# the per-frame camera table on the same edges: no interior stencil, 1-column and partial last blocks, odd sizes
+GRID += [(W, H, M, "cameras") for W, H, M in ((1, 8, 3), (2, 3, 1), (3, 3, 1), (31, 9, 3), (32, 2, 1), (33, 17, 1),
+                                              (63, 7, 3), (65, 9, 1), (97, 17, 3))]
 
 
 def test_grid_reaches_every_tile_edge():
@@ -593,6 +628,18 @@ def test_grid_reaches_every_tile_edge():
     for opt in OPTS:
         assert any(o == opt and W > 32 and W % 32 and H > 8 and H % 8 for W, H, _, o in GRID), opt
         assert {M for W, H, M, o in GRID if o == opt} == {1, 3}, opt
+    # the camera rows: both tangents differ between frames, non-integer offsets of either sign that carry the principal
+    # point across a block seam in x and in y
+    cams = [(W, H, M) for W, H, M, o in GRID if o == "cameras"]
+    r = camera_rows(3, 97, 17)
+    assert len(set(r[:, 0])) == 3 and len(set(r[:, 1])) == 3
+    assert (r[:, 2:] != np.round(r[:, 2:])).all() and (r[:, 2] > 0).any() and (r[:, 2] < 0).any()
+    x_cross = y_cross = False
+    for W, H, M in cams:
+        r = camera_rows(M, W, H)
+        x_cross |= bool((np.floor(W / 2 / 32) != np.floor((W / 2 + r[:, 2]) / 32)).any() and W > 64)
+        y_cross |= bool((np.floor(H / 2 / 8) != np.floor((H / 2 + r[:, 3]) / 8)).any() and H > 16)
+    assert x_cross and y_cross
 
 
 @pytest.mark.parametrize("W,H,M,opt", GRID)
@@ -602,7 +649,7 @@ def test_loss_and_post_kernels_elementwise(W, H, M, opt, dev):
     _check_reach(name, W, H, r["planted"], r["o"], r["dLa"])
 
 
-@pytest.mark.parametrize("W,H,M,opt", [(1001, 563, 2, "all_bkgd"), (512, 512, 8, "bench")])
+@pytest.mark.parametrize("W,H,M,opt", [(1001, 563, 2, "all_bkgd"), (512, 512, 8, "bench"), (512, 512, 8, "cameras")])
 def test_loss_kernel_large_reductions(W, H, M, opt, dev):
     """Thousands of blocks per frame: the loss terms' 7 fp32 atomics per block, against a bound that counts them."""
     name = f"{W}x{H}"
@@ -615,8 +662,10 @@ def test_loss_kernel_large_reductions(W, H, M, opt, dev):
 @pytest.mark.parametrize("H", [1, 9])
 @pytest.mark.parametrize("M", [1, 3])
 def test_feature_loss_kernel_at_tile_edges(W, H, M, dev):
-    """sr_feature_loss_batch on the same 32 x 8 grid's edges against the float64 model: exact counts, 1e-5 relative
-    per plane and per term, bitwise-deterministic planes."""
+    """sr_feature_loss_batch on the same 32 x 8 grid's edges against its restatement (tests/feature_loss_bounds.py):
+    exact counts, every plane element and per-frame term under the rounding-error bound, untouched channels exactly 0,
+    bitwise-deterministic planes."""
+    from . import feature_loss_bounds as fb
     from .feature_loss_model import feature_losses
     from .test_gpu_feature_loss import _call, _inputs
     F, Cf, gm = 22, 16, 21
@@ -624,14 +673,33 @@ def test_feature_loss_kernel_at_tile_edges(W, H, M, dev):
     w = torch.tensor([1e-2, 7e-3], device=dev)
     terms, counts, grad = _call(feat, target, mask, det, allmap, gm, w)
     n = lambda t: t.cpu().numpy()  # noqa: E731
-    rt, rc, rg = feature_losses(n(feat), n(target), n(mask), n(det), n(allmap[:, 1]), gm, [1e-2, 7e-3])
+    _, rc, _ = feature_losses(n(feat), n(target), n(mask), n(det), n(allmap[:, 1]), gm, [1e-2, 7e-3])
     assert np.array_equal(counts.cpu().numpy(), rc)
-    tt = terms.cpu().numpy().astype(np.float64)
-    for k in range(2):
-        assert np.abs(tt[:, k] - rt[:, k]).max() <= 1e-5 * np.abs(rt[:, k]).max(), (k, tt[:, k], rt[:, k])
-    g = grad.cpu().numpy().astype(np.float64)
-    assert not np.isnan(g).any()
-    for m in range(M):
-        for c in range(F):
-            assert np.abs(g[m, c] - rg[m, c]).max() <= 1e-5 * np.abs(rg[m, c]).max(), (m, c)
+    px = fb.pixel_terms(n(feat), n(target), n(mask), n(det), n(allmap[:, 1]), gm)
+    rep = fb.check(f"{W}x{H} M={M}", n(terms), n(counts), n(grad), px, n(w), gm, F)
+    print(f"\n[feature {W}x{H} M={M}] " + ", ".join(f"{k} {v:.3g}" for k, v in rep.items()))
     assert torch.equal(_call(feat, target, mask, det, allmap, gm, w)[2], grad)
+
+
+@pytest.mark.parametrize("name", list(FEATURE_CONFIGS))
+def test_feature_loss_kernel_planted(name, dev):
+    """The planted configurations of tests/feature_loss_bounds.py: features equal to the target, the Gaussian channel
+    equal to alpha, masks of 0, 0.375 and 1e-30, |d| near 1e-20, on block seams and the image border; Cf = F, Cf = 1,
+    the Gaussian-mask term alone, F = 32, frames undetected and at 0.5, a batch where nothing is positive."""
+    from . import feature_loss_bounds as fb
+    from .test_gpu_feature_loss import _call
+    feat, target, mask, det, alpha, gm, planted = fb.config_inputs(name)
+    M, F, H, W = feat.shape
+    T = lambda x: None if x is None else torch.from_numpy(np.ascontiguousarray(x)).to(dev)  # noqa: E731
+    allmap = torch.rand((M, 8, H, W), device=dev)
+    allmap[:, 1] = T(alpha)
+    w = T(fb.WEIGHTS)
+    terms, counts, grad = _call(T(feat), T(target), T(mask), T(det), allmap, gm, w)
+    n = lambda t: t.cpu().numpy()  # noqa: E731
+    px = fb.pixel_terms(feat, target, mask, det, alpha, gm)
+    rep = fb.check(name, n(terms), n(counts), n(grad), px, fb.WEIGHTS, gm, F)
+    nk = sum(int(k.sum()) for k in px["knife"].values())
+    print(f"\n[feature {name}] knife {nk} of {M * H * W} px; " + ", ".join(f"{k} {v:.3g}" for k, v in rep.items()))
+    assert nk <= 4
+    if fb.CONFIGS[name].get("empty"):
+        assert int(counts.abs().sum()) == 0 and float(terms.abs().max()) == 0 and float(grad.abs().max()) == 0
