@@ -45,11 +45,12 @@ SR_API int sr_grad_norm_flat(int32_t n_groups, const int64_t* begin, const float
 
 /*
  * One Adam step (torch.optim.Adam: amsgrad off, weight_decay 0) over params / exp_avg / exp_avg_sq, DEVICE float.
- * lr: DEVICE float [n_groups].  step: DEVICE int64, incremented first; the step runs with t = the new value and the
- * bias corrections (float)(1 - pow(beta1, t)) and (float)sqrt(1 - pow(beta2, t)) evaluated in double, as sr_adam_flat
- * does on the host.  clip_coef: DEVICE float, or NULL for 1.  The step count advances also when the buffer is empty.
+ * lr: DEVICE float [n_groups].  step: DEVICE int64, incremented first; the step runs with t = the new value, the step
+ * size (float)(lr / (1 - pow(beta1, t))) and the bias correction (float)sqrt(1 - pow(beta2, t)) evaluated in double from
+ * the double betas, as sr_adam_flat does on the host and torch.optim.Adam does in Python.  clip_coef: DEVICE float, or
+ * NULL for 1.  The step count advances also when the buffer is empty.
  */
-SR_API int sr_adam_flat_state(int32_t n_groups, const int64_t* begin, const float* lr, float beta1, float beta2, float eps,
+SR_API int sr_adam_flat_state(int32_t n_groups, const int64_t* begin, const float* lr, double beta1, double beta2, float eps,
                               int64_t* step, float grad_scale, const float* clip_coef, float* params, const float* grads,
                               float* exp_avg, float* exp_avg_sq, void* stream);
 

@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define SR_ABI_VERSION 11
+#define SR_ABI_VERSION 12
 
 #if defined(__GNUC__)
 #define SR_API __attribute__((visibility("default")))
@@ -376,8 +376,10 @@ SR_API int sr_feature_rows_backward(int32_t P, int32_t M, int32_t B, int32_t Cf,
  * Optimizer-side kernels over the FLAT surfel parameter buffer (SURVEY.md section 8(f) row N4): the Adam step of every
  * surfel parameter group in one launch (lab4d/engine/trainer.py:243-253,585-586; torch.optim.Adam semantics), and
  * densify / prune as one gather into new buffers (gs/scene/gaussian_model.py:291-446).  See csrc/optim.cu.
+ * sr_adam_flat takes the betas in double, as torch.optim.Adam holds them, and forms its constants as torch does:
+ * (float)(1 - beta), (float)beta2, (float)(lr / (1 - beta1^t)) and (float)sqrt(1 - beta2^t), the powers in double.
  */
-SR_API int sr_adam_flat(int32_t n_groups, const int64_t* begin, const float* lr, float beta1, float beta2, float eps,
+SR_API int sr_adam_flat(int32_t n_groups, const int64_t* begin, const float* lr, double beta1, double beta2, float eps,
                         int64_t step, float grad_scale, float* params, const float* grads, float* exp_avg, float* exp_avg_sq,
                         void* stream);
 SR_API int sr_surfel_compact(int32_t n_groups, const int32_t* width, const int64_t* old_begin, const int64_t* new_begin,

@@ -91,6 +91,13 @@ def _calls():
     return lib, calls, keep
 
 
+def test_adam_betas_are_double(built):
+    """Both Adam entry points take torch's double betas (their 1 - beta and bias corrections are formed in double)."""
+    from vidu4d_b200 import _capi
+    for table, name in ((_capi.PROTOTYPES, "sr_adam_flat"), (_capi.OPTIM_PROTOTYPES, "sr_adam_flat_state")):
+        assert table[name][1][3:5] == [C.c_double, C.c_double], name
+
+
 def test_covers_every_int_entry_point(built):
     from vidu4d_b200 import _capi
     _, calls, _ = _calls()

@@ -29,8 +29,9 @@ def test_frame_cameras_layout_matches_c(built, tmp_path):
     assert bit == _capi.SR_FRAME_CAMERAS
 
 
-def test_camera_header_matches_ctypes_table(built):
-    """include/surfel_camera.h <-> libsurfel_raster.so <-> _capi.CAMERA_PROTOTYPES, and the ABI version."""
+def test_camera_header_and_abi_version_match_library_and_binding(built):
+    """include/surfel_camera.h <-> libsurfel_raster.so <-> _capi.CAMERA_PROTOTYPES, and the ABI version: the
+    SR_ABI_VERSION surfel_raster.h defines is the library's and the binding's."""
     import re
     from vidu4d_b200 import _capi
     lib = _capi.load()
@@ -42,7 +43,8 @@ def test_camera_header_matches_ctypes_table(built):
         assert hasattr(lib, name)
         want = [C.c_void_p if "*" in p else kinds[p.replace("const", "").split()[0]] for p in params.split(",")]
         assert _capi.CAMERA_PROTOTYPES[name][1] == want, name
-    assert lib.sr_abi_version() == _capi.ABI_VERSION == 11
+    raster = open(os.path.join(ROOT, "include", "surfel_raster.h")).read()
+    assert lib.sr_abi_version() == _capi.ABI_VERSION == int(re.search(r"#define SR_ABI_VERSION (\d+)", raster).group(1))
 
 
 def test_flag_with_null_table_is_einval_before_any_cuda_call(built):

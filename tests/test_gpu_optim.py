@@ -158,7 +158,11 @@ def test_bias_corrections_equal_host_formula_to_step_100000(dev):
 
 def test_clip_and_step_match_torch_clip_and_adam(dev):
     """clip_grad_norm_(5.0, extras) + step() against torch.nn.utils.clip_grad_norm_ + torch.optim.Adam (seven groups
-    plus the extras, eps 1e-15) over ten steps, clipping on alternate steps."""
+    plus the extras, eps 1e-15) over ten steps, clipping on alternate steps, each step from torch's parameters and
+    moments: the surfel moments bit for bit and each surfel parameter within the rounding of the fp32 rate
+    (tests/optim_model.py rate_rounding_ok).  Where the totals differ in their last bits, so that torch's coefficient is
+    not the kernel's, torch's Adam gets the kernel's coefficient."""
+    from . import optim_model as om
     m = _model(5003, dev, seed=4)
     gen = torch.Generator(device=dev).manual_seed(2)
     extras = [torch.nn.Parameter(torch.rand(3, device=dev, generator=gen)),          # a learnable background
@@ -173,8 +177,16 @@ def test_clip_and_step_match_torch_clip_and_adam(dev):
         scale = 1.0 if step % 2 == 0 else 1e-4
         m.zero_grad_flat()
         _fill_grads(m, seed=20 + step, scale=scale)
+        with torch.no_grad():
+            for p, r in zip(m.flat_params(), ref):
+                p.copy_(r)
+            if step:
+                m.exp_avg.copy_(torch.cat([opt_ref.state[r]["exp_avg"].flatten() for r in ref]))
+                m.exp_avg_sq.copy_(torch.cat([opt_ref.state[r]["exp_avg_sq"].flatten() for r in ref]))
+        before = [r.detach().clone() for r in ref]
         for p, r in zip(m.flat_params(), ref):
             r.grad = p.grad.detach().clone()
+        raw = [r.grad.clone() for r in ref]
         for i, (p, r) in enumerate(zip(extras, ref_x)):
             if i == 2:
                 p.grad = r.grad = None
@@ -185,10 +197,18 @@ def test_clip_and_step_match_torch_clip_and_adam(dev):
         total_ref = torch.nn.utils.clip_grad_norm_(ref + ref_x, 5.0)
         assert abs(float(total) - float(total_ref)) <= 1e-6 * float(total_ref), step
         assert (float(m.clip_coef) < 1.0) == (step % 2 == 0), (step, float(total))
+        if not bool(torch.clamp(5.0 / (total_ref + 1e-6), max=1.0) == m.clip_coef):
+            for r, g0 in zip(ref, raw):
+                r.grad = g0 * m.clip_coef
         m.step()
         opt_x.step()
         opt_ref.step()
-        for p, r, n in zip(m.flat_params() + extras, ref + ref_x, NAMES + ("bkgd", "x", "no_grad")):
+        off, tot = m._offsets(m.P)
+        for p, r, n, b, a, e in zip(m.flat_params(), ref, NAMES, before, off, off[1:] + [tot]):
+            assert torch.equal(m.exp_avg[a:e], opt_ref.state[r]["exp_avg"].flatten()), (step, n)
+            assert torch.equal(m.exp_avg_sq[a:e], opt_ref.state[r]["exp_avg_sq"].flatten()), (step, n)
+            assert om.rate_rounding_ok(p.detach().cpu().numpy(), r.detach().cpu().numpy(), b.cpu().numpy()).all(), (step, n)
+        for p, r, n in zip(extras, ref_x, ("bkgd", "x", "no_grad")):
             p, r = p.detach(), r.detach()
             assert float((p - r).abs().max()) <= 1e-6 * float(r.abs().max()) + 1e-9, (step, n)
     assert int(m.device_step) == 10

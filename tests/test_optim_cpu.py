@@ -1,7 +1,7 @@
 """CPU: include/surfel_optim.h given the checks tests/test_host_cpu.py and tests/test_abi_errors_cpu.py give
 surfel_raster.h (header <-> library <-> binding, each bad argument's own message, SR_ECUDA without a device); the clip
 model (tests/optim_model.py) against torch.nn.utils.clip_grad_norm_; and the margin that lets the device's float64 pow
-reproduce the host's float32 bias corrections."""
+reproduce the host's fp32 Adam scalars."""
 import ctypes as C
 import math
 import os
@@ -176,18 +176,24 @@ def test_clip_model_matches_torch(scale):
 
 
 def test_bias_corrections_have_margin_for_device_pow():
-    """For every step 1..100 000 at Adam's default betas, every float64 value within 4 ulp of the host's pow(beta, t)
-    gives the same float32 bias correction.  The device's pow is within 2 ulp, so it reproduces the host's scalars."""
-    for t in range(1, 100001):
-        for beta, sq in ((0.9, False), (0.999, True)):
-            b = float(np.float32(beta))
-            p = math.pow(b, t)
-            lo = hi = p
-            out = {np.float32(math.sqrt(1.0 - p) if sq else 1.0 - p)}
-            for _ in range(4):
-                lo, hi = math.nextafter(lo, 0.0), math.nextafter(hi, 1.0)
-                for c in (lo, hi):
-                    out.add(np.float32(math.sqrt(1.0 - c) if sq else 1.0 - c))
-            assert len(out) == 1, (t, beta)
-    assert om.bias_corrections(0.9, 0.999, 1) == (np.float32(1 - float(np.float32(0.9))),
-                                                  np.float32(math.sqrt(1 - float(np.float32(0.999)))))
+    """For every step 2..100 000 at Adam's default betas (torch's doubles), every float64 value within 4 ulp of the host's
+    pow(beta, t) gives the same fp32 scalars: sqrt(1 - beta2^t), and lr / (1 - beta1^t) for each of the Stage-3 rates
+    as fp32 values.  The device's pow is within 2 ulp, so sr_adam_flat_state reproduces sr_adam_flat's scalars.  Step 1
+    takes beta itself, no pow, on both sides: there 2.5e-3 / (1 - 0.9) and 5e-2 / (1 - 0.9) round differently 1 ulp
+    below 0.9."""
+    t = np.arange(2, 100001)
+    lrs = np.float32([1.6e-4, 2.5e-3, 2.5e-3 / 20.0, 5e-2, 5e-3, 1e-3]).astype(np.float64)
+    for beta in (0.9, 0.999):
+        p = np.array([math.pow(beta, float(k)) for k in t])
+        outs = []
+        for shift in range(-4, 5):
+            c = p.copy()
+            for _ in range(abs(shift)):
+                c = np.nextafter(c, 1.0 if shift > 0 else 0.0)
+            if beta == 0.999:
+                outs.append(np.sqrt(1.0 - c).astype(np.float32)[None])
+            else:
+                outs.append((lrs[:, None] / (1.0 - c)[None]).astype(np.float32))
+        assert all(np.array_equal(o, outs[4]) for o in outs), beta
+    bc1, sqrt_bc2 = om.bias_corrections(0.9, 0.999, 1)
+    assert bc1 == 1.0 - 0.9 and sqrt_bc2 == np.float32(math.sqrt(1.0 - 0.999))

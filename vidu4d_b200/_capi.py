@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libsurfel_raster.so")
 
-ABI_VERSION = 11
+ABI_VERSION = 12
 SR_STATUS_OVERFLOW = 1
 SR_STATUS_PREFILTER = 4
 SR_BATCH_SUM_SHARED = 1
@@ -90,7 +90,7 @@ PROTOTYPES = {
     "sr_cycle_loss_backward": (C.c_int, [_i32] * 3 + [_p] * 17),
     "sr_feature_rows_forward": (C.c_int, [_i32] * 4 + [_p] * 14),
     "sr_feature_rows_backward": (C.c_int, [_i32] * 4 + [_p] * 19),
-    "sr_adam_flat": (C.c_int, [_i32, _p, _p, _f32, _f32, _f32, _i64, _f32] + [_p] * 5),
+    "sr_adam_flat": (C.c_int, [_i32, _p, _p, _f64, _f64, _f32, _i64, _f32] + [_p] * 5),
     "sr_surfel_compact": (C.c_int, [_i32, _p, _p, _p, _i32, _i32, _i32] + [_p] * 12),
     "sr_knn_cells": (C.c_int64, [_i32, _p, _p, _p, _p]),
     "sr_knn_mean_dist2": (C.c_int, [_i32] + [_p] * 6),
@@ -118,7 +118,7 @@ SSIM_SYMBOLS = tuple(SSIM_PROTOTYPES)
 OPTIM_PROTOTYPES = {
     "sr_grad_norm_scratch_bytes": (C.c_int64, [_i32]),
     "sr_grad_norm_flat": (C.c_int, [_i32, _p, _p, _f32, _p, _i32, _f32] + [_p] * 4 + [_i64, _p]),
-    "sr_adam_flat_state": (C.c_int, [_i32, _p, _p, _f32, _f32, _f32, _p, _f32] + [_p] * 6),
+    "sr_adam_flat_state": (C.c_int, [_i32, _p, _p, _f64, _f64, _f32, _p, _f32] + [_p] * 6),
     "sr_densify_stats": (C.c_int, [_i32, _i32, _p, _p, _f32] + [_p] * 4),
 }
 OPTIM_SYMBOLS = tuple(OPTIM_PROTOTYPES)

@@ -6,6 +6,8 @@
 // points are binned into a uniform grid (counting sort: count -> scan -> scatter) and every point searches growing cubic
 // shells of cells until its third-nearest distance is provably final.  Exact 3-NN, same result: (d0 + d1 + d2) / 3 with
 // the three smallest squared distances to OTHER points (duplicates count with distance 0, as in the reference).
+#include <cfloat>
+
 #include "common.cuh"
 
 namespace {
@@ -45,7 +47,9 @@ __global__ void knn_query_kernel(const Grid g, int P, const float* __restrict__ 
     if (i >= P) return;
     const float x = pts[3 * (size_t)i], y = pts[3 * (size_t)i + 1], z = pts[3 * (size_t)i + 2];
     const int3 c = cell_of(g, x, y, z);
-    float best[3] = {3.4e38f, 3.4e38f, 3.4e38f};
+    // FLT_MAX, as simple_knn.cu: with fewer than three other points the mean is (d0 + d1 + FLT_MAX) / 3 (3 points) or
+    // Inf (1 or 2 points)
+    float best[3] = {FLT_MAX, FLT_MAX, FLT_MAX};
     const int rmax = max(g.nx, max(g.ny, g.nz));
     for (int r = 0; r <= rmax; r++) {
         // cells at Chebyshev distance exactly r from the point's own cell

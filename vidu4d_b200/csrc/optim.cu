@@ -10,7 +10,11 @@
 //     densification_postfix, densify_and_split, densify_and_clone, prune_points) becomes ONE gather kernel that writes the
 //     new parameter, exp_avg and exp_avg_sq buffers from a source-index list, instead of ~60 torch cat / index /
 //     nn.Parameter re-creations per call.
-// Semantics are torch.optim.Adam's (amsgrad off, no weight decay) and the reference's row-wise copy rules, bit for bit.
+// Semantics are torch.optim.Adam's (amsgrad off, no weight decay; its default foreach path on CUDA) and the reference's
+// row-wise copy rules.  The Adam constants are formed as torch forms them from its double betas and rates: 1 - beta in
+// double rounded once, beta^t and lr / (1 - beta1^t) in double; every element operation is torch's, rounded where torch
+// rounds.  Both moments equal torch's bit for bit; so do the parameters when the rates are fp32 values.  Both entry
+// points take the rates as fp32, so a rate that is not one is rounded first (a step size within 3 u of torch's).
 //
 // The per-step optimizer state can also live on the device (include/surfel_optim.h): a group-wise float64 sum of squares
 // of the gradient buffer gives torch.nn.utils.clip_grad_norm_'s coefficient in a one-CTA finish, and the Adam pass reads
@@ -28,7 +32,7 @@ constexpr int MAXG = 8;
 struct AdamGroups {
     int n;
     long long begin[MAXG + 1];     // element offsets of the groups inside the flat buffer; begin[n] = total
-    float lr[MAXG];
+    float step_size[MAXG];         // sr_adam_flat: (float)(lr / (1 - beta1^t)), formed in double on the host
 };
 
 // sr_adam_flat_state's device state; unused (all NULL) in sr_adam_flat's instantiation
@@ -38,31 +42,39 @@ struct AdamDeviceState {
     const float* coef;             // clip coefficient, or NULL for 1
 };
 
-// Bias corrections exactly as sr_adam_flat forms them on the host
-__device__ __forceinline__ void adam_bias_corrections(float beta1, float beta2, long long step, float& bc1, float& sqrt_bc2) {
-    bc1 = (float)(1.0 - pow((double)beta1, (double)step));
-    sqrt_bc2 = (float)sqrt(1.0 - pow((double)beta2, (double)step));
+// torch/optim/adam.py _multi_tensor_adam's scalars, all in double: bias_correction1 = 1 - beta1 ** t,
+// step_size = lr / bias_correction1, bias_correction2_sqrt = (1 - beta2 ** t) ** 0.5; the kernels get them rounded to fp32
+// as torch's foreach ops do.  beta^1 is beta exactly, without a pow that the device library may round differently from
+// the host's: at t = 1 two of the Stage-3 rates sit within an ulp of a rounding boundary of lr / (1 - beta1)
+__host__ __device__ __forceinline__ double adam_pow(double beta, long long step) { return step == 1 ? beta : pow(beta, (double)step); }
+__host__ __device__ __forceinline__ double adam_bc1(double beta1, long long step) { return 1.0 - adam_pow(beta1, step); }
+__host__ __device__ __forceinline__ float adam_sqrt_bc2(double beta2, long long step) {
+    return (float)sqrt(1.0 - adam_pow(beta2, step));
 }
 
 // DEVICE_STATE = false: sr_adam_flat, every scalar a launch argument.  DEVICE_STATE = true: sr_adam_flat_state, the step,
-// rates and clip coefficient read from S (bc1 / sqrt_bc2 / G.lr are then ignored).
+// rates and clip coefficient read from S (sqrt_bc2 / G.step_size are then ignored).
 template <bool DEVICE_STATE>
 __global__ void __launch_bounds__(256)
 adam_flat_kernel(const AdamGroups G, float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                 float* __restrict__ v, float beta1, float beta2, float eps, float bc1, float sqrt_bc2, float grad_scale,
+                 float* __restrict__ v, double beta1, double beta2, float eps, float sqrt_bc2, float grad_scale,
                  const AdamDeviceState S) {
-    float lrs[MAXG], coef = 1.0f;
+    float steps[MAXG], coef = 1.0f;
     if constexpr (DEVICE_STATE) {
-        // one thread per CTA forms the scalars (two float64 pow), the rest read them from shared memory
-        __shared__ float sc[2 + MAXG + 1];
-        if (threadIdx.x == 0) adam_bias_corrections(beta1, beta2, *S.step, sc[0], sc[1]);
-        if (threadIdx.x < MAXG) sc[2 + threadIdx.x] = threadIdx.x < G.n ? S.lr[threadIdx.x] : 0.0f;
-        if (threadIdx.x == MAXG) sc[2 + MAXG] = S.coef ? *S.coef : 1.0f;
+        // thread q < MAXG forms group q's step size, thread MAXG the second bias correction (float64 pow each); the rest
+        // read them from shared memory
+        __shared__ float sc[MAXG + 2];
+        const long long t = *S.step;
+        if (threadIdx.x < MAXG) sc[threadIdx.x] = threadIdx.x < G.n ? (float)((double)S.lr[threadIdx.x] / adam_bc1(beta1, t)) : 0.0f;
+        if (threadIdx.x == MAXG) sc[MAXG] = adam_sqrt_bc2(beta2, t);
+        if (threadIdx.x == MAXG + 1) sc[MAXG + 1] = S.coef ? *S.coef : 1.0f;
         __syncthreads();
-        bc1 = sc[0]; sqrt_bc2 = sc[1]; coef = sc[2 + MAXG];
+        sqrt_bc2 = sc[MAXG]; coef = sc[MAXG + 1];
 #pragma unroll
-        for (int q = 0; q < MAXG; q++) lrs[q] = sc[2 + q];
+        for (int q = 0; q < MAXG; q++) steps[q] = sc[q];
     }
+    // torch's foreach scalars are fp32 (opmath) values: 1 - beta rounded once from double, beta2 rounded
+    const float c1 = (float)(1.0 - beta1), b2 = (float)beta2, c2 = (float)(1.0 - beta2);
     const long long total = G.begin[G.n];
     for (long long i = (long long)blockIdx.x * 1024 + threadIdx.x * 4; i < total; i += (long long)gridDim.x * 1024) {
         // four consecutive elements; a group boundary can fall inside them, so the rate is looked up per element
@@ -81,17 +93,22 @@ adam_flat_kernel(const AdamGroups G, float* __restrict__ p, const float* __restr
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             const long long e = i + k;
-            float lr = DEVICE_STATE ? lrs[0] : G.lr[0];
+            float step = DEVICE_STATE ? steps[0] : G.step_size[0];
 #pragma unroll
-            for (int q = 1; q < MAXG; q++) if (q < G.n && e >= G.begin[q]) lr = DEVICE_STATE ? lrs[q] : G.lr[q];
+            for (int q = 1; q < MAXG; q++) if (q < G.n && e >= G.begin[q]) step = DEVICE_STATE ? steps[q] : G.step_size[q];
             // (g * grad_scale) * coef, each product rounded: the averaging, then clip_grad_norm_'s in-place multiply
-            const float gr = DEVICE_STATE ? __fmul_rn(G4[k] * grad_scale, coef) : G4[k] * grad_scale;
-            // torch/optim/adam.py _single_tensor_adam: exp_avg.lerp_(grad, 1 - beta1); exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2);
-            // denom = exp_avg_sq.sqrt() / sqrt(bias_correction2) + eps; param.addcdiv_(exp_avg, denom, value=-lr / bias_correction1)
-            M4[k] = M4[k] + (gr - M4[k]) * (1.0f - beta1);
-            V4[k] = V4[k] * beta2 + gr * gr * (1.0f - beta2);
-            const float denom = sqrtf(V4[k]) / sqrt_bc2 + eps;
-            P4[k] = P4[k] - (lr / bc1) * (M4[k] / denom);
+            const float gr = __fmul_rn(__fmul_rn(G4[k], grad_scale), coef);
+            // torch's _multi_tensor_adam, one foreach op after another, each rounded to fp32:
+            //   exp_avg.lerp_(grad, 1 - beta1)              ATen lerp: self + w (end - self) for |w| < 0.5, else
+            //                                               end - (end - self)(1 - w), each one FMA
+            //   exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2)        addcmul: fma(value, grad * grad, self)
+            //   denom = exp_avg_sq.sqrt() / bias_correction2_sqrt + eps
+            //   param.addcdiv_(exp_avg, denom, -step_size)                    addcdiv: fma(value, exp_avg / denom, param)
+            const float d = __fsub_rn(gr, M4[k]);
+            M4[k] = c1 < 0.5f ? __fmaf_rn(c1, d, M4[k]) : __fmaf_rn(-d, __fsub_rn(1.0f, c1), gr);
+            V4[k] = __fmaf_rn(c2, __fmul_rn(gr, gr), __fmul_rn(V4[k], b2));
+            const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(V4[k]), sqrt_bc2), eps);
+            P4[k] = __fmaf_rn(-step, __fdiv_rn(M4[k], denom), P4[k]);
         }
         if (vec) {
             *reinterpret_cast<float4*>(p + i) = pp; *reinterpret_cast<float4*>(m + i) = mm; *reinterpret_cast<float4*>(v + i) = vv;
@@ -291,10 +308,10 @@ extern "C" {
 
 /* One Adam step over a flat buffer of `n_groups` back-to-back parameter groups (group g = elements [begin[g], begin[g+1])),
  * each with its own learning rate; torch.optim.Adam semantics (amsgrad off, weight_decay 0).  `step` is the 1-based step
- * count (bias correction); grad_scale multiplies every gradient first (1 / (frames x ranks) averaging).  All device
+ * count (bias correction); the betas are torch's double values; grad_scale multiplies every gradient first (1 / (frames x ranks) averaging).  All device
  * pointers, 16-byte aligned. */
 SR_API int sr_adam_flat(int32_t n_groups, const int64_t* begin /* host, n_groups + 1 */, const float* lr /* host, n_groups */,
-                        float beta1, float beta2, float eps, int64_t step, float grad_scale, float* params, const float* grads,
+                        double beta1, double beta2, float eps, int64_t step, float grad_scale, float* params, const float* grads,
                         float* exp_avg, float* exp_avg_sq, void* stream_) {
     if (n_groups < 1 || n_groups > MAXG) return sr_fail(SR_EINVAL, "sr_adam_flat: n_groups must be in [1, %d], got %d", MAXG, n_groups);
     if (!begin || !lr || !params || !grads || !exp_avg || !exp_avg_sq) return sr_fail(SR_EINVAL, "sr_adam_flat: a required pointer is NULL");
@@ -304,17 +321,16 @@ SR_API int sr_adam_flat(int32_t n_groups, const int64_t* begin /* host, n_groups
     AdamGroups G{};
     G.n = n_groups;
     for (int i = 0; i <= n_groups; i++) G.begin[i] = begin[i];
-    for (int i = 0; i < n_groups; i++) G.lr[i] = lr[i];
+    const double bc1 = adam_bc1(beta1, step);
+    for (int i = 0; i < n_groups; i++) G.step_size[i] = (float)((double)lr[i] / bc1);
     const long long total = begin[n_groups];
     if (total <= 0) return 0;
-    const float bc1 = (float)(1.0 - pow((double)beta1, (double)step));
-    const float sqrt_bc2 = (float)sqrt(1.0 - pow((double)beta2, (double)step));
     cudaStream_t s = (cudaStream_t)stream_;
     const long long blocks = (total + 1023) / 1024;
     ProfileScope ps("adam_flat", s);
     // grid-stride: at most 16 CTAs per SM of an H100 SXM (132 SMs)
     adam_flat_kernel<false><<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, s>>>(
-        G, params, grads, exp_avg, exp_avg_sq, beta1, beta2, eps, bc1, sqrt_bc2, grad_scale, AdamDeviceState{});
+        G, params, grads, exp_avg, exp_avg_sq, beta1, beta2, eps, adam_sqrt_bc2(beta2, step), grad_scale, AdamDeviceState{});
     return sr_launched(1, "sr_adam_flat");
 }
 
@@ -354,7 +370,7 @@ SR_API int sr_grad_norm_flat(int32_t n_groups, const int64_t* begin, const float
     return sr_launched(parts > 0 ? 2 : 1, "sr_grad_norm_flat");
 }
 
-SR_API int sr_adam_flat_state(int32_t n_groups, const int64_t* begin, const float* lr, float beta1, float beta2, float eps,
+SR_API int sr_adam_flat_state(int32_t n_groups, const int64_t* begin, const float* lr, double beta1, double beta2, float eps,
                               int64_t* step, float grad_scale, const float* clip_coef, float* params, const float* grads,
                               float* exp_avg, float* exp_avg_sq, void* stream_) {
     int rc = check_groups("sr_adam_flat_state", n_groups, begin);
@@ -377,7 +393,7 @@ SR_API int sr_adam_flat_state(int32_t n_groups, const int64_t* begin, const floa
     const long long blocks = (total + 1023) / 1024;
     ProfileScope ps("adam_flat_state", s);
     adam_flat_kernel<true><<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, s>>>(
-        G, params, grads, exp_avg, exp_avg_sq, beta1, beta2, eps, 1.0f, 1.0f, grad_scale,
+        G, params, grads, exp_avg, exp_avg_sq, beta1, beta2, eps, 1.0f, grad_scale,
         AdamDeviceState{lr, reinterpret_cast<const long long*>(step), clip_coef});
     return sr_launched(2, "sr_adam_flat_state");
 }
