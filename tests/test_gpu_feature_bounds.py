@@ -220,15 +220,16 @@ def _groups(feat, bgf):
     return [(np.ascontiguousarray(fp[:, 3 * k:3 * k + 3]), bp[3 * k:3 * k + 3].copy(), min(3, F - 3 * k)) for k in range(n)]
 
 
-def _oracle_fwd(name, dec, inp, means3D, feat, bgf, color, allmap, dev=None, s=None):
+def _oracle_fwd(name, dec, inp, means3D, feat, bgf, color, allmap, dev=None, s=None, off=None):
     """The colour oracle and one oracle per feature group, composited from this frame's GPU records; checks n_contrib,
     the colour/allmap planes and every feature plane within its bound outside the knife mask, every group's mask equal to
-    the colour's, and (given the scene s) every feature plane bit for bit a colour render of the same values."""
+    the colour's, and (given the scene s) every feature plane bit for bit a colour render of the same values.  off: the
+    principal-point offsets of the frame's camera-table row, for the records' check."""
     P, W, H, deg, pre = [int(v) for v in inp["meta"]]
     tan = (float(inp["tanfov"][0]), float(inp["tanfov"][1]))
     geo = (means3D, inp["opacities"], inp["scales"], inp["rotations"])
     st, ext = _oracle_frame(dec, P, W, H, *geo, None if pre else inp["shs"], inp["colors_precomp"] if pre else None, deg,
-                            inp["bg"], inp["viewmatrix"], inp["projmatrix"], inp["campos"], tan, name=name)
+                            inp["bg"], inp["viewmatrix"], inp["projmatrix"], inp["campos"], tan, off=off, name=name)
     fwd = _check_forward(name, st, ext, _np(color[:3]), _np(allmap), dec, W, H)
     ok = ~ext["knife"]
     planes = _np(color[3:])
@@ -236,7 +237,7 @@ def _oracle_fwd(name, dec, inp, means3D, feat, bgf, color, allmap, dev=None, s=N
     for k, (cols, b3, n) in enumerate(_groups(feat, bgf)):
         # the records hold the colour forward's rgb, not the group's: their geometry only
         sg, eg = _oracle_frame(dec, P, W, H, *geo, None, cols, 0, b3, inp["viewmatrix"], inp["projmatrix"], inp["campos"], tan,
-                               records=None, name=f"{name} group {k}")
+                               off=off, records=None, name=f"{name} group {k}")
         assert np.array_equal(eg["knife"], ext["knife"]), (name, "group", k, "knife mask differs from the colour's")
         for c in range(n):
             err = np.abs(planes[3 * k + c].astype(np.float64) - sg.color[c])

@@ -75,7 +75,11 @@ def _abs(v, bound):
     return _E(v, np.asarray(bound, np.float64) / U)
 
 
-def _run(name, W, H, M, with_bk, with_vis, dev, monkeypatch):
+def _run(name, W, H, M, with_bk, with_vis, dev, monkeypatch, hook=None, per_frame=False):
+    """hook(args, kwargs, out, pc): called inside the spied rasterizer backward, before the real one, with its arguments,
+    render_loss_batch's outputs and the surfel cloud; per_frame: Stage 3's per-frame positions and orientations (the
+    cloud's own, moved per frame), as means3D / rotations overrides.  Returns (out, dL/dallmap, the spied call: its
+    arguments and the real backward's gradients)."""
     from vidu4d_b200 import rasterizer as RZ
     from vidu4d_b200.renderer import PipelineParams, render_loss_batch
     from dataclasses import replace
@@ -100,19 +104,30 @@ def _run(name, W, H, M, with_bk, with_vis, dev, monkeypatch):
     wf = torch.tensor([1e-2, 7e-3], device=dev)
     wm = torch.tensor([0.1], device=dev)
     bk = torch.tensor([0.3, 0.5, 0.2], device=dev, requires_grad=True) if with_bk else None
-    seen = []
+    seen, spied, held = [], {}, {}
     real = RZ._C.rasterize_gaussians_backward_batch
+    pc = mk()
+    over = {}
+    if per_frame:
+        f_ = torch.arange(M, device=dev, dtype=torch.float32)[:, None, None]
+        dx = torch.randn((1, P, 3), device=dev, generator=g) * 0.002
+        dq = torch.randn((1, P, 4), device=dev, generator=g) * 0.02
+        over = dict(means3D=pc.get_xyz[None] + f_ * dx, rotations=torch.nn.functional.normalize(pc._rotation[None] + f_ * dq, dim=-1))
 
     def spy(*a, **k):
         seen.append((a[11].clone(), a[12].clone(), k["dL_dout_features"].clone(), k.get("grad_scale"),
                      k.get("features_grad_scale")))
-        return real(*a, **k)
+        if hook is not None:
+            hook(a, k, held["out"], pc)
+        spied.update(args=a, kwargs=k, grads=real(*a, **k))
+        return spied["grads"]
     monkeypatch.setattr(RZ._C, "rasterize_gaussians_backward_batch", staticmethod(spy))
     try:
-        out = render_loss_batch(bc, mk(), PipelineParams(), torch.zeros(3, device=dev), rgb, vis2d=vis, mask_gt=mask,
+        out = render_loss_batch(bc, pc, PipelineParams(), torch.zeros(3, device=dev), rgb, vis2d=vis, mask_gt=mask,
                                 learnable_bkgd=bk, w_rgb=W_RGB, lambda_normal=LAM_N, lambda_dist=LAM_D, features=feat,
                                 feature_target=ftgt, is_detected=det, gauss_mask_channel=GM, feature_loss_weights=wf,
-                                w_ssim=W_SSIM, mask_loss_weight=wm)
+                                w_ssim=W_SSIM, mask_loss_weight=wm, **over)
+        held["out"] = out
         (float(UP) * out["loss"] + float(CALLER) * out["features"][:, 16:21].square().mean()).backward()
         torch.cuda.synchronize()
     finally:
@@ -235,13 +250,14 @@ def _run(name, W, H, M, with_bk, with_vis, dev, monkeypatch):
           f"{knives['stencil']} feature {knives['feature']} of {M * W * H} px; "
           + ", ".join(f"{k} {v:.3g}" for k, v in report.items()))
     assert sum(knives.values()) <= 8 + 1e-3 * M * W * H, (name, knives)
-    return out, dLa
+    spied.update(feat=feat, over=over, pc=pc)
+    return out, dLa, spied
 
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_loss_pass_every_term_elementwise(name, dev, monkeypatch):
     W, H, M, with_bk, with_vis = CASES[name]
-    out, dLa = _run(name, W, H, M, with_bk, with_vis, dev, monkeypatch)
+    out, dLa, _ = _run(name, W, H, M, with_bk, with_vis, dev, monkeypatch)
     assert float(out["mask_terms"].abs().sum()) > 0 and float(out["ssim_terms"].abs().min()) > 0
     if M > 1:                   # the undetected frame: no feature count, no silhouette count
         assert int(out["feature_counts"][1, 0]) == 0 and int(out["mask_counts"][1]) == 0
