@@ -1,0 +1,59 @@
+/*
+ * surfel_render.h -- forward-only rendering of many frames: a trained sequence rendered for viewing or evaluation.
+ *
+ * The same library as surfel_raster.h (libsurfel_raster.so), the same SR_API visibility, SR_E* codes and
+ * sr_last_error() message path.  It lives in its own header because surfel_raster.h is the drop-in boundary of the
+ * reference rasterizer, whose prototypes stay as they are.
+ *
+ * sr_forward keeps, per frame, what its backward reads: the per-surfel gradient accumulator, the per-(stage, pixel)
+ * contribution masks, final_T, n_contrib and each sub-tile's deepest contributor; with F > 0 feature channels a second
+ * pass re-walks the recorded contributors.  sr_render_forward writes the same outputs, bit for bit, keeps none of that
+ * state, and composites the F feature channels inside the colour's walk.  Its scratch is one arena per frame, smaller
+ * than sr_forward's three buffers by exactly those arrays.
+ */
+#ifndef SURFEL_RENDER_H_
+#define SURFEL_RENDER_H_
+
+#include "surfel_raster.h"
+
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+/* Bytes of one frame's forward-only arena: sr_geom_bytes(P) + sr_binning_bytes(capacity, W, H) + sr_image_bytes(W, H)
+ * less the arrays only a backward reads (the geometry's gradient accumulator, the binning's contribution masks, the
+ * image's final_T, n_contrib and sub_last).  An M-frame call takes M of them, consecutively. */
+SR_API size_t sr_render_bytes(int32_t P, int64_t capacity, int32_t width, int32_t height);
+
+/* sr_forward's arguments and outputs (an sr_frame, or an sr_frame_cameras of surfel_camera.h; an sr_batch with per-input
+ * strides; F in 0..32 with a background of 3 or 3+F values), with one arena of M * sr_render_bytes(P, capacity, W, H)
+ * bytes, 16-byte aligned, instead of the three scratch buffers.  Colour, out_others, the feature planes and radii are
+ * bit-identical to sr_forward's.  capacity, num_rendered_dev / num_rendered_host and the SR_STATUS_* words mean what
+ * they mean for sr_forward: an overflowed frame is not rendered, and the caller re-runs it with a larger capacity.
+ * P = 0 zero-fills the colour, feature and out_others planes.  Nothing is kept for a backward. */
+SR_API int sr_render_forward(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+                             const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
+                             const float* scales, const float* rotations, const float* features, int32_t F,
+                             int64_t features_stride, const float* viewmatrix, const float* projmatrix, const float* campos,
+                             float* out_color, int64_t out_color_stride, float* out_features, int64_t out_features_stride,
+                             float* out_others, int32_t* radii, void* arena, int64_t capacity, uint32_t* num_rendered_dev,
+                             uint32_t* num_rendered_host, void* stream);
+
+/* sr_post_forward over M frames in one launch: frame m's allmap (allmap + m*8*H*W) and world_view_transform (+ m*16) give
+ * its acc, rend_normal, rend_dist, depth_median, depth_expected, surf_depth, surf_normal (each output packed (M, c, H, W)).
+ * cameras: optional DEVICE (M,4) table of surfel_camera.h; with it frame m's rays use its own tangents and principal
+ * point offsets (tan_fovx / tan_fovy are not read), as sr_render_loss_batch_cameras does.  Without it every frame uses
+ * tan_fovx / tan_fovy and the centred principal point, bit-identical to sr_post_forward frame by frame.
+ * learnable_bkgd: optional DEVICE [3]; with it frame m's colour planes color + m*color_stride (color_stride >= 3*H*W
+ * floats) become color + (1 - acc) * bkgd, three rounded operations, in place.  Without it color is not read. */
+SR_API int sr_post_forward_frames(int32_t M, int32_t W, int32_t H, float tan_fovx, float tan_fovy, const float* cameras,
+                                  float depth_ratio, const float* allmap, const float* world_view_transform,
+                                  const float* learnable_bkgd, float* color, int64_t color_stride, float* acc,
+                                  float* rend_normal, float* rend_dist, float* depth_median, float* depth_expected,
+                                  float* surf_depth, float* surf_normal, void* stream);
+
+#ifdef __cplusplus
+}
+#endif
+
+#endif /* SURFEL_RENDER_H_ */

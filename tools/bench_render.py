@@ -1,0 +1,191 @@
+"""Forward-only rendering of a sequence: render_frames against today's route (the training forward under no_grad, then
+sr_post_forward per frame), two arms alternating in one process.
+
+Workload: 300 K surfels (bench.py's object scene) on 64 orbiting cameras, frames_per_call 8, F in {0, 22}, at 512^2 and
+at 128^2 (the reference's default render_res), with the scalar field of view and with a per-frame camera table.  Per arm:
+frames/s (median over repeats of CUDA-event time, with min and max), per-kernel ms from sr_set_profiling in a separate
+pass, and peak allocator bytes above the inputs.  The two arms' colour, feature planes, radii and maps are compared bit
+for bit at every timed size.  Prints one JSON object; --out writes it too.
+
+Usage: python tools/bench_render.py [--frames 64] [--chunk 8] [--repeats 7] [--out bench_render.json]
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import math
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+TAN = 0.5
+FOV = 2.0 * math.atan(TAN)
+TANF = math.tan(FOV * 0.5)     # the tangent render() derives from FoV (renderer._cam_tans): both arms use it
+
+
+def _cams(T, res, dev, table):
+    from vidu4d_b200.renderer import BatchCameras
+    from vidu4d_b200.synthetic import orbit_view, projection_matrix
+    vms, cps = [], []
+    for f in range(T):
+        R, t = orbit_view(f, T)
+        W2C = np.eye(4)
+        W2C[:3, :3], W2C[:3, 3] = R, t
+        vms.append(W2C.T.astype(np.float32))
+        cps.append((-R.T @ t).astype(np.float32))
+    vm = torch.from_numpy(np.stack(vms)).to(dev).contiguous()
+    pm = (vm @ torch.from_numpy(projection_matrix(TAN, TAN)).to(dev)).contiguous()
+    intr = None
+    if table:       # per-frame tangents with off-centre principal points
+        f = torch.arange(T, dtype=torch.float32)
+        intr = torch.stack([torch.full((T,), TANF), torch.full((T,), TANF), 0.02 * res * torch.sin(f), 0.02 * res * torch.cos(f)],
+                           1).to(dev).contiguous()
+    return BatchCameras(res, res, FOV, FOV, vm, pm, torch.from_numpy(np.stack(cps)).to(dev).contiguous(), intr)
+
+
+class _PC:
+    def __init__(self, s):
+        self.get_xyz, self.get_rotation, self.get_scaling = s["means3D"], s["rotations"], s["scales"]
+        self.get_opacity, self.get_features, self.active_sh_degree = s["opacities"], s["shs"], 3
+
+
+def today(cams, pc, bg, feat, chunk):
+    """The training forward under no_grad per chunk of frames, then sr_post_forward per frame (table cameras: the loss
+    pass's per-frame rays are not reachable from sr_post_forward, so the maps are skipped there)."""
+    from vidu4d_b200 import _capi
+    from vidu4d_b200.rasterizer import _C
+    T, H, W = len(cams), cams.image_height, cams.image_width
+    dev = pc.get_xyz.device
+    e = torch.empty((0,), device=dev)
+    outs = []
+    with torch.no_grad():
+        for t0 in range(0, T, chunk):
+            c = slice(t0, min(T, t0 + chunk))
+            kw = {} if feat is None else {"features": feat, "concat": False}
+            if cams.intrinsics is not None:
+                kw["intrinsics"] = cams.intrinsics[c]
+            o = _C.rasterize_gaussians_batch(bg, pc.get_xyz, e, pc.get_opacity, pc.get_scaling, pc.get_rotation, 1.0,
+                                             cams.world_view_transform[c], cams.full_proj_transform[c], TANF, TANF, H, W,
+                                             pc.get_features, 3, cams.camera_center[c], **kw)
+            maps = []
+            if cams.intrinsics is None:
+                for f in range(o[1].shape[0]):
+                    m = [torch.empty((k, H, W), device=dev) for k in (1, 3, 1, 1, 1, 1, 3)]
+                    _capi.call("sr_post_forward", dev, W, H, TANF, TANF, 0.0, o[2][f], cams.world_view_transform[c][f], *m)
+                    maps.append(m)
+            outs.append((o[1], o[3], o[7] if feat is not None else None, maps))
+    return outs
+
+
+def new(cams, pc, bg, feat, chunk):
+    from vidu4d_b200.renderer import PipelineParams, render_frames
+    return render_frames(cams, pc, PipelineParams(), bg, features=feat, frames_per_call=chunk)
+
+
+def _same(a, b):
+    return bool(torch.equal(a.contiguous().view(torch.int32), b.contiguous().view(torch.int32)))
+
+
+def mismatches(o_today, o_new, chunk):
+    """Names of the outputs whose bits differ between the arms (empty: identical)."""
+    bad = set()
+    keys = ("acc", "rend_normal", "rend_dist", "render_depth_median", "render_depth_expected", "surf_depth", "surf_normal")
+    for i, (color, radii, feat, maps) in enumerate(o_today):
+        c = slice(i * chunk, i * chunk + color.shape[0])
+        for k, x, y in (("render", color, o_new["render"][c]), ("radii", radii, o_new["radii"][c]),
+                        ("features", feat, o_new["features"][c] if feat is not None else None)):
+            if x is not None and not _same(x, y):
+                bad.add(k)
+        for f, m in enumerate(maps):
+            for k, x in zip(keys, m):
+                y = o_new[k][c][f]
+                if not _same(x, y if y.shape[0] == x.shape[0] else y[:1]):
+                    bad.add(k)
+    return sorted(bad)
+
+
+def timed(fn, repeats):
+    times = []
+    for _ in range(repeats):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        out = fn()
+        e1.record()
+        torch.cuda.synchronize()
+        times.append(e0.elapsed_time(e1))
+        del out
+    return times
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--frames", type=int, default=64)
+    ap.add_argument("--chunk", type=int, default=8)
+    ap.add_argument("--repeats", type=int, default=7)
+    ap.add_argument("--P", type=int, default=300_000)
+    ap.add_argument("--out", default=None)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_render needs a CUDA device")
+    from vidu4d_b200 import _capi
+    from vidu4d_b200.synthetic import object_scene
+    dev = torch.device("cuda:0")
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    s = object_scene(args.P, seed=0, opacity="trained", center=(0.0, 0.0, 0.0)).to_torch(dev)
+    pc = _PC(s)
+    g = torch.Generator(device=dev).manual_seed(0)
+    results = []
+    for res in (512, 128):
+        for F in (0, 22):
+            for table in (False, True):
+                cams = _cams(args.frames, res, dev, table)
+                feat = (torch.rand((args.P, F), device=dev, generator=g) * 2 - 1) if F else None
+                bg = torch.zeros(3, device=dev)
+                arms = {"render_frames": lambda: new(cams, pc, bg, feat, args.chunk),
+                        "today": lambda: today(cams, pc, bg, feat, args.chunk)}
+                for fn in arms.values():          # warm-up: capacity hints, module loads, allocator
+                    fn()
+                torch.cuda.synchronize()
+                bad = mismatches(arms["today"](), arms["render_frames"](), args.chunk)
+                times = {k: [] for k in arms}
+                for _ in range(args.repeats):     # alternate the arms
+                    for k, fn in arms.items():
+                        times[k] += timed(fn, 1)
+                row = {"res": res, "F": F, "cameras": "table" if table else "scalar", "identical": not bad, "mismatches": bad}
+                base = torch.cuda.memory_allocated(dev)
+                for k, fn in arms.items():
+                    torch.cuda.synchronize()
+                    torch.cuda.reset_peak_memory_stats(dev)
+                    fn()
+                    torch.cuda.synchronize()
+                    peak = torch.cuda.max_memory_allocated(dev) - base
+                    _capi.set_profiling(True)
+                    fn()
+                    prof = _capi.get_profile()
+                    _capi.set_profiling(False)
+                    t = np.asarray(times[k])
+                    row[k] = {"fps_median": args.frames / (float(np.median(t)) / 1e3),
+                              "fps_min": args.frames / (float(t.max()) / 1e3), "fps_max": args.frames / (float(t.min()) / 1e3),
+                              "ms_median": float(np.median(t)), "peak_bytes_above_inputs": int(peak),
+                              "kernels_ms": {n: round(v["ms"], 4) for n, v in prof.items()}}
+                row["speedup"] = row["render_frames"]["fps_median"] / row["today"]["fps_median"]
+                print(json.dumps(row), flush=True)
+                results.append(row)
+    out = {"gpu": gpu, "frames": args.frames, "frames_per_call": args.chunk, "P": args.P, "rows": results}
+    print(json.dumps(out))
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        with open(args.out, "w") as f:
+            json.dump(out, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()

@@ -23,7 +23,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from vidu4d_b200.build import NVCC_FLAGS, _nvcc  # noqa: E402
 
-SOURCES = ["composite_tile.cu", "composite_feat.cu", "composite_det.cu", "surfel_bwd.cu", "preprocess.cu"]
+SOURCES = ["composite_tile.cu", "composite_feat.cu", "composite_det.cu", "surfel_bwd.cu", "preprocess.cu", "composite_fwd.cu",
+           "postprocess.cu"]
 # (demangled-name pattern in the base build, pattern of the same kernel in the working tree)
 KERNELS = [
     (r"composite_tile_bwd_kernel(<\(bool\)0>)?\(", r"composite_tile_bwd_kernel(<\(bool\)0>)?\("),
@@ -38,6 +39,15 @@ KERNELS = [
     (r"emit_keys_kernel\(", r"emit_keys_kernel\("),
     (r"scan_block_sums_kernel\(", r"scan_block_sums_kernel\("),
     (r"mark_visible_kernel\(", r"mark_visible_kernel\("),
+    # the training instantiation of the composite forward (the forward-only ones are <(bool)0, ...>)
+    (r"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0>)?\(", r"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0>)?\("),
+    (r"feature_fwd_kernel<\(int\)4>\(", r"feature_fwd_kernel<\(int\)4>\("),
+    (r"feature_fwd_kernel<\(int\)2>\(", r"feature_fwd_kernel<\(int\)2>\("),
+    (r"feature_fwd_kernel<\(int\)1>\(", r"feature_fwd_kernel<\(int\)1>\("),
+    # sr_post_forward's kernels (sr_post_forward_frames' are <(bool)1, ...>)
+    (r"post_fwd_kernel(<\(bool\)0, \(bool\)0>)?\(", r"post_fwd_kernel(<\(bool\)0, \(bool\)0>)?\("),
+    (r"post_normal_kernel(<\(bool\)0, \(bool\)0>)?\(", r"post_normal_kernel(<\(bool\)0, \(bool\)0>)?\("),
+    (r"post_bwd_kernel\(", r"post_bwd_kernel\("),
 ]
 
 

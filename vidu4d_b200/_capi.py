@@ -153,6 +153,16 @@ DET_PROTOTYPES = {
 }
 DET_SYMBOLS = tuple(DET_PROTOTYPES)
 
+# forward-only rendering of many frames (sr_forward's outputs without its backward state, and render()'s post-processing
+# over M frames), declared in include/surfel_render.h (own header and table for the same reason)
+RENDER_PROTOTYPES = {
+    "sr_render_bytes": (C.c_size_t, [_i32, _i64, _i32, _i32]),
+    "sr_render_forward": (C.c_int, [_FRAME, _BATCH, _p, _i32] + [_p] * 7 + [_i32, _i64] + [_p] * 3 + [_p, _i64, _p, _i64]
+                          + [_p] * 3 + [_i64, _p, _p, _p]),
+    "sr_post_forward_frames": (C.c_int, [_i32] * 3 + [_f32] * 2 + [_p, _f32] + [_p] * 4 + [_i64] + [_p] * 8),
+}
+RENDER_SYMBOLS = tuple(RENDER_PROTOTYPES)
+
 
 _lib = None
 
@@ -167,12 +177,14 @@ def load():
             f"{LIB_PATH} not found: the CUDA extension is not built. Run `python -m vidu4d_b200.build` "
             "(or __graft_entry__.build()). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for s in SYMBOLS + SSIM_SYMBOLS + OPTIM_SYMBOLS + SKIN_MLP_SYMBOLS + MASK_LOSS_SYMBOLS + CAMERA_SYMBOLS + DET_SYMBOLS:
+    for s in (SYMBOLS + SSIM_SYMBOLS + OPTIM_SYMBOLS + SKIN_MLP_SYMBOLS + MASK_LOSS_SYMBOLS + CAMERA_SYMBOLS + DET_SYMBOLS
+              + RENDER_SYMBOLS):
         if not hasattr(lib, s):
             raise SurfelRasterError(f"{LIB_PATH} does not export {s}")
     for name, (restype, argtypes) in (list(PROTOTYPES.items()) + list(SSIM_PROTOTYPES.items()) + list(OPTIM_PROTOTYPES.items())
                                       + list(SKIN_MLP_PROTOTYPES.items()) + list(MASK_LOSS_PROTOTYPES.items())
-                                      + list(CAMERA_PROTOTYPES.items()) + list(DET_PROTOTYPES.items())):
+                                      + list(CAMERA_PROTOTYPES.items()) + list(DET_PROTOTYPES.items())
+                                      + list(RENDER_PROTOTYPES.items())):
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.sr_abi_version() != ABI_VERSION:

@@ -23,7 +23,8 @@ HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "composite_commo
            os.path.join(HERE, "..", "include", "surfel_raster.h"), os.path.join(HERE, "..", "include", "surfel_ssim.h"),
            os.path.join(HERE, "..", "include", "surfel_optim.h"), os.path.join(HERE, "..", "include", "surfel_skin_mlp.h"),
            os.path.join(HERE, "..", "include", "surfel_mask_loss.h"), os.path.join(HERE, "..", "include", "surfel_camera.h"),
-           os.path.join(HERE, "..", "include", "surfel_deterministic.h")]
+           os.path.join(HERE, "..", "include", "surfel_deterministic.h"),
+           os.path.join(HERE, "..", "include", "surfel_render.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",

@@ -16,6 +16,7 @@
 #include "common.cuh"
 #include "../../include/surfel_camera.h"
 #include "../../include/surfel_deterministic.h"
+#include "../../include/surfel_render.h"
 
 namespace {
 thread_local char g_err[512] = "";
@@ -149,6 +150,10 @@ size_t sr_image_bytes(int32_t width, int32_t height) { return image_layout(width
 size_t sr_binning_bytes(int64_t capacity, int32_t width, int32_t height) {
     return bin_layout(capacity, image_layout(width > 0 ? width : 0, height > 0 ? height : 0).tiles).total;
 }
+size_t sr_render_bytes(int32_t P, int64_t capacity, int32_t width, int32_t height) {
+    const ImageLayout i = image_layout(width > 0 ? width : 0, height > 0 ? height : 0, true);
+    return geom_layout(P, true).total + bin_layout(capacity, i.tiles, true).total + i.total;
+}
 
 int sr_debug_view(int32_t P, int32_t width, int32_t height, int64_t capacity, sr_debug_layout* out) {
     if (!out) return sr_fail(SR_EINVAL, "out is NULL");
@@ -199,7 +204,7 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
                          const float* viewmatrix, const float* campos, float* out_color, int64_t color_stride,
                          float* out_others, int32_t* radii, void* geom_buffer, void* binning_buffer, void* image_buffer,
                          int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream_,
-                         FeatArgs* ft) {
+                         FeatArgs* ft, bool forward_only) {
     if (int rc = check_frame(f)) return rc;
     if (!b || b->frames < 1 || b->frames > 65535) return sr_fail(SR_EINVAL, "batch descriptor: frames must be in [1, 65535]");
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -212,6 +217,23 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
         if (color_stride < (int64_t)(3 * N)) return sr_fail(SR_EINVAL, "out_color frame stride must be >= 3*H*W");
         if (!ft->out) return sr_fail(SR_EINVAL, "out_features pointer is NULL");
         if (ft->out_stride < (long long)(ft->F * N) * 4) return sr_fail(SR_EINVAL, "out_features frame stride must be >= F*H*W");
+    }
+    if (P > 0) {   // every argument is checked before any device work
+        if (!means3D || !opacities || !scales || !rotations || !radii) return sr_fail(SR_EINVAL, "surfel attribute pointer is NULL");
+        if ((shs == nullptr) == (colors_precomp == nullptr))
+            return sr_fail(SR_EINVAL, "provide exactly one of shs / colors_precomp");
+        if (shs && f->sh_coeffs == 0) return sr_fail(SR_EINVAL, "shs given but sh_coeffs == 0");
+        if (forward_only) {
+            if (!geom_buffer) return sr_fail(SR_EINVAL, "arena is NULL");
+            if ((uintptr_t)geom_buffer & 15) return sr_fail(SR_EINVAL, "arena must be 16-byte aligned");
+        } else if (!geom_buffer || !binning_buffer || !image_buffer) {
+            return sr_fail(SR_EINVAL, "scratch buffer is NULL");
+        }
+        if (capacity <= 0 || capacity >= (1ll << 30)) return sr_fail(SR_EINVAL, "capacity must be in (0, 2^30)");
+        // 128-bit / 64-bit vector loads: rotations as float4, scales as float2, SH rows as float4 when 3M % 4 == 0
+        if (((uintptr_t)rotations & 15) || ((uintptr_t)scales & 7) || (shs && ((uintptr_t)shs & 15)) ||
+            ((b->rotations * 4) & 15) || ((b->scales * 4) & 7) || ((b->shs * 4) & 15))
+            return sr_fail(SR_EINVAL, "rotations / shs must be 16-byte aligned and scales 8-byte aligned (per frame)");
     }
     CK(cudaMemsetAsync(num_rendered_dev, 0, (size_t)M * 2 * sizeof(uint32_t), stream), "memset(num_rendered)");
     if (P == 0) {
@@ -227,16 +249,6 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
             CK(cudaMemcpyAsync(num_rendered_host, num_rendered_dev, (size_t)M * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream), "copy(num_rendered)");
         return 0;
     }
-    if (!means3D || !opacities || !scales || !rotations || !radii) return sr_fail(SR_EINVAL, "surfel attribute pointer is NULL");
-    if ((shs == nullptr) == (colors_precomp == nullptr))
-        return sr_fail(SR_EINVAL, "provide exactly one of shs / colors_precomp");
-    if (shs && f->sh_coeffs == 0) return sr_fail(SR_EINVAL, "shs given but sh_coeffs == 0");
-    if (!geom_buffer || !binning_buffer || !image_buffer) return sr_fail(SR_EINVAL, "scratch buffer is NULL");
-    if (capacity <= 0 || capacity >= (1ll << 30)) return sr_fail(SR_EINVAL, "capacity must be in (0, 2^30)");
-    // 128-bit / 64-bit vector loads: rotations as float4, scales as float2, SH rows as float4 when 3M % 4 == 0
-    if (((uintptr_t)rotations & 15) || ((uintptr_t)scales & 7) || (shs && ((uintptr_t)shs & 15)) ||
-        ((b->rotations * 4) & 15) || ((b->scales * 4) & 7) || ((b->shs * 4) & 15))
-        return sr_fail(SR_EINVAL, "rotations / shs must be 16-byte aligned and scales 8-byte aligned (per frame)");
 
     FwdArgs a{};
     a.cam = make_cam(f, viewmatrix, campos, background);
@@ -244,15 +256,19 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
     a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.opacities = opacities;
     a.scales = scales; a.rotations = rotations;
     a.out_color = out_color; a.out_others = out_others; a.radii = radii;
+    a.gl = geom_layout(P, forward_only); a.il = image_layout(f->width, f->height, forward_only);
+    a.bl = bin_layout(capacity, a.il.tiles, forward_only);
     a.geom = (char*)geom_buffer; a.bin = (char*)binning_buffer; a.img = (char*)image_buffer;
-    a.gl = geom_layout(P); a.il = image_layout(f->width, f->height); a.bl = bin_layout(capacity, a.il.tiles);
+    if (forward_only) { a.bin = a.geom + a.gl.total; a.img = a.bin + a.bl.total; }   // frame m's arena: [geom | bin | img]
     a.num_rendered_dev = num_rendered_dev;
     a.prefiltered = f->prefiltered;
     a.key_bits = 32 + (int)sr_higher_msb((uint32_t)a.il.tiles);
     a.stream = stream; a.debug = debug;
+    a.forward_only = forward_only; a.feat = ft;
     FrameStrides& fs = a.fs;
     fs.frames = M;
     fs.geom = (long long)a.gl.total; fs.bin = (long long)a.bl.total; fs.img = (long long)a.il.total; fs.nr = 2 * sizeof(uint32_t);
+    if (forward_only) fs.geom = fs.bin = fs.img = (long long)(a.gl.total + a.bl.total + a.il.total);
     fs.means3D = b->means3D * 4; fs.shs = b->shs * 4; fs.colors = b->colors_precomp * 4; fs.opac = b->opacities * 4;
     fs.scales = b->scales * 4; fs.rots = b->rotations * 4; fs.vm = 16 * sizeof(float); fs.campos = 3 * sizeof(float);
     fs.out_color = (long long)(3 * N * sizeof(float)); fs.out_others = (long long)(8 * N * sizeof(float));
@@ -260,35 +276,41 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
     fs.radii = (long long)P * sizeof(int32_t);
 
     // per frame: tile state (ranges .. end of the image buffer); sort control words + digit histograms + look-back status
-    CK(sr_memset_frames(a.img + a.il.ranges, a.il.total, a.il.total - a.il.ranges, M, stream), "memset(tile state)");
-    CK(sr_memset_frames(a.bin + a.bl.sort_ctl, a.bl.total, a.bl.total - a.bl.sort_ctl, M, stream), "memset(sort state)");
+    CK(sr_memset_frames(a.img + a.il.ranges, (size_t)fs.img, a.il.total - a.il.ranges, M, stream), "memset(tile state)");
+    CK(sr_memset_frames(a.bin + a.bl.sort_ctl, (size_t)fs.bin, a.bl.total - a.bl.sort_ctl, M, stream), "memset(sort state)");
     CK(launch_preprocess_fwd(a), "preprocess_fwd"); DBG("preprocess_fwd");
     CK(launch_scan_emit(a), "scan/emit_keys"); DBG("scan/emit_keys");
     CK(launch_sort(a), "sort"); DBG("sort");
     CK(launch_ranges_gather(a), "ranges_gather"); DBG("ranges_gather");
     CK(launch_tile_order(a), "tile_order"); DBG("tile_order");
-    if (sr_composite_tile_fwd()) { CK(launch_composite_tile_fwd(a), "composite_tile_fwd"); }
-    else { CK(launch_composite_fwd(a), "composite_fwd"); }
-    DBG("composite_fwd");
-    if (ft) { CK(launch_feature_fwd(a, *ft), "feature_fwd"); DBG("feature_fwd"); }
+    if (forward_only) {
+        // one walk: colour, allmap and the feature channels; SURFEL_COMPOSITE_FWD is not consulted
+        CK(launch_composite_fwd(a), "composite_render"); DBG("composite_render");
+    } else {
+        if (sr_composite_tile_fwd()) { CK(launch_composite_tile_fwd(a), "composite_tile_fwd"); }
+        else { CK(launch_composite_fwd(a), "composite_fwd"); }
+        DBG("composite_fwd");
+        if (ft) { CK(launch_feature_fwd(a, *ft), "feature_fwd"); DBG("feature_fwd"); }
+    }
     if (num_rendered_host)
         CK(cudaMemcpyAsync(num_rendered_host, num_rendered_dev, (size_t)M * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream), "copy(num_rendered)");
     return 0;
 }
 
-int sr_forward(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels, const float* means3D,
-               const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
-               const float* rotations, const float* features, int32_t F, int64_t features_stride, const float* viewmatrix,
-               const float* projmatrix, const float* campos, float* out_color, int64_t out_color_stride,
-               float* out_features, int64_t out_features_stride, float* out_others, int32_t* radii, void* geom_buffer,
-               void* binning_buffer, void* image_buffer, int64_t capacity, uint32_t* num_rendered_dev,
-               uint32_t* num_rendered_host, void* stream_) {
-    (void)projmatrix;   // only feeds dead code in the reference (auxiliary.h:170-172)
+namespace {
+// sr_forward and sr_render_forward: the feature arguments, then forward_batch
+int forward_entry(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels, const float* means3D,
+                  const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
+                  const float* rotations, const float* features, int32_t F, int64_t features_stride, const float* viewmatrix,
+                  const float* campos, float* out_color, int64_t out_color_stride, float* out_features,
+                  int64_t out_features_stride, float* out_others, int32_t* radii, void* geom_buffer, void* binning_buffer,
+                  void* image_buffer, int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host,
+                  void* stream_, bool forward_only) {
     if (F == 0) {
         if (int rc = check_no_features(f, features, bg_channels, out_color_stride)) return rc;
         return forward_batch(f, b, background, means3D, shs, colors_precomp, opacities, scales, rotations, viewmatrix, campos,
                              out_color, 0, out_others, radii, geom_buffer, binning_buffer, image_buffer, capacity,
-                             num_rendered_dev, num_rendered_host, stream_, nullptr);
+                             num_rendered_dev, num_rendered_host, stream_, nullptr, forward_only);
     }
     if (int rc = check_features(f, F, bg_channels, features, features_stride)) return rc;
     FeatArgs ft{};
@@ -299,7 +321,36 @@ int sr_forward(const sr_frame* f, const sr_batch* b, const float* background, in
     ft.out = out_features; ft.out_stride = out_features_stride * 4;
     return forward_batch(f, b, background, means3D, shs, colors_precomp, opacities, scales, rotations, viewmatrix, campos,
                          out_color, out_color_stride, out_others, radii, geom_buffer, binning_buffer, image_buffer, capacity,
-                         num_rendered_dev, num_rendered_host, stream_, &ft);
+                         num_rendered_dev, num_rendered_host, stream_, &ft, forward_only);
+}
+}  // namespace
+
+int sr_forward(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels, const float* means3D,
+               const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
+               const float* rotations, const float* features, int32_t F, int64_t features_stride, const float* viewmatrix,
+               const float* projmatrix, const float* campos, float* out_color, int64_t out_color_stride,
+               float* out_features, int64_t out_features_stride, float* out_others, int32_t* radii, void* geom_buffer,
+               void* binning_buffer, void* image_buffer, int64_t capacity, uint32_t* num_rendered_dev,
+               uint32_t* num_rendered_host, void* stream_) {
+    (void)projmatrix;   // only feeds dead code in the reference (auxiliary.h:170-172)
+    return forward_entry(f, b, background, bg_channels, means3D, shs, colors_precomp, opacities, scales, rotations, features, F,
+                         features_stride, viewmatrix, campos, out_color, out_color_stride, out_features, out_features_stride,
+                         out_others, radii, geom_buffer, binning_buffer, image_buffer, capacity, num_rendered_dev,
+                         num_rendered_host, stream_, false);
+}
+
+int sr_render_forward(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels, const float* means3D,
+                      const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
+                      const float* rotations, const float* features, int32_t F, int64_t features_stride,
+                      const float* viewmatrix, const float* projmatrix, const float* campos, float* out_color,
+                      int64_t out_color_stride, float* out_features, int64_t out_features_stride, float* out_others,
+                      int32_t* radii, void* arena, int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host,
+                      void* stream_) {
+    (void)projmatrix;
+    return forward_entry(f, b, background, bg_channels, means3D, shs, colors_precomp, opacities, scales, rotations, features, F,
+                         features_stride, viewmatrix, campos, out_color, out_color_stride, out_features, out_features_stride,
+                         out_others, radii, arena, nullptr, nullptr, capacity, num_rendered_dev, num_rendered_host, stream_,
+                         true);
 }
 
 static int backward_batch(const sr_frame* f, const sr_batch* b, const float* background, const float* means3D, const float* shs,

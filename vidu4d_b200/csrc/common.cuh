@@ -74,7 +74,10 @@ struct BinLayout {
     int sort_tiles;
 };
 
-static inline __host__ __device__ GeomLayout geom_layout(int P) {
+// forward_only (sr_render_forward's arena): the arrays only a backward reads -- the geometry's gradient accumulator
+// sgrad, the binning's contribution masks, the image's final_T, n_contrib and sub_last (tile_last) -- take no bytes;
+// their offsets alias the next array's and nothing touches them.
+static inline __host__ __device__ GeomLayout geom_layout(int P, bool forward_only = false) {
     GeomLayout L;
     size_t Pa = P > 0 ? (size_t)P : 1, o = 0;
     L.nblocks = (int)((Pa + 255) / 256);
@@ -84,24 +87,24 @@ static inline __host__ __device__ GeomLayout geom_layout(int P) {
     L.point_offsets = o; o = sr_align_up(o + Pa * 4);
     L.clamped = o;       o = sr_align_up(o + Pa);
     L.block_sums = o;    o = sr_align_up(o + ((size_t)L.nblocks + 1) * 4);
-    L.sgrad = o;         o = sr_align_up(o + Pa * SR_GRAD_FLOATS * 4);
+    L.sgrad = o;         if (!forward_only) o = sr_align_up(o + Pa * SR_GRAD_FLOATS * 4);
     L.total = o;
     return L;
 }
-static inline __host__ __device__ ImageLayout image_layout(int W, int H) {
+static inline __host__ __device__ ImageLayout image_layout(int W, int H, bool forward_only = false) {
     ImageLayout L;
     size_t N = (size_t)W * H, o = 0;
     L.tiles_x = (W + SR_TILE - 1) / SR_TILE; L.tiles_y = (H + SR_TILE - 1) / SR_TILE;
     L.tiles = L.tiles_x * L.tiles_y;
-    L.final_T = o;   o = sr_align_up(o + 3 * N * 4);
-    L.n_contrib = o; o = sr_align_up(o + 2 * N * 4);
+    L.final_T = o;   if (!forward_only) o = sr_align_up(o + 3 * N * 4);
+    L.n_contrib = o; if (!forward_only) o = sr_align_up(o + 2 * N * 4);
     L.ranges = o;    o = sr_align_up(o + (size_t)L.tiles * 8);
-    L.tile_last = o; o = sr_align_up(o + (size_t)L.tiles * 8 * 4);   // per 8x4 sub-tile: deepest contributor
+    L.tile_last = o; if (!forward_only) o = sr_align_up(o + (size_t)L.tiles * 8 * 4);   // per 8x4 sub-tile: deepest contributor
     L.tile_order = o; o = sr_align_up(o + (size_t)L.tiles * 4);       // tiles, longest instance list first
     L.total = o;
     return L;
 }
-static inline __host__ __device__ BinLayout bin_layout(int64_t capacity, int tiles) {
+static inline __host__ __device__ BinLayout bin_layout(int64_t capacity, int tiles, bool forward_only = false) {
     BinLayout L;
     size_t C = capacity > 0 ? (size_t)capacity : 1, o = 0;
     L.capacity = (int64_t)C;
@@ -114,7 +117,8 @@ static inline __host__ __device__ BinLayout bin_layout(int64_t capacity, int til
     // contribution masks: per (32-instance stage of a tile list, 8x4 sub-tile, pixel) the instances that
     // contributed to the pixel -- written by the forward composite, walked by the backward (contrib_word).
     // Stage s of tile t lives at index (range.x >> 5) + t + s  (<= capacity/32 + tiles in total).
-    L.contrib = o;   o = sr_align_up(o + ((C >> 5) + (size_t)(tiles > 0 ? tiles : 0) + 1) * SR_CONTRIB_STAGE_WORDS * 4);
+    L.contrib = o;
+    if (!forward_only) o = sr_align_up(o + ((C >> 5) + (size_t)(tiles > 0 ? tiles : 0) + 1) * SR_CONTRIB_STAGE_WORDS * 4);
     // the three below are zeroed together by one memset at the start of every forward
     L.sort_ctl = o;  o = sr_align_up(o + SR_CTL_WORDS * 4);
     L.hist = o;      o = sr_align_up(o + (size_t)SR_SORT_MAX_PASSES * SR_SORT_BINS * 4);
@@ -164,6 +168,7 @@ struct FrameStrides {
 };
 
 // ---- launchers implemented in the .cu files ------------------------------------------------
+struct FeatArgs;
 struct FwdArgs {
     FrameStrides fs;
     CamParams cam;
@@ -177,6 +182,10 @@ struct FwdArgs {
     int key_bits;                 // 32 + getHigherMsb(tiles)
     cudaStream_t stream;
     bool debug;
+    // sr_render_forward: the layouts are forward_only, the composite keeps no backward state and composites the feature
+    // channels `feat` (nullptr when F = 0) in its own walk
+    bool forward_only;
+    const FeatArgs* feat;
 };
 struct BwdArgs {
     FrameStrides fs;

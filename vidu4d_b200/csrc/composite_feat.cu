@@ -27,28 +27,6 @@ namespace {
 using namespace comp;
 constexpr int FC = SR_FEAT_CHUNK;
 
-// the FC channels [c0, c0 + FC) of one feature row (channels >= F read as 0); V floats per load, F % V == 0
-template <int V>
-__device__ __forceinline__ void load_chunk(const float* __restrict__ row, int c0, int F, float (&x)[FC]) {
-#pragma unroll
-    for (int k = 0; k < FC; k += V) {
-        if (c0 + k < F) {
-            if constexpr (V == 4) {
-                const float4 t = __ldg(reinterpret_cast<const float4*>(row + c0 + k));
-                x[k] = t.x; x[k + 1] = t.y; x[k + 2] = t.z; x[k + 3] = t.w;
-            } else if constexpr (V == 2) {
-                const float2 t = __ldg(reinterpret_cast<const float2*>(row + c0 + k));
-                x[k] = t.x; x[k + 1] = t.y;
-            } else {
-                x[k] = __ldg(row + c0 + k);
-            }
-        } else {
-#pragma unroll
-            for (int j = 0; j < V; j++) x[k + j] = 0.f;
-        }
-    }
-}
-
 template <int V>
 __device__ __forceinline__ void red_chunk(float* row, int c0, int F, const float (&g)[FC]) {
 #pragma unroll

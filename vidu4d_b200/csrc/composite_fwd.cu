@@ -14,7 +14,11 @@
 //     walks exactly those;
 //   * culling and the rho_cut early-out never change a result: a skipped pair provably has alpha < 1/255;
 //   * the per-pixel state, per-pair arithmetic and output words are comp::FwdPixel's, shared with the tile forward
-//     (composite_tile.cu): the two differ only in how records reach the lanes and how they stop early.
+//     (composite_tile.cu): the two differ only in how records reach the lanes and how they stop early;
+//   * two instantiations (DESIGN.md "forward-only render").  TRAIN records the contribution masks, sub_last, final_T and
+//     n_contrib for the backward; the forward-only one (sr_render_forward) records none of them and composites up to NF
+//     feature channels inside the same walk, through FwdPixel::blend's per-pair hook: acc[k] = ff(T, fm(alpha, x[k]),
+//     acc[k]) over the same contributors, weights and order as feature_fwd, so every plane has feature_fwd's bits.
 #include "composite_common.cuh"
 
 namespace {
@@ -22,12 +26,15 @@ using namespace comp;
 
 constexpr int WPC = 1;      // independent warps per CTA (2 measured slower: register pressure)
 
+// TRAIN: the training forward (V, NF unused).  Otherwise forward-only with F <= NF feature channels (NF = 0: none), rows
+// gathered V floats per load.
+template <bool TRAIN, int V, int NF>
 __global__ void __launch_bounds__(32 * WPC)
 composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, const uint32_t* __restrict__ tile_order, int n_items, int tiles_x,
                      const float4* __restrict__ irec, int W, int H,
                      const float* __restrict__ bg, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
                      float* __restrict__ out_color, float* __restrict__ out_others, uint32_t* __restrict__ sub_last,
-                     uint32_t* __restrict__ contrib_masks) {
+                     uint32_t* __restrict__ contrib_masks, const FeatArgs ft) {
     // WPC independent warps per CTA (the SM holds at most 32 CTAs): work item = (tile, 8x4 sub-tile), tiles in
     // longest-list-first order; the warps of a CTA share nothing
     __shared__ __align__(128) float4 st_all[WPC][NST][WB * REC4];
@@ -64,6 +71,20 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
     // are one 128-B store
     uint32_t cmask = 0u;
     uint32_t* cm_out = contrib_masks + contrib_word(range.x, tile, warp, lane);
+    // forward-only: this lane's feature planes, composited as feature_fwd composites them
+    const int F = ft.F;
+    const float* feat = fr(ft.feat, ft.feat_stride, f);
+    float facc[NF > 0 ? NF : 1];
+#pragma unroll
+    for (int k = 0; k < (NF > 0 ? NF : 1); k++) facc[k] = 0.f;
+    auto feat_pair = [&](float T, float alpha, const float4* __restrict__ R) {
+        if constexpr (NF > 0) {
+            float x[NF];
+            load_chunk<V>(feat + (size_t)__float_as_uint(R[4].z) * F, 0, F, x);
+#pragma unroll
+            for (int k = 0; k < NF; k++) facc[k] = ff(T, fm(alpha, x[k]), facc[k]);
+        }
+    };
 
     for (int b = 0; b < nb; b++) {
         const float4* S = ring.wait(b);
@@ -82,10 +103,14 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
             mym &= mym - 1;                              // no-op when mym == 0
             const float rho_cut = cull_rho_cut(__shfl_sync(0xffffffffu, cull, jj));   // before any divergence
             if (!act || done) continue;
-            if (px.blend(S + jj * REC4, sp.pixx, sp.pixy, rho_cut, b * WB, jj, cmask)) done = true;
+            if constexpr (TRAIN) {
+                if (px.blend(S + jj * REC4, sp.pixx, sp.pixy, rho_cut, b * WB, jj, cmask)) done = true;
+            } else {
+                if (px.blend(S + jj * REC4, sp.pixx, sp.pixy, rho_cut, b * WB, jj, cmask, feat_pair)) done = true;
+            }
         }
         __syncwarp();                                   // every lane is done reading stage b
-        cm_out[(size_t)b * SR_CONTRIB_STAGE_WORDS] = cmask;
+        if constexpr (TRAIN) cm_out[(size_t)b * SR_CONTRIB_STAGE_WORDS] = cmask;
         cmask = 0u;
         if (__all_sync(0xffffffffu, done)) {
             // drain the copies still in flight before this warp (and its CTA's smem) goes away
@@ -95,23 +120,63 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
         if (lane == 0 && b + NST < nb) ring.issue(b + NST, b + NST);
     }
 
-    // deepest list position any pixel of this sub-tile used: the backward starts its reverse walk there
-    uint32_t wmax = px.last_contributor;
+    if constexpr (TRAIN) {
+        // deepest list position any pixel of this sub-tile used: the backward starts its reverse walk there
+        uint32_t wmax = px.last_contributor;
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
-    if (lane == 0) sub_last[tile * 8 + warp] = wmax;
-    px.store(sp, W, H, bg, final_T, n_contrib, out_color, out_others);
+        for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
+        if (lane == 0) sub_last[tile * 8 + warp] = wmax;
+        px.store(sp, W, H, bg, final_T, n_contrib, out_color, out_others);
+    } else {
+        px.store(sp, W, H, bg, out_color, out_others);
+        if constexpr (NF > 0) {
+            if (sp.inside(W, H)) {
+                const size_t N = (size_t)W * H, pid = (size_t)W * sp.pix_y + sp.pix_x;
+                float* out = fr(ft.out, ft.out_stride, f);
+#pragma unroll
+                for (int k = 0; k < NF; k++)
+                    if (k < F) out[(size_t)k * N + pid] = ft.bg ? ff(px.T, __ldg(ft.bg + k), facc[k]) : ff(px.T, 0.0f, facc[k]);
+            }
+        }
+    }
+}
+
+// the forward-only instantiation for F channels (NF = F rounded up to a multiple of 8) and vector width ft.vec
+template <int NF>
+void launch_render(const FwdArgs& a, const FeatArgs& ft, unsigned grid) {
+    auto launch = [&](auto kern) {
+        kern<<<grid, 32 * WPC, 0, a.stream>>>(
+            a.fs, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles * 8, a.il.tiles_x,
+            (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, a.cam.bg, nullptr, nullptr, a.out_color, a.out_others,
+            nullptr, nullptr, ft);
+    };
+    if constexpr (NF == 0) launch(composite_fwd_kernel<false, 1, 0>);
+    else if (ft.vec == 4) launch(composite_fwd_kernel<false, 4, NF>);
+    else if (ft.vec == 2) launch(composite_fwd_kernel<false, 2, NF>);
+    else launch(composite_fwd_kernel<false, 1, NF>);
 }
 
 }  // namespace
 
 cudaError_t launch_composite_fwd(const FwdArgs& a) {
+    const unsigned grid = (unsigned)((a.il.tiles * 8 + WPC - 1) / WPC) * (unsigned)a.fs.frames;
+    if (a.forward_only) {
+        ProfileScope ps("composite_render", a.stream);
+        const FeatArgs ft = a.feat ? *a.feat : FeatArgs{};
+        if (ft.F == 0) launch_render<0>(a, ft, grid);
+        else if (ft.F <= 8) launch_render<8>(a, ft, grid);
+        else if (ft.F <= 16) launch_render<16>(a, ft, grid);
+        else if (ft.F <= 24) launch_render<24>(a, ft, grid);
+        else launch_render<32>(a, ft, grid);
+        sr_count_launch();
+        return cudaGetLastError();
+    }
     ProfileScope ps("composite_fwd", a.stream);
-    composite_fwd_kernel<<<((a.il.tiles * 8 + WPC - 1) / WPC) * a.fs.frames, 32 * WPC, 0, a.stream>>>(
+    composite_fwd_kernel<true, 1, 0><<<((a.il.tiles * 8 + WPC - 1) / WPC) * a.fs.frames, 32 * WPC, 0, a.stream>>>(
         a.fs, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles * 8, a.il.tiles_x,
         (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, a.cam.bg,
         (float*)(a.img + a.il.final_T), (uint32_t*)(a.img + a.il.n_contrib), a.out_color, a.out_others,
-        (uint32_t*)(a.img + a.il.tile_last), (uint32_t*)(a.bin + a.bl.contrib));
+        (uint32_t*)(a.img + a.il.tile_last), (uint32_t*)(a.bin + a.bl.contrib), FeatArgs{});
     sr_count_launch();
     return cudaGetLastError();
 }

@@ -8,20 +8,55 @@
 // reassociation inside a dot product).  The backward is written as a GATHER (each pixel collects the stencil
 // contributions of its four neighbours), so it has no atomics and is deterministic.
 #include "post_common.cuh"
+#include "../../include/surfel_render.h"
 
 namespace {
 using namespace post;
 
+// sr_post_forward_frames: frame blockIdx.z of M, its camera from the optional (M,4) table, and the optional learnable
+// background added into its colour planes.  FRAMES = false is sr_post_forward's one frame (Frames unused).
+struct Frames {
+    const float* cams;      // DEVICE (M,4) or nullptr
+    const float* bkgd;      // DEVICE [3] or nullptr
+    float* color;           // frame 0's colour planes (read and written only with bkgd)
+    long long color_stride; // floats between frames
+};
+// frame f's camera: row f of the table (TABLE), else the shared tangents.  The two are separate instantiations so that
+// the scalar one compiles to sr_post_forward's arithmetic, contraction for contraction.
+template <bool TABLE>
+__device__ __forceinline__ PostCam frame_cam(const Frames& fr, int f, const float* __restrict__ wvt, int W, int H, float tanx,
+                                             float tany) {
+    if constexpr (TABLE) {
+        const float* r = fr.cams + 4 * (size_t)f;
+        return load_cam(wvt, W, H, __ldg(r), __ldg(r + 1), __ldg(r + 2), __ldg(r + 3));
+    }
+    return load_cam(wvt, W, H, tanx, tany);
+}
+
+template <bool FRAMES, bool TABLE>
 __global__ void __launch_bounds__(256)
 post_fwd_kernel(int W, int H, float tanx, float tany, float depth_ratio, const float* __restrict__ allmap,
                 const float* __restrict__ wvt, float* __restrict__ acc, float* __restrict__ rend_normal,
                 float* __restrict__ rend_dist, float* __restrict__ depth_median, float* __restrict__ depth_expected,
-                float* __restrict__ surf_depth) {
+                float* __restrict__ surf_depth, const Frames fr) {
     const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
     if (x >= W || y >= H) return;
     const size_t N = (size_t)W * H, p = (size_t)y * W + x;
-    const PostCam c = load_cam(wvt, W, H, tanx, tany);
+    const int f = FRAMES ? (int)blockIdx.z : 0;
+    if constexpr (FRAMES) {
+        allmap += (size_t)f * 8 * N; wvt += (size_t)f * 16; acc += (size_t)f * N; rend_normal += (size_t)f * 3 * N;
+        rend_dist += (size_t)f * N; depth_median += (size_t)f * N; depth_expected += (size_t)f * N; surf_depth += (size_t)f * N;
+    }
+    const PostCam c = frame_cam<TABLE>(fr, f, wvt, W, H, tanx, tany);
     const float a = allmap[N + p];
+    if constexpr (FRAMES) {
+        if (fr.bkgd) {   // deformable_gaussian.py:188-190: color[:3] + (1 - acc) * bkgd, each operation rounded
+            float* col = fr.color + (size_t)f * fr.color_stride;
+            const float om = __fadd_rn(1.0f, -a);
+#pragma unroll
+            for (int k = 0; k < 3; k++) col[k * N + p] = __fadd_rn(col[k * N + p], __fmul_rn(om, __ldg(fr.bkgd + k)));
+        }
+    }
     const float n0 = allmap[2 * N + p], n1 = allmap[3 * N + p], n2 = allmap[4 * N + p];
     acc[p] = a;
     rend_normal[p] = c.R[0] * n0 + c.R[1] * n1 + c.R[2] * n2;
@@ -36,15 +71,20 @@ post_fwd_kernel(int W, int H, float tanx, float tany, float depth_ratio, const f
 }
 
 // surf_normal needs the neighbours' surf_depth: second (tiny) kernel
+template <bool FRAMES, bool TABLE>
 __global__ void __launch_bounds__(256)
 post_normal_kernel(int W, int H, float tanx, float tany, const float* __restrict__ allmap, const float* __restrict__ wvt,
-                   const float* __restrict__ surf_depth, float* __restrict__ surf_normal) {
+                   const float* __restrict__ surf_depth, float* __restrict__ surf_normal, const Frames fr) {
     const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
     if (x >= W || y >= H) return;
     const size_t N = (size_t)W * H, p = (size_t)y * W + x;
+    const int f = FRAMES ? (int)blockIdx.z : 0;
+    if constexpr (FRAMES) {
+        allmap += (size_t)f * 8 * N; wvt += (size_t)f * 16; surf_depth += (size_t)f * N; surf_normal += (size_t)f * 3 * N;
+    }
     float o0 = 0.f, o1 = 0.f, o2 = 0.f;
     if (x >= 1 && x < W - 1 && y >= 1 && y < H - 1) {
-        const PostCam c = load_cam(wvt, W, H, tanx, tany);
+        const PostCam c = frame_cam<TABLE>(fr, f, wvt, W, H, tanx, tany);
         float ax, ay, az, bx, by, bz, ex, ey, ez, fx, fy, fz;
         ray_dir(c, x, y + 1, ax, ay, az); ray_dir(c, x, y - 1, bx, by, bz);
         ray_dir(c, x + 1, y, ex, ey, ez); ray_dir(c, x - 1, y, fx, fy, fz);
@@ -142,12 +182,41 @@ SR_API int sr_post_forward(int32_t W, int32_t H, float tanx, float tany, float d
     dim3 grid((W + 31) / 32, (H + 7) / 8);
     {
         ProfileScope ps("post_fwd", s);
-        post_fwd_kernel<<<grid, 256, 0, s>>>(W, H, tanx, tany, depth_ratio, allmap, world_view_transform, acc, rend_normal,
-                                            rend_dist, depth_median, depth_expected, surf_depth);
+        post_fwd_kernel<false, false><<<grid, 256, 0, s>>>(W, H, tanx, tany, depth_ratio, allmap, world_view_transform, acc,
+                                                   rend_normal, rend_dist, depth_median, depth_expected, surf_depth, Frames{});
     }
     ProfileScope ps("post_normal", s);
-    post_normal_kernel<<<grid, 256, 0, s>>>(W, H, tanx, tany, allmap, world_view_transform, surf_depth, surf_normal);
+    post_normal_kernel<false, false><<<grid, 256, 0, s>>>(W, H, tanx, tany, allmap, world_view_transform, surf_depth, surf_normal,
+                                                  Frames{});
     return sr_launched(2, "sr_post_forward");
+}
+
+SR_API int sr_post_forward_frames(int32_t M, int32_t W, int32_t H, float tanx, float tany, const float* cameras,
+                                  float depth_ratio, const float* allmap, const float* world_view_transform,
+                                  const float* learnable_bkgd, float* color, int64_t color_stride, float* acc,
+                                  float* rend_normal, float* rend_dist, float* depth_median, float* depth_expected,
+                                  float* surf_depth, float* surf_normal, void* stream_) {
+    if (M < 1 || M > 65535) return sr_fail(SR_EINVAL, "sr_post_forward_frames: M must be in [1, 65535], got %d", M);
+    if (W <= 0 || H <= 0) return sr_fail(SR_EINVAL, "sr_post_forward_frames: image size must be positive");
+    if (!allmap || !world_view_transform || !acc || !rend_normal || !rend_dist || !depth_median || !depth_expected || !surf_depth ||
+        !surf_normal)
+        return sr_fail(SR_EINVAL, "sr_post_forward_frames: a required pointer is NULL");
+    if (learnable_bkgd && !color) return sr_fail(SR_EINVAL, "sr_post_forward_frames: learnable_bkgd is given but color is NULL");
+    if (learnable_bkgd && color_stride < 3ll * W * H)
+        return sr_fail(SR_EINVAL, "sr_post_forward_frames: color frame stride must be >= 3*H*W");
+    cudaStream_t s = (cudaStream_t)stream_;
+    const Frames fr{cameras, learnable_bkgd, color, (long long)color_stride};
+    dim3 grid((W + 31) / 32, (H + 7) / 8, M);
+    {
+        ProfileScope ps("post_fwd_frames", s);
+        auto k = cameras ? post_fwd_kernel<true, true> : post_fwd_kernel<true, false>;
+        k<<<grid, 256, 0, s>>>(W, H, tanx, tany, depth_ratio, allmap, world_view_transform, acc, rend_normal, rend_dist,
+                               depth_median, depth_expected, surf_depth, fr);
+    }
+    ProfileScope ps("post_normal_frames", s);
+    auto k = cameras ? post_normal_kernel<true, true> : post_normal_kernel<true, false>;
+    k<<<grid, 256, 0, s>>>(W, H, tanx, tany, allmap, world_view_transform, surf_depth, surf_normal, fr);
+    return sr_launched(2, "sr_post_forward_frames");
 }
 
 SR_API int sr_post_backward(int32_t W, int32_t H, float tanx, float tany, float depth_ratio, const float* allmap,

@@ -262,16 +262,28 @@ def _frame(P, degree, Msh, W, H, tan_fovx, tan_fovy, scale_modifier, prefiltered
     return fc, C.byref(fc.frame)
 
 
+class _RenderOut:
+    """Where a forward-only _forward writes: preallocated, packed views of the caller's (T,...) outputs for this call's
+    frames (color (M,3,H,W), features (M,F,H,W) or None, others (M,8,H,W), radii (M,P)), and the arena that the calls of
+    one render share (include/surfel_render.h), grown only when a call needs more."""
+    __slots__ = ("color", "features", "others", "radii", "arena")
+
+    def __init__(self, color, features, others, radii, arena=None):
+        self.color, self.features, self.others, self.radii, self.arena = color, features, others, radii, arena
+
+
 def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, scales, rotations, features, viewmatrix,
              projmatrix, campos, H, W, degree, tan_fovx, tan_fovy, scale_modifier, prefiltered, debug, concat=True,
-             intrinsics=None):
+             intrinsics=None, render=None):
     """The one sr_forward call behind every _C forward: M frames, F = 0 without features.  The caller has validated the
     inputs and made them contiguous float32 CUDA tensors; `strides` gives the floats between consecutive frames of each
     per-surfel input (absent = shared).  intrinsics: the checked (M,4) camera table, which replaces tan_fovx / tan_fovy,
     or None.  The outputs get a leading frame dimension iff frame_dim.  In sync mode an
     overflowed call is re-run with a larger instance buffer; in nosync mode the status words join _pending.
     Returns (num_rendered (list of M ints, or -1 in nosync mode), out_color, out_others, radii, geom, binning, img,
-    out_feat): with concat, out_color holds 3+F planes per frame and out_feat is the view of the last F; None when F = 0."""
+    out_feat): with concat, out_color holds 3+F planes per frame and out_feat is the view of the last F; None when F = 0.
+    render: a _RenderOut -- forward-only (sr_render_forward): the outputs are its views, the scratch is its arena, nothing
+    is kept for a backward (geom, binning and img are None), and the instance counts are read back in either sync mode."""
     lib = _capi.load()
     dev = means3D.device
     P, N = int(means3D.shape[-2]), H * W
@@ -281,7 +293,10 @@ def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, sc
     fr, frp = _frame(P, degree, Msh, W, H, tan_fovx, tan_fovy, scale_modifier, prefiltered, debug, intrinsics)
     bt = _capi.SrBatch(M, 0, *(strides.get(k, 0) for k in _STRIDED))
     with torch.cuda.device(dev):
-        if F and concat:
+        if render is not None:
+            out_color, out_feat, out_others, radii = render.color, render.features, render.others, render.radii
+            cstride, fstride = 3 * N, F * N
+        elif F and concat:
             out_color = torch.empty(lead + (3 + F, H, W), dtype=torch.float32, device=dev)
             out_feat = out_color[..., 3:, :, :]
             cstride = fstride = (3 + F) * N
@@ -289,23 +304,33 @@ def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, sc
             out_color = torch.empty(lead + (3, H, W), dtype=torch.float32, device=dev)
             out_feat = torch.empty(lead + (F, H, W), dtype=torch.float32, device=dev) if F else None
             cstride, fstride = 3 * N, F * N
-        out_others = torch.empty(lead + (8, H, W), dtype=torch.float32, device=dev)
-        radii = torch.empty(lead + (P,), dtype=torch.int32, device=dev)
-        geom = torch.empty((M * lib.sr_geom_bytes(P),), dtype=torch.uint8, device=dev)
-        img = torch.empty((M * lib.sr_image_bytes(W, H),), dtype=torch.uint8, device=dev)
+        geom = binning = img = None
+        if render is None:
+            out_others = torch.empty(lead + (8, H, W), dtype=torch.float32, device=dev)
+            radii = torch.empty(lead + (P,), dtype=torch.int32, device=dev)
+            geom = torch.empty((M * lib.sr_geom_bytes(P),), dtype=torch.uint8, device=dev)
+            img = torch.empty((M * lib.sr_image_bytes(W, H),), dtype=torch.uint8, device=dev)
         nr_dev = torch.empty((M, 2), dtype=torch.int32, device=dev)
         stream = torch.cuda.current_stream(dev)
         key = (dev.index, W, H)
         cap = _pick_capacity(key, P)
         while True:
-            binning = torch.empty((M * lib.sr_binning_bytes(cap, W, H),), dtype=torch.uint8, device=dev)
-            nosync = (not _sync_mode) and key in _cap_hint
+            nosync = render is None and (not _sync_mode) and key in _cap_hint
             host = _host_slot(M) if nosync else torch.empty((M, 2), dtype=torch.int32, pin_memory=True)
+            args = (dev, frp, C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh), _ptr(colors),
+                    _ptr(opacity), _ptr(scales), _ptr(rotations), _ptr(features), F, strides.get("features", 0),
+                    _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), out_color, cstride, _ptr(out_feat), fstride, out_others,
+                    _ptr(radii))
             # an overflow re-run below re-runs the feature pass too
-            _capi.call("sr_forward", dev, frp, C.byref(bt), _ptr(background), int(background.numel()), _ptr(means3D), _ptr(sh),
-                       _ptr(colors), _ptr(opacity), _ptr(scales), _ptr(rotations), _ptr(features), F, strides.get("features", 0),
-                       _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos), out_color, cstride, _ptr(out_feat), fstride, out_others,
-                       _ptr(radii), geom, binning, img, cap, nr_dev, host)
+            if render is None:
+                binning = torch.empty((M * lib.sr_binning_bytes(cap, W, H),), dtype=torch.uint8, device=dev)
+                _capi.call("sr_forward", *args, geom, binning, img, cap, nr_dev, host)
+            else:
+                need = M * int(lib.sr_render_bytes(P, cap, W, H))
+                if render.arena is None or render.arena.numel() < need:
+                    render.arena = None                  # release the smaller arena before allocating its successor
+                    render.arena = torch.empty((need,), dtype=torch.uint8, device=dev)
+                _capi.call("sr_render_forward", *args, render.arena, cap, nr_dev, host)
             if nosync:
                 _pending.append((host, key, cap, stream))
                 if len(_pending) > _MAX_PENDING:

@@ -674,3 +674,104 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
     if mask_loss is not None:
         out["mask_terms"], out["mask_counts"] = outs[k], outs[k + 1]
     return out
+
+
+# ---------------------------------------------------------------------------------------------
+# Forward-only rendering of a trained sequence: what lab4d/engine/model.py:186-284 (evaluate) renders frame pair by
+# frame pair under torch.no_grad(), in chunks of frames with no backward state (include/surfel_render.h).
+# ---------------------------------------------------------------------------------------------
+def _check_render_frames(T, P, device, bg_color, means3D, rotations, features, learnable_bkgd, frames_per_call):
+    """Validate render_frames' arguments before anything runs on the device; returns F."""
+    if isinstance(frames_per_call, bool) or not isinstance(frames_per_call, int) or frames_per_call < 1:
+        raise RuntimeError(f"frames_per_call must be an int >= 1, got {frames_per_call!r}")
+    for name, t, tail in (("means3D", means3D, 3), ("rotations", rotations, 4)):
+        if t is not None and (t.ndim != 3 or tuple(t.shape) != (T, P, tail)):
+            raise RuntimeError(f"{name} must be (T,P,{tail}) = ({T},{P},{tail}) or None, got {tuple(t.shape)}")
+    F = 0
+    if features is not None:
+        from .rasterizer import _check_features
+        if torch.is_tensor(features) and features.ndim == 3 and int(features.shape[0]) != T:
+            raise RuntimeError(f"features must be (P,F) or (T,P,F) with T = {T}, got {tuple(features.shape)}")
+        F = _check_features(features, P, bg_color, batched=True)
+    elif int(bg_color.numel()) != 3:
+        raise RuntimeError(f"bg_color must have 3 values without features, got {int(bg_color.numel())}")
+    if learnable_bkgd is not None:
+        if learnable_bkgd.numel() != 3:
+            raise RuntimeError(f"learnable_bkgd must have 3 elements, got shape {tuple(learnable_bkgd.shape)}")
+        if not learnable_bkgd.is_cuda or learnable_bkgd.device != device:
+            raise RuntimeError(f"learnable_bkgd must be a CUDA tensor on the rasterizer's device {device}, got {learnable_bkgd.device}")
+    return F
+
+
+def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, features=None, learnable_bkgd=None,
+                  frames_per_call=8):
+    """Render T frames forward-only: render_fused()'s outputs for every frame, with a leading frame dimension, and nothing
+    differentiable -- no autograd graph is built, even when the inputs require grad.
+
+    cameras: BatchCameras of T frames (or a list of cameras, stacked here), with or without `intrinsics`.  pc, pipe: as in
+    render().  means3D (T,P,3) / rotations (T,P,4): optional per-frame surfels (the bob-warped copies, as in
+    render_loss_batch); default pc.get_xyz / pc.get_rotation for every frame.  features: optional (P,F) or (T,P,F),
+    1 <= F <= 32, composited with the colour's weights (bg_color may then have 3+F values).  learnable_bkgd: optional (3,):
+    "render" becomes render + (1 - acc) * learnable_bkgd, as DeformableGaussian.render_view adds it
+    (deformable_gaussian.py:188-190).
+
+    The frames are rendered frames_per_call at a time (csrc/composite_fwd.cu's forward-only walk, which keeps no backward
+    state and composites the feature channels in the colour's walk; then csrc/postprocess.cu over the chunk) straight into
+    the (T,...) outputs.  One arena, sized for the largest chunk, serves every chunk; each chunk reads its instance counts
+    back once and re-runs with a larger capacity if it overflowed.  Colour, features, allmap-derived maps and radii are
+    bit-identical to the training forward's (_C.rasterize_gaussians_batch) followed by sr_post_forward per frame.
+
+    Returns {"render": (T,3,H,W), "features": (T,F,H,W) (with features), "acc": (T,1,H,W), "rend_normal": (T,3,H,W),
+    "rend_dist": (T,1,H,W), "surf_depth", "render_depth_median", "render_depth_expected": (T,3,H,W) broadcast views of one
+    plane each, "surf_normal": (T,3,H,W), "radii": (T,P) int32, "visibility_filter": (T,P) bool}."""
+    from . import _capi
+    from .rasterizer import _RenderOut, _batch_inputs, _check_intrinsics, _f32c, _forward
+    if not isinstance(cameras, BatchCameras):
+        cameras = stack_cameras(cameras)
+    T, H, W = len(cameras), int(cameras.image_height), int(cameras.image_width)
+    xyz = pc.get_xyz if means3D is None else means3D
+    P, dev = int(xyz.shape[-2]), xyz.device
+    F = _check_render_frames(T, P, dev, bg_color, means3D, rotations, features, learnable_bkgd, frames_per_call)
+    intr = _check_intrinsics(cameras.intrinsics, T, xyz)
+    tanx, tany = (0.0, 0.0) if intr is not None else _cam_tans(cameras)     # the table replaces them
+    N = H * W
+    with torch.no_grad(), torch.cuda.device(dev):
+        rot = pc.get_rotation if rotations is None else rotations
+        ins, strides = _batch_inputs(T, means3D=(xyz.detach(), (3,)), sh=(pc.get_features.detach(), None),
+                                     opacity=(pc.get_opacity.detach(), (1,)), scales=(pc.get_scaling.detach(), (2,)),
+                                     rotations=(rot.detach(), (4,)),
+                                     features=(None if features is None else features.detach(), None))
+        bg = _f32c(bg_color.detach(), "bg_color")
+        vm = _f32c(cameras.world_view_transform.detach(), "world_view_transform")
+        pm = _f32c(cameras.full_proj_transform.detach(), "full_proj_transform")
+        cp = _f32c(cameras.camera_center.detach(), "camera_center")
+        bk = None if learnable_bkgd is None else _f32c(learnable_bkgd.detach().reshape(3), "learnable_bkgd")
+        mk = lambda *shape, dtype=torch.float32: torch.empty((T,) + shape, dtype=dtype, device=dev)  # noqa: E731
+        color, feat = mk(3, H, W), (mk(F, H, W) if F else None)
+        acc, rn, dist, med, ex, sd, sn = mk(1, H, W), mk(3, H, W), mk(1, H, W), mk(1, H, W), mk(1, H, W), mk(1, H, W), mk(3, H, W)
+        radii = mk(P, dtype=torch.int32)
+        n = min(frames_per_call, T)
+        allmap = torch.empty((n, 8, H, W), dtype=torch.float32, device=dev)     # one chunk's, reused
+        out = _RenderOut(None, None, None, None)
+        for t0 in range(0, T, n):
+            t1 = min(T, t0 + n)
+            c = slice(t0, t1)
+            # per-frame inputs are sliced (their strides stay); shared ones pass whole
+            sl = {k: (v[c] if v is not None and strides.get(k, 0) else v) for k, v in ins.items()}
+            out.color, out.features, out.others, out.radii = color[c], (feat[c] if F else None), allmap[:t1 - t0], radii[c]
+            # P = 0: the empty tensors give the device and F (their pointers pass as NULL)
+            xyz_c = sl["means3D"] if sl["means3D"] is not None else xyz
+            feat_c = sl["features"] if sl["features"] is not None else features
+            _forward(t1 - t0, True, strides, bg, xyz_c, sl["sh"], None, sl["opacity"], sl["scales"], sl["rotations"],
+                     feat_c, vm[c], pm[c], cp[c], H, W, pc.active_sh_degree, tanx, tany, 1.0, False, False,
+                     intrinsics=None if intr is None else intr[c], render=out)
+            _capi.call("sr_post_forward_frames", dev, t1 - t0, W, H, tanx, tany, None if intr is None else intr[c],
+                       float(pipe.depth_ratio), out.others, vm[c], bk, color[c], 3 * N, acc[c], rn[c], dist[c], med[c], ex[c],
+                       sd[c], sn[c])
+        del out, allmap
+        rets = {"render": color, "acc": acc, "rend_normal": rn, "rend_dist": dist, "surf_depth": sd.expand(T, 3, H, W),
+                "render_depth_median": med.expand(T, 3, H, W), "render_depth_expected": ex.expand(T, 3, H, W),
+                "surf_normal": sn, "radii": radii, "visibility_filter": radii > 0}
+        if F:
+            rets["features"] = feat
+    return rets
