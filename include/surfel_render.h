@@ -39,6 +39,34 @@ SR_API int sr_render_forward(const sr_frame* f, const sr_batch* b, const float* 
                              float* out_others, int32_t* radii, void* arena, int64_t capacity, uint32_t* num_rendered_dev,
                              uint32_t* num_rendered_host, void* stream);
 
+/* Per-surfel contribution statistics, DEVICE arrays of P words each.  A pair (frame, pixel, surfel) contributes when the
+ * composite blends it; its weight is w = T * alpha rounded once to float32 (the feature plane of a feature equal to 1),
+ * and its quantised weight q(w) = round-to-nearest-even(w * 2^32), an integer below 2^32.  Over the contributing pairs:
+ *   weight_q[s]    sum of q(w)                        (unsigned 64-bit)
+ *   max_weight[s]  max of w, as its float32 bits      (non-negative floats order as unsigned integers)
+ *   pixels[s]      number of pairs                    (unsigned 64-bit)
+ * All three are integer sums or maxima: exact, and independent of the order in which pairs, frames or calls add. */
+typedef struct sr_contrib {
+    uint64_t* weight_q;
+    uint32_t* max_weight;
+    uint64_t* pixels;
+} sr_contrib;
+
+/* sr_render_forward, which it is in every argument, output and check, that also ADDS every rendered frame's contributing
+ * pairs into `contrib` (never cleared here).  An overflowed frame is not composited and adds nothing: re-running it
+ * alone with a larger capacity adds it once (re-running a whole call would add its other frames twice).  With P > 0 the
+ * three pointers must be non-NULL, weight_q and pixels 8-byte aligned, max_weight 4-byte aligned.  contrib = NULL is
+ * sr_render_forward: the same kernels and bits. */
+SR_API int sr_render_forward_contrib(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+                                     const float* means3D, const float* shs, const float* colors_precomp,
+                                     const float* opacities, const float* scales, const float* rotations,
+                                     const float* features, int32_t F, int64_t features_stride, const float* viewmatrix,
+                                     const float* projmatrix, const float* campos, float* out_color,
+                                     int64_t out_color_stride, float* out_features, int64_t out_features_stride,
+                                     float* out_others, int32_t* radii, void* arena, int64_t capacity,
+                                     uint32_t* num_rendered_dev, uint32_t* num_rendered_host, const sr_contrib* contrib,
+                                     void* stream);
+
 /* sr_post_forward over M frames in one launch: frame m's allmap (allmap + m*8*H*W) and world_view_transform (+ m*16) give
  * its acc, rend_normal, rend_dist, depth_median, depth_expected, surf_depth, surf_normal (each output packed (M, c, H, W)).
  * cameras: optional DEVICE (M,4) table of surfel_camera.h; with it frame m's rays use its own tangents and principal

@@ -7,7 +7,13 @@ frames/s (median over repeats of CUDA-event time, with min and max), per-kernel 
 pass, and peak allocator bytes above the inputs.  The two arms' colour, feature planes, radii and maps are compared bit
 for bit at every timed size.  Prints one JSON object; --out writes it too.
 
-Usage: python tools/bench_render.py [--frames 64] [--chunk 8] [--repeats 7] [--out bench_render.json]
+--contrib measures the per-surfel contribution statistics instead: render_frames without, with, and again without a
+SurfelContributions accumulator (alternating, L2 flushed by a 256 MB write before every timed call), at 512^2 and F in
+{0, 22}, scalar cameras; then the fraction of the scene prune_by_contribution's defaults remove (no frame blends them)
+and render_frames' time before and after that prune, with the renders compared bit for bit.  Every timing is repeated in
+--rounds rounds of one process.
+
+Usage: python tools/bench_render.py [--frames 64] [--chunk 8] [--repeats 7] [--contrib [--rounds 3]] [--out FILE]
 """
 from __future__ import annotations
 
@@ -124,12 +130,112 @@ def timed(fn, repeats):
     return times
 
 
+def _flushed(fn, flush, repeats, i0=0):
+    """CUDA-event ms of fn() per repeat, each after a 256 MB write that evicts L2."""
+    times = []
+    for i in range(repeats):
+        flush.fill_((i0 + i) & 255)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        out = fn()
+        e1.record()
+        torch.cuda.synchronize()
+        times.append(e0.elapsed_time(e1))
+        del out
+    return times
+
+
+def _stat(t, frames):
+    t = np.asarray(t)
+    return {"ms_median": float(np.median(t)), "ms_min": float(t.min()), "ms_max": float(t.max()),
+            "fps_median": frames / (float(np.median(t)) / 1e3)}
+
+
+def contrib_main(args, gpu):
+    """--contrib: `rounds` rounds in one process.  Each round times, for F = 0 and 22, three arms alternating -- plain,
+    with the accumulator, plain again (an A/A control: the gap between the two plain arms is the noise floor of the
+    paired comparison) -- then the prune pair (the scene before and after prune_by_contribution).  Every round's
+    medians are reported, so drift over the process shows beside the paired differences."""
+    from vidu4d_b200.renderer import SurfelContributions
+    from vidu4d_b200.synthetic import object_scene
+    dev = torch.device("cuda:0")
+    s = object_scene(args.P, seed=0, opacity="trained", center=(0.0, 0.0, 0.0)).to_torch(dev)
+    pc = _PC(s)
+    g = torch.Generator(device=dev).manual_seed(0)
+    flush = torch.empty((256 << 20,), dtype=torch.uint8, device=dev)
+    res = 512
+    cams = _cams(args.frames, res, dev, False)
+    bg = torch.zeros(3, device=dev)
+    feats = {0: None, 22: torch.rand((args.P, 22), device=dev, generator=g) * 2 - 1}
+    acc = SurfelContributions.zeros(args.P, dev)
+
+    def with_acc(feat):
+        for t in (acc.weight_q, acc.max_weight, acc.pixels, acc.frames):
+            t.zero_()
+        return render_frames_contrib(cams, pc, bg, feat, args.chunk, acc)
+
+    # what no frame blends, from one accumulated render (the statistics do not depend on F)
+    with_acc(None)
+    keep = ~acc.prune_mask()
+    pruned = {"P_before": args.P, "P_after": int(keep.sum()), "pruned_fraction": float((~keep).sum()) / args.P,
+              "kept_by_no_frame": int((acc.frames == 0).sum())}
+    pcp = _PC({k: v[keep].contiguous() for k, v in s.items()})
+    ident = {}
+    for F, feat in feats.items():
+        a, b = new(cams, pc, bg, feat, args.chunk), with_acc(feat)
+        ident[F] = all(_same(a[k], b[k]) for k in a if k != "visibility_filter")
+    a, b = new(cams, pc, bg, None, args.chunk), new(cams, pcp, bg, None, args.chunk)
+    pruned["identical_images"] = all(_same(a[k], b[k]) for k in a if k not in ("visibility_filter", "radii"))
+    del a, b
+    rounds = []
+    for rd in range(args.rounds):
+        rows = []
+        for F, feat in feats.items():
+            arms = {"plain": lambda: new(cams, pc, bg, feat, args.chunk), "contrib": lambda: with_acc(feat),
+                    "plain_again": lambda: new(cams, pc, bg, feat, args.chunk)}
+            for fn in arms.values():          # warm-up
+                fn()
+            times = {k: [] for k in arms}
+            for r in range(args.repeats):
+                for k, fn in arms.items():
+                    times[k] += _flushed(fn, flush, 1, r)
+            row = {"round": rd, "res": res, "F": F, "identical_outputs": ident[F],
+                   **{k: _stat(v, args.frames) for k, v in times.items()}}
+            base = 0.5 * (row["plain"]["ms_median"] + row["plain_again"]["ms_median"])
+            row["overhead"] = row["contrib"]["ms_median"] / base - 1.0
+            row["plain_gap"] = row["plain_again"]["ms_median"] / row["plain"]["ms_median"] - 1.0
+            print(json.dumps(row), flush=True)
+            rows.append(row)
+        arms = {"before": lambda: new(cams, pc, bg, None, args.chunk), "after": lambda: new(cams, pcp, bg, None, args.chunk)}
+        for fn in arms.values():
+            fn()
+        times = {k: [] for k in arms}
+        for r in range(args.repeats):
+            for k, fn in arms.items():
+                times[k] += _flushed(fn, flush, 1, r)
+        prune = {"round": rd, **{k: _stat(v, args.frames) for k, v in times.items()}}
+        prune["speedup"] = prune["before"]["ms_median"] / prune["after"]["ms_median"]
+        print(json.dumps(prune), flush=True)
+        rounds.append({"rows": rows, "prune": prune})
+    out = {"gpu": gpu, "frames": args.frames, "frames_per_call": args.chunk, "P": args.P, "repeats": args.repeats,
+           "pruned": pruned, "rounds": rounds}
+    print(json.dumps(out))
+    return out
+
+
+def render_frames_contrib(cams, pc, bg, feat, chunk, acc):
+    from vidu4d_b200.renderer import PipelineParams, render_frames
+    return render_frames(cams, pc, PipelineParams(), bg, features=feat, frames_per_call=chunk, contributions=acc)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=64)
     ap.add_argument("--chunk", type=int, default=8)
     ap.add_argument("--repeats", type=int, default=7)
     ap.add_argument("--P", type=int, default=300_000)
+    ap.add_argument("--contrib", action="store_true", help="measure the contribution statistics and the prune by them")
+    ap.add_argument("--rounds", type=int, default=3, help="--contrib: rounds of every measurement in one process")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -139,6 +245,13 @@ def main():
     dev = torch.device("cuda:0")
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip()
+    if args.contrib:
+        out = contrib_main(args, gpu)
+        if args.out:
+            os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+            with open(args.out, "w") as f:
+                json.dump(out, f, indent=1)
+        return
     s = object_scene(args.P, seed=0, opacity="trained", center=(0.0, 0.0, 0.0)).to_torch(dev)
     pc = _PC(s)
     g = torch.Generator(device=dev).manual_seed(0)

@@ -39,8 +39,16 @@ KERNELS = [
     (r"emit_keys_kernel\(", r"emit_keys_kernel\("),
     (r"scan_block_sums_kernel\(", r"scan_block_sums_kernel\("),
     (r"mark_visible_kernel\(", r"mark_visible_kernel\("),
-    # the training instantiation of the composite forward (the forward-only ones are <(bool)0, ...>)
-    (r"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0>)?\(", r"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0>)?\("),
+    # the training instantiation of the composite forward (the forward-only ones are <(bool)0, ...>); a fourth template
+    # parameter, STATS = (bool)0, names the instantiations that gather no contribution statistics
+    (r"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0(, \(bool\)0)?>)?\(",
+     r"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0(, \(bool\)0)?>)?\("),
+    # the forward-only instantiations: (V, NF) = (1, 0), and V in {4, 2, 1} for NF in {8, 16, 24, 32}
+] + [
+    (rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}(, \(bool\)0)?>\(",
+     rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}(, \(bool\)0)?>\(")
+    for v, nf in [(1, 0)] + [(v, nf) for nf in (8, 16, 24, 32) for v in (4, 2, 1)]
+] + [
     (r"feature_fwd_kernel<\(int\)4>\(", r"feature_fwd_kernel<\(int\)4>\("),
     (r"feature_fwd_kernel<\(int\)2>\(", r"feature_fwd_kernel<\(int\)2>\("),
     (r"feature_fwd_kernel<\(int\)1>\(", r"feature_fwd_kernel<\(int\)1>\("),

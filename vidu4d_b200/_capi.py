@@ -45,6 +45,11 @@ class SrBatchDet(C.Structure):
     _fields_ = [("batch", SrBatch), ("scratch", C.c_void_p), ("scratch_bytes", C.c_int64)]
 
 
+class SrContrib(C.Structure):
+    """sr_contrib (include/surfel_render.h): the DEVICE per-surfel statistics sr_render_forward_contrib adds into."""
+    _fields_ = [("weight_q", C.c_void_p), ("max_weight", C.c_void_p), ("pixels", C.c_void_p)]
+
+
 class SrDebugLayout(C.Structure):
     _fields_ = [
         ("surfel_rec", C.c_size_t), ("depths", C.c_size_t), ("tiles_touched", C.c_size_t),
@@ -159,6 +164,8 @@ RENDER_PROTOTYPES = {
     "sr_render_bytes": (C.c_size_t, [_i32, _i64, _i32, _i32]),
     "sr_render_forward": (C.c_int, [_FRAME, _BATCH, _p, _i32] + [_p] * 7 + [_i32, _i64] + [_p] * 3 + [_p, _i64, _p, _i64]
                           + [_p] * 3 + [_i64, _p, _p, _p]),
+    "sr_render_forward_contrib": (C.c_int, [_FRAME, _BATCH, _p, _i32] + [_p] * 7 + [_i32, _i64] + [_p] * 3
+                                  + [_p, _i64, _p, _i64] + [_p] * 3 + [_i64, _p, _p, _p, _p]),
     "sr_post_forward_frames": (C.c_int, [_i32] * 3 + [_f32] * 2 + [_p, _f32] + [_p] * 4 + [_i64] + [_p] * 8),
 }
 RENDER_SYMBOLS = tuple(RENDER_PROTOTYPES)

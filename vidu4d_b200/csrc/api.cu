@@ -204,7 +204,7 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
                          const float* viewmatrix, const float* campos, float* out_color, int64_t color_stride,
                          float* out_others, int32_t* radii, void* geom_buffer, void* binning_buffer, void* image_buffer,
                          int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host, void* stream_,
-                         FeatArgs* ft, bool forward_only) {
+                         FeatArgs* ft, bool forward_only, const ContribArgs* contrib) {
     if (int rc = check_frame(f)) return rc;
     if (!b || b->frames < 1 || b->frames > 65535) return sr_fail(SR_EINVAL, "batch descriptor: frames must be in [1, 65535]");
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -230,6 +230,12 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
             return sr_fail(SR_EINVAL, "scratch buffer is NULL");
         }
         if (capacity <= 0 || capacity >= (1ll << 30)) return sr_fail(SR_EINVAL, "capacity must be in (0, 2^30)");
+        if (contrib) {
+            if (!contrib->weight_q || !contrib->max_weight || !contrib->pixels)
+                return sr_fail(SR_EINVAL, "contribution statistics pointer is NULL");
+            if (((uintptr_t)contrib->weight_q & 7) || ((uintptr_t)contrib->pixels & 7) || ((uintptr_t)contrib->max_weight & 3))
+                return sr_fail(SR_EINVAL, "contribution statistics: weight_q / pixels must be 8-byte aligned, max_weight 4-byte aligned");
+        }
         // 128-bit / 64-bit vector loads: rotations as float4, scales as float2, SH rows as float4 when 3M % 4 == 0
         if (((uintptr_t)rotations & 15) || ((uintptr_t)scales & 7) || (shs && ((uintptr_t)shs & 15)) ||
             ((b->rotations * 4) & 15) || ((b->scales * 4) & 7) || ((b->shs * 4) & 15))
@@ -264,7 +270,7 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
     a.prefiltered = f->prefiltered;
     a.key_bits = 32 + (int)sr_higher_msb((uint32_t)a.il.tiles);
     a.stream = stream; a.debug = debug;
-    a.forward_only = forward_only; a.feat = ft;
+    a.forward_only = forward_only; a.feat = ft; a.contrib = contrib;
     FrameStrides& fs = a.fs;
     fs.frames = M;
     fs.geom = (long long)a.gl.total; fs.bin = (long long)a.bl.total; fs.img = (long long)a.il.total; fs.nr = 2 * sizeof(uint32_t);
@@ -298,19 +304,19 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
 }
 
 namespace {
-// sr_forward and sr_render_forward: the feature arguments, then forward_batch
+// sr_forward, sr_render_forward and sr_render_forward_contrib: the feature arguments, then forward_batch
 int forward_entry(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels, const float* means3D,
                   const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
                   const float* rotations, const float* features, int32_t F, int64_t features_stride, const float* viewmatrix,
                   const float* campos, float* out_color, int64_t out_color_stride, float* out_features,
                   int64_t out_features_stride, float* out_others, int32_t* radii, void* geom_buffer, void* binning_buffer,
                   void* image_buffer, int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host,
-                  void* stream_, bool forward_only) {
+                  void* stream_, bool forward_only, const ContribArgs* contrib = nullptr) {
     if (F == 0) {
         if (int rc = check_no_features(f, features, bg_channels, out_color_stride)) return rc;
         return forward_batch(f, b, background, means3D, shs, colors_precomp, opacities, scales, rotations, viewmatrix, campos,
                              out_color, 0, out_others, radii, geom_buffer, binning_buffer, image_buffer, capacity,
-                             num_rendered_dev, num_rendered_host, stream_, nullptr, forward_only);
+                             num_rendered_dev, num_rendered_host, stream_, nullptr, forward_only, contrib);
     }
     if (int rc = check_features(f, F, bg_channels, features, features_stride)) return rc;
     FeatArgs ft{};
@@ -321,7 +327,7 @@ int forward_entry(const sr_frame* f, const sr_batch* b, const float* background,
     ft.out = out_features; ft.out_stride = out_features_stride * 4;
     return forward_batch(f, b, background, means3D, shs, colors_precomp, opacities, scales, rotations, viewmatrix, campos,
                          out_color, out_color_stride, out_others, radii, geom_buffer, binning_buffer, image_buffer, capacity,
-                         num_rendered_dev, num_rendered_host, stream_, &ft, forward_only);
+                         num_rendered_dev, num_rendered_host, stream_, &ft, forward_only, contrib);
 }
 }  // namespace
 
@@ -351,6 +357,26 @@ int sr_render_forward(const sr_frame* f, const sr_batch* b, const float* backgro
                          features_stride, viewmatrix, campos, out_color, out_color_stride, out_features, out_features_stride,
                          out_others, radii, arena, nullptr, nullptr, capacity, num_rendered_dev, num_rendered_host, stream_,
                          true);
+}
+
+int sr_render_forward_contrib(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+                              const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
+                              const float* scales, const float* rotations, const float* features, int32_t F,
+                              int64_t features_stride, const float* viewmatrix, const float* projmatrix, const float* campos,
+                              float* out_color, int64_t out_color_stride, float* out_features, int64_t out_features_stride,
+                              float* out_others, int32_t* radii, void* arena, int64_t capacity, uint32_t* num_rendered_dev,
+                              uint32_t* num_rendered_host, const sr_contrib* contrib, void* stream_) {
+    (void)projmatrix;
+    ContribArgs cs{};
+    if (contrib) {
+        cs.weight_q = reinterpret_cast<unsigned long long*>(contrib->weight_q);
+        cs.max_weight = contrib->max_weight;
+        cs.pixels = reinterpret_cast<unsigned long long*>(contrib->pixels);
+    }
+    return forward_entry(f, b, background, bg_channels, means3D, shs, colors_precomp, opacities, scales, rotations, features, F,
+                         features_stride, viewmatrix, campos, out_color, out_color_stride, out_features, out_features_stride,
+                         out_others, radii, arena, nullptr, nullptr, capacity, num_rendered_dev, num_rendered_host, stream_,
+                         true, contrib ? &cs : nullptr);
 }
 
 static int backward_batch(const sr_frame* f, const sr_batch* b, const float* background, const float* means3D, const float* shs,

@@ -169,6 +169,13 @@ struct FrameStrides {
 
 // ---- launchers implemented in the .cu files ------------------------------------------------
 struct FeatArgs;
+// Per-surfel contribution statistics of sr_render_forward_contrib (include/surfel_render.h), added into by every
+// contributing (frame, pixel, surfel) pair of the forward-only walk, w = T alpha rounded once
+struct ContribArgs {
+    unsigned long long* weight_q;  // [P] sum of rn(w 2^32)
+    uint32_t* max_weight;          // [P] max of w, as float bits
+    unsigned long long* pixels;    // [P] number of pairs
+};
 struct FwdArgs {
     FrameStrides fs;
     CamParams cam;
@@ -186,6 +193,7 @@ struct FwdArgs {
     // channels `feat` (nullptr when F = 0) in its own walk
     bool forward_only;
     const FeatArgs* feat;
+    const ContribArgs* contrib;   // forward-only: the statistics to add into, or nullptr
 };
 struct BwdArgs {
     FrameStrides fs;

@@ -18,7 +18,12 @@
 //   * two instantiations (DESIGN.md "forward-only render").  TRAIN records the contribution masks, sub_last, final_T and
 //     n_contrib for the backward; the forward-only one (sr_render_forward) records none of them and composites up to NF
 //     feature channels inside the same walk, through FwdPixel::blend's per-pair hook: acc[k] = ff(T, fm(alpha, x[k]),
-//     acc[k]) over the same contributors, weights and order as feature_fwd, so every plane has feature_fwd's bits.
+//     acc[k]) over the same contributors, weights and order as feature_fwd, so every plane has feature_fwd's bits;
+//   * STATS (sr_render_forward_contrib, DESIGN.md "contribution statistics"): the same hook also gathers each surfel's
+//     blending weight w = ff(T, alpha, 0) -- the feature plane of a feature equal to 1 -- into per-warp shared slots, one
+//     per instance of the stage, with integer shared atomics; after the stage lane i adds slot i to its surfel with one
+//     global integer atomic each.  Integer sums and an unsigned max are exact and order-independent: the totals have
+//     the same bits whatever the order of the pairs, frames, chunks or ranks.
 #include "composite_common.cuh"
 
 namespace {
@@ -26,15 +31,29 @@ using namespace comp;
 
 constexpr int WPC = 1;      // independent warps per CTA (2 measured slower: register pressure)
 
-// TRAIN: the training forward (V, NF unused).  Otherwise forward-only with F <= NF feature channels (NF = 0: none), rows
-// gathered V floats per load.
-template <bool TRAIN, int V, int NF>
+// A stage's statistics slots, per warp and instance jj: lo[jj] sums the low 16 bits of q = rn(w 2^32), hc[jj] the high
+// 16 bits plus 2^21 per pair.  q < 2^32 (w <= 0.99) and a stage has at most 32 pairs per instance, so neither word
+// overflows (32 (2^16 - 1) < 2^21, 32 < 2^11) and the stage's sum is (hc mod 2^21) 2^16 + lo, its pair count hc >> 21.
+struct StatSlots {
+    uint32_t lo[WB], hc[WB], mx[WB];
+};
+__device__ __forceinline__ void stat_pair(StatSlots* ss, int jj, float T, float alpha) {
+    const float w = ff(T, alpha, 0.0f);
+    const uint32_t q = __float2uint_rn(fm(w, 4294967296.0f));
+    atomicAdd(&ss->lo[jj], q & 0xffffu);
+    atomicAdd(&ss->hc[jj], (q >> 16) + (1u << 21));
+    atomicMax(&ss->mx[jj], __float_as_uint(w));
+}
+
+// TRAIN: the training forward (V, NF, STATS unused).  Otherwise forward-only with F <= NF feature channels (NF = 0:
+// none), rows gathered V floats per load, and with STATS the contribution statistics added into cs.
+template <bool TRAIN, int V, int NF, bool STATS = false>
 __global__ void __launch_bounds__(32 * WPC)
 composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, const uint32_t* __restrict__ tile_order, int n_items, int tiles_x,
                      const float4* __restrict__ irec, int W, int H,
                      const float* __restrict__ bg, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
                      float* __restrict__ out_color, float* __restrict__ out_others, uint32_t* __restrict__ sub_last,
-                     uint32_t* __restrict__ contrib_masks, const FeatArgs ft) {
+                     uint32_t* __restrict__ contrib_masks, const FeatArgs ft, const ContribArgs cs) {
     // WPC independent warps per CTA (the SM holds at most 32 CTAs): work item = (tile, 8x4 sub-tile), tiles in
     // longest-list-first order; the warps of a CTA share nothing
     __shared__ __align__(128) float4 st_all[WPC][NST][WB * REC4];
@@ -62,6 +81,12 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
     if (lane == 0) {
         ring.init();
         for (int b = 0; b < NST && b < nb; b++) ring.issue(b, b);
+    }
+    StatSlots* ss = nullptr;
+    if constexpr (STATS) {
+        __shared__ StatSlots ss_all[WPC];
+        ss = &ss_all[threadIdx.x >> 5];
+        ss->lo[lane] = 0u; ss->hc[lane] = 0u; ss->mx[lane] = 0u;
     }
     __syncwarp();
 
@@ -105,11 +130,29 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
             if (!act || done) continue;
             if constexpr (TRAIN) {
                 if (px.blend(S + jj * REC4, sp.pixx, sp.pixy, rho_cut, b * WB, jj, cmask)) done = true;
-            } else {
+            } else if constexpr (!STATS) {
                 if (px.blend(S + jj * REC4, sp.pixx, sp.pixy, rho_cut, b * WB, jj, cmask, feat_pair)) done = true;
+            } else {
+                auto pair = [&](float T, float alpha, const float4* __restrict__ R) {
+                    feat_pair(T, alpha, R);
+                    stat_pair(ss, jj, T, alpha);
+                };
+                if (px.blend(S + jj * REC4, sp.pixx, sp.pixy, rho_cut, b * WB, jj, cmask, pair)) done = true;
             }
         }
         __syncwarp();                                   // every lane is done reading stage b
+        if constexpr (STATS) {
+            // lane = instance: its stage totals go to its surfel, and its slot is cleared for the next stage
+            const uint32_t hc = ss->hc[lane];
+            if (hc != 0u) {
+                const uint32_t id = __float_as_uint(S[lane * REC4 + 4].z);
+                atomicAdd(cs.weight_q + id, ((unsigned long long)(hc & 0x1fffffu) << 16) + ss->lo[lane]);
+                atomicMax(cs.max_weight + id, ss->mx[lane]);
+                atomicAdd(cs.pixels + id, (unsigned long long)(hc >> 21));
+                ss->lo[lane] = 0u; ss->hc[lane] = 0u; ss->mx[lane] = 0u;
+            }
+            __syncwarp();                               // slots cleared and stage b read before its slot is refilled
+        }
         if constexpr (TRAIN) cm_out[(size_t)b * SR_CONTRIB_STAGE_WORDS] = cmask;
         cmask = 0u;
         if (__all_sync(0xffffffffu, done)) {
@@ -141,19 +184,28 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
     }
 }
 
-// the forward-only instantiation for F channels (NF = F rounded up to a multiple of 8) and vector width ft.vec
-template <int NF>
-void launch_render(const FwdArgs& a, const FeatArgs& ft, unsigned grid) {
+// the forward-only instantiation for F channels (NF = F rounded up to a multiple of 8), vector width ft.vec and, with
+// STATS, the statistics cs
+template <int NF, bool STATS>
+void launch_render(const FwdArgs& a, const FeatArgs& ft, const ContribArgs& cs, unsigned grid) {
     auto launch = [&](auto kern) {
         kern<<<grid, 32 * WPC, 0, a.stream>>>(
             a.fs, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles * 8, a.il.tiles_x,
             (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, a.cam.bg, nullptr, nullptr, a.out_color, a.out_others,
-            nullptr, nullptr, ft);
+            nullptr, nullptr, ft, cs);
     };
-    if constexpr (NF == 0) launch(composite_fwd_kernel<false, 1, 0>);
-    else if (ft.vec == 4) launch(composite_fwd_kernel<false, 4, NF>);
-    else if (ft.vec == 2) launch(composite_fwd_kernel<false, 2, NF>);
-    else launch(composite_fwd_kernel<false, 1, NF>);
+    if constexpr (NF == 0) launch(composite_fwd_kernel<false, 1, 0, STATS>);
+    else if (ft.vec == 4) launch(composite_fwd_kernel<false, 4, NF, STATS>);
+    else if (ft.vec == 2) launch(composite_fwd_kernel<false, 2, NF, STATS>);
+    else launch(composite_fwd_kernel<false, 1, NF, STATS>);
+}
+template <bool STATS>
+void launch_render_f(const FwdArgs& a, const FeatArgs& ft, const ContribArgs& cs, unsigned grid) {
+    if (ft.F == 0) launch_render<0, STATS>(a, ft, cs, grid);
+    else if (ft.F <= 8) launch_render<8, STATS>(a, ft, cs, grid);
+    else if (ft.F <= 16) launch_render<16, STATS>(a, ft, cs, grid);
+    else if (ft.F <= 24) launch_render<24, STATS>(a, ft, cs, grid);
+    else launch_render<32, STATS>(a, ft, cs, grid);
 }
 
 }  // namespace
@@ -163,11 +215,8 @@ cudaError_t launch_composite_fwd(const FwdArgs& a) {
     if (a.forward_only) {
         ProfileScope ps("composite_render", a.stream);
         const FeatArgs ft = a.feat ? *a.feat : FeatArgs{};
-        if (ft.F == 0) launch_render<0>(a, ft, grid);
-        else if (ft.F <= 8) launch_render<8>(a, ft, grid);
-        else if (ft.F <= 16) launch_render<16>(a, ft, grid);
-        else if (ft.F <= 24) launch_render<24>(a, ft, grid);
-        else launch_render<32>(a, ft, grid);
+        if (a.contrib) launch_render_f<true>(a, ft, *a.contrib, grid);
+        else launch_render_f<false>(a, ft, ContribArgs{}, grid);
         sr_count_launch();
         return cudaGetLastError();
     }
@@ -176,7 +225,7 @@ cudaError_t launch_composite_fwd(const FwdArgs& a) {
         a.fs, (const uint2*)(a.img + a.il.ranges), (const uint32_t*)(a.img + a.il.tile_order), a.il.tiles * 8, a.il.tiles_x,
         (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, a.cam.bg,
         (float*)(a.img + a.il.final_T), (uint32_t*)(a.img + a.il.n_contrib), a.out_color, a.out_others,
-        (uint32_t*)(a.img + a.il.tile_last), (uint32_t*)(a.bin + a.bl.contrib), FeatArgs{});
+        (uint32_t*)(a.img + a.il.tile_last), (uint32_t*)(a.bin + a.bl.contrib), FeatArgs{}, ContribArgs{});
     sr_count_launch();
     return cudaGetLastError();
 }

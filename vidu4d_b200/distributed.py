@@ -11,6 +11,7 @@ backward) and the canonical-surfel gradients are summed across ranks once per op
                      A FlatSurfelModel, whose size changes with densification, uses its own allreduce_grads_.
     shared_generator()   the same random stream on every rank (densify_and_prune's split noise)
     check_replicas()     raise if the ranks' copies of some tensors differ in any bit (a debugging and test aid)
+    allreduce_contributions()   every rank's per-surfel contribution statistics summed over the ranks, exactly
 """
 from __future__ import annotations
 
@@ -111,6 +112,19 @@ def check_replicas(named_tensors: dict, group=None) -> None:
         if bad:
             what = "value or size" if int(got[bad[0], k, 0]) != int(got[0, k, 0]) else "bits"
             raise RuntimeError(f"replicas differ in {name!r} ({what}): ranks {bad} of the group differ from its rank 0")
+
+
+def allreduce_contributions(contrib, group=None):
+    """Make every rank's renderer.SurfelContributions those of all the ranks' frames: SUM over weight_q, pixels and
+    frames (int64 words; the totals stay below 2^63), MAX over max_weight (the float bits as int32, which order as the
+    non-negative floats do).  Integer collectives are exact, so every rank ends with the same bits, those one rank
+    rendering every frame would have, and FlatSurfelModel.prune_by_contribution prunes the same surfels everywhere.
+    In place; returns contrib.  No-op on one rank."""
+    if _multi_rank(group):
+        for t in (contrib.weight_q, contrib.pixels, contrib.frames):
+            dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
+        dist.all_reduce(contrib.max_weight, op=dist.ReduceOp.MAX, group=group)
+    return contrib
 
 
 class FlatGrads:

@@ -265,11 +265,14 @@ def _frame(P, degree, Msh, W, H, tan_fovx, tan_fovy, scale_modifier, prefiltered
 class _RenderOut:
     """Where a forward-only _forward writes: preallocated, packed views of the caller's (T,...) outputs for this call's
     frames (color (M,3,H,W), features (M,F,H,W) or None, others (M,8,H,W), radii (M,P)), and the arena that the calls of
-    one render share (include/surfel_render.h), grown only when a call needs more."""
-    __slots__ = ("color", "features", "others", "radii", "arena")
+    one render share (include/surfel_render.h), grown only when a call needs more.  contrib: an _capi.SrContrib the call
+    adds its contribution statistics into (sr_render_forward_contrib), or None.  With it, a call of M > 1 frames that
+    overflows is not re-run -- its other frames have added already -- and `overflowed` lists the frames to re-run alone."""
+    __slots__ = ("color", "features", "others", "radii", "arena", "contrib", "overflowed")
 
-    def __init__(self, color, features, others, radii, arena=None):
+    def __init__(self, color, features, others, radii, arena=None, contrib=None):
         self.color, self.features, self.others, self.radii, self.arena = color, features, others, radii, arena
+        self.contrib, self.overflowed = contrib, []
 
 
 def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, scales, rotations, features, viewmatrix,
@@ -330,7 +333,10 @@ def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, sc
                 if render.arena is None or render.arena.numel() < need:
                     render.arena = None                  # release the smaller arena before allocating its successor
                     render.arena = torch.empty((need,), dtype=torch.uint8, device=dev)
-                _capi.call("sr_render_forward", *args, render.arena, cap, nr_dev, host)
+                if render.contrib is None:
+                    _capi.call("sr_render_forward", *args, render.arena, cap, nr_dev, host)
+                else:
+                    _capi.call("sr_render_forward_contrib", *args, render.arena, cap, nr_dev, host, C.byref(render.contrib))
             if nosync:
                 _pending.append((host, key, cap, stream))
                 if len(_pending) > _MAX_PENDING:
@@ -347,6 +353,9 @@ def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, sc
             if status & _capi.SR_STATUS_PREFILTER:
                 raise RuntimeError("Point is filtered although prefiltered is set. This shouldn't happen!")
             if status & _capi.SR_STATUS_OVERFLOW:
+                if render is not None and render.contrib is not None and M > 1:
+                    render.overflowed = [m for m, (_, st) in enumerate(words) if st & _capi.SR_STATUS_OVERFLOW]
+                    break
                 cap = _round_cap(int(max(num_rendered) * 1.1) + 4096)
                 continue
             break

@@ -680,6 +680,56 @@ def render_loss_batch(cameras, pc, pipe, bg_color, target_rgb, vis2d=None, mask_
 # Forward-only rendering of a trained sequence: what lab4d/engine/model.py:186-284 (evaluate) renders frame pair by
 # frame pair under torch.no_grad(), in chunks of frames with no backward state (include/surfel_render.h).
 # ---------------------------------------------------------------------------------------------
+@dataclass
+class SurfelContributions:
+    """What every surfel contributes to a set of rendered frames, added into by render_frames(contributions=...).
+
+    A pair (frame, pixel, surfel) contributes when the composite blends it; its weight is w = T * alpha, rounded once to
+    float32 (the feature plane of a feature equal to 1), and its quantised weight q(w) = round-half-even(w * 2^32).  Per
+    surfel, over every contributing pair (include/surfel_render.h, sr_contrib):
+      weight_q   (P,) int64: the sum of q(w), an unsigned 64-bit word (it stays below 2^63)
+      max_weight (P,) int32: the largest w, as its float32 bits (max_weight.view(torch.float32) is the value)
+      pixels     (P,) int64: the number of contributing (frame, pixel) pairs
+      frames     (P,) int64: the number of rendered frames with radii > 0 (those whose preprocess kept the surfel)
+    Every entry is an integer sum or maximum, so the totals have the same bits for any order of the frames, any chunking
+    and, after distributed.allreduce_contributions, any split over ranks.  torch's collectives take no unsigned 64-bit
+    type: the words live in int64 and int32 tensors."""
+    weight_q: torch.Tensor
+    max_weight: torch.Tensor
+    pixels: torch.Tensor
+    frames: torch.Tensor
+
+    @classmethod
+    def zeros(cls, P: int, device) -> "SurfelContributions":
+        z = lambda dt: torch.zeros((int(P),), dtype=dt, device=device)  # noqa: E731
+        return cls(z(torch.int64), z(torch.int32), z(torch.int64), z(torch.int64))
+
+    @property
+    def P(self) -> int:
+        return int(self.weight_q.shape[0])
+
+    @property
+    def weight(self) -> torch.Tensor:
+        """(P,) float64: each surfel's summed weight, weight_q / 2^32."""
+        return self.weight_q.to(torch.float64) / 4294967296.0
+
+    def prune_mask(self, min_weight: float = 0.0, min_pixels: int = 1) -> torch.Tensor:
+        """(P,) bool: the surfels with weight < min_weight or pixels < min_pixels."""
+        return (self.weight < float(min_weight)) | (self.pixels < int(min_pixels))
+
+    def check(self, P: int, device) -> None:
+        """Raise RuntimeError unless the four tensors are contiguous (P,) tensors of their dtypes on `device`."""
+        for name, dt in (("weight_q", torch.int64), ("max_weight", torch.int32), ("pixels", torch.int64),
+                         ("frames", torch.int64)):
+            t = getattr(self, name)
+            if not torch.is_tensor(t) or t.dtype != dt or tuple(t.shape) != (P,) or not t.is_contiguous():
+                raise RuntimeError(f"contributions.{name} must be a contiguous {dt} (P,) = ({P},) tensor, got "
+                                   f"{tuple(t.shape) if torch.is_tensor(t) else type(t).__name__}"
+                                   f"{' ' + str(t.dtype) if torch.is_tensor(t) else ''}")
+            if t.device != torch.device(device):
+                raise RuntimeError(f"contributions.{name} must be on the rasterizer's device {device}, got {t.device}")
+
+
 def _check_render_frames(T, P, device, bg_color, means3D, rotations, features, learnable_bkgd, frames_per_call):
     """Validate render_frames' arguments before anything runs on the device; returns F."""
     if isinstance(frames_per_call, bool) or not isinstance(frames_per_call, int) or frames_per_call < 1:
@@ -704,7 +754,7 @@ def _check_render_frames(T, P, device, bg_color, means3D, rotations, features, l
 
 
 def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, features=None, learnable_bkgd=None,
-                  frames_per_call=8):
+                  frames_per_call=8, contributions=None):
     """Render T frames forward-only: render_fused()'s outputs for every frame, with a leading frame dimension, and nothing
     differentiable -- no autograd graph is built, even when the inputs require grad.
 
@@ -721,6 +771,12 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
     back once and re-runs with a larger capacity if it overflowed.  Colour, features, allmap-derived maps and radii are
     bit-identical to the training forward's (_C.rasterize_gaussians_batch) followed by sr_post_forward per frame.
 
+    contributions: optional SurfelContributions of P surfels on the surfels' device (SurfelContributions.zeros(P, device)),
+    added into in place with every rendered frame's per-surfel statistics, gathered in the same walk
+    (sr_render_forward_contrib).  A sequence rendered in several calls, in any order and with any frames_per_call, adds
+    the same bits as one call; a chunk that overflows re-runs only its overflowed frames, so no frame adds twice.  The
+    rendered outputs are the same with and without it.
+
     Returns {"render": (T,3,H,W), "features": (T,F,H,W) (with features), "acc": (T,1,H,W), "rend_normal": (T,3,H,W),
     "rend_dist": (T,1,H,W), "surf_depth", "render_depth_median", "render_depth_expected": (T,3,H,W) broadcast views of one
     plane each, "surf_normal": (T,3,H,W), "radii": (T,P) int32, "visibility_filter": (T,P) bool}."""
@@ -732,6 +788,10 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
     xyz = pc.get_xyz if means3D is None else means3D
     P, dev = int(xyz.shape[-2]), xyz.device
     F = _check_render_frames(T, P, dev, bg_color, means3D, rotations, features, learnable_bkgd, frames_per_call)
+    if contributions is not None:
+        if not isinstance(contributions, SurfelContributions):
+            raise RuntimeError(f"contributions must be a SurfelContributions, got {type(contributions).__name__}")
+        contributions.check(P, dev)
     intr = _check_intrinsics(cameras.intrinsics, T, xyz)
     tanx, tany = (0.0, 0.0) if intr is not None else _cam_tans(cameras)     # the table replaces them
     N = H * W
@@ -753,20 +813,36 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
         n = min(frames_per_call, T)
         allmap = torch.empty((n, 8, H, W), dtype=torch.float32, device=dev)     # one chunk's, reused
         out = _RenderOut(None, None, None, None)
-        for t0 in range(0, T, n):
-            t1 = min(T, t0 + n)
-            c = slice(t0, t1)
+        if contributions is not None:
+            out.contrib = _capi.SrContrib(contributions.weight_q.data_ptr(), contributions.max_weight.data_ptr(),
+                                          contributions.pixels.data_ptr())
+
+        def forward(a, b, t0):
+            """frames [a, b) of the chunk that starts at t0"""
+            c = slice(a, b)
             # per-frame inputs are sliced (their strides stay); shared ones pass whole
             sl = {k: (v[c] if v is not None and strides.get(k, 0) else v) for k, v in ins.items()}
-            out.color, out.features, out.others, out.radii = color[c], (feat[c] if F else None), allmap[:t1 - t0], radii[c]
+            out.color, out.features, out.others, out.radii = color[c], (feat[c] if F else None), allmap[a - t0:b - t0], radii[c]
             # P = 0: the empty tensors give the device and F (their pointers pass as NULL)
             xyz_c = sl["means3D"] if sl["means3D"] is not None else xyz
             feat_c = sl["features"] if sl["features"] is not None else features
-            _forward(t1 - t0, True, strides, bg, xyz_c, sl["sh"], None, sl["opacity"], sl["scales"], sl["rotations"],
+            _forward(b - a, True, strides, bg, xyz_c, sl["sh"], None, sl["opacity"], sl["scales"], sl["rotations"],
                      feat_c, vm[c], pm[c], cp[c], H, W, pc.active_sh_degree, tanx, tany, 1.0, False, False,
                      intrinsics=None if intr is None else intr[c], render=out)
+
+        for t0 in range(0, T, n):
+            t1 = min(T, t0 + n)
+            c = slice(t0, t1)
+            out.overflowed = []
+            forward(t0, t1, t0)
+            # with contributions an overflowed chunk is not re-run whole: its frames that fit have added already
+            for m in list(out.overflowed):
+                forward(t0 + m, t0 + m + 1, t0)
+            if contributions is not None:
+                contributions.frames += (radii[c] > 0).sum(0)
+            # the whole chunk's allmap: after a one-frame re-run out.others is that frame's slice alone
             _capi.call("sr_post_forward_frames", dev, t1 - t0, W, H, tanx, tany, None if intr is None else intr[c],
-                       float(pipe.depth_ratio), out.others, vm[c], bk, color[c], 3 * N, acc[c], rn[c], dist[c], med[c], ex[c],
+                       float(pipe.depth_ratio), allmap[:t1 - t0], vm[c], bk, color[c], 3 * N, acc[c], rn[c], dist[c], med[c], ex[c],
                        sd[c], sn[c])
         del out, allmap
         rets = {"render": color, "acc": acc, "rend_normal": rn, "rend_dist": dist, "surf_depth": sd.expand(T, 3, H, W),

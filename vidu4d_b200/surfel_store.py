@@ -392,6 +392,23 @@ class FlatSurfelModel(torch.nn.Module):
         return n
 
     @torch.no_grad()
+    def prune_by_contribution(self, contrib, min_weight: float = 0.0, min_pixels: int = 1) -> int:
+        """Prune every surfel whose summed blending weight over the rendered frames is below min_weight, or that
+        contributed to fewer than min_pixels (frame, pixel) pairs: with the defaults, every surfel no frame blends (each
+        view sees it behind opaque ones, or culls it).  contrib: a renderer.SurfelContributions of this store's P surfels,
+        filled by render_frames(contributions=) -- on several ranks, after distributed.allreduce_contributions, so that
+        every rank prunes the same surfels.  Goes through prune_points: the Adam moments, statistics and regist_feat
+        follow.  Returns the number pruned.  When none is, the buffers are left as they are (same addresses)."""
+        self._live("prune_by_contribution")
+        if contrib.P != self.P:
+            raise RuntimeError(f"contributions are for {contrib.P} surfels, the store has {self.P}")
+        mask = contrib.prune_mask(min_weight, min_pixels).to(self.flat.device)
+        n = int(mask.sum())
+        if n:
+            self.prune_points(mask)
+        return n
+
+    @torch.no_grad()
     def densify_and_prune(self, max_grad, min_opacity, extent, max_screen_size, generator=None):
         """gaussian_model.py:431-446 in ONE pass over the buffers.  The reference builds the result in four steps (clone ->
         cat; split -> cat, prune the split parents; prune by opacity / size), re-creating every parameter and both Adam
