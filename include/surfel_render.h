@@ -67,6 +67,35 @@ SR_API int sr_render_forward_contrib(const sr_frame* f, const sr_batch* b, const
                                      uint32_t* num_rendered_dev, uint32_t* num_rendered_host, const sr_contrib* contrib,
                                      void* stream);
 
+/* Foreground masks and the per-surfel share of the contribution statistics that lands on background pixels.
+ *   mask         DEVICE bytes: frame m's H*W pixels, row-major, at mask + m * mask_stride; nonzero = foreground
+ *   mask_stride  bytes between consecutive frames' masks, >= H*W
+ *   weight_bg_q  DEVICE [P] (unsigned 64-bit): sum of q(w) over the contributing pairs on background pixels
+ *   pixels_bg    DEVICE [P] (unsigned 64-bit): the number of those pairs
+ * Integer sums, like sr_contrib's: exact and independent of the order of pairs, frames or calls. */
+typedef struct sr_contrib_mask {
+    const uint8_t* mask;
+    int64_t mask_stride;
+    uint64_t* weight_bg_q;
+    uint64_t* pixels_bg;
+} sr_contrib_mask;
+
+/* sr_render_forward_contrib, which it is in every argument, output and check, that also ADDS every rendered frame's
+ * contributing pairs on background pixels into mask->weight_bg_q and mask->pixels_bg (never cleared here).  contrib's
+ * three words get exactly the bits sr_render_forward_contrib gives, and so do the rendered outputs.  An overflowed frame
+ * adds nothing.  mask = NULL, or mask->mask = NULL, is sr_render_forward_contrib: the same kernels and bits.  Otherwise
+ * contrib must be non-NULL, mask_stride >= H*W and, with P > 0, weight_bg_q and pixels_bg non-NULL and 8-byte aligned. */
+SR_API int sr_render_forward_contrib_masked(const sr_frame* f, const sr_batch* b, const float* background,
+                                            int32_t bg_channels, const float* means3D, const float* shs,
+                                            const float* colors_precomp, const float* opacities, const float* scales,
+                                            const float* rotations, const float* features, int32_t F,
+                                            int64_t features_stride, const float* viewmatrix, const float* projmatrix,
+                                            const float* campos, float* out_color, int64_t out_color_stride,
+                                            float* out_features, int64_t out_features_stride, float* out_others,
+                                            int32_t* radii, void* arena, int64_t capacity, uint32_t* num_rendered_dev,
+                                            uint32_t* num_rendered_host, const sr_contrib* contrib,
+                                            const sr_contrib_mask* mask, void* stream);
+
 /* sr_post_forward over M frames in one launch: frame m's allmap (allmap + m*8*H*W) and world_view_transform (+ m*16) give
  * its acc, rend_normal, rend_dist, depth_median, depth_expected, surf_depth, surf_normal (each output packed (M, c, H, W)).
  * cameras: optional DEVICE (M,4) table of surfel_camera.h; with it frame m's rays use its own tangents and principal

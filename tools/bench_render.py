@@ -13,7 +13,13 @@ SurfelContributions accumulator (alternating, L2 flushed by a 256 MB write befor
 and render_frames' time before and after that prune, with the renders compared bit for bit.  Every timing is repeated in
 --rounds rounds of one process.
 
-Usage: python tools/bench_render.py [--frames 64] [--chunk 8] [--repeats 7] [--contrib [--rounds 3]] [--out FILE]
+--silhouette measures the background share of the statistics: render_frames without statistics, with a
+SurfelContributions accumulator, with one that has the background words and the frames' silhouettes as masks, and
+without statistics again (alternating, L2 flushed before every timed call), at 512^2 and F in {0, 22}, scalar cameras.
+The silhouettes are the plain render's acc > 0.5.  Outputs and the four older words are compared bit for bit.
+
+Usage: python tools/bench_render.py [--frames 64] [--chunk 8] [--repeats 7] [--contrib | --silhouette [--rounds 3]]
+                                    [--out FILE]
 """
 from __future__ import annotations
 
@@ -223,9 +229,72 @@ def contrib_main(args, gpu):
     return out
 
 
-def render_frames_contrib(cams, pc, bg, feat, chunk, acc):
+def render_frames_contrib(cams, pc, bg, feat, chunk, acc, masks=None):
     from vidu4d_b200.renderer import PipelineParams, render_frames
-    return render_frames(cams, pc, PipelineParams(), bg, features=feat, frames_per_call=chunk, contributions=acc)
+    return render_frames(cams, pc, PipelineParams(), bg, features=feat, frames_per_call=chunk, contributions=acc,
+                         masks=masks)
+
+
+def silhouette_main(args, gpu):
+    """--silhouette: `rounds` rounds in one process; each times, for F = 0 and 22, four arms alternating -- plain, with
+    the accumulator, with the accumulator and masks, plain again (the A/A control)."""
+    from vidu4d_b200.renderer import SurfelContributions
+    from vidu4d_b200.synthetic import object_scene
+    dev = torch.device("cuda:0")
+    s = object_scene(args.P, seed=0, opacity="trained", center=(0.0, 0.0, 0.0)).to_torch(dev)
+    pc = _PC(s)
+    g = torch.Generator(device=dev).manual_seed(0)
+    flush = torch.empty((256 << 20,), dtype=torch.uint8, device=dev)
+    res = 512
+    cams = _cams(args.frames, res, dev, False)
+    bg = torch.zeros(3, device=dev)
+    feats = {0: None, 22: torch.rand((args.P, 22), device=dev, generator=g) * 2 - 1}
+    acc = SurfelContributions.zeros(args.P, dev)
+    acc_bg = SurfelContributions.zeros(args.P, dev, silhouettes=True)
+    masks = new(cams, pc, bg, None, args.chunk)["acc"][:, 0] > 0.5          # (T, H, W) silhouettes
+
+    def stats(feat, a, m=None):
+        for t in (a.weight_q, a.max_weight, a.pixels, a.frames) + ((a.weight_bg_q, a.pixels_bg) if m is not None else ()):
+            t.zero_()
+        return render_frames_contrib(cams, pc, bg, feat, args.chunk, a, m)
+
+    check = {}
+    for F, feat in feats.items():
+        a, b, c = new(cams, pc, bg, feat, args.chunk), stats(feat, acc), stats(feat, acc_bg, masks)
+        check[F] = {"identical_outputs": all(_same(a[k], b[k]) and _same(a[k], c[k]) for k in a if k != "visibility_filter"),
+                    "identical_words": all(torch.equal(getattr(acc, k), getattr(acc_bg, k))
+                                           for k in ("weight_q", "max_weight", "pixels", "frames"))}
+        del a, b, c
+    frac = acc_bg.background_fraction
+    scene = {"foreground_pixel_fraction": float(masks.float().mean()),
+             "background_pair_fraction": float(acc_bg.pixels_bg.sum()) / max(1, int(acc_bg.pixels.sum())),
+             "surfels_over_half_background": int((frac > 0.5).sum()), "surfels_all_background": int((frac == 1.0).sum())}
+    print(json.dumps({"check": check, "scene": scene}), flush=True)
+    rounds = []
+    for rd in range(args.rounds):
+        rows = []
+        for F, feat in feats.items():
+            arms = {"plain": lambda: new(cams, pc, bg, feat, args.chunk), "contrib": lambda: stats(feat, acc),
+                    "masked": lambda: stats(feat, acc_bg, masks), "plain_again": lambda: new(cams, pc, bg, feat, args.chunk)}
+            for fn in arms.values():          # warm-up
+                fn()
+            times = {k: [] for k in arms}
+            for r in range(args.repeats):
+                for k, fn in arms.items():
+                    times[k] += _flushed(fn, flush, 1, r)
+            row = {"round": rd, "res": res, "F": F, **check[F], **{k: _stat(v, args.frames) for k, v in times.items()}}
+            base = 0.5 * (row["plain"]["ms_median"] + row["plain_again"]["ms_median"])
+            row["contrib_overhead"] = row["contrib"]["ms_median"] / base - 1.0
+            row["masked_overhead"] = row["masked"]["ms_median"] / base - 1.0
+            row["masked_over_contrib"] = row["masked"]["ms_median"] / row["contrib"]["ms_median"] - 1.0
+            row["plain_gap"] = row["plain_again"]["ms_median"] / row["plain"]["ms_median"] - 1.0
+            print(json.dumps(row), flush=True)
+            rows.append(row)
+        rounds.append(rows)
+    out = {"gpu": gpu, "frames": args.frames, "frames_per_call": args.chunk, "P": args.P, "repeats": args.repeats,
+           "scene": scene, "rounds": rounds}
+    print(json.dumps(out))
+    return out
 
 
 def main():
@@ -235,7 +304,8 @@ def main():
     ap.add_argument("--repeats", type=int, default=7)
     ap.add_argument("--P", type=int, default=300_000)
     ap.add_argument("--contrib", action="store_true", help="measure the contribution statistics and the prune by them")
-    ap.add_argument("--rounds", type=int, default=3, help="--contrib: rounds of every measurement in one process")
+    ap.add_argument("--silhouette", action="store_true", help="measure the background share of the statistics")
+    ap.add_argument("--rounds", type=int, default=3, help="--contrib / --silhouette: rounds of every measurement in one process")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -245,8 +315,8 @@ def main():
     dev = torch.device("cuda:0")
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip()
-    if args.contrib:
-        out = contrib_main(args, gpu)
+    if args.contrib or args.silhouette:
+        out = contrib_main(args, gpu) if args.contrib else silhouette_main(args, gpu)
         if args.out:
             os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
             with open(args.out, "w") as f:

@@ -25,6 +25,8 @@ from vidu4d_b200.build import NVCC_FLAGS, _nvcc  # noqa: E402
 
 SOURCES = ["composite_tile.cu", "composite_feat.cu", "composite_det.cu", "surfel_bwd.cu", "preprocess.cu", "composite_fwd.cu",
            "postprocess.cu"]
+_STATS = r"\((?:bool|<unnamed>::Stats)\)"      # composite_fwd_kernel's fourth template argument, either spelling
+_FWD_ONLY = [(1, 0)] + [(v, nf) for nf in (8, 16, 24, 32) for v in (4, 2, 1)]
 # (demangled-name pattern in the base build, pattern of the same kernel in the working tree)
 KERNELS = [
     (r"composite_tile_bwd_kernel(<\(bool\)0>)?\(", r"composite_tile_bwd_kernel(<\(bool\)0>)?\("),
@@ -39,15 +41,21 @@ KERNELS = [
     (r"emit_keys_kernel\(", r"emit_keys_kernel\("),
     (r"scan_block_sums_kernel\(", r"scan_block_sums_kernel\("),
     (r"mark_visible_kernel\(", r"mark_visible_kernel\("),
-    # the training instantiation of the composite forward (the forward-only ones are <(bool)0, ...>); a fourth template
-    # parameter, STATS = (bool)0, names the instantiations that gather no contribution statistics
-    (r"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0(, \(bool\)0)?>)?\(",
-     r"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0(, \(bool\)0)?>)?\("),
-    # the forward-only instantiations: (V, NF) = (1, 0), and V in {4, 2, 1} for NF in {8, 16, 24, 32}
+    # the training instantiation of the composite forward (the forward-only ones are <(bool)0, ...>).  A fourth template
+    # parameter names what the forward-only walk gathers: (bool)0 / (bool)1 before the silhouette statistics, then the
+    # Stats enum's OFF = 0, WEIGHTS = 1 (the contribution statistics) and MASKED = 2 (their background share, new)
+    (rf"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0(, {_STATS}0)?>)?\(",
+     rf"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0(, {_STATS}0)?>)?\("),
+    # the forward-only instantiations without and with the contribution statistics: (V, NF) = (1, 0), and V in {4, 2, 1}
+    # for NF in {8, 16, 24, 32}
 ] + [
-    (rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}(, \(bool\)0)?>\(",
-     rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}(, \(bool\)0)?>\(")
-    for v, nf in [(1, 0)] + [(v, nf) for nf in (8, 16, 24, 32) for v in (4, 2, 1)]
+    (rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}(, {_STATS}0)?>\(",
+     rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}(, {_STATS}0)?>\(")
+    for v, nf in _FWD_ONLY
+] + [
+    (rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}, {_STATS}1>\(",
+     rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}, {_STATS}1>\(")
+    for v, nf in _FWD_ONLY
 ] + [
     (r"feature_fwd_kernel<\(int\)4>\(", r"feature_fwd_kernel<\(int\)4>\("),
     (r"feature_fwd_kernel<\(int\)2>\(", r"feature_fwd_kernel<\(int\)2>\("),

@@ -50,6 +50,12 @@ class SrContrib(C.Structure):
     _fields_ = [("weight_q", C.c_void_p), ("max_weight", C.c_void_p), ("pixels", C.c_void_p)]
 
 
+class SrContribMask(C.Structure):
+    """sr_contrib_mask (include/surfel_render.h): the DEVICE foreground masks (frame m at mask + m*mask_stride bytes) and
+    the per-surfel background words sr_render_forward_contrib_masked adds into."""
+    _fields_ = [("mask", C.c_void_p), ("mask_stride", C.c_int64), ("weight_bg_q", C.c_void_p), ("pixels_bg", C.c_void_p)]
+
+
 class SrDebugLayout(C.Structure):
     _fields_ = [
         ("surfel_rec", C.c_size_t), ("depths", C.c_size_t), ("tiles_touched", C.c_size_t),
@@ -166,6 +172,8 @@ RENDER_PROTOTYPES = {
                           + [_p] * 3 + [_i64, _p, _p, _p]),
     "sr_render_forward_contrib": (C.c_int, [_FRAME, _BATCH, _p, _i32] + [_p] * 7 + [_i32, _i64] + [_p] * 3
                                   + [_p, _i64, _p, _i64] + [_p] * 3 + [_i64, _p, _p, _p, _p]),
+    "sr_render_forward_contrib_masked": (C.c_int, [_FRAME, _BATCH, _p, _i32] + [_p] * 7 + [_i32, _i64] + [_p] * 3
+                                         + [_p, _i64, _p, _i64] + [_p] * 3 + [_i64, _p, _p, _p, _p, _p]),
     "sr_post_forward_frames": (C.c_int, [_i32] * 3 + [_f32] * 2 + [_p, _f32] + [_p] * 4 + [_i64] + [_p] * 8),
 }
 RENDER_SYMBOLS = tuple(RENDER_PROTOTYPES)

@@ -213,6 +213,8 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
     const size_t N = (size_t)f->width * f->height;
     if (!out_color || !out_others || !num_rendered_dev) return sr_fail(SR_EINVAL, "output pointer is NULL");
     if (!background || !viewmatrix || !campos) return sr_fail(SR_EINVAL, "camera / background pointer is NULL");
+    if (contrib && contrib->mask && contrib->mask_stride < (long long)N)
+        return sr_fail(SR_EINVAL, "silhouette mask frame stride must be >= H*W bytes");
     if (ft) {
         if (color_stride < (int64_t)(3 * N)) return sr_fail(SR_EINVAL, "out_color frame stride must be >= 3*H*W");
         if (!ft->out) return sr_fail(SR_EINVAL, "out_features pointer is NULL");
@@ -235,6 +237,12 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
                 return sr_fail(SR_EINVAL, "contribution statistics pointer is NULL");
             if (((uintptr_t)contrib->weight_q & 7) || ((uintptr_t)contrib->pixels & 7) || ((uintptr_t)contrib->max_weight & 3))
                 return sr_fail(SR_EINVAL, "contribution statistics: weight_q / pixels must be 8-byte aligned, max_weight 4-byte aligned");
+            if (contrib->mask) {
+                if (!contrib->weight_bg_q || !contrib->pixels_bg)
+                    return sr_fail(SR_EINVAL, "silhouette statistics pointer is NULL");
+                if (((uintptr_t)contrib->weight_bg_q & 7) || ((uintptr_t)contrib->pixels_bg & 7))
+                    return sr_fail(SR_EINVAL, "silhouette statistics: weight_bg_q / pixels_bg must be 8-byte aligned");
+            }
         }
         // 128-bit / 64-bit vector loads: rotations as float4, scales as float2, SH rows as float4 when 3M % 4 == 0
         if (((uintptr_t)rotations & 15) || ((uintptr_t)scales & 7) || (shs && ((uintptr_t)shs & 15)) ||
@@ -366,12 +374,36 @@ int sr_render_forward_contrib(const sr_frame* f, const sr_batch* b, const float*
                               float* out_color, int64_t out_color_stride, float* out_features, int64_t out_features_stride,
                               float* out_others, int32_t* radii, void* arena, int64_t capacity, uint32_t* num_rendered_dev,
                               uint32_t* num_rendered_host, const sr_contrib* contrib, void* stream_) {
+    return sr_render_forward_contrib_masked(f, b, background, bg_channels, means3D, shs, colors_precomp, opacities, scales,
+                                            rotations, features, F, features_stride, viewmatrix, projmatrix, campos,
+                                            out_color, out_color_stride, out_features, out_features_stride, out_others,
+                                            radii, arena, capacity, num_rendered_dev, num_rendered_host, contrib, nullptr,
+                                            stream_);
+}
+
+int sr_render_forward_contrib_masked(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+                                     const float* means3D, const float* shs, const float* colors_precomp,
+                                     const float* opacities, const float* scales, const float* rotations,
+                                     const float* features, int32_t F, int64_t features_stride, const float* viewmatrix,
+                                     const float* projmatrix, const float* campos, float* out_color,
+                                     int64_t out_color_stride, float* out_features, int64_t out_features_stride,
+                                     float* out_others, int32_t* radii, void* arena, int64_t capacity,
+                                     uint32_t* num_rendered_dev, uint32_t* num_rendered_host, const sr_contrib* contrib,
+                                     const sr_contrib_mask* mask, void* stream_) {
     (void)projmatrix;
+    const bool masked = mask && mask->mask;
+    if (masked && !contrib) return sr_fail(SR_EINVAL, "a silhouette mask needs the contribution statistics (contrib is NULL)");
     ContribArgs cs{};
     if (contrib) {
         cs.weight_q = reinterpret_cast<unsigned long long*>(contrib->weight_q);
         cs.max_weight = contrib->max_weight;
         cs.pixels = reinterpret_cast<unsigned long long*>(contrib->pixels);
+    }
+    if (masked) {
+        cs.mask = mask->mask;
+        cs.mask_stride = mask->mask_stride;
+        cs.weight_bg_q = reinterpret_cast<unsigned long long*>(mask->weight_bg_q);
+        cs.pixels_bg = reinterpret_cast<unsigned long long*>(mask->pixels_bg);
     }
     return forward_entry(f, b, background, bg_channels, means3D, shs, colors_precomp, opacities, scales, rotations, features, F,
                          features_stride, viewmatrix, campos, out_color, out_color_stride, out_features, out_features_stride,

@@ -175,6 +175,12 @@ struct ContribArgs {
     unsigned long long* weight_q;  // [P] sum of rn(w 2^32)
     uint32_t* max_weight;          // [P] max of w, as float bits
     unsigned long long* pixels;    // [P] number of pairs
+    // sr_render_forward_contrib_masked: frame m's H*W foreground bytes at mask + m*mask_stride (0 = background), and
+    // the two sums over the pairs on background pixels; mask = nullptr gathers the three words above alone
+    const uint8_t* mask;
+    long long mask_stride;         // bytes
+    unsigned long long* weight_bg_q;  // [P] sum of rn(w 2^32) over the background pairs
+    unsigned long long* pixels_bg;    // [P] number of background pairs
 };
 struct FwdArgs {
     FrameStrides fs;

@@ -23,13 +23,21 @@
 //     blending weight w = ff(T, alpha, 0) -- the feature plane of a feature equal to 1 -- into per-warp shared slots, one
 //     per instance of the stage, with integer shared atomics; after the stage lane i adds slot i to its surfel with one
 //     global integer atomic each.  Integer sums and an unsigned max are exact and order-independent: the totals have
-//     the same bits whatever the order of the pairs, frames, chunks or ranks.
+//     the same bits whatever the order of the pairs, frames, chunks or ranks;
+//   * MASKED statistics (sr_render_forward_contrib_masked): each lane reads its pixel's foreground byte once, before
+//     the walk, and adds its pairs into a foreground or a background set of slots.  The flush adds both sets into the
+//     three words above, which get the unmasked walk's bits, and the background set alone into weight_bg_q and
+//     pixels_bg.
 #include "composite_common.cuh"
 
 namespace {
 using namespace comp;
 
 constexpr int WPC = 1;      // independent warps per CTA (2 measured slower: register pressure)
+
+// What the forward-only walk gathers besides its outputs: nothing, the contribution statistics, or the statistics and
+// their share on the frame's background pixels
+enum class Stats { OFF, WEIGHTS, MASKED };
 
 // A stage's statistics slots, per warp and instance jj: lo[jj] sums the low 16 bits of q = rn(w 2^32), hc[jj] the high
 // 16 bits plus 2^21 per pair.  q < 2^32 (w <= 0.99) and a stage has at most 32 pairs per instance, so neither word
@@ -44,10 +52,16 @@ __device__ __forceinline__ void stat_pair(StatSlots* ss, int jj, float T, float 
     atomicAdd(&ss->hc[jj], (q >> 16) + (1u << 21));
     atomicMax(&ss->mx[jj], __float_as_uint(w));
 }
+// MASKED: two such sets, [0] for the pairs on foreground pixels and [1] for those on background pixels.  A lane's pixel
+// is one or the other for the whole walk, so each lane adds into one set with stat_pair's three atomics; the flush adds
+// both sets into weight_q / max_weight / pixels and set [1] alone into weight_bg_q / pixels_bg.
+struct MaskedSlots {
+    StatSlots set[2];
+};
 
 // TRAIN: the training forward (V, NF, STATS unused).  Otherwise forward-only with F <= NF feature channels (NF = 0:
-// none), rows gathered V floats per load, and with STATS the contribution statistics added into cs.
-template <bool TRAIN, int V, int NF, bool STATS = false>
+// none), rows gathered V floats per load, and with STATS != OFF the contribution statistics added into cs.
+template <bool TRAIN, int V, int NF, Stats STATS = Stats::OFF>
 __global__ void __launch_bounds__(32 * WPC)
 composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, const uint32_t* __restrict__ tile_order, int n_items, int tiles_x,
                      const float4* __restrict__ irec, int W, int H,
@@ -83,10 +97,21 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
         for (int b = 0; b < NST && b < nb; b++) ring.issue(b, b);
     }
     StatSlots* ss = nullptr;
-    if constexpr (STATS) {
+    if constexpr (STATS == Stats::WEIGHTS) {
         __shared__ StatSlots ss_all[WPC];
         ss = &ss_all[threadIdx.x >> 5];
         ss->lo[lane] = 0u; ss->hc[lane] = 0u; ss->mx[lane] = 0u;
+    }
+    // MASKED: the warp's two sets, and the one this lane's pairs add into, chosen by its pixel's mask byte in frame f,
+    // read once here (a pixel outside the image has no pairs)
+    MaskedSlots* sm = nullptr;
+    if constexpr (STATS == Stats::MASKED) {
+        __shared__ MaskedSlots sm_all[WPC];
+        sm = &sm_all[threadIdx.x >> 5];
+        for (int k = 0; k < 2; k++) { sm->set[k].lo[lane] = 0u; sm->set[k].hc[lane] = 0u; sm->set[k].mx[lane] = 0u; }
+        const bool bg_pixel =
+            sp.inside(W, H) && __ldg(fr(cs.mask, cs.mask_stride, f) + (size_t)W * sp.pix_y + sp.pix_x) == 0;
+        ss = &sm->set[bg_pixel ? 1 : 0];
     }
     __syncwarp();
 
@@ -130,7 +155,7 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
             if (!act || done) continue;
             if constexpr (TRAIN) {
                 if (px.blend(S + jj * REC4, sp.pixx, sp.pixy, rho_cut, b * WB, jj, cmask)) done = true;
-            } else if constexpr (!STATS) {
+            } else if constexpr (STATS == Stats::OFF) {
                 if (px.blend(S + jj * REC4, sp.pixx, sp.pixy, rho_cut, b * WB, jj, cmask, feat_pair)) done = true;
             } else {
                 auto pair = [&](float T, float alpha, const float4* __restrict__ R) {
@@ -141,7 +166,7 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
             }
         }
         __syncwarp();                                   // every lane is done reading stage b
-        if constexpr (STATS) {
+        if constexpr (STATS == Stats::WEIGHTS) {
             // lane = instance: its stage totals go to its surfel, and its slot is cleared for the next stage
             const uint32_t hc = ss->hc[lane];
             if (hc != 0u) {
@@ -151,6 +176,27 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
                 atomicAdd(cs.pixels + id, (unsigned long long)(hc >> 21));
                 ss->lo[lane] = 0u; ss->hc[lane] = 0u; ss->mx[lane] = 0u;
             }
+        }
+        if constexpr (STATS == Stats::MASKED) {
+            // the same, with both sets' totals in the three words and the background set's in its two
+            StatSlots& fg = sm->set[0];
+            StatSlots& bk = sm->set[1];
+            const uint32_t hf = fg.hc[lane], hb = bk.hc[lane];
+            if ((hf | hb) != 0u) {
+                const uint32_t id = __float_as_uint(S[lane * REC4 + 4].z);
+                const unsigned long long qf = ((unsigned long long)(hf & 0x1fffffu) << 16) + fg.lo[lane];
+                const unsigned long long qb = ((unsigned long long)(hb & 0x1fffffu) << 16) + bk.lo[lane];
+                atomicAdd(cs.weight_q + id, qf + qb);
+                atomicMax(cs.max_weight + id, max(fg.mx[lane], bk.mx[lane]));
+                atomicAdd(cs.pixels + id, (unsigned long long)((hf >> 21) + (hb >> 21)));
+                if (hb != 0u) {
+                    atomicAdd(cs.weight_bg_q + id, qb);
+                    atomicAdd(cs.pixels_bg + id, (unsigned long long)(hb >> 21));
+                }
+                for (int k = 0; k < 2; k++) { sm->set[k].lo[lane] = 0u; sm->set[k].hc[lane] = 0u; sm->set[k].mx[lane] = 0u; }
+            }
+        }
+        if constexpr (STATS != Stats::OFF) {
             __syncwarp();                               // slots cleared and stage b read before its slot is refilled
         }
         if constexpr (TRAIN) cm_out[(size_t)b * SR_CONTRIB_STAGE_WORDS] = cmask;
@@ -185,8 +231,8 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
 }
 
 // the forward-only instantiation for F channels (NF = F rounded up to a multiple of 8), vector width ft.vec and, with
-// STATS, the statistics cs
-template <int NF, bool STATS>
+// STATS != OFF, the statistics cs
+template <int NF, Stats STATS>
 void launch_render(const FwdArgs& a, const FeatArgs& ft, const ContribArgs& cs, unsigned grid) {
     auto launch = [&](auto kern) {
         kern<<<grid, 32 * WPC, 0, a.stream>>>(
@@ -199,7 +245,7 @@ void launch_render(const FwdArgs& a, const FeatArgs& ft, const ContribArgs& cs, 
     else if (ft.vec == 2) launch(composite_fwd_kernel<false, 2, NF, STATS>);
     else launch(composite_fwd_kernel<false, 1, NF, STATS>);
 }
-template <bool STATS>
+template <Stats STATS>
 void launch_render_f(const FwdArgs& a, const FeatArgs& ft, const ContribArgs& cs, unsigned grid) {
     if (ft.F == 0) launch_render<0, STATS>(a, ft, cs, grid);
     else if (ft.F <= 8) launch_render<8, STATS>(a, ft, cs, grid);
@@ -215,8 +261,9 @@ cudaError_t launch_composite_fwd(const FwdArgs& a) {
     if (a.forward_only) {
         ProfileScope ps("composite_render", a.stream);
         const FeatArgs ft = a.feat ? *a.feat : FeatArgs{};
-        if (a.contrib) launch_render_f<true>(a, ft, *a.contrib, grid);
-        else launch_render_f<false>(a, ft, ContribArgs{}, grid);
+        if (!a.contrib) launch_render_f<Stats::OFF>(a, ft, ContribArgs{}, grid);
+        else if (a.contrib->mask) launch_render_f<Stats::MASKED>(a, ft, *a.contrib, grid);
+        else launch_render_f<Stats::WEIGHTS>(a, ft, *a.contrib, grid);
         sr_count_launch();
         return cudaGetLastError();
     }

@@ -116,12 +116,15 @@ def check_replicas(named_tensors: dict, group=None) -> None:
 
 def allreduce_contributions(contrib, group=None):
     """Make every rank's renderer.SurfelContributions those of all the ranks' frames: SUM over weight_q, pixels and
-    frames (int64 words; the totals stay below 2^63), MAX over max_weight (the float bits as int32, which order as the
-    non-negative floats do).  Integer collectives are exact, so every rank ends with the same bits, those one rank
+    frames, and over weight_bg_q and pixels_bg when present (int64 words; the totals stay below 2^63), MAX over
+    max_weight (the float bits as int32, which order as the non-negative floats do).  Integer collectives are exact, so every rank ends with the same bits, those one rank
     rendering every frame would have, and FlatSurfelModel.prune_by_contribution prunes the same surfels everywhere.
     In place; returns contrib.  No-op on one rank."""
     if _multi_rank(group):
-        for t in (contrib.weight_q, contrib.pixels, contrib.frames):
+        sums = [contrib.weight_q, contrib.pixels, contrib.frames]
+        if contrib.silhouettes:
+            sums += [contrib.weight_bg_q, contrib.pixels_bg]
+        for t in sums:
             dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
         dist.all_reduce(contrib.max_weight, op=dist.ReduceOp.MAX, group=group)
     return contrib

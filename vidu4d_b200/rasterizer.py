@@ -267,12 +267,14 @@ class _RenderOut:
     frames (color (M,3,H,W), features (M,F,H,W) or None, others (M,8,H,W), radii (M,P)), and the arena that the calls of
     one render share (include/surfel_render.h), grown only when a call needs more.  contrib: an _capi.SrContrib the call
     adds its contribution statistics into (sr_render_forward_contrib), or None.  With it, a call of M > 1 frames that
-    overflows is not re-run -- its other frames have added already -- and `overflowed` lists the frames to re-run alone."""
-    __slots__ = ("color", "features", "others", "radii", "arena", "contrib", "overflowed")
+    overflows is not re-run -- its other frames have added already -- and `overflowed` lists the frames to re-run alone.
+    mask: with contrib, an _capi.SrContribMask whose `mask` points at this call's first frame's foreground mask: the call
+    also adds the background share of the statistics (sr_render_forward_contrib_masked); or None."""
+    __slots__ = ("color", "features", "others", "radii", "arena", "contrib", "overflowed", "mask")
 
-    def __init__(self, color, features, others, radii, arena=None, contrib=None):
+    def __init__(self, color, features, others, radii, arena=None, contrib=None, mask=None):
         self.color, self.features, self.others, self.radii, self.arena = color, features, others, radii, arena
-        self.contrib, self.overflowed = contrib, []
+        self.contrib, self.overflowed, self.mask = contrib, [], mask
 
 
 def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, scales, rotations, features, viewmatrix,
@@ -335,6 +337,9 @@ def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, sc
                     render.arena = torch.empty((need,), dtype=torch.uint8, device=dev)
                 if render.contrib is None:
                     _capi.call("sr_render_forward", *args, render.arena, cap, nr_dev, host)
+                elif render.mask is not None:
+                    _capi.call("sr_render_forward_contrib_masked", *args, render.arena, cap, nr_dev, host,
+                               C.byref(render.contrib), C.byref(render.mask))
                 else:
                     _capi.call("sr_render_forward_contrib", *args, render.arena, cap, nr_dev, host, C.byref(render.contrib))
             if nosync:

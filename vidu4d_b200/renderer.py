@@ -691,18 +691,30 @@ class SurfelContributions:
       max_weight (P,) int32: the largest w, as its float32 bits (max_weight.view(torch.float32) is the value)
       pixels     (P,) int64: the number of contributing (frame, pixel) pairs
       frames     (P,) int64: the number of rendered frames with radii > 0 (those whose preprocess kept the surfel)
-    Every entry is an integer sum or maximum, so the totals have the same bits for any order of the frames, any chunking
-    and, after distributed.allreduce_contributions, any split over ranks.  torch's collectives take no unsigned 64-bit
-    type: the words live in int64 and int32 tensors."""
+    With silhouettes (zeros(..., silhouettes=True); render_frames(..., masks=) fills them, include/surfel_render.h,
+    sr_contrib_mask), over the contributing pairs on the frames' background pixels:
+      weight_bg_q (P,) int64: the sum of q(w)
+      pixels_bg   (P,) int64: the number of those pairs
+    Without them both are None.  Every entry is an integer sum or maximum, so the totals have the same bits for any order
+    of the frames, any chunking and, after distributed.allreduce_contributions, any split over ranks.  torch's
+    collectives take no unsigned 64-bit type: the words live in int64 and int32 tensors."""
     weight_q: torch.Tensor
     max_weight: torch.Tensor
     pixels: torch.Tensor
     frames: torch.Tensor
+    weight_bg_q: Optional[torch.Tensor] = None
+    pixels_bg: Optional[torch.Tensor] = None
 
     @classmethod
-    def zeros(cls, P: int, device) -> "SurfelContributions":
+    def zeros(cls, P: int, device, silhouettes: bool = False) -> "SurfelContributions":
         z = lambda dt: torch.zeros((int(P),), dtype=dt, device=device)  # noqa: E731
-        return cls(z(torch.int64), z(torch.int32), z(torch.int64), z(torch.int64))
+        bg = (z(torch.int64), z(torch.int64)) if silhouettes else (None, None)
+        return cls(z(torch.int64), z(torch.int32), z(torch.int64), z(torch.int64), *bg)
+
+    @property
+    def silhouettes(self) -> bool:
+        """True when the background words are present."""
+        return self.weight_bg_q is not None or self.pixels_bg is not None
 
     @property
     def P(self) -> int:
@@ -713,14 +725,37 @@ class SurfelContributions:
         """(P,) float64: each surfel's summed weight, weight_q / 2^32."""
         return self.weight_q.to(torch.float64) / 4294967296.0
 
-    def prune_mask(self, min_weight: float = 0.0, min_pixels: int = 1) -> torch.Tensor:
-        """(P,) bool: the surfels with weight < min_weight or pixels < min_pixels."""
-        return (self.weight < float(min_weight)) | (self.pixels < int(min_pixels))
+    @property
+    def background_fraction(self) -> torch.Tensor:
+        """(P,) float64: the share of each surfel's summed weight that fell on background pixels, weight_bg_q / weight_q
+        (each word converted to float64, then divided); 0 where weight_q == 0.  Needs the background words."""
+        if self.weight_bg_q is None:
+            raise RuntimeError("background_fraction needs the background words: SurfelContributions.zeros(P, device, "
+                               "silhouettes=True), filled by render_frames(..., masks=)")
+        wq = self.weight_q.to(torch.float64)
+        return torch.where(wq > 0, self.weight_bg_q.to(torch.float64) / wq.clamp_min(1.0), torch.zeros_like(wq))
+
+    def prune_mask(self, min_weight: float = 0.0, min_pixels: int = 1,
+                   max_background_fraction: Optional[float] = None) -> torch.Tensor:
+        """(P,) bool: the surfels with weight < min_weight or pixels < min_pixels and, when max_background_fraction f is
+        given (it needs the background words), those whose background_fraction is above f."""
+        mask = (self.weight < float(min_weight)) | (self.pixels < int(min_pixels))
+        if max_background_fraction is not None:
+            f = max_background_fraction
+            if isinstance(f, bool) or not isinstance(f, (int, float)) or not 0.0 <= float(f) <= 1.0:
+                raise RuntimeError(f"max_background_fraction must be a number in [0, 1] or None, got {f!r}")
+            mask |= self.background_fraction > float(f)
+        return mask
 
     def check(self, P: int, device) -> None:
-        """Raise RuntimeError unless the four tensors are contiguous (P,) tensors of their dtypes on `device`."""
-        for name, dt in (("weight_q", torch.int64), ("max_weight", torch.int32), ("pixels", torch.int64),
-                         ("frames", torch.int64)):
+        """Raise RuntimeError unless the four tensors, and the two background words when present (both or neither), are
+        contiguous (P,) tensors of their dtypes on `device`."""
+        if (self.weight_bg_q is None) != (self.pixels_bg is None):
+            raise RuntimeError("contributions.weight_bg_q and contributions.pixels_bg must both be tensors or both None")
+        names = [("weight_q", torch.int64), ("max_weight", torch.int32), ("pixels", torch.int64), ("frames", torch.int64)]
+        if self.silhouettes:
+            names += [("weight_bg_q", torch.int64), ("pixels_bg", torch.int64)]
+        for name, dt in names:
             t = getattr(self, name)
             if not torch.is_tensor(t) or t.dtype != dt or tuple(t.shape) != (P,) or not t.is_contiguous():
                 raise RuntimeError(f"contributions.{name} must be a contiguous {dt} (P,) = ({P},) tensor, got "
@@ -753,8 +788,27 @@ def _check_render_frames(T, P, device, bg_color, means3D, rotations, features, l
     return F
 
 
+def _silhouette_masks(masks, T, H, W, device):
+    """render_frames' masks as one contiguous (T,H,W) uint8 tensor on `device`, nonzero = foreground: bool and uint8
+    pass as they are (bool is viewed as bytes), a floating mask is foreground where > 0.5, converted once here."""
+    if not torch.is_tensor(masks):
+        raise RuntimeError(f"masks must be a tensor, got {type(masks).__name__}")
+    if tuple(masks.shape) not in ((T, H, W), (T, 1, H, W)):
+        raise RuntimeError(f"masks must be (T,H,W) or (T,1,H,W) = ({T},{H},{W}), got {tuple(masks.shape)}")
+    if masks.device != torch.device(device):
+        raise RuntimeError(f"masks must be on the rasterizer's device {device}, got {masks.device}")
+    m = masks.detach().reshape(T, H, W)
+    if m.dtype == torch.bool:
+        return m.contiguous().view(torch.uint8)
+    if m.dtype == torch.uint8:
+        return m.contiguous()
+    if m.is_floating_point():
+        return (m > 0.5).view(torch.uint8)
+    raise RuntimeError(f"masks must be bool, uint8 or floating point, got {m.dtype}")
+
+
 def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, features=None, learnable_bkgd=None,
-                  frames_per_call=8, contributions=None):
+                  frames_per_call=8, contributions=None, masks=None):
     """Render T frames forward-only: render_fused()'s outputs for every frame, with a leading frame dimension, and nothing
     differentiable -- no autograd graph is built, even when the inputs require grad.
 
@@ -777,6 +831,13 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
     the same bits as one call; a chunk that overflows re-runs only its overflowed frames, so no frame adds twice.  The
     rendered outputs are the same with and without it.
 
+    masks: optional foreground masks, (T,H,W) or (T,1,H,W), on the surfels' device: bool or uint8 (nonzero =
+    foreground) or floating point (foreground where > 0.5).  With them `contributions` must have the background words
+    (SurfelContributions.zeros(P, device, silhouettes=True)), and each surfel's contributing pairs on background pixels
+    are added into weight_bg_q and pixels_bg in the same walk (sr_render_forward_contrib_masked).  The rendered outputs
+    and the other statistics have the same bits as without masks.  A pixel the frame cannot judge -- outside vis2d --
+    should not count as background: pass masks = mask | ~vis2d.
+
     Returns {"render": (T,3,H,W), "features": (T,F,H,W) (with features), "acc": (T,1,H,W), "rend_normal": (T,3,H,W),
     "rend_dist": (T,1,H,W), "surf_depth", "render_depth_median", "render_depth_expected": (T,3,H,W) broadcast views of one
     plane each, "surf_normal": (T,3,H,W), "radii": (T,P) int32, "visibility_filter": (T,P) bool}."""
@@ -792,6 +853,13 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
         if not isinstance(contributions, SurfelContributions):
             raise RuntimeError(f"contributions must be a SurfelContributions, got {type(contributions).__name__}")
         contributions.check(P, dev)
+        if contributions.silhouettes and masks is None:
+            raise RuntimeError("contributions has the background words (weight_bg_q, pixels_bg) but no masks were given")
+    if masks is not None:
+        if contributions is None or not contributions.silhouettes:
+            raise RuntimeError("masks need contributions with the background words: "
+                               "SurfelContributions.zeros(P, device, silhouettes=True)")
+        masks = _silhouette_masks(masks, T, H, W, dev)
     intr = _check_intrinsics(cameras.intrinsics, T, xyz)
     tanx, tany = (0.0, 0.0) if intr is not None else _cam_tans(cameras)     # the table replaces them
     N = H * W
@@ -816,6 +884,8 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
         if contributions is not None:
             out.contrib = _capi.SrContrib(contributions.weight_q.data_ptr(), contributions.max_weight.data_ptr(),
                                           contributions.pixels.data_ptr())
+        if masks is not None:
+            out.mask = _capi.SrContribMask(None, N, contributions.weight_bg_q.data_ptr(), contributions.pixels_bg.data_ptr())
 
         def forward(a, b, t0):
             """frames [a, b) of the chunk that starts at t0"""
@@ -823,6 +893,8 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
             # per-frame inputs are sliced (their strides stay); shared ones pass whole
             sl = {k: (v[c] if v is not None and strides.get(k, 0) else v) for k, v in ins.items()}
             out.color, out.features, out.others, out.radii = color[c], (feat[c] if F else None), allmap[a - t0:b - t0], radii[c]
+            if out.mask is not None:
+                out.mask.mask = masks[a].data_ptr()                 # this call's frames: a, a + 1, ... (stride H*W)
             # P = 0: the empty tensors give the device and F (their pointers pass as NULL)
             xyz_c = sl["means3D"] if sl["means3D"] is not None else xyz
             feat_c = sl["features"] if sl["features"] is not None else features
@@ -844,7 +916,7 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
             _capi.call("sr_post_forward_frames", dev, t1 - t0, W, H, tanx, tany, None if intr is None else intr[c],
                        float(pipe.depth_ratio), allmap[:t1 - t0], vm[c], bk, color[c], 3 * N, acc[c], rn[c], dist[c], med[c], ex[c],
                        sd[c], sn[c])
-        del out, allmap
+        del out, allmap, masks
         rets = {"render": color, "acc": acc, "rend_normal": rn, "rend_dist": dist, "surf_depth": sd.expand(T, 3, H, W),
                 "render_depth_median": med.expand(T, 3, H, W), "render_depth_expected": ex.expand(T, 3, H, W),
                 "surf_normal": sn, "radii": radii, "visibility_filter": radii > 0}

@@ -392,17 +392,21 @@ class FlatSurfelModel(torch.nn.Module):
         return n
 
     @torch.no_grad()
-    def prune_by_contribution(self, contrib, min_weight: float = 0.0, min_pixels: int = 1) -> int:
+    def prune_by_contribution(self, contrib, min_weight: float = 0.0, min_pixels: int = 1,
+                              max_background_fraction=None) -> int:
         """Prune every surfel whose summed blending weight over the rendered frames is below min_weight, or that
         contributed to fewer than min_pixels (frame, pixel) pairs: with the defaults, every surfel no frame blends (each
-        view sees it behind opaque ones, or culls it).  contrib: a renderer.SurfelContributions of this store's P surfels,
+        view sees it behind opaque ones, or culls it).  With max_background_fraction f, also every surfel whose share of
+        weight on the frames' background pixels (contrib.background_fraction, gathered by render_frames(...,
+        masks=)) is above f: a clump that floats off the object, which every view blends over background.  The default
+        None leaves the decision to the first two tests.  contrib: a renderer.SurfelContributions of this store's P surfels,
         filled by render_frames(contributions=) -- on several ranks, after distributed.allreduce_contributions, so that
         every rank prunes the same surfels.  Goes through prune_points: the Adam moments, statistics and regist_feat
         follow.  Returns the number pruned.  When none is, the buffers are left as they are (same addresses)."""
         self._live("prune_by_contribution")
         if contrib.P != self.P:
             raise RuntimeError(f"contributions are for {contrib.P} surfels, the store has {self.P}")
-        mask = contrib.prune_mask(min_weight, min_pixels).to(self.flat.device)
+        mask = contrib.prune_mask(min_weight, min_pixels, max_background_fraction).to(self.flat.device)
         n = int(mask.sum())
         if n:
             self.prune_points(mask)
