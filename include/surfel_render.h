@@ -96,6 +96,46 @@ SR_API int sr_render_forward_contrib_masked(const sr_frame* f, const sr_batch* b
                                             uint32_t* num_rendered_host, const sr_contrib* contrib,
                                             const sr_contrib_mask* mask, void* stream);
 
+/* Per-pixel maps lifted onto the surfels: each surfel's blending-weighted sum of C caller-supplied channels.
+ *   values         DEVICE floats: frame m's (C, H, W) planes, row-major, at values + m * values_stride
+ *   C              channels, 1..32
+ *   values_stride  floats between consecutive frames' values, >= C*H*W
+ *   scale_log2     s, in SR_LIFT_SCALE_MIN..SR_LIFT_SCALE_MAX.  A caller whose values stay within |v| <= B picks
+ *                  s = 32 - ceil(log2 B) once and keeps it for every call that adds into the same sums
+ *   sums           DEVICE [P * C] (signed 64-bit, row-major (P, C)): over the contributing pairs of surfel i,
+ *                  sums[i*C + c] += q,  q = round-to-nearest-even(fl(w * v) * 2^s),  fl(w * v) the float32 product of
+ *                  sr_contrib's weight w and the pixel's value v of channel c.  |q| <= 2^32 when |v| <= 2^(32-s).
+ *   saturated      DEVICE [1] (unsigned 64-bit): the number of (pair, channel) terms that were not exact -- a non-finite
+ *                  value, which contributes 0, or |fl(w * v) * 2^s| > 2^32, which contributes +-2^32.
+ * Two's-complement integer sums: exact, and independent of the order of pairs, frames, calls or ranks.  With v = 1 and
+ * s = 32, q is sr_contrib's q(w). */
+#define SR_LIFT_MAX_CHANNELS 32
+#define SR_LIFT_SCALE_MIN (-64)
+#define SR_LIFT_SCALE_MAX 64
+typedef struct sr_lift {
+    const float* values;
+    int32_t C;
+    int64_t values_stride;
+    int32_t scale_log2;
+    int64_t* sums;
+    uint64_t* saturated;
+} sr_lift;
+
+/* sr_render_forward_contrib, which it is in every argument, output and check, that also ADDS every rendered frame's
+ * lifted values into lift->sums and lift->saturated (never cleared here).  contrib's three words and the rendered
+ * outputs get exactly the bits sr_render_forward_contrib gives.  An overflowed frame adds nothing.  lift = NULL is
+ * sr_render_forward_contrib: the same kernels and bits.  Otherwise contrib must be non-NULL, F must be 0 (a lift is a
+ * colour-only walk), C in 1..32, values_stride >= C*H*W, scale_log2 in range and, with P > 0, values non-NULL and 4-byte
+ * aligned, sums and saturated non-NULL and 8-byte aligned. */
+SR_API int sr_render_forward_lift(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+                                  const float* means3D, const float* shs, const float* colors_precomp,
+                                  const float* opacities, const float* scales, const float* rotations,
+                                  const float* features, int32_t F, int64_t features_stride, const float* viewmatrix,
+                                  const float* projmatrix, const float* campos, float* out_color, int64_t out_color_stride,
+                                  float* out_features, int64_t out_features_stride, float* out_others, int32_t* radii,
+                                  void* arena, int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host,
+                                  const sr_contrib* contrib, const sr_lift* lift, void* stream);
+
 /* sr_post_forward over M frames in one launch: frame m's allmap (allmap + m*8*H*W) and world_view_transform (+ m*16) give
  * its acc, rend_normal, rend_dist, depth_median, depth_expected, surf_depth, surf_normal (each output packed (M, c, H, W)).
  * cameras: optional DEVICE (M,4) table of surfel_camera.h; with it frame m's rays use its own tangents and principal

@@ -18,8 +18,13 @@ SurfelContributions accumulator, with one that has the background words and the 
 without statistics again (alternating, L2 flushed before every timed call), at 512^2 and F in {0, 22}, scalar cameras.
 The silhouettes are the plain render's acc > 0.5.  Outputs and the four older words are compared bit for bit.
 
-Usage: python tools/bench_render.py [--frames 64] [--chunk 8] [--repeats 7] [--contrib | --silhouette [--rounds 3]]
-                                    [--out FILE]
+--lift measures lifting per-pixel maps onto the surfels: render_frames with a SurfelContributions accumulator alone,
+with it and a SurfelLift of C = 1, 16 and 32 channels (uniform values in [-1, 1], value bound 1), and with the
+accumulator alone again as the A/A control (alternating, L2 flushed before every timed call), at 512^2, F = 0, scalar
+cameras.  Outputs and the statistics are compared bit for bit with the accumulator-only arm.
+
+Usage: python tools/bench_render.py [--frames 64] [--chunk 8] [--repeats 7] [--contrib | --silhouette | --lift
+                                    [--rounds 3]] [--out FILE]
 """
 from __future__ import annotations
 
@@ -229,10 +234,10 @@ def contrib_main(args, gpu):
     return out
 
 
-def render_frames_contrib(cams, pc, bg, feat, chunk, acc, masks=None):
+def render_frames_contrib(cams, pc, bg, feat, chunk, acc, masks=None, lift=None, values=None):
     from vidu4d_b200.renderer import PipelineParams, render_frames
     return render_frames(cams, pc, PipelineParams(), bg, features=feat, frames_per_call=chunk, contributions=acc,
-                         masks=masks)
+                         masks=masks, lift=lift, values=values)
 
 
 def silhouette_main(args, gpu):
@@ -297,6 +302,68 @@ def silhouette_main(args, gpu):
     return out
 
 
+def lift_main(args, gpu):
+    """--lift: `rounds` rounds in one process; each times five arms alternating -- the accumulator alone, with lifts of
+    C = 1, 16 and 32 channels, and the accumulator alone again (the A/A control)."""
+    from vidu4d_b200.renderer import SurfelContributions, SurfelLift
+    from vidu4d_b200.synthetic import object_scene
+    dev = torch.device("cuda:0")
+    s = object_scene(args.P, seed=0, opacity="trained", center=(0.0, 0.0, 0.0)).to_torch(dev)
+    pc = _PC(s)
+    g = torch.Generator(device=dev).manual_seed(0)
+    flush = torch.empty((256 << 20,), dtype=torch.uint8, device=dev)
+    res = 512
+    cams = _cams(args.frames, res, dev, False)
+    bg = torch.zeros(3, device=dev)
+    Cs = (1, 16, 32)
+    values = {C: torch.rand((args.frames, C, res, res), device=dev, generator=g) * 2 - 1 for C in Cs}
+    acc = SurfelContributions.zeros(args.P, dev)
+    accs = {C: SurfelContributions.zeros(args.P, dev) for C in Cs}
+    lifts = {C: SurfelLift.zeros(args.P, C, dev) for C in Cs}
+
+    def stats(a, C=None):
+        for t in (a.weight_q, a.max_weight, a.pixels, a.frames):
+            t.zero_()
+        if C is None:
+            return render_frames_contrib(cams, pc, bg, None, args.chunk, a)
+        lifts[C].sums.zero_()
+        lifts[C].saturated.zero_()
+        return render_frames_contrib(cams, pc, bg, None, args.chunk, a, lift=lifts[C], values=values[C])
+
+    base = stats(acc)
+    check = {}
+    for C in Cs:
+        out = stats(accs[C], C)
+        check[C] = {"identical_outputs": all(_same(base[k], out[k]) for k in base if k != "visibility_filter"),
+                    "identical_words": all(torch.equal(getattr(acc, k), getattr(accs[C], k))
+                                           for k in ("weight_q", "max_weight", "pixels", "frames")),
+                    "saturated": int(lifts[C].saturated), "nonzero_sums": int((lifts[C].sums != 0).sum())}
+        del out
+    del base
+    print(json.dumps({"check": check, "pairs": int(acc.pixels.sum())}), flush=True)
+    rounds = []
+    for rd in range(args.rounds):
+        arms = {"contrib": lambda: stats(acc), **{f"lift{C}": (lambda C=C: stats(accs[C], C)) for C in Cs},
+                "contrib_again": lambda: stats(acc)}
+        for fn in arms.values():          # warm-up
+            fn()
+        times = {k: [] for k in arms}
+        for r in range(args.repeats):
+            for k, fn in arms.items():
+                times[k] += _flushed(fn, flush, 1, r)
+        row = {"round": rd, "res": res, "F": 0, **{k: _stat(v, args.frames) for k, v in times.items()}}
+        base_ms = 0.5 * (row["contrib"]["ms_median"] + row["contrib_again"]["ms_median"])
+        for C in Cs:
+            row[f"lift{C}_over_contrib"] = row[f"lift{C}"]["ms_median"] / base_ms - 1.0
+        row["contrib_gap"] = row["contrib_again"]["ms_median"] / row["contrib"]["ms_median"] - 1.0
+        print(json.dumps(row), flush=True)
+        rounds.append(row)
+    out = {"gpu": gpu, "frames": args.frames, "frames_per_call": args.chunk, "P": args.P, "repeats": args.repeats,
+           "check": {str(C): v for C, v in check.items()}, "rounds": rounds}
+    print(json.dumps(out))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=64)
@@ -305,7 +372,9 @@ def main():
     ap.add_argument("--P", type=int, default=300_000)
     ap.add_argument("--contrib", action="store_true", help="measure the contribution statistics and the prune by them")
     ap.add_argument("--silhouette", action="store_true", help="measure the background share of the statistics")
-    ap.add_argument("--rounds", type=int, default=3, help="--contrib / --silhouette: rounds of every measurement in one process")
+    ap.add_argument("--lift", action="store_true", help="measure lifting per-pixel maps onto the surfels")
+    ap.add_argument("--rounds", type=int, default=3,
+                    help="--contrib / --silhouette / --lift: rounds of every measurement in one process")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -315,8 +384,8 @@ def main():
     dev = torch.device("cuda:0")
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip()
-    if args.contrib or args.silhouette:
-        out = contrib_main(args, gpu) if args.contrib else silhouette_main(args, gpu)
+    if args.contrib or args.silhouette or args.lift:
+        out = contrib_main(args, gpu) if args.contrib else silhouette_main(args, gpu) if args.silhouette else lift_main(args, gpu)
         if args.out:
             os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
             with open(args.out, "w") as f:

@@ -26,6 +26,7 @@ from vidu4d_b200.build import NVCC_FLAGS, _nvcc  # noqa: E402
 SOURCES = ["composite_tile.cu", "composite_feat.cu", "composite_det.cu", "surfel_bwd.cu", "preprocess.cu", "composite_fwd.cu",
            "postprocess.cu"]
 _STATS = r"\((?:bool|<unnamed>::Stats)\)"      # composite_fwd_kernel's fourth template argument, either spelling
+_LW = r"(, \(int\)0)?"                          # its fifth, the lift's channel width, absent before the lift
 _FWD_ONLY = [(1, 0)] + [(v, nf) for nf in (8, 16, 24, 32) for v in (4, 2, 1)]
 # (demangled-name pattern in the base build, pattern of the same kernel in the working tree)
 KERNELS = [
@@ -43,19 +44,20 @@ KERNELS = [
     (r"mark_visible_kernel\(", r"mark_visible_kernel\("),
     # the training instantiation of the composite forward (the forward-only ones are <(bool)0, ...>).  A fourth template
     # parameter names what the forward-only walk gathers: (bool)0 / (bool)1 before the silhouette statistics, then the
-    # Stats enum's OFF = 0, WEIGHTS = 1 (the contribution statistics) and MASKED = 2 (their background share, new)
-    (rf"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0(, {_STATS}0)?>)?\(",
-     rf"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0(, {_STATS}0)?>)?\("),
-    # the forward-only instantiations without and with the contribution statistics: (V, NF) = (1, 0), and V in {4, 2, 1}
-    # for NF in {8, 16, 24, 32}
+    # Stats enum's OFF = 0, WEIGHTS = 1 (the contribution statistics), MASKED = 2 (their background share) and LIFT = 3
+    # (the lifted maps, new); a fifth, the lift's channel width, is (int)0 in every other instantiation
+    (rf"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0(, {_STATS}0{_LW})?>)?\(",
+     rf"composite_fwd_kernel(<\(bool\)1, \(int\)1, \(int\)0(, {_STATS}0{_LW})?>)?\("),
+    # the forward-only instantiations without and with the contribution statistics and with their background share:
+    # (V, NF) = (1, 0), and V in {4, 2, 1} for NF in {8, 16, 24, 32}
 ] + [
-    (rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}(, {_STATS}0)?>\(",
-     rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}(, {_STATS}0)?>\(")
+    (rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}(, {_STATS}0{_LW})?>\(",
+     rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}(, {_STATS}0{_LW})?>\(")
     for v, nf in _FWD_ONLY
 ] + [
-    (rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}, {_STATS}1>\(",
-     rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}, {_STATS}1>\(")
-    for v, nf in _FWD_ONLY
+    (rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}, {_STATS}{st}{_LW}>\(",
+     rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}, {_STATS}{st}{_LW}>\(")
+    for st in (1, 2) for v, nf in _FWD_ONLY
 ] + [
     (r"feature_fwd_kernel<\(int\)4>\(", r"feature_fwd_kernel<\(int\)4>\("),
     (r"feature_fwd_kernel<\(int\)2>\(", r"feature_fwd_kernel<\(int\)2>\("),

@@ -56,6 +56,18 @@ class SrContribMask(C.Structure):
     _fields_ = [("mask", C.c_void_p), ("mask_stride", C.c_int64), ("weight_bg_q", C.c_void_p), ("pixels_bg", C.c_void_p)]
 
 
+class SrLift(C.Structure):
+    """sr_lift (include/surfel_render.h): the DEVICE per-pixel values (frame m's (C,H,W) at values + m*values_stride
+    floats), the scale 2^scale_log2, and the DEVICE (P,C) int64 sums and [1] saturated counter sr_render_forward_lift
+    adds into."""
+    _fields_ = [("values", C.c_void_p), ("C", C.c_int32), ("values_stride", C.c_int64), ("scale_log2", C.c_int32),
+                ("sums", C.c_void_p), ("saturated", C.c_void_p)]
+
+
+LIFT_MAX_CHANNELS = 32                       # SR_LIFT_MAX_CHANNELS
+LIFT_SCALE_MIN, LIFT_SCALE_MAX = -64, 64     # SR_LIFT_SCALE_MIN, SR_LIFT_SCALE_MAX
+
+
 class SrDebugLayout(C.Structure):
     _fields_ = [
         ("surfel_rec", C.c_size_t), ("depths", C.c_size_t), ("tiles_touched", C.c_size_t),
@@ -174,6 +186,8 @@ RENDER_PROTOTYPES = {
                                   + [_p, _i64, _p, _i64] + [_p] * 3 + [_i64, _p, _p, _p, _p]),
     "sr_render_forward_contrib_masked": (C.c_int, [_FRAME, _BATCH, _p, _i32] + [_p] * 7 + [_i32, _i64] + [_p] * 3
                                          + [_p, _i64, _p, _i64] + [_p] * 3 + [_i64, _p, _p, _p, _p, _p]),
+    "sr_render_forward_lift": (C.c_int, [_FRAME, _BATCH, _p, _i32] + [_p] * 7 + [_i32, _i64] + [_p] * 3
+                               + [_p, _i64, _p, _i64] + [_p] * 3 + [_i64, _p, _p, _p, _p, _p]),
     "sr_post_forward_frames": (C.c_int, [_i32] * 3 + [_f32] * 2 + [_p, _f32] + [_p] * 4 + [_i64] + [_p] * 8),
 }
 RENDER_SYMBOLS = tuple(RENDER_PROTOTYPES)

@@ -215,6 +215,16 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
     if (!background || !viewmatrix || !campos) return sr_fail(SR_EINVAL, "camera / background pointer is NULL");
     if (contrib && contrib->mask && contrib->mask_stride < (long long)N)
         return sr_fail(SR_EINVAL, "silhouette mask frame stride must be >= H*W bytes");
+    if (contrib && contrib->lift) {
+        if (contrib->lift_C < 1 || contrib->lift_C > SR_LIFT_MAX_CHANNELS)
+            return sr_fail(SR_EINVAL, "lift: C must be in [1, %d], got %d", SR_LIFT_MAX_CHANNELS, contrib->lift_C);
+        if (ft) return sr_fail(SR_EINVAL, "lift: feature channels cannot be composited in the same call (F must be 0)");
+        if (contrib->lift_stride / 4 < (long long)contrib->lift_C * (long long)N)
+            return sr_fail(SR_EINVAL, "lift: values frame stride must be >= C*H*W floats");
+        if (contrib->lift_scale_log2 < SR_LIFT_SCALE_MIN || contrib->lift_scale_log2 > SR_LIFT_SCALE_MAX)
+            return sr_fail(SR_EINVAL, "lift: scale_log2 must be in [%d, %d], got %d", SR_LIFT_SCALE_MIN, SR_LIFT_SCALE_MAX,
+                           contrib->lift_scale_log2);
+    }
     if (ft) {
         if (color_stride < (int64_t)(3 * N)) return sr_fail(SR_EINVAL, "out_color frame stride must be >= 3*H*W");
         if (!ft->out) return sr_fail(SR_EINVAL, "out_features pointer is NULL");
@@ -242,6 +252,14 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
                     return sr_fail(SR_EINVAL, "silhouette statistics pointer is NULL");
                 if (((uintptr_t)contrib->weight_bg_q & 7) || ((uintptr_t)contrib->pixels_bg & 7))
                     return sr_fail(SR_EINVAL, "silhouette statistics: weight_bg_q / pixels_bg must be 8-byte aligned");
+            }
+            if (contrib->lift) {
+                if (!contrib->lift_values || !contrib->lift_sums || !contrib->lift_saturated)
+                    return sr_fail(SR_EINVAL, "lift: values / sums / saturated pointer is NULL");
+                if ((uintptr_t)contrib->lift_values & 3)
+                    return sr_fail(SR_EINVAL, "lift: values must be 4-byte aligned");
+                if (((uintptr_t)contrib->lift_sums & 7) || ((uintptr_t)contrib->lift_saturated & 7))
+                    return sr_fail(SR_EINVAL, "lift: sums / saturated must be 8-byte aligned");
             }
         }
         // 128-bit / 64-bit vector loads: rotations as float4, scales as float2, SH rows as float4 when 3M % 4 == 0
@@ -367,6 +385,46 @@ int sr_render_forward(const sr_frame* f, const sr_batch* b, const float* backgro
                          true);
 }
 
+// sr_render_forward_contrib_masked and sr_render_forward_lift: the statistics' arguments, then forward_entry
+static int render_forward_stats(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+                                const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
+                                const float* scales, const float* rotations, const float* features, int32_t F,
+                                int64_t features_stride, const float* viewmatrix, const float* campos, float* out_color,
+                                int64_t out_color_stride, float* out_features, int64_t out_features_stride,
+                                float* out_others, int32_t* radii, void* arena, int64_t capacity,
+                                uint32_t* num_rendered_dev, uint32_t* num_rendered_host, const sr_contrib* contrib,
+                                const sr_contrib_mask* mask, const sr_lift* lift, void* stream_) {
+    const bool masked = mask && mask->mask;
+    if (masked && !contrib) return sr_fail(SR_EINVAL, "a silhouette mask needs the contribution statistics (contrib is NULL)");
+    if (lift && !contrib) return sr_fail(SR_EINVAL, "a lift needs the contribution statistics (contrib is NULL)");
+    ContribArgs cs{};
+    if (lift) {
+        cs.lift = true;
+        cs.lift_C = lift->C;
+        cs.lift_values = lift->values;
+        cs.lift_stride = lift->values_stride * 4;
+        cs.lift_scale_log2 = lift->scale_log2;
+        cs.lift_scale = ldexpf(1.0f, lift->scale_log2);
+        cs.lift_sums = reinterpret_cast<long long*>(lift->sums);
+        cs.lift_saturated = reinterpret_cast<unsigned long long*>(lift->saturated);
+    }
+    if (contrib) {
+        cs.weight_q = reinterpret_cast<unsigned long long*>(contrib->weight_q);
+        cs.max_weight = contrib->max_weight;
+        cs.pixels = reinterpret_cast<unsigned long long*>(contrib->pixels);
+    }
+    if (masked) {
+        cs.mask = mask->mask;
+        cs.mask_stride = mask->mask_stride;
+        cs.weight_bg_q = reinterpret_cast<unsigned long long*>(mask->weight_bg_q);
+        cs.pixels_bg = reinterpret_cast<unsigned long long*>(mask->pixels_bg);
+    }
+    return forward_entry(f, b, background, bg_channels, means3D, shs, colors_precomp, opacities, scales, rotations, features, F,
+                         features_stride, viewmatrix, campos, out_color, out_color_stride, out_features, out_features_stride,
+                         out_others, radii, arena, nullptr, nullptr, capacity, num_rendered_dev, num_rendered_host, stream_,
+                         true, contrib ? &cs : nullptr);
+}
+
 int sr_render_forward_contrib(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
                               const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
                               const float* scales, const float* rotations, const float* features, int32_t F,
@@ -391,25 +449,26 @@ int sr_render_forward_contrib_masked(const sr_frame* f, const sr_batch* b, const
                                      uint32_t* num_rendered_dev, uint32_t* num_rendered_host, const sr_contrib* contrib,
                                      const sr_contrib_mask* mask, void* stream_) {
     (void)projmatrix;
-    const bool masked = mask && mask->mask;
-    if (masked && !contrib) return sr_fail(SR_EINVAL, "a silhouette mask needs the contribution statistics (contrib is NULL)");
-    ContribArgs cs{};
-    if (contrib) {
-        cs.weight_q = reinterpret_cast<unsigned long long*>(contrib->weight_q);
-        cs.max_weight = contrib->max_weight;
-        cs.pixels = reinterpret_cast<unsigned long long*>(contrib->pixels);
-    }
-    if (masked) {
-        cs.mask = mask->mask;
-        cs.mask_stride = mask->mask_stride;
-        cs.weight_bg_q = reinterpret_cast<unsigned long long*>(mask->weight_bg_q);
-        cs.pixels_bg = reinterpret_cast<unsigned long long*>(mask->pixels_bg);
-    }
-    return forward_entry(f, b, background, bg_channels, means3D, shs, colors_precomp, opacities, scales, rotations, features, F,
-                         features_stride, viewmatrix, campos, out_color, out_color_stride, out_features, out_features_stride,
-                         out_others, radii, arena, nullptr, nullptr, capacity, num_rendered_dev, num_rendered_host, stream_,
-                         true, contrib ? &cs : nullptr);
+    return render_forward_stats(f, b, background, bg_channels, means3D, shs, colors_precomp, opacities, scales, rotations,
+                                features, F, features_stride, viewmatrix, campos, out_color, out_color_stride, out_features,
+                                out_features_stride, out_others, radii, arena, capacity, num_rendered_dev, num_rendered_host,
+                                contrib, mask, nullptr, stream_);
 }
+
+int sr_render_forward_lift(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+                           const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
+                           const float* scales, const float* rotations, const float* features, int32_t F,
+                           int64_t features_stride, const float* viewmatrix, const float* projmatrix, const float* campos,
+                           float* out_color, int64_t out_color_stride, float* out_features, int64_t out_features_stride,
+                           float* out_others, int32_t* radii, void* arena, int64_t capacity, uint32_t* num_rendered_dev,
+                           uint32_t* num_rendered_host, const sr_contrib* contrib, const sr_lift* lift, void* stream_) {
+    (void)projmatrix;
+    return render_forward_stats(f, b, background, bg_channels, means3D, shs, colors_precomp, opacities, scales, rotations,
+                                features, F, features_stride, viewmatrix, campos, out_color, out_color_stride, out_features,
+                                out_features_stride, out_others, radii, arena, capacity, num_rendered_dev, num_rendered_host,
+                                contrib, nullptr, lift, stream_);
+}
+
 
 static int backward_batch(const sr_frame* f, const sr_batch* b, const float* background, const float* means3D, const float* shs,
                           const float* colors_precomp, const float* scales, const float* rotations, const float* viewmatrix,

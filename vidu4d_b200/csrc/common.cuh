@@ -181,6 +181,16 @@ struct ContribArgs {
     long long mask_stride;         // bytes
     unsigned long long* weight_bg_q;  // [P] sum of rn(w 2^32) over the background pairs
     unsigned long long* pixels_bg;    // [P] number of background pairs
+    // sr_render_forward_lift (lift = true): frame m's (C, H, W) values at lift_values + m*lift_stride, each pair's
+    // rn(w v 2^s) added into lift_sums[surfel * C + c], clamped and non-finite values counted in lift_saturated
+    bool lift;
+    int lift_C;                    // 1..32
+    const float* lift_values;
+    long long lift_stride;         // bytes
+    float lift_scale;              // 2^s
+    int lift_scale_log2;           // s
+    long long* lift_sums;          // [P * C]
+    unsigned long long* lift_saturated;  // [1]
 };
 struct FwdArgs {
     FrameStrides fs;

@@ -27,7 +27,12 @@
 //   * MASKED statistics (sr_render_forward_contrib_masked): each lane reads its pixel's foreground byte once, before
 //     the walk, and adds its pairs into a foreground or a background set of slots.  The flush adds both sets into the
 //     three words above, which get the unmasked walk's bits, and the background set alone into weight_bg_q and
-//     pixels_bg.
+//     pixels_bg;
+//   * LIFT (sr_render_forward_lift, DESIGN.md "lifting maps"): the WEIGHTS words, plus each surfel's weighted sum of
+//     C <= LW caller-supplied per-pixel values.  Each lane reads its pixel's C values once, before the walk; per pair and
+//     channel q = rn(fm(fm(w, v), 2^s)) is added into per-warp shared slots with two native 32-bit shared atomics, and
+//     after the stage lane i adds its instance's non-zero slots to lift[surfel * C + c] with 64-bit global atomics.
+//     Colour only (NF = 0): the staged values take the feature accumulator's registers.
 #include "composite_common.cuh"
 
 namespace {
@@ -35,9 +40,9 @@ using namespace comp;
 
 constexpr int WPC = 1;      // independent warps per CTA (2 measured slower: register pressure)
 
-// What the forward-only walk gathers besides its outputs: nothing, the contribution statistics, or the statistics and
-// their share on the frame's background pixels
-enum class Stats { OFF, WEIGHTS, MASKED };
+// What the forward-only walk gathers besides its outputs: nothing, the contribution statistics, the statistics and
+// their share on the frame's background pixels, or the statistics and the lifted per-pixel values
+enum class Stats { OFF, WEIGHTS, MASKED, LIFT };
 
 // A stage's statistics slots, per warp and instance jj: lo[jj] sums the low 16 bits of q = rn(w 2^32), hc[jj] the high
 // 16 bits plus 2^21 per pair.  q < 2^32 (w <= 0.99) and a stage has at most 32 pairs per instance, so neither word
@@ -58,16 +63,52 @@ __device__ __forceinline__ void stat_pair(StatSlots* ss, int jj, float T, float 
 struct MaskedSlots {
     StatSlots set[2];
 };
+// LIFT: a stage's channel sums, per warp, channel c and instance jj, as q = hi 2^16 + lo: lo[c][jj] sums the low 16 bits
+// of each q, hi[c][jj] the rest (q >> 16, arithmetic).  sm_90 has no native 64-bit shared add (atomicAdd on a 64-bit
+// shared word is a compare-and-swap loop); two 32-bit adds are.  |q| <= 2^32 and a stage has at most 32 pairs per
+// instance, so neither word overflows (32 (2^16 - 1) < 2^21, 32 (2^16 + 1) < 2^31).  Channel-major, so that the
+// flush's lanes (lane = instance) read consecutive words.
+template <int LW>
+struct LiftSlots {
+    uint32_t lo[LW][WB];
+    int32_t hi[LW][WB];
+};
+// One pair's C <= LW channels: q = rn(fm(fm(w, v), scale)), scale = 2^s, clamped to +-2^32 (each clamp counts in sat).
+// v holds the lane's staged values, 0 for a non-finite one, and nbad the number of those, which count once per pair:
+// they contribute 0.  fm(p, 2^s) is exact unless it leaves float's normal range; below it the exact product rounds to
+// 0 as well, above it is clamped.  A zero q skips its atomics (padding channels are always 0).
+template <int LW>
+__device__ __forceinline__ void lift_pair(LiftSlots<LW>* ls, int jj, float w, const float (&v)[LW], float scale,
+                                          uint32_t nbad, uint32_t& sat) {
+    sat += nbad;
+#pragma unroll
+    for (int c = 0; c < LW; c++) {
+        const float x = fm(fm(w, v[c]), scale);
+        long long q;
+        if (fabsf(x) > 4294967296.0f) {
+            q = x > 0.0f ? (1ll << 32) : -(1ll << 32);
+            sat++;
+        } else {
+            q = __float2ll_rn(x);
+        }
+        if (q != 0) {
+            atomicAdd(&ls->lo[c][jj], (uint32_t)q & 0xffffu);
+            atomicAdd(&ls->hi[c][jj], (int32_t)(q >> 16));
+        }
+    }
+}
 
-// TRAIN: the training forward (V, NF, STATS unused).  Otherwise forward-only with F <= NF feature channels (NF = 0:
-// none), rows gathered V floats per load, and with STATS != OFF the contribution statistics added into cs.
-template <bool TRAIN, int V, int NF, Stats STATS = Stats::OFF>
+// TRAIN: the training forward (V, NF, STATS, LW unused).  Otherwise forward-only with F <= NF feature channels (NF = 0:
+// none), rows gathered V floats per load, and with STATS != OFF the contribution statistics added into cs; with
+// STATS == LIFT (NF = 0) also the lift of cs.lift_C <= LW channels.
+template <bool TRAIN, int V, int NF, Stats STATS = Stats::OFF, int LW = 0>
 __global__ void __launch_bounds__(32 * WPC)
 composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, const uint32_t* __restrict__ tile_order, int n_items, int tiles_x,
                      const float4* __restrict__ irec, int W, int H,
                      const float* __restrict__ bg, float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
                      float* __restrict__ out_color, float* __restrict__ out_others, uint32_t* __restrict__ sub_last,
                      uint32_t* __restrict__ contrib_masks, const FeatArgs ft, const ContribArgs cs) {
+    static_assert(STATS != Stats::LIFT || (NF == 0 && LW > 0 && LW <= 32), "a lift is a colour-only walk of 1..32 channels");
     // WPC independent warps per CTA (the SM holds at most 32 CTAs): work item = (tile, 8x4 sub-tile), tiles in
     // longest-list-first order; the warps of a CTA share nothing
     __shared__ __align__(128) float4 st_all[WPC][NST][WB * REC4];
@@ -97,10 +138,31 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
         for (int b = 0; b < NST && b < nb; b++) ring.issue(b, b);
     }
     StatSlots* ss = nullptr;
-    if constexpr (STATS == Stats::WEIGHTS) {
+    if constexpr (STATS == Stats::WEIGHTS || STATS == Stats::LIFT) {
         __shared__ StatSlots ss_all[WPC];
         ss = &ss_all[threadIdx.x >> 5];
         ss->lo[lane] = 0u; ss->hc[lane] = 0u; ss->mx[lane] = 0u;
+    }
+    // LIFT: the warp's channel slots, and this lane's pixel's values in frame f, read once here (0 outside the image, for
+    // the padding channels c >= C and for a non-finite value, which nbad counts)
+    constexpr int LS = LW > 0 ? LW : 1;
+    LiftSlots<LS>* ls = nullptr;
+    float lv[LS];
+    uint32_t nbad = 0u, sat = 0u;
+    if constexpr (STATS == Stats::LIFT) {
+        __shared__ LiftSlots<LW> ls_all[WPC];
+        ls = &ls_all[threadIdx.x >> 5];
+        const bool in = sp.inside(W, H);
+        const size_t N = (size_t)W * H;
+        const float* v = fr(cs.lift_values, cs.lift_stride, f) + (in ? (size_t)W * sp.pix_y + sp.pix_x : 0);
+#pragma unroll
+        for (int c = 0; c < LW; c++) {
+            ls->lo[c][lane] = 0u; ls->hi[c][lane] = 0;
+            const float x = (in && c < cs.lift_C) ? __ldg(v + (size_t)c * N) : 0.0f;
+            const bool ok = isfinite(x);
+            nbad += ok ? 0u : 1u;
+            lv[c] = ok ? x : 0.0f;
+        }
     }
     // MASKED: the warp's two sets, and the one this lane's pairs add into, chosen by its pixel's mask byte in frame f,
     // read once here (a pixel outside the image has no pairs)
@@ -161,12 +223,13 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
                 auto pair = [&](float T, float alpha, const float4* __restrict__ R) {
                     feat_pair(T, alpha, R);
                     stat_pair(ss, jj, T, alpha);
+                    if constexpr (STATS == Stats::LIFT) lift_pair(ls, jj, ff(T, alpha, 0.0f), lv, cs.lift_scale, nbad, sat);
                 };
                 if (px.blend(S + jj * REC4, sp.pixx, sp.pixy, rho_cut, b * WB, jj, cmask, pair)) done = true;
             }
         }
         __syncwarp();                                   // every lane is done reading stage b
-        if constexpr (STATS == Stats::WEIGHTS) {
+        if constexpr (STATS == Stats::WEIGHTS || STATS == Stats::LIFT) {
             // lane = instance: its stage totals go to its surfel, and its slot is cleared for the next stage
             const uint32_t hc = ss->hc[lane];
             if (hc != 0u) {
@@ -175,6 +238,20 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
                 atomicMax(cs.max_weight + id, ss->mx[lane]);
                 atomicAdd(cs.pixels + id, (unsigned long long)(hc >> 21));
                 ss->lo[lane] = 0u; ss->hc[lane] = 0u; ss->mx[lane] = 0u;
+                if constexpr (STATS == Stats::LIFT) {
+                    // and its non-zero channel sums to lift[id * C + c] (two's complement: an unsigned add)
+                    unsigned long long* dst = reinterpret_cast<unsigned long long*>(cs.lift_sums) + (size_t)id * cs.lift_C;
+#pragma unroll
+                    for (int c = 0; c < LW; c++) {
+                        const uint32_t lo = ls->lo[c][lane];
+                        const int32_t hi = ls->hi[c][lane];
+                        if ((lo | (uint32_t)hi) != 0u) {
+                            const long long q = (long long)hi * 65536 + (long long)lo;
+                            if (q != 0) atomicAdd(dst + c, (unsigned long long)q);
+                            ls->lo[c][lane] = 0u; ls->hi[c][lane] = 0;
+                        }
+                    }
+                }
             }
         }
         if constexpr (STATS == Stats::MASKED) {
@@ -217,6 +294,13 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
         if (lane == 0) sub_last[tile * 8 + warp] = wmax;
         px.store(sp, W, H, bg, final_T, n_contrib, out_color, out_others);
     } else {
+        if constexpr (STATS == Stats::LIFT) {
+            // the warp's clamped and non-finite (pair, channel) count: one global atomic per warp, when non-zero
+            unsigned long long n = sat;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+            if (lane == 0 && n != 0ull) atomicAdd(cs.lift_saturated, n);
+        }
         px.store(sp, W, H, bg, out_color, out_others);
         if constexpr (NF > 0) {
             if (sp.inside(W, H)) {
@@ -232,7 +316,7 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
 
 // the forward-only instantiation for F channels (NF = F rounded up to a multiple of 8), vector width ft.vec and, with
 // STATS != OFF, the statistics cs
-template <int NF, Stats STATS>
+template <int NF, Stats STATS, int LW = 0>
 void launch_render(const FwdArgs& a, const FeatArgs& ft, const ContribArgs& cs, unsigned grid) {
     auto launch = [&](auto kern) {
         kern<<<grid, 32 * WPC, 0, a.stream>>>(
@@ -240,7 +324,7 @@ void launch_render(const FwdArgs& a, const FeatArgs& ft, const ContribArgs& cs, 
             (const float4*)(a.bin + a.bl.inst_rec), a.cam.W, a.cam.H, a.cam.bg, nullptr, nullptr, a.out_color, a.out_others,
             nullptr, nullptr, ft, cs);
     };
-    if constexpr (NF == 0) launch(composite_fwd_kernel<false, 1, 0, STATS>);
+    if constexpr (NF == 0) launch(composite_fwd_kernel<false, 1, 0, STATS, LW>);
     else if (ft.vec == 4) launch(composite_fwd_kernel<false, 4, NF, STATS>);
     else if (ft.vec == 2) launch(composite_fwd_kernel<false, 2, NF, STATS>);
     else launch(composite_fwd_kernel<false, 1, NF, STATS>);
@@ -253,6 +337,14 @@ void launch_render_f(const FwdArgs& a, const FeatArgs& ft, const ContribArgs& cs
     else if (ft.F <= 24) launch_render<24, STATS>(a, ft, cs, grid);
     else launch_render<32, STATS>(a, ft, cs, grid);
 }
+// the lift's instantiation for C channels (LW = C rounded up to a multiple of 8); no feature channels
+void launch_lift(const FwdArgs& a, const ContribArgs& cs, unsigned grid) {
+    const FeatArgs ft{};
+    if (cs.lift_C <= 8) launch_render<0, Stats::LIFT, 8>(a, ft, cs, grid);
+    else if (cs.lift_C <= 16) launch_render<0, Stats::LIFT, 16>(a, ft, cs, grid);
+    else if (cs.lift_C <= 24) launch_render<0, Stats::LIFT, 24>(a, ft, cs, grid);
+    else launch_render<0, Stats::LIFT, 32>(a, ft, cs, grid);
+}
 
 }  // namespace
 
@@ -262,6 +354,7 @@ cudaError_t launch_composite_fwd(const FwdArgs& a) {
         ProfileScope ps("composite_render", a.stream);
         const FeatArgs ft = a.feat ? *a.feat : FeatArgs{};
         if (!a.contrib) launch_render_f<Stats::OFF>(a, ft, ContribArgs{}, grid);
+        else if (a.contrib->lift) launch_lift(a, *a.contrib, grid);
         else if (a.contrib->mask) launch_render_f<Stats::MASKED>(a, ft, *a.contrib, grid);
         else launch_render_f<Stats::WEIGHTS>(a, ft, *a.contrib, grid);
         sr_count_launch();

@@ -12,6 +12,7 @@ backward) and the canonical-surfel gradients are summed across ranks once per op
     shared_generator()   the same random stream on every rank (densify_and_prune's split noise)
     check_replicas()     raise if the ranks' copies of some tensors differ in any bit (a debugging and test aid)
     allreduce_contributions()   every rank's per-surfel contribution statistics summed over the ranks, exactly
+    allreduce_lift()            every rank's lifted per-surfel sums summed over the ranks, exactly
 """
 from __future__ import annotations
 
@@ -128,6 +129,21 @@ def allreduce_contributions(contrib, group=None):
             dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
         dist.all_reduce(contrib.max_weight, op=dist.ReduceOp.MAX, group=group)
     return contrib
+
+
+def allreduce_lift(lift, group=None):
+    """Make every rank's renderer.SurfelLift that of all the ranks' frames: SUM over sums and saturated (int64, two's
+    complement: exact, whatever the order).  With allreduce_contributions over the same frames, every rank's
+    lift.mean(contrib) has the same bits.  Every rank must use the same scale_log2 (checked).  In place; returns lift.
+    No-op on one rank."""
+    if _multi_rank(group):
+        s = torch.tensor([lift.scale_log2, -lift.scale_log2], dtype=torch.int64, device=lift.sums.device)
+        dist.all_reduce(s, op=dist.ReduceOp.MAX, group=group)
+        if int(s[0]) != lift.scale_log2 or -int(s[1]) != lift.scale_log2:
+            raise RuntimeError(f"lift scales differ across ranks: scale_log2 from {-int(s[1])} to {int(s[0])}")
+        dist.all_reduce(lift.sums, op=dist.ReduceOp.SUM, group=group)
+        dist.all_reduce(lift.saturated, op=dist.ReduceOp.SUM, group=group)
+    return lift
 
 
 class FlatGrads:

@@ -269,12 +269,14 @@ class _RenderOut:
     adds its contribution statistics into (sr_render_forward_contrib), or None.  With it, a call of M > 1 frames that
     overflows is not re-run -- its other frames have added already -- and `overflowed` lists the frames to re-run alone.
     mask: with contrib, an _capi.SrContribMask whose `mask` points at this call's first frame's foreground mask: the call
-    also adds the background share of the statistics (sr_render_forward_contrib_masked); or None."""
-    __slots__ = ("color", "features", "others", "radii", "arena", "contrib", "overflowed", "mask")
+    also adds the background share of the statistics (sr_render_forward_contrib_masked); or None.  lift: with contrib,
+    an _capi.SrLift whose `values` points at this call's first frame's values: the call also adds its lifted values
+    (sr_render_forward_lift); or None."""
+    __slots__ = ("color", "features", "others", "radii", "arena", "contrib", "overflowed", "mask", "lift")
 
-    def __init__(self, color, features, others, radii, arena=None, contrib=None, mask=None):
+    def __init__(self, color, features, others, radii, arena=None, contrib=None, mask=None, lift=None):
         self.color, self.features, self.others, self.radii, self.arena = color, features, others, radii, arena
-        self.contrib, self.overflowed, self.mask = contrib, [], mask
+        self.contrib, self.overflowed, self.mask, self.lift = contrib, [], mask, lift
 
 
 def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, scales, rotations, features, viewmatrix,
@@ -337,6 +339,9 @@ def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, sc
                     render.arena = torch.empty((need,), dtype=torch.uint8, device=dev)
                 if render.contrib is None:
                     _capi.call("sr_render_forward", *args, render.arena, cap, nr_dev, host)
+                elif render.lift is not None:
+                    _capi.call("sr_render_forward_lift", *args, render.arena, cap, nr_dev, host, C.byref(render.contrib),
+                               C.byref(render.lift))
                 elif render.mask is not None:
                     _capi.call("sr_render_forward_contrib_masked", *args, render.arena, cap, nr_dev, host,
                                C.byref(render.contrib), C.byref(render.mask))

@@ -765,6 +765,104 @@ class SurfelContributions:
                 raise RuntimeError(f"contributions.{name} must be on the rasterizer's device {device}, got {t.device}")
 
 
+@dataclass
+class SurfelLift:
+    """Per-pixel maps lifted onto the surfels, added into by render_frames(..., contributions=, lift=, values=): for each
+    surfel i and channel c, over the contributing pairs (frame, pixel, surfel i) of the rendered frames,
+
+      sums[i, c] += q,   q = round-half-even(fl(w * v) * 2^scale_log2),
+
+    w the pair's weight (SurfelContributions' w = T * alpha) and v the pixel's value of channel c (include/surfel_render.h,
+    sr_lift).  sums is (P,C) int64, an exact two's-complement sum: the same bits for any order of the frames, any chunking
+    and, after distributed.allreduce_lift, any split over ranks.  saturated (1,) int64 counts the (pair, channel) terms
+    that were not exact: a non-finite value contributes 0, and |fl(w * v) * 2^s| > 2^32 contributes +-2^32.
+
+    scale_log2 s is fixed when the accumulator is made, from a bound B on |v|: s = 32 - ceil(log2 B), so that |q| <= 2^32
+    for every |v| <= B and a sum cannot overflow below 2^31 pairs.  It is never chosen from the data: sums made with
+    different scales do not add.  With v = 1 and B = 1, q is SurfelContributions' q(w), so sums[:, c] == weight_q."""
+    sums: torch.Tensor
+    saturated: torch.Tensor
+    scale_log2: int
+
+    @staticmethod
+    def scale_for(value_bound: float) -> int:
+        """s = 32 - ceil(log2 B), exactly (no floating-point logarithm); B must be in (2^-33, 2^96]."""
+        from . import _capi
+        B = value_bound
+        if isinstance(B, bool) or not isinstance(B, (int, float)) or not math.isfinite(float(B)) or float(B) <= 0.0:
+            raise RuntimeError(f"value_bound must be a finite positive number, got {B!r}")
+        m, e = math.frexp(float(B))                  # B = m 2^e, 0.5 <= m < 1
+        s = 32 - (e - 1 if m == 0.5 else e)
+        if not _capi.LIFT_SCALE_MIN <= s <= _capi.LIFT_SCALE_MAX:
+            raise RuntimeError(f"value_bound {B!r} gives scale_log2 {s}, outside [{_capi.LIFT_SCALE_MIN}, "
+                               f"{_capi.LIFT_SCALE_MAX}]: value_bound must be in (2^-33, 2^96]")
+        return s
+
+    @classmethod
+    def zeros(cls, P: int, C: int, device, value_bound: float = 1.0) -> "SurfelLift":
+        """An empty accumulator of C channels (1 <= C <= 32) for P surfels, for values with |v| <= value_bound."""
+        if isinstance(C, bool) or not isinstance(C, int) or not 1 <= C <= 32:
+            raise RuntimeError(f"C must be an int in [1, 32], got {C!r}")
+        return cls(torch.zeros((int(P), C), dtype=torch.int64, device=device),
+                   torch.zeros((1,), dtype=torch.int64, device=device), cls.scale_for(value_bound))
+
+    @property
+    def P(self) -> int:
+        return int(self.sums.shape[0])
+
+    @property
+    def C(self) -> int:
+        return int(self.sums.shape[1])
+
+    def mean(self, contrib: "SurfelContributions") -> torch.Tensor:
+        """(P,C) float64: each surfel's weighted mean of the lifted values, (sums 2^-s) / (weight_q 2^-32), each word
+        converted to float64 first; 0 where weight_q == 0.  contrib: the SurfelContributions the same render_frames calls
+        filled (on several ranks, both all-reduced)."""
+        if contrib.P != self.P:
+            raise RuntimeError(f"contributions are for {contrib.P} surfels, the lift for {self.P}")
+        wq = contrib.weight_q.to(self.sums.device, torch.float64)[:, None] * 2.0 ** -32
+        v = self.sums.to(torch.float64) * 2.0 ** -self.scale_log2
+        return torch.where(wq > 0, v / torch.where(wq > 0, wq, torch.ones_like(wq)), torch.zeros_like(v))
+
+    def check(self, P: int, device) -> None:
+        """Raise RuntimeError unless sums is a contiguous (P,C) int64 tensor with 1 <= C <= 32, saturated a (1,) int64
+        tensor, both on `device`, and scale_log2 an int in the library's range."""
+        from . import _capi
+        t = self.sums
+        if not torch.is_tensor(t) or t.dtype != torch.int64 or t.ndim != 2 or int(t.shape[0]) != P \
+                or not 1 <= int(t.shape[1]) <= 32 or not t.is_contiguous():
+            raise RuntimeError(f"lift.sums must be a contiguous torch.int64 (P,C) tensor with P = {P} and 1 <= C <= 32, "
+                               f"got {tuple(t.shape) if torch.is_tensor(t) else type(t).__name__}"
+                               f"{' ' + str(t.dtype) if torch.is_tensor(t) else ''}")
+        u = self.saturated
+        if not torch.is_tensor(u) or u.dtype != torch.int64 or tuple(u.shape) != (1,):
+            raise RuntimeError("lift.saturated must be a (1,) torch.int64 tensor")
+        for name, x in (("sums", t), ("saturated", u)):
+            if x.device != torch.device(device):
+                raise RuntimeError(f"lift.{name} must be on the rasterizer's device {device}, got {x.device}")
+        s = self.scale_log2
+        if isinstance(s, bool) or not isinstance(s, int) or not _capi.LIFT_SCALE_MIN <= s <= _capi.LIFT_SCALE_MAX:
+            raise RuntimeError(f"lift.scale_log2 must be an int in [{_capi.LIFT_SCALE_MIN}, {_capi.LIFT_SCALE_MAX}], "
+                               f"got {s!r}")
+
+
+def _lift_values(values, T, C, H, W, device):
+    """render_frames' values, checked: a contiguous (T,C,H,W) float32 tensor on `device`.  Nothing is converted or
+    copied here; a channels-last (T,H,W,C) map passes as maps.permute(0, 3, 1, 2).contiguous(), one explicit copy."""
+    if not torch.is_tensor(values):
+        raise RuntimeError(f"values must be a tensor, got {type(values).__name__}")
+    if tuple(values.shape) != (T, C, H, W):
+        raise RuntimeError(f"values must be (T,C,H,W) = ({T},{C},{H},{W}), got {tuple(values.shape)}")
+    if values.dtype != torch.float32:
+        raise RuntimeError(f"values must be float32, got {values.dtype}")
+    if values.device != torch.device(device):
+        raise RuntimeError(f"values must be on the rasterizer's device {device}, got {values.device}")
+    if not values.is_contiguous():
+        raise RuntimeError("values must be contiguous; a channels-last (T,H,W,C) map passes as "
+                           "maps.permute(0, 3, 1, 2).contiguous()")
+    return values.detach()
+
+
 def _check_render_frames(T, P, device, bg_color, means3D, rotations, features, learnable_bkgd, frames_per_call):
     """Validate render_frames' arguments before anything runs on the device; returns F."""
     if isinstance(frames_per_call, bool) or not isinstance(frames_per_call, int) or frames_per_call < 1:
@@ -808,7 +906,7 @@ def _silhouette_masks(masks, T, H, W, device):
 
 
 def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, features=None, learnable_bkgd=None,
-                  frames_per_call=8, contributions=None, masks=None):
+                  frames_per_call=8, contributions=None, masks=None, lift=None, values=None):
     """Render T frames forward-only: render_fused()'s outputs for every frame, with a leading frame dimension, and nothing
     differentiable -- no autograd graph is built, even when the inputs require grad.
 
@@ -838,6 +936,14 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
     and the other statistics have the same bits as without masks.  A pixel the frame cannot judge -- outside vis2d --
     should not count as background: pass masks = mask | ~vis2d.
 
+    lift, values: optional SurfelLift of P surfels and C channels (SurfelLift.zeros(P, C, device, value_bound)) and the
+    per-pixel maps to lift, a contiguous (T,C,H,W) float32 tensor on the surfels' device (a channels-last (T,H,W,C) map
+    passes as maps.permute(0, 3, 1, 2).contiguous(), one explicit copy).  Each surfel's weighted sums of the values at
+    its contributing pairs are added into lift.sums in the same walk (sr_render_forward_lift), with the same frame
+    bookkeeping as `contributions`, which a lift needs.  A lift renders colour only (no features) and takes no masks: a
+    background indicator channel, 1 on background pixels, lifted with value_bound 1, gives weight_bg_q.  The rendered
+    outputs and the statistics have the same bits as without a lift.
+
     Returns {"render": (T,3,H,W), "features": (T,F,H,W) (with features), "acc": (T,1,H,W), "rend_normal": (T,3,H,W),
     "rend_dist": (T,1,H,W), "surf_depth", "render_depth_median", "render_depth_expected": (T,3,H,W) broadcast views of one
     plane each, "surf_normal": (T,3,H,W), "radii": (T,P) int32, "visibility_filter": (T,P) bool}."""
@@ -848,6 +954,8 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
     T, H, W = len(cameras), int(cameras.image_height), int(cameras.image_width)
     xyz = pc.get_xyz if means3D is None else means3D
     P, dev = int(xyz.shape[-2]), xyz.device
+    if lift is not None and features is not None:
+        raise RuntimeError("lift renders colour only: features must be None")
     F = _check_render_frames(T, P, dev, bg_color, means3D, rotations, features, learnable_bkgd, frames_per_call)
     if contributions is not None:
         if not isinstance(contributions, SurfelContributions):
@@ -860,6 +968,19 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
             raise RuntimeError("masks need contributions with the background words: "
                                "SurfelContributions.zeros(P, device, silhouettes=True)")
         masks = _silhouette_masks(masks, T, H, W, dev)
+    if lift is not None:
+        if not isinstance(lift, SurfelLift):
+            raise RuntimeError(f"lift must be a SurfelLift, got {type(lift).__name__}")
+        if contributions is None:
+            raise RuntimeError("lift needs contributions: SurfelContributions.zeros(P, device)")
+        if masks is not None:
+            raise RuntimeError("lift and masks cannot be combined in one call: lift a background indicator channel instead")
+        lift.check(P, dev)
+        if values is None:
+            raise RuntimeError("lift needs values: the (T,C,H,W) maps to lift")
+        values = _lift_values(values, T, lift.C, H, W, dev)
+    elif values is not None:
+        raise RuntimeError("values are lifted into a SurfelLift: pass lift=SurfelLift.zeros(P, C, device)")
     intr = _check_intrinsics(cameras.intrinsics, T, xyz)
     tanx, tany = (0.0, 0.0) if intr is not None else _cam_tans(cameras)     # the table replaces them
     N = H * W
@@ -886,6 +1007,9 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
                                           contributions.pixels.data_ptr())
         if masks is not None:
             out.mask = _capi.SrContribMask(None, N, contributions.weight_bg_q.data_ptr(), contributions.pixels_bg.data_ptr())
+        if lift is not None:
+            out.lift = _capi.SrLift(None, lift.C, lift.C * N, lift.scale_log2, lift.sums.data_ptr(),
+                                    lift.saturated.data_ptr())
 
         def forward(a, b, t0):
             """frames [a, b) of the chunk that starts at t0"""
@@ -895,6 +1019,8 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
             out.color, out.features, out.others, out.radii = color[c], (feat[c] if F else None), allmap[a - t0:b - t0], radii[c]
             if out.mask is not None:
                 out.mask.mask = masks[a].data_ptr()                 # this call's frames: a, a + 1, ... (stride H*W)
+            if out.lift is not None:
+                out.lift.values = values[a].data_ptr()              # (stride C*H*W)
             # P = 0: the empty tensors give the device and F (their pointers pass as NULL)
             xyz_c = sl["means3D"] if sl["means3D"] is not None else xyz
             feat_c = sl["features"] if sl["features"] is not None else features
@@ -916,7 +1042,7 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
             _capi.call("sr_post_forward_frames", dev, t1 - t0, W, H, tanx, tany, None if intr is None else intr[c],
                        float(pipe.depth_ratio), allmap[:t1 - t0], vm[c], bk, color[c], 3 * N, acc[c], rn[c], dist[c], med[c], ex[c],
                        sd[c], sn[c])
-        del out, allmap, masks
+        del out, allmap, masks, values
         rets = {"render": color, "acc": acc, "rend_normal": rn, "rend_dist": dist, "surf_depth": sd.expand(T, 3, H, W),
                 "render_depth_median": med.expand(T, 3, H, W), "render_depth_expected": ex.expand(T, 3, H, W),
                 "surf_normal": sn, "radii": radii, "visibility_filter": radii > 0}
