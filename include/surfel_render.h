@@ -136,6 +136,41 @@ SR_API int sr_render_forward_lift(const sr_frame* f, const sr_batch* b, const fl
                                   void* arena, int64_t capacity, uint32_t* num_rendered_dev, uint32_t* num_rendered_host,
                                   const sr_contrib* contrib, const sr_lift* lift, void* stream);
 
+/* Each pixel's K heaviest contributing pairs, its anchors on the surfels.
+ *   K        slots per pixel: 1, 2, 4 or 8
+ *   stride   elements between consecutive frames of ids and weights, >= K*H*W; uv's frames are 2*stride apart
+ *   ids      DEVICE (frame, K, H, W) int32: the pair's surfel, -1 for an empty slot
+ *   weights  DEVICE (frame, K, H, W): the pair's w, sr_contrib's weight, 0 for an empty slot
+ *   uv       DEVICE (frame, K, 2, H, W): where the pixel's ray hits the surfel's disc, in its scaled tangent frame: the
+ *            surface point is mean + u*s_u*t_u + v*s_v*t_v, t_u and t_v the first two columns of the rotation and
+ *            s the scale, as the forward builds its homography.  A pair on the screen-space filter branch (its rho2d
+ *            below its rho3d, where the depth is the centre's) stores (0, 0), the centre.  (0, 0) for an empty slot.
+ * The slots are sorted by w, descending.  A pair enters only if its w is strictly larger than the last slot's, so among
+ * equal weights the earlier pair of the front-to-back walk stays ahead: the result is deterministic. */
+#define SR_ANCHORS_MAX 8
+typedef struct sr_anchors {
+    int32_t K;
+    int64_t stride;
+    int32_t* ids;
+    float* weights;
+    float* uv;
+} sr_anchors;
+
+/* sr_render_forward, which it is in every argument, output and check, that also WRITES every rendered frame's anchors
+ * (overwritten, never added into); the rendered outputs get exactly the bits sr_render_forward gives.  An overflowed
+ * frame writes no anchors: the caller re-runs it with a larger capacity.  P = 0 writes empty slots.  anchors must be
+ * non-NULL, K in {1, 2, 4, 8}, F must be 0 (anchors are a colour-only walk), stride >= K*H*W, and ids, weights and uv
+ * non-NULL and 4-byte aligned. */
+SR_API int sr_render_forward_anchors(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+                                     const float* means3D, const float* shs, const float* colors_precomp,
+                                     const float* opacities, const float* scales, const float* rotations,
+                                     const float* features, int32_t F, int64_t features_stride, const float* viewmatrix,
+                                     const float* projmatrix, const float* campos, float* out_color,
+                                     int64_t out_color_stride, float* out_features, int64_t out_features_stride,
+                                     float* out_others, int32_t* radii, void* arena, int64_t capacity,
+                                     uint32_t* num_rendered_dev, uint32_t* num_rendered_host, const sr_anchors* anchors,
+                                     void* stream);
+
 /* sr_post_forward over M frames in one launch: frame m's allmap (allmap + m*8*H*W) and world_view_transform (+ m*16) give
  * its acc, rend_normal, rend_dist, depth_median, depth_expected, surf_depth, surf_normal (each output packed (M, c, H, W)).
  * cameras: optional DEVICE (M,4) table of surfel_camera.h; with it frame m's rays use its own tangents and principal

@@ -23,8 +23,12 @@ with it and a SurfelLift of C = 1, 16 and 32 channels (uniform values in [-1, 1]
 accumulator alone again as the A/A control (alternating, L2 flushed before every timed call), at 512^2, F = 0, scalar
 cameras.  Outputs and the statistics are compared bit for bit with the accumulator-only arm.
 
-Usage: python tools/bench_render.py [--frames 64] [--chunk 8] [--repeats 7] [--contrib | --silhouette | --lift
-                                    [--rounds 3]] [--out FILE]
+--anchors measures keeping each pixel's heaviest pairs: render_frames plain, with anchors=1, 4 and 8, and plain again
+as the A/A control (alternating, L2 flushed before every timed call), at 512^2, F = 0, scalar cameras.  Outputs are
+compared bit for bit with the plain arm.
+
+Usage: python tools/bench_render.py [--frames 64] [--chunk 8] [--repeats 7] [--contrib | --silhouette | --lift |
+                                    --anchors [--rounds 3]] [--out FILE]
 """
 from __future__ import annotations
 
@@ -364,6 +368,54 @@ def lift_main(args, gpu):
     return out
 
 
+def anchors_main(args, gpu):
+    """--anchors: `rounds` rounds in one process; each times five arms alternating -- the plain render, with anchors of
+    K = 1, 4 and 8 slots, and the plain render again (the A/A control)."""
+    from vidu4d_b200.renderer import PipelineParams, render_frames
+    from vidu4d_b200.synthetic import object_scene
+    dev = torch.device("cuda:0")
+    s = object_scene(args.P, seed=0, opacity="trained", center=(0.0, 0.0, 0.0)).to_torch(dev)
+    pc = _PC(s)
+    flush = torch.empty((256 << 20,), dtype=torch.uint8, device=dev)
+    res = 512
+    cams = _cams(args.frames, res, dev, False)
+    bg = torch.zeros(3, device=dev)
+    Ks = (1, 4, 8)
+
+    def run(K=None):
+        return render_frames(cams, pc, PipelineParams(), bg, frames_per_call=args.chunk, anchors=K)
+
+    base = run()
+    check = {}
+    for K in Ks:
+        out = run(K)
+        check[K] = {"identical_outputs": all(_same(base[k], out[k]) for k in base if k != "visibility_filter"),
+                    "filled_slots": int((out["anchor_ids"] >= 0).sum())}
+        del out
+    del base
+    print(json.dumps({"check": check}), flush=True)
+    rounds = []
+    for rd in range(args.rounds):
+        arms = {"plain": lambda: run(), **{f"anchors{K}": (lambda K=K: run(K)) for K in Ks}, "plain_again": lambda: run()}
+        for fn in arms.values():          # warm-up
+            fn()
+        times = {k: [] for k in arms}
+        for r in range(args.repeats):
+            for k, fn in arms.items():
+                times[k] += _flushed(fn, flush, 1, r)
+        row = {"round": rd, "res": res, "F": 0, **{k: _stat(v, args.frames) for k, v in times.items()}}
+        base_ms = 0.5 * (row["plain"]["ms_median"] + row["plain_again"]["ms_median"])
+        for K in Ks:
+            row[f"anchors{K}_over_plain"] = row[f"anchors{K}"]["ms_median"] / base_ms - 1.0
+        row["plain_gap"] = row["plain_again"]["ms_median"] / row["plain"]["ms_median"] - 1.0
+        print(json.dumps(row), flush=True)
+        rounds.append(row)
+    out = {"gpu": gpu, "frames": args.frames, "frames_per_call": args.chunk, "P": args.P, "repeats": args.repeats,
+           "check": {str(K): v for K, v in check.items()}, "rounds": rounds}
+    print(json.dumps(out))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=64)
@@ -373,8 +425,9 @@ def main():
     ap.add_argument("--contrib", action="store_true", help="measure the contribution statistics and the prune by them")
     ap.add_argument("--silhouette", action="store_true", help="measure the background share of the statistics")
     ap.add_argument("--lift", action="store_true", help="measure lifting per-pixel maps onto the surfels")
+    ap.add_argument("--anchors", action="store_true", help="measure keeping each pixel's heaviest pairs")
     ap.add_argument("--rounds", type=int, default=3,
-                    help="--contrib / --silhouette / --lift: rounds of every measurement in one process")
+                    help="--contrib / --silhouette / --lift / --anchors: rounds of every measurement in one process")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -384,8 +437,9 @@ def main():
     dev = torch.device("cuda:0")
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip()
-    if args.contrib or args.silhouette or args.lift:
-        out = contrib_main(args, gpu) if args.contrib else silhouette_main(args, gpu) if args.silhouette else lift_main(args, gpu)
+    if args.contrib or args.silhouette or args.lift or args.anchors:
+        out = (contrib_main(args, gpu) if args.contrib else silhouette_main(args, gpu) if args.silhouette
+               else lift_main(args, gpu) if args.lift else anchors_main(args, gpu))
         if args.out:
             os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
             with open(args.out, "w") as f:

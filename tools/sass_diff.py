@@ -59,6 +59,11 @@ KERNELS = [
      rf"composite_fwd_kernel<\(bool\)0, \(int\){v}, \(int\){nf}, {_STATS}{st}{_LW}>\(")
     for st in (1, 2) for v, nf in _FWD_ONLY
 ] + [
+    # the lifts, colour-only walks of LW = 8, 16, 24 and 32 channels; the anchors (Stats 4) are new
+    (rf"composite_fwd_kernel<\(bool\)0, \(int\)1, \(int\)0, {_STATS}3, \(int\){lw}>\(",
+     rf"composite_fwd_kernel<\(bool\)0, \(int\)1, \(int\)0, {_STATS}3, \(int\){lw}>\(")
+    for lw in (8, 16, 24, 32)
+] + [
     (r"feature_fwd_kernel<\(int\)4>\(", r"feature_fwd_kernel<\(int\)4>\("),
     (r"feature_fwd_kernel<\(int\)2>\(", r"feature_fwd_kernel<\(int\)2>\("),
     (r"feature_fwd_kernel<\(int\)1>\(", r"feature_fwd_kernel<\(int\)1>\("),

@@ -68,6 +68,15 @@ LIFT_MAX_CHANNELS = 32                       # SR_LIFT_MAX_CHANNELS
 LIFT_SCALE_MIN, LIFT_SCALE_MAX = -64, 64     # SR_LIFT_SCALE_MIN, SR_LIFT_SCALE_MAX
 
 
+class SrAnchors(C.Structure):
+    """sr_anchors (include/surfel_render.h): K slots per pixel, the elements between frames of the DEVICE (frame,K,H,W)
+    ids and weights (uv's frames are twice as far apart), and the three DEVICE arrays sr_render_forward_anchors writes."""
+    _fields_ = [("K", C.c_int32), ("stride", C.c_int64), ("ids", C.c_void_p), ("weights", C.c_void_p), ("uv", C.c_void_p)]
+
+
+ANCHOR_SLOTS = (1, 2, 4, 8)                  # the K sr_render_forward_anchors takes (SR_ANCHORS_MAX = 8)
+
+
 class SrDebugLayout(C.Structure):
     _fields_ = [
         ("surfel_rec", C.c_size_t), ("depths", C.c_size_t), ("tiles_touched", C.c_size_t),
@@ -188,9 +197,19 @@ RENDER_PROTOTYPES = {
                                          + [_p, _i64, _p, _i64] + [_p] * 3 + [_i64, _p, _p, _p, _p, _p]),
     "sr_render_forward_lift": (C.c_int, [_FRAME, _BATCH, _p, _i32] + [_p] * 7 + [_i32, _i64] + [_p] * 3
                                + [_p, _i64, _p, _i64] + [_p] * 3 + [_i64, _p, _p, _p, _p, _p]),
+    "sr_render_forward_anchors": (C.c_int, [_FRAME, _BATCH, _p, _i32] + [_p] * 7 + [_i32, _i64] + [_p] * 3
+                                  + [_p, _i64, _p, _i64] + [_p] * 3 + [_i64, _p, _p, _p, _p]),
     "sr_post_forward_frames": (C.c_int, [_i32] * 3 + [_f32] * 2 + [_p, _f32] + [_p] * 4 + [_i64] + [_p] * 8),
 }
 RENDER_SYMBOLS = tuple(RENDER_PROTOTYPES)
+
+# tracking pixels through a sequence on their anchors, declared in include/surfel_track.h (own header and table for the
+# same reason)
+TRACK_PROTOTYPES = {
+    "sr_track_pixels": (C.c_int, [_i32] * 7 + [_p] * 4 + [_i64] + [_p, _i64, _p, _p, _i64] + [_p, _f32, _f32, _p]
+                        + [_p, _f32] + [_p] * 5),
+}
+TRACK_SYMBOLS = tuple(TRACK_PROTOTYPES)
 
 
 _lib = None
@@ -207,13 +226,13 @@ def load():
             "(or __graft_entry__.build()). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for s in (SYMBOLS + SSIM_SYMBOLS + OPTIM_SYMBOLS + SKIN_MLP_SYMBOLS + MASK_LOSS_SYMBOLS + CAMERA_SYMBOLS + DET_SYMBOLS
-              + RENDER_SYMBOLS):
+              + RENDER_SYMBOLS + TRACK_SYMBOLS):
         if not hasattr(lib, s):
             raise SurfelRasterError(f"{LIB_PATH} does not export {s}")
     for name, (restype, argtypes) in (list(PROTOTYPES.items()) + list(SSIM_PROTOTYPES.items()) + list(OPTIM_PROTOTYPES.items())
                                       + list(SKIN_MLP_PROTOTYPES.items()) + list(MASK_LOSS_PROTOTYPES.items())
                                       + list(CAMERA_PROTOTYPES.items()) + list(DET_PROTOTYPES.items())
-                                      + list(RENDER_PROTOTYPES.items())):
+                                      + list(RENDER_PROTOTYPES.items()) + list(TRACK_PROTOTYPES.items())):
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.sr_abi_version() != ABI_VERSION:

@@ -17,14 +17,14 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libsurfel_raster.so")
 SOURCES = ["api.cu", "preprocess.cu", "sort.cu", "composite_fwd.cu", "composite_tile.cu", "composite_feat.cu", "surfel_bwd.cu",
            "postprocess.cu", "loss.cu", "warp.cu", "match.cu", "cycle.cu", "feature_rows.cu", "optim.cu", "knn.cu", "outlier.cu", "ssim.cu",
-           "skin_mlp.cu", "mask_loss.cu", "composite_det.cu"]
+           "skin_mlp.cu", "mask_loss.cu", "composite_det.cu", "track.cu"]
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "composite_common.cuh"), os.path.join(CSRC, "post_common.cuh"),
-           os.path.join(CSRC, "warp_common.cuh"),
+           os.path.join(CSRC, "warp_common.cuh"), os.path.join(CSRC, "surfel_geom.cuh"),
            os.path.join(HERE, "..", "include", "surfel_raster.h"), os.path.join(HERE, "..", "include", "surfel_ssim.h"),
            os.path.join(HERE, "..", "include", "surfel_optim.h"), os.path.join(HERE, "..", "include", "surfel_skin_mlp.h"),
            os.path.join(HERE, "..", "include", "surfel_mask_loss.h"), os.path.join(HERE, "..", "include", "surfel_camera.h"),
            os.path.join(HERE, "..", "include", "surfel_deterministic.h"),
-           os.path.join(HERE, "..", "include", "surfel_render.h")]
+           os.path.join(HERE, "..", "include", "surfel_render.h"), os.path.join(HERE, "..", "include", "surfel_track.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",

@@ -26,6 +26,7 @@ std::atomic<uint64_t> g_launches{0};
     do {                                                     \
         if (debug) CK(cudaStreamSynchronize(stream), where); \
     } while (0)
+}  // namespace
 
 CamParams make_cam(const sr_frame* f, const float* vm, const float* campos, const float* bg) {
     CamParams c{};
@@ -48,6 +49,8 @@ CamParams make_cam(const sr_frame* f, const float* vm, const float* campos, cons
     c.cams = (f->flags & SR_FRAME_CAMERAS) ? reinterpret_cast<const sr_frame_cameras*>(f)->cameras : nullptr;
     return c;
 }
+
+namespace {
 
 int check_frame(const sr_frame* f) {
     if (!f) return sr_fail(SR_EINVAL, "frame descriptor is NULL");
@@ -213,9 +216,10 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
     const size_t N = (size_t)f->width * f->height;
     if (!out_color || !out_others || !num_rendered_dev) return sr_fail(SR_EINVAL, "output pointer is NULL");
     if (!background || !viewmatrix || !campos) return sr_fail(SR_EINVAL, "camera / background pointer is NULL");
-    if (contrib && contrib->mask && contrib->mask_stride < (long long)N)
+    const bool stats = contrib && !contrib->anchors;   // anchors gather none of the statistics
+    if (stats && contrib->mask && contrib->mask_stride < (long long)N)
         return sr_fail(SR_EINVAL, "silhouette mask frame stride must be >= H*W bytes");
-    if (contrib && contrib->lift) {
+    if (stats && contrib->lift) {
         if (contrib->lift_C < 1 || contrib->lift_C > SR_LIFT_MAX_CHANNELS)
             return sr_fail(SR_EINVAL, "lift: C must be in [1, %d], got %d", SR_LIFT_MAX_CHANNELS, contrib->lift_C);
         if (ft) return sr_fail(SR_EINVAL, "lift: feature channels cannot be composited in the same call (F must be 0)");
@@ -242,7 +246,7 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
             return sr_fail(SR_EINVAL, "scratch buffer is NULL");
         }
         if (capacity <= 0 || capacity >= (1ll << 30)) return sr_fail(SR_EINVAL, "capacity must be in (0, 2^30)");
-        if (contrib) {
+        if (stats) {
             if (!contrib->weight_q || !contrib->max_weight || !contrib->pixels)
                 return sr_fail(SR_EINVAL, "contribution statistics pointer is NULL");
             if (((uintptr_t)contrib->weight_q & 7) || ((uintptr_t)contrib->pixels & 7) || ((uintptr_t)contrib->max_weight & 3))
@@ -277,6 +281,13 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
             CK(cudaMemsetAsync(out_color, 0, (size_t)M * 3 * N * sizeof(float), stream), "memset(out_color)");
         }
         CK(cudaMemsetAsync(out_others, 0, (size_t)M * 8 * N * sizeof(float), stream), "memset(out_others)");
+        if (contrib && contrib->anchors) {
+            // every slot empty: id -1 (all bits set), w 0, uv (0, 0)
+            const size_t K = (size_t)contrib->anchor_K, pitch = (size_t)contrib->anchor_stride * 4;
+            CK(cudaMemset2DAsync(contrib->anchor_ids, pitch, 0xff, K * N * 4, (size_t)M, stream), "memset(anchor_ids)");
+            CK(cudaMemset2DAsync(contrib->anchor_w, pitch, 0, K * N * 4, (size_t)M, stream), "memset(anchor_weights)");
+            CK(cudaMemset2DAsync(contrib->anchor_uv, 2 * pitch, 0, 2 * K * N * 4, (size_t)M, stream), "memset(anchor_uv)");
+        }
         if (num_rendered_host)
             CK(cudaMemcpyAsync(num_rendered_host, num_rendered_dev, (size_t)M * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream), "copy(num_rendered)");
         return 0;
@@ -297,6 +308,12 @@ static int forward_batch(const sr_frame* f, const sr_batch* b, const float* back
     a.key_bits = 32 + (int)sr_higher_msb((uint32_t)a.il.tiles);
     a.stream = stream; a.debug = debug;
     a.forward_only = forward_only; a.feat = ft; a.contrib = contrib;
+    ContribArgs anchors{};
+    if (contrib && contrib->anchors) {   // the kernel reads each frame's status word to skip an overflowed frame
+        anchors = *contrib;
+        anchors.anchor_status = num_rendered_dev + 1;
+        a.contrib = &anchors;
+    }
     FrameStrides& fs = a.fs;
     fs.frames = M;
     fs.geom = (long long)a.gl.total; fs.bin = (long long)a.bl.total; fs.img = (long long)a.il.total; fs.nr = 2 * sizeof(uint32_t);
@@ -469,6 +486,36 @@ int sr_render_forward_lift(const sr_frame* f, const sr_batch* b, const float* ba
                                 contrib, nullptr, lift, stream_);
 }
 
+int sr_render_forward_anchors(const sr_frame* f, const sr_batch* b, const float* background, int32_t bg_channels,
+                              const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
+                              const float* scales, const float* rotations, const float* features, int32_t F,
+                              int64_t features_stride, const float* viewmatrix, const float* projmatrix, const float* campos,
+                              float* out_color, int64_t out_color_stride, float* out_features, int64_t out_features_stride,
+                              float* out_others, int32_t* radii, void* arena, int64_t capacity, uint32_t* num_rendered_dev,
+                              uint32_t* num_rendered_host, const sr_anchors* anchors, void* stream_) {
+    (void)projmatrix;
+    if (!anchors) return sr_fail(SR_EINVAL, "anchors is NULL");
+    const int K = anchors->K;
+    if (K != 1 && K != 2 && K != 4 && K != 8) return sr_fail(SR_EINVAL, "anchors: K must be 1, 2, 4 or 8, got %d", K);
+    if (F != 0) return sr_fail(SR_EINVAL, "anchors: feature channels cannot be composited in the same call (F must be 0)");
+    if (f && f->width > 0 && f->height > 0 && anchors->stride < (int64_t)K * f->width * f->height)
+        return sr_fail(SR_EINVAL, "anchors: frame stride must be >= K*H*W elements");
+    if (!anchors->ids || !anchors->weights || !anchors->uv)
+        return sr_fail(SR_EINVAL, "anchors: ids / weights / uv pointer is NULL");
+    if (((uintptr_t)anchors->ids & 3) || ((uintptr_t)anchors->weights & 3) || ((uintptr_t)anchors->uv & 3))
+        return sr_fail(SR_EINVAL, "anchors: ids / weights / uv must be 4-byte aligned");
+    ContribArgs cs{};
+    cs.anchors = true;
+    cs.anchor_K = K;
+    cs.anchor_stride = anchors->stride;
+    cs.anchor_ids = anchors->ids;
+    cs.anchor_w = anchors->weights;
+    cs.anchor_uv = anchors->uv;
+    return forward_entry(f, b, background, bg_channels, means3D, shs, colors_precomp, opacities, scales, rotations, features, F,
+                         features_stride, viewmatrix, campos, out_color, out_color_stride, out_features, out_features_stride,
+                         out_others, radii, arena, nullptr, nullptr, capacity, num_rendered_dev, num_rendered_host, stream_,
+                         true, &cs);
+}
 
 static int backward_batch(const sr_frame* f, const sr_batch* b, const float* background, const float* means3D, const float* shs,
                           const float* colors_precomp, const float* scales, const float* rotations, const float* viewmatrix,

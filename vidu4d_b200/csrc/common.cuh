@@ -170,20 +170,38 @@ struct FrameStrides {
 // ---- launchers implemented in the .cu files ------------------------------------------------
 struct FeatArgs;
 // Per-surfel contribution statistics of sr_render_forward_contrib (include/surfel_render.h), added into by every
-// contributing (frame, pixel, surfel) pair of the forward-only walk, w = T alpha rounded once
+// contributing (frame, pixel, surfel) pair of the forward-only walk, w = T alpha rounded once; or, with `anchors`, where
+// sr_render_forward_anchors writes each pixel's heaviest pairs instead.  The anchors' words share the statistics' bytes
+// and their flag the lift flag's padding, so that the kernel parameter keeps its size and the other walks their code.
 struct ContribArgs {
-    unsigned long long* weight_q;  // [P] sum of rn(w 2^32)
-    uint32_t* max_weight;          // [P] max of w, as float bits
-    unsigned long long* pixels;    // [P] number of pairs
-    // sr_render_forward_contrib_masked: frame m's H*W foreground bytes at mask + m*mask_stride (0 = background), and
-    // the two sums over the pairs on background pixels; mask = nullptr gathers the three words above alone
-    const uint8_t* mask;
-    long long mask_stride;         // bytes
-    unsigned long long* weight_bg_q;  // [P] sum of rn(w 2^32) over the background pairs
-    unsigned long long* pixels_bg;    // [P] number of background pairs
+    union {
+        struct {
+            unsigned long long* weight_q;  // [P] sum of rn(w 2^32)
+            uint32_t* max_weight;          // [P] max of w, as float bits
+            unsigned long long* pixels;    // [P] number of pairs
+            // sr_render_forward_contrib_masked: frame m's H*W foreground bytes at mask + m*mask_stride (0 = background),
+            // and the two sums over the pairs on background pixels; mask = nullptr gathers the three words above alone
+            const uint8_t* mask;
+            long long mask_stride;         // bytes
+            unsigned long long* weight_bg_q;  // [P] sum of rn(w 2^32) over the background pairs
+            unsigned long long* pixels_bg;    // [P] number of background pairs
+        };
+        struct {
+            // sr_render_forward_anchors: each pixel's anchor_K heaviest contributing pairs, frame m's (K, H, W) ids and
+            // weights at + m*anchor_stride elements, its (K, 2, H, W) hit coordinates at anchor_uv + 2m*anchor_stride; a
+            // frame whose status word (anchor_status + m*fs.nr bytes) has SR_STATUS_OVERFLOW set writes none
+            int32_t* anchor_ids;
+            float* anchor_w;
+            float* anchor_uv;
+            const uint32_t* anchor_status;
+            long long anchor_stride;       // elements
+            int anchor_K;                  // 1, 2, 4 or 8
+        };
+    };
     // sr_render_forward_lift (lift = true): frame m's (C, H, W) values at lift_values + m*lift_stride, each pair's
     // rn(w v 2^s) added into lift_sums[surfel * C + c], clamped and non-finite values counted in lift_saturated
     bool lift;
+    bool anchors;                  // sr_render_forward_anchors: the union holds the anchors' words, no statistics
     int lift_C;                    // 1..32
     const float* lift_values;
     long long lift_stride;         // bytes
@@ -240,6 +258,9 @@ struct FeatArgs {
     const float* grad_scale;                       // optional DEVICE scalar multiplying dout (nullptr = 1)
     float* dfeat;       long long dfeat_stride;    // backward: dL/dfeatures [P*F], zeroed by the launcher
 };
+
+// the forward's camera of an sr_frame (api.cu): intrinsics from its tangents, or its per-frame table
+CamParams make_cam(const sr_frame* f, const float* vm, const float* campos, const float* bg);
 
 cudaError_t launch_preprocess_fwd(const FwdArgs& a);      // preprocess.cu
 cudaError_t launch_scan_emit(const FwdArgs& a);           // preprocess.cu

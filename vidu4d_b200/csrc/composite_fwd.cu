@@ -33,6 +33,9 @@
 //     channel q = rn(fm(fm(w, v), 2^s)) is added into per-warp shared slots with two native 32-bit shared atomics, and
 //     after the stage lane i adds its instance's non-zero slots to lift[surfel * C + c] with 64-bit global atomics.
 //     Colour only (NF = 0): the staged values take the feature accumulator's registers.
+//   * ANCHORS (sr_render_forward_anchors, DESIGN.md "anchors"): each lane keeps its pixel's KA heaviest contributing pairs
+//     in registers as (surfel id, w, u, v), w the statistics' weight and (u, v) where the pixel's ray hits the disc, and
+//     writes them after the walk.  No atomics and no cross-lane traffic; colour only (NF = 0).
 #include "composite_common.cuh"
 
 namespace {
@@ -41,8 +44,9 @@ using namespace comp;
 constexpr int WPC = 1;      // independent warps per CTA (2 measured slower: register pressure)
 
 // What the forward-only walk gathers besides its outputs: nothing, the contribution statistics, the statistics and
-// their share on the frame's background pixels, or the statistics and the lifted per-pixel values
-enum class Stats { OFF, WEIGHTS, MASKED, LIFT };
+// their share on the frame's background pixels, the statistics and the lifted per-pixel values, or each pixel's
+// heaviest pairs alone
+enum class Stats { OFF, WEIGHTS, MASKED, LIFT, ANCHORS };
 
 // A stage's statistics slots, per warp and instance jj: lo[jj] sums the low 16 bits of q = rn(w 2^32), hc[jj] the high
 // 16 bits plus 2^21 per pair.  q < 2^32 (w <= 0.99) and a stage has at most 32 pairs per instance, so neither word
@@ -98,9 +102,35 @@ __device__ __forceinline__ void lift_pair(LiftSlots<LW>* ls, int jj, float w, co
     }
 }
 
+// ANCHORS: a pixel's KA heaviest pairs so far, sorted by w descending; among equal weights the earlier pair (the
+// front-most: the walk's order is fixed) stays ahead.  Empty slots hold id -1, w 0 and uv (0, 0); every contributing
+// pair has w > 0 (T >= 1e-4, alpha >= 1/255), so it enters an empty slot.
+template <int KA>
+struct AnchorSlots {
+    int32_t id[KA];
+    float w[KA], u[KA], v[KA];
+    __device__ __forceinline__ void clear() {
+#pragma unroll
+        for (int k = 0; k < KA; k++) { id[k] = -1; w[k] = 0.f; u[k] = 0.f; v[k] = 0.f; }
+    }
+    // A pair enters if its w is strictly larger than the last slot's: it takes the first slot of smaller weight and
+    // every slot from there on takes its predecessor's content (selects only: the slots stay in registers).
+    __device__ __forceinline__ void add(int32_t pid, float pw, float pu, float pv) {
+        bool shift = false;
+#pragma unroll
+        for (int k = 0; k < KA; k++) {
+            const bool take = shift || pw > w[k];
+            const int32_t ti = id[k]; const float tw = w[k], tu = u[k], tv = v[k];
+            if (take) { id[k] = pid; w[k] = pw; u[k] = pu; v[k] = pv; pid = ti; pw = tw; pu = tu; pv = tv; }
+            shift = take;
+        }
+    }
+};
+
 // TRAIN: the training forward (V, NF, STATS, LW unused).  Otherwise forward-only with F <= NF feature channels (NF = 0:
 // none), rows gathered V floats per load, and with STATS != OFF the contribution statistics added into cs; with
-// STATS == LIFT (NF = 0) also the lift of cs.lift_C <= LW channels.
+// STATS == LIFT (NF = 0) also the lift of cs.lift_C <= LW channels.  With STATS == ANCHORS (NF = 0) LW is the slot
+// count KA instead, and nothing is added into the statistics.
 template <bool TRAIN, int V, int NF, Stats STATS = Stats::OFF, int LW = 0>
 __global__ void __launch_bounds__(32 * WPC)
 composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, const uint32_t* __restrict__ tile_order, int n_items, int tiles_x,
@@ -109,6 +139,8 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
                      float* __restrict__ out_color, float* __restrict__ out_others, uint32_t* __restrict__ sub_last,
                      uint32_t* __restrict__ contrib_masks, const FeatArgs ft, const ContribArgs cs) {
     static_assert(STATS != Stats::LIFT || (NF == 0 && LW > 0 && LW <= 32), "a lift is a colour-only walk of 1..32 channels");
+    static_assert(STATS != Stats::ANCHORS || (NF == 0 && (LW == 1 || LW == 2 || LW == 4 || LW == 8)),
+                  "anchors are a colour-only walk of 1, 2, 4 or 8 slots");
     // WPC independent warps per CTA (the SM holds at most 32 CTAs): work item = (tile, 8x4 sub-tile), tiles in
     // longest-list-first order; the warps of a CTA share nothing
     __shared__ __align__(128) float4 st_all[WPC][NST][WB * REC4];
@@ -176,6 +208,10 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
         ss = &sm->set[bg_pixel ? 1 : 0];
     }
     __syncwarp();
+    // ANCHORS: this lane's pixel's slots
+    constexpr int KA = STATS == Stats::ANCHORS ? LW : 1;
+    AnchorSlots<KA> anc;
+    if constexpr (STATS == Stats::ANCHORS) anc.clear();
 
     FwdPixel px;
     bool done = !sp.inside(W, H);
@@ -219,6 +255,12 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
                 if (px.blend(S + jj * REC4, sp.pixx, sp.pixy, rho_cut, b * WB, jj, cmask)) done = true;
             } else if constexpr (STATS == Stats::OFF) {
                 if (px.blend(S + jj * REC4, sp.pixx, sp.pixy, rho_cut, b * WB, jj, cmask, feat_pair)) done = true;
+            } else if constexpr (STATS == Stats::ANCHORS) {
+                // the screen-space filter branch blends the centre's depth: its anchor is the centre, (0, 0)
+                auto pair = [&](float T, float alpha, const float4* __restrict__ R, float sx, float sy, bool disc) {
+                    anc.add((int32_t)__float_as_uint(R[4].z), ff(T, alpha, 0.0f), disc ? sx : 0.0f, disc ? sy : 0.0f);
+                };
+                if (px.blend(S + jj * REC4, sp.pixx, sp.pixy, rho_cut, b * WB, jj, cmask, pair)) done = true;
             } else {
                 auto pair = [&](float T, float alpha, const float4* __restrict__ R) {
                     feat_pair(T, alpha, R);
@@ -273,7 +315,7 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
                 for (int k = 0; k < 2; k++) { sm->set[k].lo[lane] = 0u; sm->set[k].hc[lane] = 0u; sm->set[k].mx[lane] = 0u; }
             }
         }
-        if constexpr (STATS != Stats::OFF) {
+        if constexpr (STATS != Stats::OFF && STATS != Stats::ANCHORS) {
             __syncwarp();                               // slots cleared and stage b read before its slot is refilled
         }
         if constexpr (TRAIN) cm_out[(size_t)b * SR_CONTRIB_STAGE_WORDS] = cmask;
@@ -302,6 +344,22 @@ composite_fwd_kernel(const FrameStrides fs, const uint2* __restrict__ ranges, co
             if (lane == 0 && n != 0ull) atomicAdd(cs.lift_saturated, n);
         }
         px.store(sp, W, H, bg, out_color, out_others);
+        if constexpr (STATS == Stats::ANCHORS) {
+            // every slot, empty ones included, unless the frame overflowed (its walk saw no pairs; the caller re-runs it)
+            if (sp.inside(W, H) && !(__ldg(fr(cs.anchor_status, fs.nr, f)) & SR_STATUS_OVERFLOW)) {
+                const size_t N = (size_t)W * H, pid = (size_t)W * sp.pix_y + sp.pix_x;
+                int32_t* ids = fr(cs.anchor_ids, cs.anchor_stride * 4, f) + pid;
+                float* ws = fr(cs.anchor_w, cs.anchor_stride * 4, f) + pid;
+                float* uv = fr(cs.anchor_uv, cs.anchor_stride * 8, f) + pid;
+#pragma unroll
+                for (int k = 0; k < KA; k++) {
+                    ids[k * N] = anc.id[k];
+                    ws[k * N] = anc.w[k];
+                    uv[2 * k * N] = anc.u[k];
+                    uv[(2 * k + 1) * N] = anc.v[k];
+                }
+            }
+        }
         if constexpr (NF > 0) {
             if (sp.inside(W, H)) {
                 const size_t N = (size_t)W * H, pid = (size_t)W * sp.pix_y + sp.pix_x;
@@ -345,6 +403,14 @@ void launch_lift(const FwdArgs& a, const ContribArgs& cs, unsigned grid) {
     else if (cs.lift_C <= 24) launch_render<0, Stats::LIFT, 24>(a, ft, cs, grid);
     else launch_render<0, Stats::LIFT, 32>(a, ft, cs, grid);
 }
+// the anchors' instantiation for K slots; no feature channels
+void launch_anchors(const FwdArgs& a, const ContribArgs& cs, unsigned grid) {
+    const FeatArgs ft{};
+    if (cs.anchor_K == 1) launch_render<0, Stats::ANCHORS, 1>(a, ft, cs, grid);
+    else if (cs.anchor_K == 2) launch_render<0, Stats::ANCHORS, 2>(a, ft, cs, grid);
+    else if (cs.anchor_K == 4) launch_render<0, Stats::ANCHORS, 4>(a, ft, cs, grid);
+    else launch_render<0, Stats::ANCHORS, 8>(a, ft, cs, grid);
+}
 
 }  // namespace
 
@@ -354,6 +420,7 @@ cudaError_t launch_composite_fwd(const FwdArgs& a) {
         ProfileScope ps("composite_render", a.stream);
         const FeatArgs ft = a.feat ? *a.feat : FeatArgs{};
         if (!a.contrib) launch_render_f<Stats::OFF>(a, ft, ContribArgs{}, grid);
+        else if (a.contrib->anchors) launch_anchors(a, *a.contrib, grid);
         else if (a.contrib->lift) launch_lift(a, *a.contrib, grid);
         else if (a.contrib->mask) launch_render_f<Stats::MASKED>(a, ft, *a.contrib, grid);
         else launch_render_f<Stats::WEIGHTS>(a, ft, *a.contrib, grid);

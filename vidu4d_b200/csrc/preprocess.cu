@@ -16,6 +16,7 @@
 // contraction pattern of the reference's sm_100a SASS (DESIGN.md "FMA map"), so tile assignment and
 // sort keys are identical to the reference build, not merely close.
 #include "common.cuh"
+#include "surfel_geom.cuh"
 
 namespace {
 
@@ -31,23 +32,12 @@ __constant__ float kSH_C3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.457
                                 0.3731763325901154f, -0.4570457994644658f, 1.445305721320277f,
                                 -0.5900435899266435f};
 
-struct View { float m[16]; };
-__device__ __forceinline__ View load_view(const float* __restrict__ vm) {
-    View v;
-#pragma unroll
-    for (int i = 0; i < 16; i++) v.m[i] = __ldg(vm + i);
-    return v;
-}
-// view-space z exactly as transformPoint4x3 contracts it in the reference build
-__device__ __forceinline__ float view_z(const View& c, float x, float y, float z) {
-    return fa(ff(z, c.m[10], ff(x, c.m[2], fm(y, c.m[6]))), c.m[14]);
-}
-// glm mat3(W) * v
-__device__ __forceinline__ float3 w_mul(const View& c, float3 v) {
-    return make_float3(ff(v.z, c.m[8], ff(v.x, c.m[0], fm(v.y, c.m[4]))),
-                       ff(v.z, c.m[9], ff(v.x, c.m[1], fm(v.y, c.m[5]))),
-                       ff(v.z, c.m[10], ff(v.x, c.m[2], fm(v.y, c.m[6]))));
-}
+// the view transform and the rotation matrix: one copy in surfel_geom.cuh, shared with the tracking kernel
+using sgeo::View;
+using sgeo::load_view;
+using sgeo::view_z;
+using sgeo::w_mul;
+using sgeo::rot_matrix;
 
 // auxiliary.h:64-74: one copy in common.cuh, shared with the deterministic backward's emission index
 __device__ __forceinline__ void get_rect(float px, float py, int max_radius, int gx, int gy, uint2& rmin, uint2& rmax) {
@@ -148,24 +138,6 @@ __device__ __forceinline__ void stage_sh(float* shbuf, const float* __restrict__
     } else {
         for (int i = threadIdx.x; i < total; i += 256) { const int r = i / M3; shbuf[r * stride + (i - r * M3)] = __ldg(gsrc + i); }
     }
-}
-
-// computeTransMat's rotation matrix R (row-major) of the quaternion q = (w,x,y,z); glm names .x=w .y=x .z=y .w=z
-__device__ __forceinline__ void rot_matrix(float4 q, float R[9]) {
-    const float n2 = ff(q.z, q.z, ff(q.y, q.y, ff(q.w, q.w, fm(q.x, q.x))));
-    const float s = rsqrtf(n2);
-    const float w = fm(q.x, s), x = fm(q.y, s), y = fm(q.z, s), z = fm(q.w, s);
-    const float wz = fm(w, z), wy = fm(w, y), wx = fm(w, x), yy = fm(y, y), zz = fm(z, z);
-    float t;
-    t = fa(yy, zz);        R[0] = fa(1.f, -fa(t, t));
-    t = ff(x, y, wz);      R[1] = fa(t, t);
-    t = ff(x, z, -wy);     R[2] = fa(t, t);
-    t = ff(x, y, -wz);     R[3] = fa(t, t);
-    t = ff(x, x, zz);      R[4] = fa(1.f, -fa(t, t));
-    t = ff(y, z, wx);      R[5] = fa(t, t);
-    t = ff(x, z, wy);      R[6] = fa(t, t);
-    t = ff(y, z, -wx);     R[7] = fa(t, t);
-    t = ff(x, x, yy);      R[8] = fa(1.f, -fa(t, t));
 }
 
 // One thread owns one surfel for every frame of the batch (grid = ceil(P/256) blocks).  An input whose frame stride is 0

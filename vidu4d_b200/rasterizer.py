@@ -271,12 +271,14 @@ class _RenderOut:
     mask: with contrib, an _capi.SrContribMask whose `mask` points at this call's first frame's foreground mask: the call
     also adds the background share of the statistics (sr_render_forward_contrib_masked); or None.  lift: with contrib,
     an _capi.SrLift whose `values` points at this call's first frame's values: the call also adds its lifted values
-    (sr_render_forward_lift); or None."""
-    __slots__ = ("color", "features", "others", "radii", "arena", "contrib", "overflowed", "mask", "lift")
+    (sr_render_forward_lift); or None.  anchors: without contrib, an _capi.SrAnchors whose arrays point at this call's
+    first frame's slots: the call also writes each pixel's heaviest pairs (sr_render_forward_anchors), overwriting them,
+    so an overflowed call re-runs whole as the plain render does; or None."""
+    __slots__ = ("color", "features", "others", "radii", "arena", "contrib", "overflowed", "mask", "lift", "anchors")
 
-    def __init__(self, color, features, others, radii, arena=None, contrib=None, mask=None, lift=None):
+    def __init__(self, color, features, others, radii, arena=None, contrib=None, mask=None, lift=None, anchors=None):
         self.color, self.features, self.others, self.radii, self.arena = color, features, others, radii, arena
-        self.contrib, self.overflowed, self.mask, self.lift = contrib, [], mask, lift
+        self.contrib, self.overflowed, self.mask, self.lift, self.anchors = contrib, [], mask, lift, anchors
 
 
 def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, scales, rotations, features, viewmatrix,
@@ -337,7 +339,9 @@ def _forward(M, frame_dim, strides, background, means3D, sh, colors, opacity, sc
                 if render.arena is None or render.arena.numel() < need:
                     render.arena = None                  # release the smaller arena before allocating its successor
                     render.arena = torch.empty((need,), dtype=torch.uint8, device=dev)
-                if render.contrib is None:
+                if render.anchors is not None:
+                    _capi.call("sr_render_forward_anchors", *args, render.arena, cap, nr_dev, host, C.byref(render.anchors))
+                elif render.contrib is None:
                     _capi.call("sr_render_forward", *args, render.arena, cap, nr_dev, host)
                 elif render.lift is not None:
                     _capi.call("sr_render_forward_lift", *args, render.arena, cap, nr_dev, host, C.byref(render.contrib),

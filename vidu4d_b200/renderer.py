@@ -906,7 +906,7 @@ def _silhouette_masks(masks, T, H, W, device):
 
 
 def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, features=None, learnable_bkgd=None,
-                  frames_per_call=8, contributions=None, masks=None, lift=None, values=None):
+                  frames_per_call=8, contributions=None, masks=None, lift=None, values=None, anchors=None):
     """Render T frames forward-only: render_fused()'s outputs for every frame, with a leading frame dimension, and nothing
     differentiable -- no autograd graph is built, even when the inputs require grad.
 
@@ -944,6 +944,15 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
     background indicator channel, 1 on background pixels, lifted with value_bound 1, gives weight_bg_q.  The rendered
     outputs and the statistics have the same bits as without a lift.
 
+    anchors: optional slot count K in {1, 2, 4, 8}.  Each pixel's K heaviest contributing pairs are kept in the same walk
+    (sr_render_forward_anchors) and returned as "anchor_ids" (T,K,H,W) int32 (the surfel, -1 for an empty slot),
+    "anchor_weights" (T,K,H,W) (the pair's w, SurfelContributions' weight; 0 for an empty slot), sorted descending with
+    the front-most pair first among equal weights, and "anchor_uv" (T,K,2,H,W) (where the pixel's ray hits the disc, in
+    its scaled tangent frame: the point mean + u*s_u*t_u + v*s_v*t_v; (0, 0), the centre, on the screen-space filter
+    branch and in an empty slot).  tracking.track_pixels follows these pixels through the sequence.  Anchors render
+    colour only and combine with none of features, contributions, masks or lift.  Every other output has the same bits
+    as without anchors.  They take 16 B per slot and pixel: K = 4 at 512 x 512 is 16.8 MB per frame.
+
     Returns {"render": (T,3,H,W), "features": (T,F,H,W) (with features), "acc": (T,1,H,W), "rend_normal": (T,3,H,W),
     "rend_dist": (T,1,H,W), "surf_depth", "render_depth_median", "render_depth_expected": (T,3,H,W) broadcast views of one
     plane each, "surf_normal": (T,3,H,W), "radii": (T,P) int32, "visibility_filter": (T,P) bool}."""
@@ -956,6 +965,12 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
     P, dev = int(xyz.shape[-2]), xyz.device
     if lift is not None and features is not None:
         raise RuntimeError("lift renders colour only: features must be None")
+    if anchors is not None:
+        if isinstance(anchors, bool) or not isinstance(anchors, int) or anchors not in _capi.ANCHOR_SLOTS:
+            raise RuntimeError(f"anchors must be a slot count in {_capi.ANCHOR_SLOTS}, got {anchors!r}")
+        for name, arg in (("features", features), ("contributions", contributions), ("masks", masks), ("lift", lift)):
+            if arg is not None:
+                raise RuntimeError(f"anchors render colour only and gather no statistics: {name} must be None")
     F = _check_render_frames(T, P, dev, bg_color, means3D, rotations, features, learnable_bkgd, frames_per_call)
     if contributions is not None:
         if not isinstance(contributions, SurfelContributions):
@@ -1007,6 +1022,11 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
                                           contributions.pixels.data_ptr())
         if masks is not None:
             out.mask = _capi.SrContribMask(None, N, contributions.weight_bg_q.data_ptr(), contributions.pixels_bg.data_ptr())
+        if anchors is not None:
+            K = anchors
+            a_ids = torch.empty((T, K, H, W), dtype=torch.int32, device=dev)
+            a_w, a_uv = mk(K, H, W), mk(K, 2, H, W)
+            out.anchors = _capi.SrAnchors(K, K * N, None, None, None)
         if lift is not None:
             out.lift = _capi.SrLift(None, lift.C, lift.C * N, lift.scale_log2, lift.sums.data_ptr(),
                                     lift.saturated.data_ptr())
@@ -1021,6 +1041,9 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
                 out.mask.mask = masks[a].data_ptr()                 # this call's frames: a, a + 1, ... (stride H*W)
             if out.lift is not None:
                 out.lift.values = values[a].data_ptr()              # (stride C*H*W)
+            if out.anchors is not None:                             # (stride K*H*W; uv 2*K*H*W)
+                out.anchors.ids, out.anchors.weights, out.anchors.uv = (a_ids[a].data_ptr(), a_w[a].data_ptr(),
+                                                                        a_uv[a].data_ptr())
             # P = 0: the empty tensors give the device and F (their pointers pass as NULL)
             xyz_c = sl["means3D"] if sl["means3D"] is not None else xyz
             feat_c = sl["features"] if sl["features"] is not None else features
@@ -1048,4 +1071,6 @@ def render_frames(cameras, pc, pipe, bg_color, means3D=None, rotations=None, fea
                 "surf_normal": sn, "radii": radii, "visibility_filter": radii > 0}
         if F:
             rets["features"] = feat
+        if anchors is not None:
+            rets["anchor_ids"], rets["anchor_weights"], rets["anchor_uv"] = a_ids, a_w, a_uv
     return rets
